@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- BIN hot path on B200: 720p frame-windows/sec (BASELINE.json metric).
+"""bench.py -- BIN hot path on H100: 720p frame-windows/sec (BASELINE.json metric).
 
 One "step" = `--windows-per-step` (default 5) forwards of the shipped 6-frame bin_stage4 network (the path test.py
 runs, SURVEY 8d config 2b) on independent synthetic 1280x720 windows per GPU; windows are independent, so N GPUs run
@@ -8,12 +8,15 @@ excluded from the timed region and timed separately).  Five windows per step mak
 20-step run ~3 s, long enough that one slow rank shows up in the per-rank record instead of in the noise.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference|reference-cuda]
-                    [--height H --width W] [--windows-per-step S] [--no-extras]
+                    [--height H --width W] [--windows-per-step S] [--no-extras] [--dump-outputs DIR]
 
 Prints ONE JSON line (rank 0).  `value` = device-resident windows/s, `e2e` = the same metric through the module call
 with pinned-host inputs (6 frames H2D per window) and the 3 images test.py writes (outputs 13, 8, 12) copied back D2H
 inside the timed region.  `--impl reference` times the reference's CPU PyTorch path (the unmodified reference when it
-is present on the machine, else the line-cited oracle port) on REAL 1280x720 windows.
+is present under baseline/_ref, else the line-cited oracle port) on REAL 1280x720 windows.
+`--dump-outputs DIR` writes, after the timed steps, the 14 outputs of every window of the last timed step (recomputed
+untimed from the same inputs and checked bit for bit against the last window's timed outputs) as
+DIR/window<i>_out<k>.npy (float32; a fixed seeded sample of each flattened output when all of them would exceed 64 MB).
 """
 from __future__ import annotations
 
@@ -37,7 +40,8 @@ LAUNCHES_PER_WINDOW = 4 * (1 + 42 + 12) + 3
 
 
 def peaks():
-    p = {"bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "hbm_gbs": 6650.0, "source": "fallback"}
+    # fallback = the H100 SXM data sheet (dense fp16/bf16, HBM3): peaks to divide by, not rates this code reaches
+    p = {"bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "hbm_gbs": 3350.0, "source": "fallback"}
     try:
         d = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         p.update({k: d[k] for k in ("bf16_tflops", "bf16_tflops_sustained", "hbm_gbs") if k in d})
@@ -99,16 +103,13 @@ class ClockSampler:
 
 # ------------------------------------------------------------------------------------------------ CPU reference
 def _reference_root():
-    """The unmodified reference, when it exists on this machine (the authoring container; never the GPU box)."""
-    for cand in ("/root/reference", os.path.join(ROOT, "baseline", "_ref")):
-        if os.path.isfile(os.path.join(cand, "models", "archs", "RDN.py")):
-            return cand
-    return None
+    """The unmodified reference, when a copy of it is installed under baseline/_ref."""
+    cand = os.path.join(ROOT, "baseline", "_ref")
+    return cand if os.path.isfile(os.path.join(cand, "models", "archs", "RDN.py")) else None
 
 
 def cpu_window_runner():
-    """Returns (run(frames) -> outputs, kind): the reference's own bin_stage4_lstm on CPU when /root/reference (or
-    baseline/_ref) is present -- kind "reference" -- else oracle/bin_oracle.py, the line-cited restatement that
+    """Returns (run(frames) -> outputs, kind): the reference's own bin_stage4_lstm on CPU when baseline/_ref is present -- kind "reference" -- else oracle/bin_oracle.py, the line-cited restatement that
     tests/golden pins to the reference's outputs -- kind "port".  Both are fp32 PyTorch CPU (oneDNN) graphs."""
     import torch
     from oracle import bin_oracle as O
@@ -140,9 +141,8 @@ def cpu_window_runner():
 
 
 def pick_cpu_threads(run, budget_s=20.0):
-    """torch's CPU convolutions slow down when oversubscribed (measured on the 128-core GPU host in round 1: a 128x128
-    window takes 0.89 / 0.74 / 1.33 / 3.1 s on 8 / 16 / 32 / 64 threads), so "all the host threads it can use" is
-    found by a short sweep on a 192x320 window instead of assumed."""
+    """torch's CPU convolutions slow down when oversubscribed, so "all the host threads it can use" is found by a short
+    sweep on a 192x320 window instead of assumed."""
     import torch
     from oracle import bin_oracle as O
     ncpu = os.cpu_count() or 1
@@ -209,7 +209,7 @@ def run_reference(args):
 
 
 def eager_cuda_numbers(torch, dev, H, W, steps=3):
-    """The bar a PyTorch user sees today: the oracle port (the reference's own torch ops) run eagerly on the SAME B200
+    """The bar a PyTorch user sees today: the oracle port (the reference's own torch ops) run eagerly on the SAME GPU
     through cuDNN, fp32 (TF32 as torch defaults: cudnn.allow_tf32=True) and fp16-autocast, cudnn.benchmark=True as
     test.py:148 sets it.  All 20 backbone calls + 12 ConvLSTM calls per window, CUDA-event timed."""
     from oracle import bin_oracle as O
@@ -293,7 +293,6 @@ def dominant_kernel_roofline(torch, ops, pk, ncalls, h, w):
     tail = {"bound": "hbm", "kernel": "rdb_tail (conv3 + LFF + residual fused)",
             "achieved": tail_bytes / (tail_ms * 1e-3) / 1e9, "peak": hbm, "unit": "GB/s",
             "frac": tail_bytes / (tail_ms * 1e-3) / 1e9 / hbm,
-            "traffic": 636.8e6 if (ncalls, h, w) == (5, 360, 640) else None,     # profiles/r02_prof_tail.md (442.9 MB read + 193.9 MB written)
             "algorithmic_bytes_per_launch": tail_bytes,
             "tflops": tail_flops / (tail_ms * 1e-3) / 1e12, "tensor_frac": tail_flops / (tail_ms * 1e-3) / 1e12 / peak,
             "ms_per_launch": tail_ms}
@@ -312,19 +311,10 @@ def dominant_kernel_roofline(torch, ops, pk, ncalls, h, w):
                                         "frac": lstm_bytes / (lstm_ms * 1e-3) / 1e9 / hbm, "algorithmic_bytes": lstm_bytes}}
     return {"bound": "tensor", "kernel": "RDB 3x3 convs 0..2, x-stacked implicit GEMM (3 shapes)", "achieved": ach,
             "peak": peak, "unit": "TFLOP/s", "frac": ach / peak,
-            # dram__bytes_read.sum + dram__bytes_write.sum of the three launches at this exact shape, from the committed
-            # `ncu --set full` capture profiles/r02_prof_conv_quad.md (885.1 MB read + 167.6 MB written; a constant of that
-            # capture, not re-measured by this run); algorithmic: reads 5*230400*(192+256+320) B, writes 3*5*230400*64 B
-            "traffic": 1052.7e6 if (ncalls, h, w) == (5, 360, 640) else None,
-            "traffic_source": "profiles/r02_prof_conv_quad.md (ncu --set full, same shapes)",
+            # algorithmic: reads 5*230400*(192+256+320) B, writes 3*5*230400*64 B
             "algorithmic_bytes_per_launch_set": ncalls * h * w * (192 + 256 + 320) + 3 * ncalls * h * w * 64,
-            "peak_source": f"MEASURED_PEAKS.json bf16_tflops ({pk['source']}, burst: kernel timed alone)",
+            "peak_source": f"bf16_tflops ({pk['source']}: H100 SXM data sheet unless MEASURED_PEAKS.json; kernel timed alone)",
             "algorithmic_flops_per_launch_set": tot_flops, "ms_per_launch_set": tot_ms,
-            # DESIGN 4a: every 128x96x16 MMA fetches A (4 KB) + B (3 KB) from shared memory at 128 B/clk = 56 cycles against
-            # 48 cycles of tensor time, so this formulation tops out at 0.857 of the tensor peak before TMA fill / epilogue
-            "on_chip_limit": {"resource": "shared-memory operand port", "bytes_per_mma": 7168, "port_cycles_per_mma": 56,
-                              "tensor_cycles_per_mma": 48, "ceiling_frac_of_peak": 48.0 / 56.0,
-                              "frac_of_ceiling": ach / peak / (48.0 / 56.0)},
             "second_kernel": tail,
             "memory_bound_kernels": mem}
 
@@ -373,6 +363,27 @@ def train_step_numbers(torch, dev, steps=4, warm=2, B=8, H=256, W=256, ddp=None)
     del net, model, opt, fr, gt
     torch.cuda.empty_cache()
     return res
+
+
+DUMP_BYTES = 60 << 20                 # sample budget: with the .npy headers the files stay under 64 MB
+
+
+def dump_outputs(out_dir, windows):
+    """windows[i][k] = output k of window i of the last timed step -> out_dir/window<i>_out<k>.npy, float32.  When all
+    outputs together exceed DUMP_BYTES, each one is reduced to the same fixed seeded sample of its flattened elements
+    (sorted indices, generator seed 0), so two builds run with the same arguments write comparable files."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    n_all = sum(o.numel() for w_ in windows for o in w_)
+    for i, w_ in enumerate(windows):
+        for k, o in enumerate(w_):
+            flat = o.detach().float().reshape(-1)
+            cap = max(1, DUMP_BYTES // 4 // len(windows) // len(w_))
+            if n_all * 4 > DUMP_BYTES and flat.numel() > cap:
+                idx = torch.randperm(flat.numel(), generator=torch.Generator().manual_seed(0))[:cap].sort().values
+                flat = flat[idx.to(flat.device)]
+            np.save(os.path.join(out_dir, f"window{i}_out{k:02d}.npy"), flat.cpu().numpy().astype(np.float32))
 
 
 def run_ours(args):
@@ -466,6 +477,14 @@ def run_ours(args):
         ms_dev = e0.elapsed_time(e1)
         step_ms = [a.elapsed_time(b) for a, b in zip([e0] + marks[:-1], marks)]
         clocks = sampler.stop()
+        if args.dump_outputs and rank == 0:
+            # the last step's windows once more, untimed (keeping all their outputs alive inside the timed region would
+            # add allocations to it); the path is deterministic, which the last window's timed outputs confirm bit for bit
+            last_step = [net(*w_) for w_ in wins_dev]
+            if not all(torch.equal(a, b) for a, b in zip(last_step[-1], outs)):
+                raise SystemExit("--dump-outputs: re-running the last step did not reproduce its timed outputs")
+            dump_outputs(args.dump_outputs, last_step)
+            del last_step
         # ---- end-to-end: pinned host -> device, forward, 3 result images -> pinned host -----------
         from bin_b200.pipeline import WindowPipeline
         pipe = WindowPipeline(net, dev)
@@ -545,7 +564,7 @@ def run_ours(args):
             ms32 = _time_ms(torch, lambda: net(*wins_dev[0]), reps=4, warm=0)
             rdn.set_precision(net, "fp16")
             extras["fp32_mode"] = {"value": 1e3 / ms32, "unit": UNIT, "ms_per_window": ms32,
-                                   "note": "set_precision(net, 'fp32'): split-fp16 x3 on the same tcgen05 kernels, <= 1e-5 vs the fp32 oracle (tests)"}
+                                   "note": "set_precision(net, 'fp32'): split-fp16 x3 on the same wgmma kernels, <= 1e-5 vs the fp32 oracle (tests)"}
         rdn.release_workspaces()
         torch.cuda.empty_cache()
         extras["eager_cuda"] = eager_cuda_numbers(torch, dev, H, W)
@@ -579,9 +598,9 @@ def run_ours(args):
             "dtype": "f16", "data": "synthetic",
             "config": {"workload": f"bin_stage4 6-frame window {W}x{H} (SURVEY 8d config 2b; what test.py runs)",
                        "frames": 6, "windows_per_gpu_per_step": S, "outputs": 14,
-                       "arithmetic": "fp16 operands / fp32 accumulate (tcgen05 kind::f16), fp32 frames in/out, fp32 ConvLSTM",
+                       "arithmetic": "fp16 operands / fp32 accumulate (wgmma f32.f16.f16), fp32 frames in/out, fp32 ConvLSTM",
                        "warmup_policy": "--warmup steps, then untimed settle steps (>= 2.5 s, until 3 consecutive steps agree within 1.5 %, <= 6 s; per_rank[].settle) so that the timed steps see the governor's steady state",
-                       "l2": f"{S} distinct windows per step, per-window working set (>1 GB of activations per backbone stage) >> 126 MB L2; no explicit flush",
+                       "l2": f"{S} distinct windows per step, per-window working set (>1 GB of activations per backbone stage) >> 50 MB L2; no explicit flush",
                        "executed_flop_fraction": EXECUTED_FRACTION, "weights": "synthetic U(+-1/sqrt(fan_in)) seed 0",
                        "nccl_init_ms": nccl_init_ms, "weight_broadcast_ms": bcast_ms, "weight_broadcast_bytes": bcast_bytes},
             "window_tflops_reference_as_executed": flops / (ms_step * 1e-3) / 1e12,
@@ -614,6 +633,9 @@ def main():
     ap.add_argument("--width", type=int, default=1280)
     ap.add_argument("--windows-per-step", type=int, default=5)
     ap.add_argument("--no-extras", action="store_true", help="skip roofline / cpu_baseline / eager / train extras")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the outputs of the last timed step to DIR/*.npy (float32, <= 64 MB in all; recomputed after the "
+                         "timed region, so the timing is that of a run without the flag)")
     args = ap.parse_args()
     if args.impl == "reference-cuda":
         run_reference_cuda(args)

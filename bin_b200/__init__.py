@@ -1,4 +1,4 @@
-"""bin_b200 -- B200-native (sm_100a) implementation of the BIN deblur+interpolation hot path.
+"""bin_b200 -- Hopper-native (H100, sm_90a) implementation of the BIN deblur+interpolation hot path.
 
 Python here is host-side plumbing only (module mirror, weight packing cache, window sharding);
 all arithmetic runs in hand-written CUDA kernels inside libbin_b200.so (see include/bin_b200.h).

@@ -97,11 +97,6 @@ _SIGS = {
     "bin_adam_step": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int] + [C.c_float] * 8 + [C.c_void_p]),
     "bin_blur_average_u8": (C.c_int, [C.c_void_p, C.c_int, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
 }
-# measurement tooling (libbin_b200_tools.so, csrc/tools_abi.h) -- bound only when BIN_B200_LIB points at that library
-_TOOLS_SIGS = {
-    "bin_tools_microbench_mma": (C.c_int, [C.c_int, C.c_int, C.c_int, C.POINTER(C.c_float)]),
-    "bin_tools_debug_timeline": (C.c_int, [C.POINTER(C.c_longlong), C.c_int]),
-}
 
 _lib = None
 
@@ -110,27 +105,22 @@ def lib() -> C.CDLL:
     """Load (once) and return the shared library; raises if it has not been built."""
     global _lib
     if _lib is None:
-        path = os.environ.get("BIN_B200_LIB") or LIB_PATH          # tools point this at libbin_b200_tools.so
-        tools = os.path.basename(path) == "libbin_b200_tools.so"
+        path = LIB_PATH
         # A fresh checkout carries sources only, and an in-tree library may be older than the sources: (re)build when the
         # source digest differs from the stamp next to the .so (a no-op otherwise; ~1 min with nvcc).  If that is not
         # possible and no library exists the package is unusable -- there is deliberately no CPU / PyTorch fallback.
         try:
             from . import build as _build
-            if path in (LIB_PATH, _build.TOOLS_LIB):
-                _build.build(tools=tools)
+            _build.build()
         except Exception as e:  # noqa: BLE001
             if not os.path.exists(path) or "failed" in str(e):       # a compile/link error is never papered over
                 raise BinB200Error(
                     f"{path} not found and building it failed ({e}). Build with `python -m bin_b200.build` "
-                    "(nvcc, sm_100a). bin_b200 has no CPU/PyTorch fallback.") from e
+                    "(nvcc, sm_90a). bin_b200 has no CPU/PyTorch fallback.") from e
             import warnings
             warnings.warn(f"bin_b200: could not verify/rebuild {path} against the sources ({e}); using it as is")
         L = C.CDLL(path)
-        sigs = dict(_SIGS)
-        if tools:
-            sigs.update(_TOOLS_SIGS)
-        for name, (res, args) in sigs.items():
+        for name, (res, args) in _SIGS.items():
             fn = getattr(L, name)          # AttributeError here = header/library mismatch
             fn.restype = res
             fn.argtypes = args

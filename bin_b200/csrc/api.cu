@@ -24,13 +24,6 @@ static Options read_options() {
   const char* e;
   o.debug = (e = env("BIN_B200_DEBUG")) ? atoi(e) : 0;
   o.fuse_lff = !((e = env("BIN_B200_FUSE_LFF")) && *e == '0');
-  o.tail_streams = !((e = env("BIN_B200_TAIL_STREAMS")) && *e == '0');
-  o.pair = (e = env("BIN_B200_PAIR")) && *e == '1';     // CTA-pair kernels: opt-in until verified on hardware
-  o.msplit = (e = env("BIN_B200_MSPLIT")) && *e == '1';
-  o.quad = !((e = env("BIN_B200_QUAD")) && *e == '0');  // four MMA warps in the x-stacked conv: default (measured +8 %)
-  o.tailq = (e = env("BIN_B200_TAILQ")) && *e == '1';
-  o.spread = (e = env("BIN_B200_SPREAD")) && *e == '1';
-  o.polite = (e = env("BIN_B200_POLITE")) && *e == '1';
   o.zigzag = (e = env("BIN_B200_ZIGZAG")) && *e == '1';
   o.stage_mmas = (e = env("BIN_B200_STAGE_MMAS")) ? atoi(e) : 12;
   if (o.stage_mmas < 1) o.stage_mmas = 12;
@@ -38,14 +31,8 @@ static Options read_options() {
   return o;
 }
 const Options& options() {
-#ifdef BIN_B200_TOOLS
-  static thread_local Options o;
-  o = read_options();
-  return o;
-#else
   static const Options o = read_options();
   return o;
-#endif
 }
 
 int num_sms() {
@@ -55,7 +42,7 @@ int num_sms() {
   int v = cache[dev & 63].load(std::memory_order_relaxed);
   if (v == 0) {
     cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
-    if (v <= 0) v = 148;
+    if (v <= 0) v = 132;
     cache[dev & 63].store(v, std::memory_order_relaxed);
   }
   return v;
@@ -191,17 +178,16 @@ static bin_conv_args_t conv_args(const void* blob, const ConvSpec& c, int x3 = 0
 // An RDB run layer-by-layer over the whole (batched) image moves 2 240 B/position through HBM
 // (each conv re-reads the growing concat); measured, that makes the RDB convs HBM-bound at ~50 % of
 // the tensor peak.  Walking the RDB band by band -- all 5 layers for one band before the next --
-// keeps x (192 B/px) + growth scratch (256 B/px) + x' (192 B/px) of the band inside the 126 MB L2,
+// keeps x (192 B/px) + growth scratch (256 B/px) + x' (192 B/px) of the band inside the 50 MB L2,
 // so only x in / x' out (384 B/position) touch HBM.  Bands overlap by the 3-row receptive field of
 // the chained 3x3 convs (rows are recomputed, values identical).  Boundaries sit at rows 8k-3 so
 // every layer of a band has the same number of 8-row tile rows, and k is chosen to minimise the
-// number of 148-CTA waves.
+// number of one-CTA-per-SM waves.
 struct Band { int b0, nb, y0, y1; };   // batch items [b0,b0+nb), LFF output rows [y0,y1)
 constexpr size_t kBandBytesPerPx = 640;
 static size_t band_budget() {            // BIN_B200_BAND_BUDGET_KB overrides (tests force many bands)
-  // Measured on B200 (720p, 5 batched calls): with 10 bands the 10x launch count costs more
-  // (prologue + drain per launch, ~4 us each) than the L2 residency saves: 41.5 ms vs 31.8 ms per
-  // window.  Default = one band (off).
+  // Default = one band (off): every band is a further launch of every RDB conv (prologue and drain per
+  // launch), and at 720p a band that fits the 50 MB L2 is only a few dozen rows.
   return options().band_budget;
 }
 
@@ -275,7 +261,7 @@ static int run_rdb(const void* blob, const BackboneLayout& L, int i, const bin_a
       const int lo = bd.y0 - ext < 0 ? 0 : bd.y0 - ext, hi = bd.y1 + ext > h ? h : bd.y1 + ext;
       a.b_begin = bd.b0; a.b_count = bd.nb; a.y_begin = lo; a.y_count = hi - lo;
       // zigzag: conv0 forward, conv1 backward, conv2 forward, tail backward -- every launch starts on the tiles its
-      // predecessor touched last, which are the ones still in the 126 MB L2 (the tail ends at tile 0, where the next
+      // predecessor touched last, which are the ones still in the 50 MB L2 (the tail ends at tile 0, where the next
       // RDB's conv0 starts)
       BIN_TRY(launch_conv(a, s, options().zigzag && (c & 1)));
     }
@@ -567,7 +553,7 @@ int bin_check_device(void) {
   BIN_CUDA_OK(cudaGetDevice(&dev));
   cudaDeviceProp prop;
   BIN_CUDA_OK(cudaGetDeviceProperties(&prop, dev));
-  if (prop.major != 10) return fail(BIN_ERR_UNSUPPORTED, std::string("bin_b200 needs an sm_100 device, found sm_") +
+  if (prop.major != 9) return fail(BIN_ERR_UNSUPPORTED, std::string("bin_b200 needs an sm_90 device, found sm_") +
                                                           std::to_string(prop.major) + std::to_string(prop.minor));
   return BIN_OK;
 }

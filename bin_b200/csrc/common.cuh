@@ -1,6 +1,6 @@
-// bin_b200 -- PTX wrappers for sm_100a (tcgen05 / TMEM / TMA / mbarrier).
-// Hand-written; no CUTLASS dependency.  Bit layouts of the UMMA descriptors follow the
-// PTX ISA "tcgen05 matrix descriptor" / "instruction descriptor" tables.
+// bin_b200 -- PTX wrappers for sm_90a (wgmma / TMA / mbarrier).
+// Hand-written; no CUTLASS dependency.  The bit layout of the shared-memory matrix descriptor follows the
+// PTX ISA "matrix descriptor" table of wgmma.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -9,7 +9,8 @@
 #include <stdio.h>
 
 #ifndef BIN_SPIN_LIMIT
-#define BIN_SPIN_LIMIT (1u << 27)   // mbarrier wait watchdog: trap instead of hanging the GPU
+#define BIN_SPIN_LIMIT (1u << 27)   // mbarrier wait watchdog: trap instead of hanging the GPU (no printf: a call in a
+                                    // kernel makes ptxas serialise every wgmma of it)
 #endif
 
 namespace binb {
@@ -49,41 +50,15 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// `tag` identifies the waiter in the watchdog message (kernel instantiation / role / iteration), 0 = untagged.
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, unsigned long long tag = 0ull) {
+__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
-#ifdef BIN_B200_TOOLS
-    if (tag >> 63) __nanosleep(64);          // experiment: polite polling (tag bit 63)
-#endif
     if (++spins > BIN_SPIN_LIMIT) {
-      printf("bin_b200: mbarrier watchdog (block %d/%d thread %d bar %p parity %u tag %llx)\n", blockIdx.x, gridDim.x,
-             threadIdx.x, (void*)bar, parity, tag);
-      __trap();
+__trap();
     }
   }
 }
 
-// Polite wait for roles that are NOT on the latency-critical path (TMA producers waiting for a ring slot, epilogue warps
-// waiting for an accumulator): sleep between polls.  These warps spin for thousands of cycles per tile; on a power-capped
-// part (the pool's B200s run at 1.45-1.7 GHz under sw_power_cap) every issued instruction of a spin loop is clock taken
-// from the tensor pipe.
-__device__ __forceinline__ void mbar_wait_polite(uint64_t* bar, uint32_t parity, uint32_t ns, unsigned long long tag = 0ull) {
-  uint32_t spins = 0;
-  while (!mbar_try_wait(bar, parity)) {
-    __nanosleep(ns);
-    if (++spins > BIN_SPIN_LIMIT) {
-      printf("bin_b200: mbarrier watchdog (block %d/%d thread %d bar %p parity %u tag %llx)\n", blockIdx.x, gridDim.x,
-             threadIdx.x, (void*)bar, parity, tag);
-      __trap();
-    }
-  }
-}
-
-// NOTE (measured, round 2): letting ONE lane poll and parking the other 31 at __syncwarp() does NOT make a warp-wide
-// wait cheaper -- a wait on an already-completed phase still costs 300-450 cycles while the tensor pipe is streaming
-// operands from shared memory -- and it serialised the two tile streams of rdb_tail_kernel (0.21 -> 0.28 ms).  All lanes
-// poll.
 // ---------------------------------------------------------------- TMA
 __device__ __forceinline__ void tma_prefetch_desc(const void* tmap) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(tmap) : "memory");
@@ -114,158 +89,27 @@ __device__ __forceinline__ void bulk_load_1d(void* smem_dst, const void* gsrc, u
                : "memory");
 }
 
-// Warp-converged single-lane election: keeps the surrounding values warp-uniform for the compiler
-// (descriptors stay in uniform registers; no per-instruction ELECT loop around UTCHMMA).
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n\t.reg .b32 rx;\n\t.reg .pred px;\n\t"
-      "elect.sync rx|px, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, px;\n\t}"
-      : "=r"(pred));
-  return pred != 0;
+// ---------------------------------------------------------------- wgmma (sm_90a)
+// Shared-memory matrix descriptor, SWIZZLE_NONE ("interleave"), 8 x 16-byte core matrices:
+//   K-major : element (row r, k) lives at start + (r%8)*16 + (r/8)*SBO + (k/8)*LBO + (k%8)*2     [fp16]
+//   MN-major: element (k, col n) lives at start + (k%8)*16 + (k/8)*LBO + (n/8)*SBO + (n%8)*2
+// bits [0,14) start>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [62,64) layout = 0 (no swizzle)
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+  return (uint64_t)((smem_addr >> 4) & 0x3FFFu) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16) |
+         ((uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32);
 }
-
-// ---------------------------------------------------------------- tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {   // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
+// before the first wgmma of a group that reads / writes accumulator registers the warp has touched
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across a wgmma wait
+template <int K>
+__device__ __forceinline__ void acc_fence(float (&d)[K]) {
+#pragma unroll
+  for (int i = 0; i < K; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {      // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem] * B[smem], kind::f16 (fp16/bf16 inputs, fp32 accumulate), one CTA.
-__device__ __forceinline__ void umma_f16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier once all previously issued tcgen05.mma of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// TMEM -> registers: this warp's 32 lanes x 16 consecutive fp32 columns.
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// Shared-memory matrix descriptor, K-major, SWIZZLE_NONE ("interleave"):
-//   element (row r, k) lives at start + (r%8)*16 + (r/8)*SBO + (k/8)*LBO + (k%8)*2   [fp16]
-// bits [0,14) start>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [46,48) version=1 | [61,64) layout=0
-__device__ __forceinline__ uint64_t umma_desc_kmajor_noswz(uint32_t smem_addr, uint32_t lbo_bytes,
-                                                           uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr >> 4) & 0x3FFFu);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= (uint64_t)1 << 46;
-  return d;
-}
-// Instruction descriptor, kind::f16: fp16 A/B (K-major both), fp32 D, MxN.
-__host__ __device__ constexpr uint32_t umma_idesc_f16(int M, int N) {
-  return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
-}  // namespace binb
-
-// ================================================================ CTA pairs (cta_group::2)
-// Two CTAs of a (2,1,1) cluster sit on the two SMs of one TPC.  One tcgen05.mma.cta_group::2, issued by the leader
-// (cluster rank 0), multiplies A = 128 rows from EACH CTA's shared memory (same offset in both) with B = N/2 rows from
-// each CTA (rows [0,N/2) from the leader, [N/2,N) from the peer) into 128 x N accumulators at the same TMEM address of
-// each CTA.  Per SM the operand fetch drops from 4 KB + 32 N to 4 KB + 16 N bytes per K = 16 step.
-namespace binb {
-
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-// shared::cta address of this CTA -> shared::cluster address of the same offset in CTA `rank` of the cluster
-__device__ __forceinline__ uint32_t mapa_u32(uint32_t smem_addr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_addr), "r"(rank));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {      // every thread of both CTAs
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// arrive on an mbarrier that may live in the peer CTA (address from mapa_u32); release at cluster scope
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// wait on a LOCAL mbarrier whose arrivals may come from the peer CTA: acquire at cluster scope
-__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {
-  uint32_t spins = 0;
-  for (;;) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(smem_u32(bar)), "r"(parity)
-        : "memory");
-    if (ok) return;
-    if (++spins > BIN_SPIN_LIMIT) {
-      printf("bin_b200: cluster mbarrier watchdog (block %d thread %d bar %p parity %u)\n", blockIdx.x, threadIdx.x,
-             (void*)bar, parity);
-      __trap();
-    }
-  }
-}
-// 4-D tiled load into THIS CTA's shared memory whose completion bytes are credited to an mbarrier given as a
-// shared::cluster address (the leader's barrier): needs the .cta_group::2 form.
-__device__ __forceinline__ void tma_load_4d_pair(void* smem_dst, const void* tmap, uint32_t bar_cluster_addr, int c0,
-                                                 int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.tile.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5, %6}], [%2];" ::"r"(smem_u32(smem_dst)),
-      "l"(tmap), "r"(bar_cluster_addr), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t* dst_smem, uint32_t ncols) {   // one warp in EACH CTA, same dst offset
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_pair() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_f16_ss_pair(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                                 uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive (once) on the mbarrier at this offset in every CTA of `mask` when all MMAs issued so far have completed
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar, uint16_t mask = 3) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                   smem_u32(bar)),
-               "h"(mask)
-               : "memory");
-}
+// barrier over the 128 threads of one consumer warpgroup (ids 1.. are free; 0 is __syncthreads)
+__device__ __forceinline__ void wg_sync(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
 
 }  // namespace binb

@@ -1,4 +1,4 @@
-// bin_b200 -- implicit-GEMM convolution for sm_100a (tcgen05.mma + TMEM + TMA).
+// bin_b200 -- implicit-GEMM convolution for sm_90a (wgmma + TMA + mbarrier).
 //
 // Replaces every nn.Conv2d on the BIN hot path (reference models/archs/RDN.py:141,162,187-188,
 // 199-200,205,207 and the 36/60-channel twins): stride 1, zero padding k/2, bias, optional ReLU
@@ -6,36 +6,27 @@
 // (RDN.py:206) or the final "+ mean(input frames)" fp32 NCHW store (RDN.py:221,279,333).
 //
 // GEMM view: M = pixels, N = Cout, K = taps x Cin.  Activations are P8 fp16
-// [B][C/8][H][W][8]: one pixel of one 8-channel plane is exactly one 16-byte row of a UMMA
+// [B][C/8][H][W][8]: one pixel of one 8-channel plane is exactly one 16-byte row of a wgmma
 // K-major / no-swizzle core matrix, and pixels are contiguous, so the A operand of tap (ky,kx)
 // is the SAME shared-memory tile addressed through a descriptor whose start is shifted by
 // (ky*32+kx)*16 bytes -- no im2col, the halo tile is fetched once per 32-channel chunk by one
-// 5-D TMA box load whose out-of-bounds zero fill implements the conv's zero padding.
-// Tile: 8 rows x 32-pixel smem pitch = 256 GEMM rows = two 128xN fp32 accumulators in TMEM;
-// the 2*PAD right-most columns of each row are junk rows that are never stored.
-//
-// Warp roles (256 threads, 1 CTA/SM, persistent over tiles):
-//   warp 0 lane 0 : TMA producer (activation box + weight slab per stage, mbarrier ring)
-//   warp 1 lane 0 : tcgen05.mma issuer (accumulates taps x k-steps into TMEM)
-//   warp 2        : TMEM allocator
-//   warps 4..7    : epilogue (tcgen05.ld -> bias/ReLU/residual -> 128-bit fp16 stores),
-//                   double-buffered against the next tile's MMAs through tmem_full/empty.
-// Weight sets that fit (RDB convs, LFF, SFENet2, GFF.1, UPNet.2) stay resident in shared memory.
+// 4-D TMA box load whose out-of-bounds zero fill implements the conv's zero padding.
+// Tile: 8 rows x 32-pixel smem pitch = 256 GEMM rows = four 64-row wgmma blocks, fp32 accumulators in
+// registers; the 2*PAD right-most columns of each row are junk rows that are never stored.
 #include <stdio.h>
 #include <stdlib.h>
 
 #include "common.cuh"
 #include "internal.h"
+#include "wgmma.cuh"
 
 namespace binb {
 
 // SX ("stack x"): the KS horizontal taps are folded into the GEMM N dimension -- B rows are
 // (kx, cout), the A operand is NOT shifted in x, and the epilogue adds the kx-th column group of
-// the accumulator row of pixel p+kx (a warp shuffle: each epilogue warp holds exactly one 32-pixel
-// tile row, and the lanes that would need the next row are the junk columns).  One MMA then does
-// 128 x (KS*NT) x 16 instead of 128 x NT x 16 for the same 4 KB A read, which lifts the Cout=32
-// RDB convs from 40 % to 86 % of the shared-memory-bound tcgen05 issue rate
-// (measured: MMA(128xNx16) costs max(N/2, 32+N/4) cycles).
+// the accumulator row of pixel p+kx.  One wgmma then does 64 x (KS*NT) x 16 instead of 64 x NT x 16
+// for the same A read: the Cout=32 RDB convs would otherwise issue N=32 instructions, whose operand
+// traffic per FLOP is three times as high.
 template <int NT, int KS, bool SX>
 struct ConvCfg {
   static constexpr int PAD = KS / 2;
@@ -44,30 +35,25 @@ struct ConvCfg {
   static constexpr int ROWS = ROWSPLIT ? kTH : kTH + 2 * PAD;
   static constexpr int A_PLANE = ROWS * kTWH * 16;       // bytes of one plane of a stage
   static constexpr int A_BYTES = kKPL * A_PLANE;
-  static constexpr int NMMA = SX ? NT * KS : NT;         // N of one tcgen05.mma
+  static constexpr int NMMA = SX ? NT * KS : NT;         // N of one wgmma
   static constexpr int TAPS_C = SX ? KS : KS * KS;       // B slabs ("taps") per chunk
   static constexpr int TAPS_S = (SX || ROWSPLIT) ? KS : KS * KS;  // taps per stage
   static constexpr int NSUB = ROWSPLIT ? KS : 1;         // stages per chunk
   static constexpr int W_TAP = kKPL * NMMA * 16;         // bytes per tap per chunk
   static constexpr int W_STAGE = TAPS_S * W_TAP;
   static constexpr int W_CHUNK = TAPS_C * W_TAP;
-  static constexpr int ACC_COLS = kMT * NMMA;
-  static constexpr int TMEM_COLS = (2 * ACC_COLS <= 32) ? 32 : (2 * ACC_COLS <= 64) ? 64
-                                   : (2 * ACC_COLS <= 128) ? 128 : (2 * ACC_COLS <= 256) ? 256 : 512;
-  static_assert(2 * ACC_COLS <= 512, "TMEM overflow");
+  // SX: the kx = 1, 2 column groups of a 64-row accumulator block (+2 rows read by the junk columns) go through shared
+  // memory to reach the thread that holds pixel p; pitch padded by 4 words against bank conflicts
+  static constexpr int XPITCH = 2 * NT + 4;
+  static constexpr int XBYTES = SX ? 66 * XPITCH * 4 : 0;   // per consumer warpgroup
   static_assert(!(SX && ROWSPLIT), "SX is only used for 3x3");
-  static_assert(NMMA % 16 == 0 && NMMA <= 256, "invalid UMMA N");
+  static_assert(NMMA % 16 == 0 && NMMA <= 256, "invalid wgmma N");
 };
 
 struct Ctrl {
   uint64_t full[kMaxStages];
   uint64_t empty[kMaxStages];
   uint64_t wfull[kMaxResidentChunks];
-  uint64_t tmem_full[2];
-  uint64_t tmem_empty[2];
-  uint64_t wready;            // PAIR: the peer's resident weight halves have landed (leader's copy is used)
-  uint32_t tmem_base;
-  volatile uint32_t issued[2];   // per accumulator (QUAD) / [0] only: number of pipeline stages whose MMAs have been issued (hand-off)
 };
 static_assert(sizeof(Ctrl) <= 1024, "ctrl block");
 
@@ -80,102 +66,50 @@ __device__ __forceinline__ float2 unpack_h2(uint32_t u) {
   return __half22float2(h);
 }
 
-// perf-debug timeline (BIN_B200_DEBUG=8): block 0 records clock64 at role milestones.
-// layout: dbg[role*4096 + iter*4 + k], role 0 = producer A, 1 = MMA warp A, 2 = epilogue (warp 4).
-__device__ __forceinline__ void dbg_rec(const ConvParams& p, int role, uint32_t iter, int k) {
-#ifdef BIN_B200_TOOLS       // the product library carries no timeline hooks
-  if ((p.debug & 8) && blockIdx.x == 0 && iter < 1024) p.dbg[role * 4096 + iter * 4 + k] = clock64();
-#endif
-}
+constexpr int kThreads = 384;   // warpgroup 0: TMA producer (one thread); warpgroups 1, 2: wgmma + epilogue
 
-// tools build: which epilogue warp the timeline records (BIN_B200_DEBUG bits 12..14 -> warps 4..11)
-__device__ __forceinline__ int kDbgEpiWarp(const ConvParams& p) {
-#ifdef BIN_B200_TOOLS
-  return 4 + ((p.debug >> 12) & 7);
-#else
-  return 4;
-#endif
-}
-
-constexpr int kThreads = 384;   // 12 warps, see the role table below
-
-// Warp roles (384 threads, 1 CTA/SM, persistent over tiles).  Measured on B200: one mbarrier poll
-// costs 200-350 cycles even when the phase is already complete, so a single MMA warp that polls
-// once per 12-MMA stage leaves the tensor pipe idle ~50 % of the time.  Hence every role that sits
-// on a latency chain is doubled and the two copies work on alternating items:
-//   warp 0 lane 0 : TMA producer A                              warp 2 : TMEM alloc, then TMA producer B
-//   warp 1        : MMA issuer  A  (accumulator 0)              warp 3 : MMA issuer B (accumulator 1)
-//   warps 4..11   : epilogue, warp w handles TMEM lane quarter w%4 of accumulator tile (w-4)/4
-// One ring of S (even) smem stages; stage i is filled by producer i%2 and its MMAs are issued by MMA
-// warp i%2, which is also the only waiter of that stage's full barrier.  The two MMA warps hand the
-// tensor pipe to each other through a shared-memory counter (strict stage order), so one warp's
-// barrier poll / descriptor setup overlaps the other's issue phase.  The two
-// TMEM accumulator buffers alternate per tile and are released by the epilogue (tmem_full counts
-// one tcgen05.commit per MMA warp).
-// A pipeline stage holds up to p.cps "units" (unit = one 32-channel chunk, or one (chunk, ky) for 5x5).
 // X3 ("fp32-accurate" mode, 1e-5 parity bar): every value is carried as an fp16 pair hi + lo (22 significant bits).
 // Tensors hold, per 32-channel chunk, 4 planes of hi followed by 4 planes of lo; a logical K chunk becomes three
 // physical chunks  x_hi*W_hi + x_lo*W_hi + x_hi*W_lo  (the lo*lo term is below 2^-22), the weights are packed
 // pre-scaled by 2^8 so that W_lo stays a normal fp16 number, and the epilogue un-scales the fp32 accumulator and
 // splits its result into (hi, lo) again.  Same kernel, same descriptors: 3x the MMAs, 2x the activation bytes.
 __device__ __forceinline__ int x3_plane(int logical_plane) { return 2 * (logical_plane & ~3) + (logical_plane & 3); }
-__device__ __forceinline__ void split_store(__half* base_hi, __half* base_lo, const float* f) {
-  uint4 hi, lo;
-  uint32_t* hp = reinterpret_cast<uint32_t*>(&hi);
-  uint32_t* lp = reinterpret_cast<uint32_t*>(&lo);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const __half h0 = __float2half_rn(f[2 * i]), h1 = __float2half_rn(f[2 * i + 1]);
+// stores 2 consecutive channels (4 bytes) of one pixel, or their (hi, lo) split
+template <bool X3>
+__device__ __forceinline__ void store_pair(__half* p, size_t lo_off, float a, float b) {
+  if constexpr (X3) {
+    const __half h0 = __float2half_rn(a), h1 = __float2half_rn(b);
     const __half2 hh = __halves2half2(h0, h1);
-    const __half2 ll = __floats2half2_rn(f[2 * i] - __half2float(h0), f[2 * i + 1] - __half2float(h1));
-    hp[i] = *reinterpret_cast<const uint32_t*>(&hh);
-    lp[i] = *reinterpret_cast<const uint32_t*>(&ll);
+    *reinterpret_cast<__half2*>(p) = hh;
+    *reinterpret_cast<__half2*>(p + lo_off) = __floats2half2_rn(a - __half2float(h0), b - __half2float(h1));
+  } else {
+    *reinterpret_cast<uint32_t*>(p) = pack_h2(a, b);
   }
-  *reinterpret_cast<uint4*>(base_hi) = hi;
-  *reinterpret_cast<uint4*>(base_lo) = lo;
+}
+template <bool X3>
+__device__ __forceinline__ void store_one(__half* p, size_t lo_off, float a) {
+  const __half h = __float2half_rn(a);
+  *p = h;
+  if constexpr (X3) p[lo_off] = __float2half_rn(a - __half2float(h));
 }
 
-// PAIR (cta_group::2, launched as (2,1,1) clusters; x-stacked resident-weight convs only): the two CTAs of a cluster each
-// run their own 256-pixel tile with their own producers, accumulators and epilogue warps, but the B operand -- the
-// resident weights -- is split between them (48 of the 96 rows of every slab per CTA) and ONE 256 x 96 x 16 MMA issued by
-// the leader's MMA warps feeds both: 5.5 KB instead of 7 KB of shared-memory operand traffic per SM and MMA (the limiter
-// of this kernel, DESIGN.md 4), and half the resident-weight footprint (two more ring slots for the 160-channel conv).
-// Barriers as in rdb_tail_pair_kernel: `full` in the leader (2 x bytes, both CTAs' TMA credit it), `empty` / `tmem_full`
-// by multicast commit into both CTAs, `tmem_empty` in the leader counting the epilogue threads of both CTAs.
-// QUAD (448 threads; every fp16 conv with a P8 / PixelShuffle epilogue, single CTA): FOUR MMA warps -- accumulator m of the tile is fed by the two warps
-// (m, stage parity 0 / 1), which alternate stages and hand over through issued[m] exactly as the two warps of the default
-// scheme do.  The role timelines show a single issuing warp sustaining one MMA per ~82 cycles while two warps issuing
-// CONCURRENTLY reach the isolated rate (57); with four warps two are always issuing (one per accumulator) while the other
-// two wait on their next barrier.  The MMA order per accumulator is unchanged -> bit-identical results.
-template <int NT, int KS, int EPI, bool SX, bool X3, bool PAIR = false, bool QUAD = false>
-__global__ void __launch_bounds__(QUAD ? kThreads + 64 : kThreads, 1) conv_igemm_kernel(const __grid_constant__ ConvParams p) {
+// Roles (384 threads, 1 CTA/SM, persistent over tiles):
+//   warp 0 lane 0 : TMA producer (activation box + weight slab per stage, mbarrier ring)
+//   warpgroup 1+m : accumulator m = tile rows [128 m, 128 m + 128) as two 64-row wgmma blocks held in registers; it
+//                   waits for each stage, issues its wgmmas, releases the stage one stage later (wait_group 1), and
+//                   runs the epilogue of its rows straight from the accumulator fragments.
+// Weight sets that fit (RDB convs, LFF, SFENet2, GFF.1, UPNet.2) stay resident in shared memory.
+// A pipeline stage holds up to p.cps "units" (unit = one 32-channel chunk, or one (chunk, ky) for 5x5).
+template <int NT, int KS, int EPI, bool SX, bool X3>
+__global__ void __launch_bounds__(kThreads, 1) conv_igemm_kernel(const __grid_constant__ ConvParams p) {
   using C = ConvCfg<NT, KS, SX>;
-  static_assert(!PAIR || (SX && !X3 && EPI == BIN_EPI_P8), "the CTA-pair form exists for the x-stacked fp16 convs");
-  static_assert(!QUAD || (!X3 && !PAIR && EPI != BIN_EPI_FINAL), "the four-MMA-warp form exists for the fp16 P8 / PixelShuffle convs");
-  const uint32_t rank = PAIR ? cluster_ctarank() : 0u;
-  // tile sequence of this CTA: single CTA -> tiles blockIdx.x, +gridDim.x, ...; pair -> tile pair q = cluster, +nclusters, ...
-  // with tile 2q + rank (the peer of an odd tail re-runs the last tile with its stores suppressed)
-  const int tq0 = PAIR ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
-  const int tqstep = PAIR ? (int)(gridDim.x >> 1) : (int)gridDim.x;
-  const int tqn = PAIR ? (p.ntiles + 1) >> 1 : p.ntiles;
-  // watchdog tag: instantiation | role | pipeline iteration
-  constexpr unsigned long long kTag0 = ((unsigned long long)NT << 48) | ((unsigned long long)KS << 44) | ((unsigned long long)EPI << 40) |
-                                       ((unsigned long long)SX << 38) | ((unsigned long long)X3 << 37) | ((unsigned long long)PAIR << 36);
-  const unsigned long long kTag = kTag0 | ((p.debug & 512) ? (1ull << 63) : 0ull);   // tools build: bit 63 = polite polling experiment
-  auto tile_at = [&](int tq, bool& live) {
-    int t = PAIR ? 2 * tq + (int)rank : tq;
-    live = t < p.ntiles;
-    if (!live) t = p.ntiles - 1;
-    return p.reverse ? p.ntiles - 1 - t : t;
-  };
+  constexpr int NA = C::NMMA / 2;                              // accumulator registers per thread and 64-row block
+  auto tile_at = [&](int tq) { return p.reverse ? p.ntiles - 1 - tq : tq; };
   extern __shared__ __align__(1024) uint8_t smem[];
   Ctrl* ctrl = reinterpret_cast<Ctrl*>(smem);
   float* sbias = reinterpret_cast<float*>(smem + 1024);
 
-  const int warp = threadIdx.x >> 5;
-  // Role index.  QUAD + p.spread: the fourth MMA warp swaps places with producer B (physical warp 2 <-> 13), so that the four
-  // MMA issuers sit on four different SM sub-partitions (warp % 4) instead of two of them sharing sub-partition 1.
-  const int rw = (QUAD && p.spread) ? (warp == 2 ? 13 : (warp == 13 ? 2 : warp)) : warp;
+  const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);   // provably warp-uniform for the compiler
   const int lane = threadIdx.x & 31;
   const uint32_t S = p.nstages;
   const int nchunks = p.nch0 + p.nch1;
@@ -184,10 +118,8 @@ __global__ void __launch_bounds__(QUAD ? kThreads + 64 : kThreads, 1) conv_igemm
   const int spt = (nunits + cps - 1) / cps;                   // stages per tile
   const int unit_bytes = C::A_BYTES + (p.resident ? 0 : C::W_STAGE);
   const int stage_bytes = cps * unit_bytes;
-  constexpr int WH = PAIR ? 2 : 1;                             // resident B bytes per CTA = 1 / WH of the slab
-  constexpr int B_PLANE = C::NMMA * 16 / WH;                   // bytes of one 8-channel plane of a B slab in this CTA
   uint8_t* res_w = smem + kCtrlBytes;
-  uint8_t* stage0 = res_w + (p.resident ? nchunks * (C::W_CHUNK / WH) : 0);
+  uint8_t* stage0 = res_w + (p.resident ? nchunks * C::W_CHUNK : 0);
 
   // ------------------------------------------------------------ one-time setup
   if (threadIdx.x == 0) {
@@ -195,487 +127,213 @@ __global__ void __launch_bounds__(QUAD ? kThreads + 64 : kThreads, 1) conv_igemm
     if (p.nch1 > 0) tma_prefetch_desc(&p.tmap1);
     for (int i = 0; i < kMaxStages; ++i) {
       mbar_init(&ctrl->full[i], 1);
-      mbar_init(&ctrl->empty[i], (QUAD || p.msplit) ? 2 : 1);   // M-split / QUAD: two MMA warps consume every stage
+      mbar_init(&ctrl->empty[i], 8);                           // one arrival per consumer warp
     }
     for (int i = 0; i < kMaxResidentChunks; ++i) mbar_init(&ctrl->wfull[i], 1);
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&ctrl->tmem_full[i], QUAD ? 4 : 2);        // one tcgen05.commit per MMA warp
-      mbar_init(&ctrl->tmem_empty[i], PAIR ? 16 : 8);      // ONE arrival per epilogue warp (of both CTAs): 256 threads
-                                                           // arriving on one mbarrier serialise in the shared-memory
-                                                           // atomic unit (~1 500 cycles per tile, measured by ablation)
-    }
-    mbar_init(&ctrl->wready, 1);
-    ctrl->issued[0] = ctrl->issued[1] = 0;
     fence_barrier_init();
   }
   const bool bias_in_smem = NT * p.nh <= 256;                  // else (wide data-gradient launches) read it from global
   if (bias_in_smem)
     for (int i = threadIdx.x; i < NT * p.nh; i += blockDim.x) sbias[i] = p.bias[i];
   const float* bsrc = bias_in_smem ? sbias : p.bias;
-  if (rw == 2) {
-    if constexpr (PAIR) { tmem_alloc_pair(&ctrl->tmem_base, C::TMEM_COLS); tmem_relinquish_pair(); }
-    else { tmem_alloc(&ctrl->tmem_base, C::TMEM_COLS); tmem_relinquish(); }
-  }
-  tc_fence_before();
   __syncthreads();
-  if constexpr (PAIR) cluster_sync_all();                      // both CTAs' barriers are initialised
-  tc_fence_after();
-  const uint32_t tmem_base = ctrl->tmem_base;
 
-  if ((rw == 0 || rw == 2) && lane == 0) {
-    // ========================================================== TMA producers (stage i -> producer i%2)
-    const uint32_t Y = rw >> 1;
-    if (p.resident && Y == 0) {
+  if (warp == 0) {
+    if (lane != 0) return;
+    // ========================================================== TMA producer
+    if (p.resident) {
       for (int c = 0; c < nchunks; ++c) {
-        mbar_expect_tx(&ctrl->wfull[c], C::W_CHUNK / WH);
-        if constexpr (PAIR) {                                  // this CTA's rows [48 r, 48 r + 48) of every plane of every tap
-          for (int tp = 0; tp < C::TAPS_C; ++tp)
-            for (int pl = 0; pl < kKPL; ++pl)
-              bulk_load_1d(res_w + c * (C::W_CHUNK / 2) + tp * (C::W_TAP / 2) + pl * B_PLANE,
-                           reinterpret_cast<const uint8_t*>(p.w) + (size_t)c * C::W_CHUNK + tp * C::W_TAP + pl * (C::NMMA * 16) +
-                               rank * B_PLANE,
-                           B_PLANE, &ctrl->wfull[c]);
-        } else {
-          bulk_load_1d(res_w + c * C::W_CHUNK, reinterpret_cast<const uint8_t*>(p.w) + (size_t)c * C::W_CHUNK,
-                       C::W_CHUNK, &ctrl->wfull[c]);
-        }
+        mbar_expect_tx(&ctrl->wfull[c], C::W_CHUNK);
+        bulk_load_1d(res_w + c * C::W_CHUNK, reinterpret_cast<const uint8_t*>(p.w) + (size_t)c * C::W_CHUNK, C::W_CHUNK,
+                     &ctrl->wfull[c]);
       }
     }
-    const uint32_t full0 = PAIR ? mapa_u32(smem_u32(&ctrl->full[0]), 0) : 0u;   // the LEADER's full barriers
-    uint32_t it = 0, s = 0, ph = 0;
-    for (int tq = tq0; tq < tqn; tq += tqstep) {
-      bool live;
-      const int tile = tile_at(tq, live);
-      int t = tile;
+    uint32_t s = 0, ph = 0;
+    for (int tq = blockIdx.x; tq < p.ntiles; tq += gridDim.x) {
+      int t = tile_at(tq);
       const int nh = t % p.nh; t /= p.nh;
       const int txi = t % p.tiles_x; t /= p.tiles_x;
       const int tyi = t % p.tiles_y;
       const int b = p.b0 + t / p.tiles_y;
       const int x0 = txi * C::TW - C::PAD, y0 = p.y0 + tyi * kTH - C::PAD;
       int unit = 0;
-      for (int j = 0; j < spt; ++j, ++it) {
+      for (int j = 0; j < spt; ++j) {
         const int nu = (nunits - unit < cps) ? nunits - unit : cps;
-        if ((it & 1u) == Y) {
-          if (Y == 0) dbg_rec(p, 0, it >> 1, 0);
-          if (p.polite) mbar_wait_polite(&ctrl->empty[s], ph ^ 1, 200, kTag | (1ull << 32) | it);
-          else mbar_wait(&ctrl->empty[s], ph ^ 1, kTag | (1ull << 32) | it);
-          if (Y == 0) dbg_rec(p, 0, it >> 1, 1);
-          uint8_t* dst = stage0 + (size_t)s * stage_bytes;
-#ifdef BIN_B200_TOOLS      // ablation (timing only): no global -> shared input traffic at all = what ANY fusion that keeps the
-          if (!PAIR && p.resident && (p.debug & 1024)) {   // inputs on chip could at best save (BIN_B200_DEBUG bit 10)
-            mbar_arrive(&ctrl->full[s]);
-            unit += nu;
-            if (++s == S) { s = 0; ph ^= 1; }
-            continue;
-          }
-#endif
-          if (!PAIR || rank == 0) mbar_expect_tx(&ctrl->full[s], (uint32_t)((PAIR ? 2 : 1) * nu * unit_bytes));
-          for (int u = 0; u < nu; ++u) {
-            const int c = (unit + u) / C::NSUB, sub = (unit + u) % C::NSUB;
-            const int lc = X3 ? c / 3 : c;                     // logical 32-channel chunk
-            const bool seg1 = lc >= p.nch0l;
-            const void* tmap = seg1 ? (const void*)&p.tmap1 : (const void*)&p.tmap0;
-            const int lplane = seg1 ? p.plane0_1 + (lc - p.nch0l) * kKPL : p.plane0_0 + lc * kKPL;
-            const int plane = X3 ? 2 * lplane + ((c % 3) == 1 ? 4 : 0) : lplane;   // X3: hi, lo, hi again
-            if constexpr (PAIR)
-              tma_load_4d_pair(dst + (size_t)u * unit_bytes, tmap, full0 + s * 8, x0 * 8, y0, plane, b);
-            else
-              tma_load_4d(dst + (size_t)u * unit_bytes, tmap, &ctrl->full[s], x0 * 8, y0 + (C::ROWSPLIT ? sub : 0), plane, b);
-            if (!p.resident) {
-              const size_t woff = ((size_t)(nh * nchunks + c) * C::TAPS_C + (C::ROWSPLIT ? sub * KS : 0)) * C::W_TAP;
-              bulk_load_1d(dst + (size_t)u * unit_bytes + C::A_BYTES, reinterpret_cast<const uint8_t*>(p.w) + woff,
-                           C::W_STAGE, &ctrl->full[s]);
-            }
+        mbar_wait(&ctrl->empty[s], ph ^ 1);
+        uint8_t* dst = stage0 + (size_t)s * stage_bytes;
+        mbar_expect_tx(&ctrl->full[s], (uint32_t)(nu * unit_bytes));
+        for (int u = 0; u < nu; ++u) {
+          const int c = (unit + u) / C::NSUB, sub = (unit + u) % C::NSUB;
+          const int lc = X3 ? c / 3 : c;                     // logical 32-channel chunk
+          const bool seg1 = lc >= p.nch0l;
+          const void* tmap = seg1 ? (const void*)&p.tmap1 : (const void*)&p.tmap0;
+          const int lplane = seg1 ? p.plane0_1 + (lc - p.nch0l) * kKPL : p.plane0_0 + lc * kKPL;
+          const int plane = X3 ? 2 * lplane + ((c % 3) == 1 ? 4 : 0) : lplane;   // X3: hi, lo, hi again
+          tma_load_4d(dst + (size_t)u * unit_bytes, tmap, &ctrl->full[s], x0 * 8, y0 + (C::ROWSPLIT ? sub : 0), plane, b);
+          if (!p.resident) {
+            const size_t woff = ((size_t)(nh * nchunks + c) * C::TAPS_C + (C::ROWSPLIT ? sub * KS : 0)) * C::W_TAP;
+            bulk_load_1d(dst + (size_t)u * unit_bytes + C::A_BYTES, reinterpret_cast<const uint8_t*>(p.w) + woff,
+                         C::W_STAGE, &ctrl->full[s]);
           }
         }
         unit += nu;
         if (++s == S) { s = 0; ph ^= 1; }
       }
     }
-  } else if (PAIR && rw == 1 && rank == 1) {
-    // ========================================================== peer: tell the leader when this CTA's B halves have landed
-    for (int c = 0; c < nchunks; ++c) mbar_wait(&ctrl->wfull[c], 0);
-    if (lane == 0) mbar_arrive_cluster(mapa_u32(smem_u32(&ctrl->wready), 0));
-  } else if ((rw == 1 || rw == 3 || (QUAD && rw >= 12)) && rank == 0) {
-    // ========================================================== MMA issuers (warp converged, one elected lane; PAIR: leader only)
-    const uint32_t Y = QUAD ? ((rw == 1 || rw == 12) ? 0u : 1u) : (uint32_t)(rw >> 1);   // stage parity this warp issues
-    const uint32_t mq = (QUAD && rw >= 12) ? 1u : 0u;                                        // QUAD: its accumulator
-    constexpr uint32_t idesc = umma_idesc_f16(PAIR ? 256 : 128, C::NMMA);
-    constexpr uint32_t D_HI = (128u >> 4) | (1u << 14);            // SBO=128 B, descriptor version 1
-    constexpr uint32_t A_LBO = ((uint32_t)C::A_PLANE >> 4) << 16;
-    constexpr uint32_t B_LBO = ((uint32_t)B_PLANE >> 4) << 16;
-    uint32_t it = 0, s = 0, ph = 0, tl = 0, dbg_it = 0;
-    for (int tq = tq0; tq < tqn; tq += tqstep, ++tl) {
-      const uint32_t as = tl & 1, aph = (tl >> 1) & 1;
-      if constexpr (PAIR) mbar_wait_cluster(&ctrl->tmem_empty[as], aph ^ 1);
-      else mbar_wait(&ctrl->tmem_empty[as], aph ^ 1, kTag | (3ull << 32) | tl);
-      tc_fence_after();
-      int unit = 0;
-      for (int j = 0; j < spt; ++j, ++it) {
-        const int nu = (nunits - unit < cps) ? nunits - unit : cps;
-        // Two ways to share the tensor pipe between the two MMA warps:
-        //  * stage alternation (msplit = 0): warp it%2 issues ALL MMAs of stage `it`, then hands the pipe over through
-        //    ctrl->issued -- every hand-off is a bubble of a few hundred cycles (in situ 64-75 cycles per N=96 MMA against
-        //    56 in isolation);
-        //  * M-split (msplit = 1): both warps consume EVERY stage, warp Y issues only the MMAs of accumulator Y (tile rows
-        //    128 Y .. 128 Y + 127).  The two accumulators are independent, so nothing orders the warps against each other
-        //    (no hand-off, no shared counter); a stage is recycled when both have committed (empty count 2), so neither
-        //    waiter can be lapped.  The per-accumulator MMA order is unchanged -> bit-identical results.
-        const bool mine = (!QUAD && p.msplit) ? true : (it & 1u) == Y;
-        if (mine && rw == 1 && lane == 0) dbg_rec(p, 1, dbg_it, 0);
-        if (mine) {
-          // Each MMA warp waits ONLY on the stages it issues (S is even, so stage parity = warp): a parity-tracked
-          // mbarrier must never be waited on by a thread that can fall a whole phase behind -- mbarrier.try_wait may
-          // suspend the thread, and a waiter that wakes after the barrier completed TWO phases sees "not complete" and
-          // hangs.  (Both warps used to observe every full barrier; the warp that only observed could be lapped while
-          // suspended: a rare watchdog under load, seen once at 720p in the split-fp16 mode.)  Ordering between the two
-          // warps is carried by ctrl->issued alone.
-          mbar_wait(&ctrl->full[s], ph, kTag | (2ull << 32) | it);
-          if (p.resident && tl == 0) {
-            for (int u = 0; u < nu; ++u)
-              if ((unit + u) % C::NSUB == 0) mbar_wait(&ctrl->wfull[(unit + u) / C::NSUB], 0);
-            if (PAIR) mbar_wait_cluster(&ctrl->wready, 0);
-          }
-          if (QUAD || !p.msplit)
-            while (ctrl->issued[mq] < it) __nanosleep(32);  // stage it-1 fully issued by the other warp (a tight
-                                                            // shared-memory spin would compete with the MMA operand fetch)
-          if (rw == 1 && lane == 0) dbg_rec(p, 1, dbg_it, 1);
-          tc_fence_after();
-          const uint32_t st_base = smem_u32(stage0 + (size_t)s * stage_bytes);
-          for (int u = 0; u < nu; ++u) {
-            const int c = (unit + u) / C::NSUB, sub = (unit + u) % C::NSUB;
-            const uint32_t a_base = st_base + u * unit_bytes;
-            const uint32_t w_base = p.resident
-                                        ? smem_u32(res_w + c * (C::W_CHUNK / WH)) + (C::ROWSPLIT ? sub * KS * C::W_TAP : 0)
-                                        : a_base + C::A_BYTES;
-            const uint32_t a_lo = ((a_base >> 4) & 0x3FFFu) | A_LBO;
-            const uint32_t b_lo = ((w_base >> 4) & 0x3FFFu) | B_LBO;
-            const uint32_t not_first = (unit + u) != 0 ? 1u : 0u;
-            if (elect_one()) {
+    return;
+  }
+  if (warp < 4) return;
+
+  // ============================================================ consumer warpgroups
+  const int m = (warp - 4) >> 2;                               // accumulator: tile rows [128 m, 128 m + 128)
+  const int wq = warp & 3;                                     // warp within the warpgroup: 16 rows of each 64-row block
+  const int k4 = lane & 3;                                     // fragment column pair: columns 8 i + 2 k4, +1
+  float* xbuf = reinterpret_cast<float*>(stage0 + (size_t)S * stage_bytes + m * C::XBYTES);
+  float acc[2][NA];
+  constexpr float kAcc = X3 ? (1.f / 256.f) : 1.f;            // X3 weights are packed scaled by 2^8
+  uint32_t s = 0, ph = 0;
+  for (int tq = blockIdx.x; tq < p.ntiles; tq += gridDim.x) {
+    // ---------------------------------------------------------- main loop: K = chunks x taps
+    int unit = 0, prev = -1;
+    for (int j = 0; j < spt; ++j) {
+      const int nu = (nunits - unit < cps) ? nunits - unit : cps;
+      mbar_wait(&ctrl->full[s], ph);
+      if (p.resident && tq == (int)blockIdx.x) {
+        for (int u = 0; u < nu; ++u)
+          if ((unit + u) % C::NSUB == 0) mbar_wait(&ctrl->wfull[(unit + u) / C::NSUB], 0);
+      }
+      const uint32_t st_base = smem_u32(stage0 + (size_t)s * stage_bytes);
+      wgmma_fence();
+      for (int u = 0; u < nu; ++u) {
+        const int c = (unit + u) / C::NSUB, sub = (unit + u) % C::NSUB;
+        const uint32_t a_base = st_base + u * unit_bytes;
+        const uint32_t w_base = p.resident ? smem_u32(res_w + c * C::W_CHUNK) + (C::ROWSPLIT ? sub * KS * C::W_TAP : 0)
+                                           : a_base + C::A_BYTES;
+        const uint32_t not_first = (unit + u) != 0 ? 1u : 0u;
 #pragma unroll
-              for (int m = 0; m < kMT; ++m) {
-                if (QUAD ? (uint32_t)m != mq : (p.msplit && (uint32_t)m != Y)) continue;
-                const uint32_t d = tmem_base + as * C::ACC_COLS + m * C::NMMA;
+        for (int tp = 0; tp < C::TAPS_S; ++tp) {
+          const int ky = SX ? tp : (C::ROWSPLIT ? 0 : tp / KS);
+          const int kx = SX ? 0 : (C::ROWSPLIT ? tp : tp % KS);
 #pragma unroll
-                for (int tp = 0; tp < C::TAPS_S; ++tp) {
-                  const int ky = SX ? tp : (C::ROWSPLIT ? 0 : tp / KS);
-                  const int kx = SX ? 0 : (C::ROWSPLIT ? tp : tp % KS);
-                  const uint32_t a_off = (uint32_t)(m * 128 + ky * kTWH + kx);   // in 16-byte rows
+          for (int jj = 0; jj < kKC / 16; ++jj) {
+            const uint64_t bd = gmma_desc(w_base + tp * C::W_TAP + jj * 2 * C::NMMA * 16, C::NMMA * 16, 128);
 #pragma unroll
-                  for (int jj = 0; jj < kKC / 16; ++jj) {
-                    const uint64_t ad = ((uint64_t)D_HI << 32) | (a_lo + a_off + jj * 2 * (C::A_PLANE >> 4));
-                    const uint64_t bd = ((uint64_t)D_HI << 32) | (b_lo + (tp * (C::W_TAP / WH) + jj * 2 * B_PLANE) / 16);
-                    if constexpr (PAIR) umma_f16_ss_pair(d, ad, bd, idesc, (tp == 0 && jj == 0) ? not_first : 1u);
-                    else umma_f16_ss(d, ad, bd, idesc, (tp == 0 && jj == 0) ? not_first : 1u);
-                  }
-                }
-              }
+            for (int mb = 0; mb < 2; ++mb) {
+              const uint32_t a_row = (uint32_t)(m * 128 + mb * 64 + ky * kTWH + kx);   // 16-byte rows
+              const uint64_t ad = gmma_desc(a_base + a_row * 16 + jj * 2 * C::A_PLANE, C::A_PLANE, 128);
+              Wgmma<C::NMMA>::mma(acc[mb], ad, bd, (tp == 0 && jj == 0) ? not_first : 1u);
             }
-            __syncwarp();
           }
-          if (elect_one()) {                               // frees the smem stage (in both CTAs) once these MMAs retire
-            if constexpr (PAIR) umma_commit_pair(&ctrl->empty[s]);
-            else umma_commit(&ctrl->empty[s]);
-          }
-          tc_fence_before();                               // order this warp's tcgen05.mma before the flag (the
-          __syncwarp();                                    // other warp pairs it with tc_fence_after above)
-          if (lane == 0 && (QUAD || !p.msplit)) ctrl->issued[mq] = it + 1;   // hand over to the warp of the other stage parity
-          if (rw == 1 && lane == 0) dbg_rec(p, 1, dbg_it, 2);
-          ++dbg_it;
         }
-        unit += nu;
-        if (++s == S) { s = 0; ph ^= 1; }
       }
-      if (elect_one()) {                                   // this warp's share of the tile's MMAs
-        if constexpr (PAIR) umma_commit_pair(&ctrl->tmem_full[as]);
-        else umma_commit(&ctrl->tmem_full[as]);
-      }
-      __syncwarp();
+      wgmma_commit();
+      wgmma_wait<1>();                                         // the previous stage's wgmmas have retired
+      if (prev >= 0 && lane == 0) mbar_arrive(&ctrl->empty[prev]);
+      prev = (int)s;
+      unit += nu;
+      if (++s == S) { s = 0; ph ^= 1; }
     }
-  } else if (warp >= 4 && warp < 12) {
-    // ========================================================== epilogue
-    const int q = warp & 3;
-    const int m = (warp - 4) >> 2;                      // which 128-row accumulator of the tile
-    uint32_t acc_it = 0;
-    // FINAL epilogue: the mean of the input frames (RDN.py:221/279/333) of tile t+1 is loaded while tile t is being
-    // processed (one tile of software pipelining: a cold DRAM round trip per tile was the kernel's critical path).
-    constexpr int NFV = (EPI == BIN_EPI_FINAL) ? 3 * BIN_MAX_FRAMES : 1;
-    float fv[NFV];                                  // raw frame samples of the tile being processed
-    auto frame_load = [&](int tile_, float (&dst)[NFV]) {   // loads only: consumed one tile later
-      if constexpr (EPI == BIN_EPI_FINAL) {
-        int t = tile_ / p.nh;
-        const int txi_ = t % p.tiles_x; t /= p.tiles_x;
-        const int tyi_ = t % p.tiles_y;
-        const int b_ = p.b0 + t / p.tiles_y;
-        const int L_ = m * 128 + q * 32 + lane;
-        const int y_ = p.y0 + tyi_ * kTH + (L_ >> 5), x_ = txi_ * C::TW + (L_ & 31);
-        const bool valid_ = tile_ < p.ntiles && ((L_ & 31) < C::TW) && (y_ < p.y0 + p.ny) && (x_ < p.W);
-        const int call = b_ / p.fr.Bc, bb = b_ % p.fr.Bc;
-        const size_t hw = (size_t)p.H * p.W;
+    wgmma_wait<0>();
+    acc_fence(acc[0]);
+    acc_fence(acc[1]);
+    if (lane == 0) mbar_arrive(&ctrl->empty[prev]);
+
+    // ---------------------------------------------------------- epilogue from the accumulator fragments
+    // fragment of a 64-row block: acc[mb][4 i + 2 h + e] = row 16 wq + lane/4 + 8 h, column 8 i + 2 k4 + e
+    int t = tile_at(tq);
+    const int nh = t % p.nh; t /= p.nh;
+    const int txi = t % p.tiles_x; t /= p.tiles_x;
+    const int tyi = t % p.tiles_y;
+    const int b = p.b0 + t / p.tiles_y;
+    const int yend = p.y0 + p.ny;
 #pragma unroll
-        for (int c = 0; c < 3; ++c) {
-          const size_t off = ((size_t)bb * 3 + c) * hw + (size_t)y_ * p.W + x_;
+    for (int mb = 0; mb < 2; ++mb) {
+      if constexpr (SX) {                                      // kx = 1, 2 column groups -> shared memory
 #pragma unroll
-          for (int fi = 0; fi < BIN_MAX_FRAMES; ++fi)
-            dst[c * BIN_MAX_FRAMES + fi] = (valid_ && fi < p.fr.nframes) ? __ldg(p.fr.frame[call][fi] + off) : 0.f;
-        }
-      }
-    };
-    frame_load(blockIdx.x, fv);
-    const uint32_t tempty0 = PAIR ? mapa_u32(smem_u32(&ctrl->tmem_empty[0]), 0) : 0u;   // the LEADER's barriers
-    // Tile coordinates are advanced incrementally (mixed-radix add of the per-iteration step) instead of being decoded
-    // with six integer divisions per tile: with four MMA warps the epilogue is the kernel's critical path and those
-    // divisions were ~300 cycles of it per tile.  (Pair / reversed launches keep the division form.)
-    constexpr bool kIncr = !PAIR;
-    int c_nh = 0, c_tx = 0, c_ty = 0, c_b = 0, d_nh = 0, d_tx = 0, d_ty = 0, d_b = 0;
-    if (kIncr && !p.reverse) {
-      int t = tq0;
-      c_nh = t % p.nh; t /= p.nh; c_tx = t % p.tiles_x; t /= p.tiles_x; c_ty = t % p.tiles_y; c_b = t / p.tiles_y;
-      t = tqstep;
-      d_nh = t % p.nh; t /= p.nh; d_tx = t % p.tiles_x; t /= p.tiles_x; d_ty = t % p.tiles_y; d_b = t / p.tiles_y;
-    }
-    // x-stacked conv: the 32 biases of the tile's output channels live in registers for the whole persistent loop (they were
-    // 8 LDS.128 per warp and tile on the shared-memory pipe the MMA operands need)
-    float breg[(SX && EPI == BIN_EPI_P8) ? NT : 1];
-    if constexpr (SX && EPI == BIN_EPI_P8) {
+        for (int i = NT / 8; i < C::NMMA / 8; ++i)
 #pragma unroll
-      for (int i = 0; i < NT; ++i) breg[i] = bsrc[i];
-    }
-    for (int tq = tq0; tq < tqn; tq += tqstep, ++acc_it) {
-      bool live = true;
-      int tile, nh, txi, tyi, b;
-      if (kIncr && !p.reverse) {
-        tile = tq; nh = c_nh; txi = c_tx; tyi = c_ty; b = p.b0 + c_b;
-        c_nh += d_nh; if (c_nh >= p.nh) { c_nh -= p.nh; ++c_tx; }            // next tile's coordinates
-        c_tx += d_tx; if (c_tx >= p.tiles_x) { c_tx -= p.tiles_x; ++c_ty; }
-        c_ty += d_ty; if (c_ty >= p.tiles_y) { c_ty -= p.tiles_y; ++c_b; }
-        c_b += d_b;
-      } else {
-        tile = tile_at(tq, live);
-        int t = tile;
-        nh = t % p.nh; t /= p.nh;
-        txi = t % p.tiles_x; t /= p.tiles_x;
-        tyi = t % p.tiles_y;
-        b = p.b0 + t / p.tiles_y;
-      }
-      const int yend = p.y0 + p.ny;
-      const uint32_t as = acc_it & 1, aph = (acc_it >> 1) & 1;
-      float fmean[(EPI == BIN_EPI_FINAL) ? 3 : 1];
-      if constexpr (EPI == BIN_EPI_FINAL) {
-#pragma unroll
-        for (int c = 0; c < 3; ++c) {
-          float acc = fv[c * BIN_MAX_FRAMES];
-#pragma unroll
-          for (int fi = 1; fi < BIN_MAX_FRAMES; ++fi) acc += fv[c * BIN_MAX_FRAMES + fi];   // left-to-right like the reference
-          fmean[c] = acc / (float)p.fr.nframes;
-        }
-      }
-      frame_load(tile + (int)gridDim.x, fv);                      // next tile's samples: in flight during this tile's wait + stores
-      const int L = m * 128 + q * 32 + lane;
-      const int ty = L >> 5, tx = L & 31;
-      const int y = p.y0 + tyi * kTH + ty, x = txi * C::TW + tx;
-      const bool valid = live && (tx < C::TW) && (y < yend) && (x < p.W);
-      // operands of the epilogue that do not depend on the accumulators are fetched BEFORE waiting for
-      // them, so their global-load latency overlaps the MMAs: the residual tile (RDN.py:165, :219) ...
-      uint4 rbuf[(EPI == BIN_EPI_P8 && !SX) ? (X3 ? 2 : 1) * (NT / 8) : 1];
-      if constexpr (EPI == BIN_EPI_P8 && !SX) {
-        if (p.res != nullptr) {
-#pragma unroll
-          for (int k = 0; k < NT / 8; ++k) {
-            const int lp = p.res_plane0 + (nh * NT) / 8 + k;
-            const bool ok = valid && (nh * NT) / 8 + k < p.store_planes;
-            const size_t off = ((((size_t)b * p.res_planes + (X3 ? x3_plane(lp) : lp)) * p.H + y) * p.W + x) * 8;
-            rbuf[k] = ok ? *reinterpret_cast<const uint4*>(p.res + off) : make_uint4(0, 0, 0, 0);
-            if constexpr (X3)
-              rbuf[NT / 8 + k] = ok ? *reinterpret_cast<const uint4*>(p.res + off + (size_t)4 * p.H * p.W * 8) : make_uint4(0, 0, 0, 0);
+          for (int h = 0; h < 2; ++h) {
+            const int r = wq * 16 + (lane >> 2) + 8 * h;
+            *reinterpret_cast<float2*>(xbuf + r * C::XPITCH + 8 * i - NT + 2 * k4) =
+                make_float2(acc[mb][4 * i + 2 * h], acc[mb][4 * i + 2 * h + 1]);
           }
-        }
+        wg_sync(1 + m);
       }
-      constexpr float kAcc = X3 ? (1.f / 256.f) : 1.f;      // X3 weights are packed scaled by 2^8
-      if (warp == kDbgEpiWarp(p) && lane == 0) dbg_rec(p, 2, acc_it, 0);
-      if (p.polite) mbar_wait_polite(&ctrl->tmem_full[as], aph, 40, kTag | (4ull << 32) | acc_it);
-      else mbar_wait(&ctrl->tmem_full[as], aph, kTag | (4ull << 32) | acc_it);
-      if (warp == kDbgEpiWarp(p) && lane == 0) dbg_rec(p, 2, acc_it, 1);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + as * C::ACC_COLS + m * C::NMMA;
-      if constexpr (EPI == BIN_EPI_P8) {
-        // TMEM loads are issued in batches (tcgen05.wait::ld waits for ALL outstanding loads, so one wait per
-        // 16 columns serialised a ~200-cycle round trip six times per tile and made the LFF epilogue the bottleneck)
-        constexpr int GRP = SX ? 32 : (NT % 48 == 0 ? 48 : (NT % 32 == 0 ? 32 : 16));   // output channels per batch
 #pragma unroll
-        for (int g0 = 0; g0 < NT; g0 += GRP) {
-          uint32_t v[(SX ? 3 : 1) * GRP];
-#ifdef BIN_B200_TOOLS      // epilogue ablations for the timeline tool (timing only, results are garbage): BIN_B200_DEBUG bits 5..8
-          const bool abl_ld = p.debug & 32, abl_bias = p.debug & 64, abl_shfl = p.debug & 128, abl_st = p.debug & 256;
-          if (abl_ld) {
-#pragma unroll
-            for (int i = 0; i < (SX ? 3 : 1) * GRP; ++i) v[i] = lane + i;
-          } else
-#else
-          constexpr bool abl_bias = false, abl_shfl = false, abl_st = false;
-#endif
-#pragma unroll
-          for (int j = 0; j < GRP / 16; ++j) {
-            if constexpr (SX) {
-              tmem_ld16(taddr + g0 + 16 * j, *reinterpret_cast<uint32_t(*)[16]>(&v[16 * j]));
-              tmem_ld16(taddr + NT + g0 + 16 * j, *reinterpret_cast<uint32_t(*)[16]>(&v[GRP + 16 * j]));
-              tmem_ld16(taddr + 2 * NT + g0 + 16 * j, *reinterpret_cast<uint32_t(*)[16]>(&v[2 * GRP + 16 * j]));
-            } else {
-              tmem_ld16(taddr + g0 + 16 * j, *reinterpret_cast<uint32_t(*)[16]>(&v[16 * j]));
-            }
+      for (int h = 0; h < 2; ++h) {
+        const int r = wq * 16 + (lane >> 2) + 8 * h;           // row within the 64-row block
+        const int L = m * 128 + mb * 64 + r;
+        const int ty = L >> 5, tx = L & 31;
+        const int y = p.y0 + tyi * kTH + ty, x = txi * C::TW + tx;
+        const bool valid = (tx < C::TW) && (y < yend) && (x < p.W);
+        // value of output channel column 8 i + 2 k4 + e of this pixel (x-stacked: out[p] = D0[p] + D1[p+1] + D2[p+2])
+        auto val = [&](int i, int e) {
+          const float d0 = acc[mb][4 * i + 2 * h + e];
+          if constexpr (SX) {
+            const int col = 8 * i + 2 * k4 + e;
+            return ((d0 + xbuf[(r + 1) * C::XPITCH + col]) + xbuf[(r + 2) * C::XPITCH + NT + col]) * kAcc;
+          } else {
+            return d0 * kAcc;
           }
-          tmem_ld_wait();
-          if (warp == kDbgEpiWarp(p) && lane == 0 && g0 == 0) dbg_rec(p, 2, acc_it, 3);        // tools build: TMEM loads have landed
-#pragma unroll
-          for (int j = 0; j < GRP / 16; ++j) {
-            const int n0 = g0 + 16 * j;
-            float f[16];
-            if constexpr (SX) {
-              // out[p] = D[p][kx=0] + D[p+1][kx=1] + D[p+2][kx=2]; p+1, p+2 are lanes +1, +2 of this warp
-#pragma unroll
-              for (int i = 0; i < 16; ++i) {
-                const float b1 = abl_shfl ? __uint_as_float(v[GRP + 16 * j + i]) : __shfl_down_sync(0xffffffffu, __uint_as_float(v[GRP + 16 * j + i]), 1);
-                const float b2 = abl_shfl ? __uint_as_float(v[2 * GRP + 16 * j + i]) : __shfl_down_sync(0xffffffffu, __uint_as_float(v[2 * GRP + 16 * j + i]), 2);
-                f[i] = ((__uint_as_float(v[16 * j + i]) + b1) + b2) * kAcc + (abl_bias ? 0.25f : breg[n0 + i]);
-              }
-            } else {
-#pragma unroll
-              for (int i = 0; i < 16; ++i) f[i] = __uint_as_float(v[16 * j + i]) * kAcc + bsrc[nh * NT + n0 + i];
-            }
-            if (valid) {
-              if (p.relu) {
-#pragma unroll
-                for (int i = 0; i < 16; ++i) f[i] = fmaxf(f[i], 0.f);
-              }
-              const int cpl = (nh * NT + n0) >> 3;   // channel plane of f[0]
-              if (!SX && p.res != nullptr) {
-#pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                  const uint4 r = rbuf[SX ? 0 : n0 / 8 + h];
-                  const uint32_t rr[4] = {r.x, r.y, r.z, r.w};
-#pragma unroll
-                  for (int i = 0; i < 4; ++i) {
-                    const float2 g = unpack_h2(rr[i]);
-                    f[h * 8 + 2 * i] += g.x;
-                    f[h * 8 + 2 * i + 1] += g.y;
-                  }
-                  if constexpr (X3 && !SX) {
-                    const uint4 r2 = rbuf[NT / 8 + n0 / 8 + h];
-                    const uint32_t rl[4] = {r2.x, r2.y, r2.z, r2.w};
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) {
-                      const float2 g = unpack_h2(rl[i]);
-                      f[h * 8 + 2 * i] += g.x;
-                      f[h * 8 + 2 * i + 1] += g.y;
-                    }
-                  }
-                }
-              }
-#pragma unroll
-              for (int h = 0; h < 2; ++h) {
-                if constexpr (X3) {
-                  const size_t off = ((((size_t)b * p.out_planes + x3_plane(p.out_plane0 + cpl + h)) * p.H + y) * p.W + x) * 8;
-                  if (cpl + h < p.store_planes) split_store(p.out + off, p.out + off + (size_t)4 * p.H * p.W * 8, f + h * 8);
-                } else {
-                  uint4 o;
-                  o.x = pack_h2(f[h * 8 + 0], f[h * 8 + 1]);
-                  o.y = pack_h2(f[h * 8 + 2], f[h * 8 + 3]);
-                  o.z = pack_h2(f[h * 8 + 4], f[h * 8 + 5]);
-                  o.w = pack_h2(f[h * 8 + 6], f[h * 8 + 7]);
-                  const size_t off = ((((size_t)b * p.out_planes + p.out_plane0 + cpl + h) * p.H + y) * p.W + x) * 8;
-                  if (cpl + h < p.store_planes && !abl_st) *reinterpret_cast<uint4*>(p.out + off) = o;
-                }
-              }
-            }
-          }
-        }
-      } else if constexpr (EPI == BIN_EPI_PIXSHUF) {
-        // out[c, 2y+i, 2x+j] = conv[4c+2i+j, y, x]   (nn.PixelShuffle(2), RDN.py:206)
-#pragma unroll 2
-        for (int n0 = 0; n0 < NT; n0 += 32) {
-          uint32_t v0[16], v1[16];
-          tmem_ld16(taddr + n0, v0);
-          tmem_ld16(taddr + n0 + 16, v1);
-          tmem_ld_wait();
+        };
+        if constexpr (EPI == BIN_EPI_P8) {
           if (valid) {
-            float f[32];
 #pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              f[i] = __uint_as_float(v0[i]) * kAcc + sbias[nh * NT + n0 + i];
-              f[16 + i] = __uint_as_float(v1[i]) * kAcc + sbias[nh * NT + n0 + 16 + i];
+            for (int i = 0; i < NT / 8; ++i) {
+              const int rel = (nh * NT) / 8 + i;                // channel plane relative to out_plane0
+              if (rel >= p.store_planes) continue;
+              const int n = nh * NT + 8 * i + 2 * k4;
+              float f0 = val(i, 0) + bsrc[n], f1 = val(i, 1) + bsrc[n + 1];
+              if (p.relu) { f0 = fmaxf(f0, 0.f); f1 = fmaxf(f1, 0.f); }
+              if (!SX && p.res != nullptr) {
+                const int lp = p.res_plane0 + rel;
+                const size_t off = ((((size_t)b * p.res_planes + (X3 ? x3_plane(lp) : lp)) * p.H + y) * p.W + x) * 8 + 2 * k4;
+                const float2 g = unpack_h2(*reinterpret_cast<const uint32_t*>(p.res + off));
+                f0 += g.x; f1 += g.y;
+                if constexpr (X3) {
+                  const float2 g2 = unpack_h2(*reinterpret_cast<const uint32_t*>(p.res + off + (size_t)4 * p.H * p.W * 8));
+                  f0 += g2.x; f1 += g2.y;
+                }
+              }
+              const int op = p.out_plane0 + rel;
+              const size_t off = ((((size_t)b * p.out_planes + (X3 ? x3_plane(op) : op)) * p.H + y) * p.W + x) * 8 + 2 * k4;
+              store_pair<X3>(p.out + off, (size_t)4 * p.H * p.W * 8, f0, f1);
             }
-            const int opl = (nh * NT + n0) >> 5;   // output plane (8 channels = 32 conv channels)
+          }
+        } else if constexpr (EPI == BIN_EPI_PIXSHUF) {
+          // out[c, 2y+i, 2x+j] = conv[4c+2i+j, y, x]   (nn.PixelShuffle(2), RDN.py:206)
+          if (valid) {
             const int H2 = 2 * p.H, W2 = 2 * p.W;
 #pragma unroll
-            for (int ij = 0; ij < 4; ++ij) {
-              const int yy = 2 * y + (ij >> 1), xx = 2 * x + (ij & 1);
-              if constexpr (X3) {
-                float g8[8];
+            for (int i = 0; i < NT / 8; ++i) {
 #pragma unroll
-                for (int cc = 0; cc < 8; ++cc) g8[cc] = f[cc * 4 + ij];
-                const size_t off = ((((size_t)b * p.out_planes + x3_plane(p.out_plane0 + opl)) * H2 + yy) * W2 + xx) * 8;
-                split_store(p.out + off, p.out + off + (size_t)4 * H2 * W2 * 8, g8);
-              } else {
-                uint4 o;
-                o.x = pack_h2(f[0 * 4 + ij], f[1 * 4 + ij]);
-                o.y = pack_h2(f[2 * 4 + ij], f[3 * 4 + ij]);
-                o.z = pack_h2(f[4 * 4 + ij], f[5 * 4 + ij]);
-                o.w = pack_h2(f[6 * 4 + ij], f[7 * 4 + ij]);
-                const size_t off = ((((size_t)b * p.out_planes + p.out_plane0 + opl) * H2 + yy) * W2 + xx) * 8;
-                *reinterpret_cast<uint4*>(p.out + off) = o;
+              for (int e = 0; e < 2; ++e) {
+                const int n = nh * NT + 8 * i + 2 * k4 + e;
+                const int c = n >> 2, yy = 2 * y + ((n >> 1) & 1), xx = 2 * x + (n & 1);
+                const int op = p.out_plane0 + (c >> 3);
+                const size_t off = ((((size_t)b * p.out_planes + (X3 ? x3_plane(op) : op)) * H2 + yy) * W2 + xx) * 8 + (c & 7);
+                store_one<X3>(p.out + off, (size_t)4 * H2 * W2 * 8, val(i, e) + sbias[n]);
               }
             }
           }
-        }
-      } else {  // BIN_EPI_FINAL: fp32 NCHW = conv + bias + mean(frames)
-        float cv[3];
-        if constexpr (SX) {
-          uint32_t v0[16], v1[16], v2[16];
-          tmem_ld16(taddr, v0);
-          tmem_ld16(taddr + NT, v1);
-          tmem_ld16(taddr + 2 * NT, v2);
-          tmem_ld_wait();
+        } else {  // BIN_EPI_FINAL: fp32 NCHW = conv + bias + mean(frames) (RDN.py:221/279/333); channels 0..2
+          if (valid && k4 < 2) {
+            const int call = b / p.fr.Bc, bb = b % p.fr.Bc;
+            const size_t hw = (size_t)p.H * p.W;
 #pragma unroll
-          for (int c = 0; c < 3; ++c) {
-            const float b1 = __shfl_down_sync(0xffffffffu, __uint_as_float(v1[c]), 1);
-            const float b2 = __shfl_down_sync(0xffffffffu, __uint_as_float(v2[c]), 2);
-            cv[c] = ((__uint_as_float(v0[c]) + b1) + b2) * kAcc;
-          }
-        } else {
-          uint32_t v[16];
-          tmem_ld16(taddr, v);
-          tmem_ld_wait();
-#pragma unroll
-          for (int c = 0; c < 3; ++c) cv[c] = __uint_as_float(v[c]) * kAcc;
-        }
-        if (valid) {
-          const int call = b / p.fr.Bc, bb = b % p.fr.Bc;
-          const size_t hw = (size_t)p.H * p.W;
-#pragma unroll
-          for (int c = 0; c < 3; ++c) {
-            const size_t off = ((size_t)bb * 3 + c) * hw + (size_t)y * p.W + x;
-            p.fr.out[call][off] = (cv[c] + sbias[c]) + fmean[c];
+            for (int e = 0; e < 2; ++e) {
+              const int c = 2 * k4 + e;
+              if (c >= 3) continue;
+              const size_t off = ((size_t)bb * 3 + c) * hw + (size_t)y * p.W + x;
+              float fm = __ldg(p.fr.frame[call][0] + off);
+              for (int fi = 1; fi < p.fr.nframes; ++fi) fm += __ldg(p.fr.frame[call][fi] + off);   // left to right
+              p.fr.out[call][off] = (val(0, e) + sbias[c]) + fm / (float)p.fr.nframes;
+            }
           }
         }
       }
-      tc_fence_before();
-      __syncwarp();                                        // every lane's tcgen05.ld has completed (wait::ld above)
-      if (lane == 0) {
-        if constexpr (PAIR) mbar_arrive_cluster(tempty0 + as * 8);
-        else mbar_arrive(&ctrl->tmem_empty[as]);
-      }
-      if (warp == kDbgEpiWarp(p) && lane == 0) dbg_rec(p, 2, acc_it, 2);
+      if constexpr (SX) wg_sync(1 + m);                       // xbuf is rewritten by the next block
     }
-  }
-
-  // ------------------------------------------------------------ teardown
-  tc_fence_before();
-  __syncthreads();
-  if constexpr (PAIR) cluster_sync_all();                      // the leader's MMAs touch the peer's smem / TMEM
-  if (rw == 2) {
-    tc_fence_after();
-    if constexpr (PAIR) tmem_dealloc_pair(tmem_base, C::TMEM_COLS);
-    else tmem_dealloc(tmem_base, C::TMEM_COLS);
   }
 }
 
@@ -713,8 +371,6 @@ int make_p8_tmap(CUtensorMap* m, const bin_act_t& t, int box_rows) {
   if (r != CUDA_SUCCESS) return fail(BIN_ERR_CUDA, "cuTensorMapEncodeTiled failed with code " + std::to_string((int)r));
   return BIN_OK;
 }
-
-long long* g_dbg = nullptr;   // perf-debug timeline buffer (tools only)
 
 // Generic P8 box: box_px pixels x box_rows rows x box_planes planes (used by the weight-gradient kernel).
 int make_p8_tmap_box(CUtensorMap* m, const bin_act_t& t, int box_px, int box_rows, int box_planes) {
@@ -760,81 +416,31 @@ static int launch_inst(const bin_conv_args_t& a, cudaStream_t s, bool reverse) {
   p.ntiles = nb * p.tiles_x * p.tiles_y * p.nh;
   p.relu = a.relu;
   const int nchunks = p.nch0 + p.nch1;
-  // CTA pairs (cta_group::2) for the x-stacked RDB convs: the resident weights are split between the two CTAs
-  constexpr bool kPairable = SX && KS == 3 && NT == 32 && EPI == BIN_EPI_P8 && !X3;
-  const int wh = (kPairable && options().pair) ? 2 : 1;
+  const int xbytes = kMT * C::XBYTES;
   // keep the whole weight set resident in smem when it leaves room for >= 3 activation stages
   p.resident = (p.nh == 1 && nchunks <= kMaxResidentChunks &&
-                kCtrlBytes + nchunks * C::W_CHUNK / wh + 3 * C::A_BYTES + 256 <= kSmemMax) ? 1 : 0;
-  const bool pair = wh == 2 && p.resident;
-  const int res_bytes = p.resident ? nchunks * C::W_CHUNK / (pair ? 2 : 1) : 0;
+                kCtrlBytes + nchunks * C::W_CHUNK + xbytes + 3 * C::A_BYTES + 256 <= kSmemMax) ? 1 : 0;
+  const int res_bytes = p.resident ? nchunks * C::W_CHUNK : 0;
   const int unit_bytes = C::A_BYTES + (p.resident ? 0 : C::W_STAGE);
   const int nunits = nchunks * C::NSUB;
   // units per pipeline stage: an mbarrier round trip costs a few hundred cycles, so a stage should
-  // carry >= ~12 MMAs (>= ~700 tensor-pipe cycles); one 1x1 unit is only 4 MMAs.
+  // carry >= ~12 wgmma instructions per warpgroup; one 1x1 unit is only 4.
   const int mma_per_unit = kMT * C::TAPS_S * (kKC / 16);
   int cps = (options().stage_mmas + mma_per_unit - 1) / mma_per_unit;
   if (cps > nunits) cps = nunits;
-  const int avail = kSmemMax - kCtrlBytes - res_bytes - 256;
+  const int avail = kSmemMax - kCtrlBytes - res_bytes - xbytes - 256;
   while (cps > 1 && avail / (cps * unit_bytes) < 2) --cps;
   int S = avail / (cps * unit_bytes);
   if (S > kMaxStages) S = kMaxStages;
-  S &= ~1;                                     // even: producer i%2 must always see the same slots
   if (S < 2) return fail(BIN_ERR_UNSUPPORTED, "conv configuration does not fit in shared memory");
   p.nstages = S;
   p.cps = cps;
-  const int smem_bytes = kCtrlBytes + res_bytes + S * cps * unit_bytes + 256;
+  const int smem_bytes = kCtrlBytes + res_bytes + S * cps * unit_bytes + xbytes + 256;
   p.out = reinterpret_cast<__half*>(a.out.ptr); p.out_planes = a.out.planes; p.out_plane0 = a.out_plane0;
   p.store_planes = a.store_planes > 0 ? a.store_planes : a.cout_pad / 8;
   p.res = reinterpret_cast<const __half*>(a.res.ptr); p.res_planes = a.res.planes; p.res_plane0 = a.res_plane0;
   p.fr = a.fr;
-  p.debug = options().debug;
-  p.msplit = options().msplit ? 1 : 0;
-  p.polite = options().polite ? 1 : 0;
-  p.spread = options().spread ? 1 : 0;
-  p.reverse = (reverse && EPI == BIN_EPI_P8) ? 1 : 0;     // (the FINAL epilogue prefetches tile + gridDim.x: forward only)
-#ifdef BIN_B200_TOOLS
-  if (p.debug & 8) {
-    if (!g_dbg) { BIN_CUDA_OK(cudaMalloc(&g_dbg, 3 * 4096 * sizeof(long long))); }
-    BIN_CUDA_OK(cudaMemsetAsync(g_dbg, 0, 3 * 4096 * sizeof(long long), s));
-    p.dbg = g_dbg;
-  }
-#endif
-  if constexpr (kPairable) {
-    if (pair) {
-      if (cps != 1) return fail(BIN_ERR_UNSUPPORTED, "conv pair kernel expects one unit per stage");
-      auto kp = conv_igemm_kernel<NT, KS, EPI, SX, X3, true>;
-      static std::atomic<unsigned long long> pair_opted{0};   // per device
-      BIN_TRY(ensure_dynamic_smem(kp, kSmemMax, pair_opted));
-      const int npt = (p.ntiles + 1) / 2, maxc = num_sms() / 2;
-      const int nclusters = npt < maxc ? npt : maxc;
-      if (nclusters < 1) return BIN_OK;
-      cudaLaunchConfig_t cfg;
-      memset(&cfg, 0, sizeof(cfg));
-      cfg.gridDim = dim3(2 * nclusters); cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = smem_bytes; cfg.stream = s;
-      cudaLaunchAttribute at[1];
-      at[0].id = cudaLaunchAttributeClusterDimension;
-      at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-      cfg.attrs = at; cfg.numAttrs = 1;
-      BIN_CUDA_OK(cudaLaunchKernelEx(&cfg, kp, p));
-      return BIN_OK;
-    }
-  }
-  constexpr bool kQuadable = !X3 && EPI != BIN_EPI_FINAL;
-  if constexpr (kQuadable) {
-    // (not with a residual / accumulate epilogue: its prefetch registers do not fit under the 448-thread bound without
-    // spills, and the data-gradient convs of the training step measured 1.5 % slower with it)
-    if (options().quad && (SX || a.res.ptr == nullptr)) {
-      auto kq = conv_igemm_kernel<NT, KS, EPI, SX, X3, false, true>;
-      static std::atomic<unsigned long long> quad_opted{0};   // per instantiation, per device
-      BIN_TRY(ensure_dynamic_smem(kq, kSmemMax, quad_opted));
-      const int gq = p.ntiles < num_sms() ? p.ntiles : num_sms();
-      if (gq < 1) return BIN_OK;
-      kq<<<gq, kThreads + 64, smem_bytes, s>>>(p);
-      BIN_CUDA_OK(cudaGetLastError());
-      return BIN_OK;
-    }
-  }
+  p.reverse = (reverse && EPI == BIN_EPI_P8) ? 1 : 0;
   auto kern = conv_igemm_kernel<NT, KS, EPI, SX, X3>;
   static std::atomic<unsigned long long> smem_opted{0};   // per instantiation, per device
   BIN_TRY(ensure_dynamic_smem(kern, kSmemMax, smem_opted));
@@ -842,7 +448,7 @@ static int launch_inst(const bin_conv_args_t& a, cudaStream_t s, bool reverse) {
   if (grid < 1) return BIN_OK;
   kern<<<grid, kThreads, smem_bytes, s>>>(p);
   BIN_CUDA_OK(cudaGetLastError());
-  if (p.debug & 16) {                       // debugging aid: synchronise and name the failing launch
+  if (options().debug & 16) {              // debugging aid: synchronise and name the failing launch
     cudaError_t e = cudaStreamSynchronize(s);
     if (e != cudaSuccess)
       return fail(BIN_ERR_CUDA, std::string("conv launch failed: ") + cudaGetErrorString(e) + " NT=" + std::to_string(NT) +

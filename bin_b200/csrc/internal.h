@@ -41,30 +41,21 @@ inline int ensure_dynamic_smem(Kernel kern, int bytes, std::atomic<unsigned long
 }
 
 // ------------------------------------------------------------------ process options
-// Environment knobs of the library (documented in DESIGN.md).  The product build reads them ONCE per process (no
-// getenv on the launch path); the tools build (-DBIN_B200_TOOLS) re-reads them on every call so that a tool can A/B
-// configurations inside one process.
+// Environment knobs of the library (documented in DESIGN.md), read once per process (no getenv on the launch path).
 struct Options {
-  int debug;                 // BIN_B200_DEBUG   bit 3: role timeline (tools build only), bit 4: synchronise after each conv launch
+  int debug;                 // BIN_B200_DEBUG   bit 4: synchronise after each conv launch
   bool fuse_lff;             // BIN_B200_FUSE_LFF=0 runs conv3 and LFF as two launches instead of rdb_tail_kernel
-  bool tail_streams;         // BIN_B200_TAIL_STREAMS=0 selects the hand-off variant of rdb_tail_kernel
-  bool pair;                 // BIN_B200_PAIR=1 selects the CTA-pair (cta_group::2) kernels (measured slower: opt-in)
-  bool msplit;               // BIN_B200_MSPLIT: conv MMA warps split the tile's two accumulators instead of alternating stages
-  bool quad;                 // BIN_B200_QUAD=0 falls back to two MMA warps in the x-stacked conv kernel (default: four)
-  bool tailq;                // BIN_B200_TAILQ: two MMA warps per tile stream in rdb_tail_kernel (448 threads)
-  bool spread;               // BIN_B200_SPREAD: QUAD convs put one MMA warp on each SM sub-partition
-  bool polite;               // BIN_B200_POLITE: producers / epilogue warps sleep between barrier polls (power)
   bool zigzag;               // BIN_B200_ZIGZAG: consecutive RDB launches walk the tiles in opposite directions (L2 reuse)
-  int stage_mmas;            // BIN_B200_STAGE_MMAS: target MMAs per pipeline stage of the conv kernel (default 12)
+  int stage_mmas;            // BIN_B200_STAGE_MMAS: target wgmma instructions per pipeline stage of the conv kernel (default 12)
   size_t band_budget;        // BIN_B200_BAND_BUDGET_KB (L2 band walker; default: one band)
 };
 const Options& options();
 int num_sms();               // SM count of the current device (cached per device)
 
 // ------------------------------------------------------------------ tile geometry of the conv kernel
-constexpr int kTWH = 32;   // smem row pitch of an activation tile, in pixels (= 4 UMMA row groups)
+constexpr int kTWH = 32;   // smem row pitch of an activation tile, in pixels (= 4 core-matrix row groups)
 constexpr int kTH = 8;     // output rows per CTA tile
-constexpr int kMT = 2;     // 128-row accumulators per CTA tile (kTH*kTWH/128)
+constexpr int kMT = 2;     // 128-row accumulators per CTA tile (kTH*kTWH/128), one per consumer warpgroup
 constexpr int kKC = 32;    // input channels per pipeline stage
 constexpr int kKPL = 4;    // P8 planes per stage
 constexpr int kCtrlBytes = 2048;
@@ -81,13 +72,11 @@ struct alignas(64) ConvParams {
   int H, W, Btot;                      // conv resolution
   int b0, y0, ny;                      // batch / row sub-range processed by this launch
   int tiles_x, tiles_y, ntiles, nh;    // nh = cout_pad / NT
-  int relu, resident, nstages, cps, debug, msplit, reverse, polite, spread;
+  int relu, resident, nstages, cps, reverse;
   __half* out; int out_planes, out_plane0, store_planes;
   const __half* res; int res_planes, res_plane0;
   bin_frames_t fr;
-  long long* dbg;
 };
-extern long long* g_dbg;
 
 int launch_conv(const bin_conv_args_t& a, cudaStream_t s, bool reverse = false);   // reverse: walk the tiles last-to-first
 

@@ -1,54 +1,49 @@
-// bin_b200 -- fused tail of a residual dense block for sm_100a:
+// bin_b200 -- fused tail of a residual dense block for sm_90a:
 //   g3 = ReLU(conv3x3(cat(x, g0, g1, g2)))        RDN.py:141-147 (RDB_Conv, the 4th of RDN.py:156-160)
 //   x' = LFF(cat(x, g0, g1, g2, g3)) + x          RDN.py:162-165 (1x1 conv 224 -> 96, local residual)
-// in ONE kernel.  Layer by layer these two move 448 + 832 bytes per position through HBM and are bound by it
-// (DESIGN.md 5); fused, the 192 input channels are fetched once (the 1x1 LFF reads the centre of the very halo tile
-// the 3x3 conv already has in shared memory), g3 never leaves the SM, and only x' is written: 768 bytes per position.
+// in ONE kernel.  Layer by layer these two move 448 + 832 bytes per position through HBM; fused, the 192 input
+// channels are fetched once (the 1x1 LFF reads the centre of the very halo tile the 3x3 conv already has in shared
+// memory), g3 never leaves the SM, and only x' is written: 768 bytes per position.
 //
 // GEMM view per 128-pixel tile (4 rows x 32-pixel smem pitch, 30 valid columns) and 32-channel chunk c = 0..5:
 //   conv accumulator  (128 x 96, the three kx taps stacked in N as in conv_igemm.cu)  += A(ky) * Wc[c][ky],  ky = 0..2
 //   LFF accumulator   (128 x 96)                                                      += A(centre) * Wl[c]
-// then, once the conv accumulator is complete, the epilogue-A warps add the kx column groups (warp shuffles), apply
-// bias + ReLU, and write g3 of the tile as a K-major fp16 operand into shared memory, and ONE more K = 32 step
-//   LFF accumulator += g3 * Wl[6]
-// finishes x'.  That "tail" step of tile t is issued AFTER the main loop of tile t+1, so the tensor pipe never waits
-// for the epilogue: TMEM holds two conv accumulators and three LFF accumulators (2*96 + 3*96 = 480 columns).
-// All weights (6 x 4 slabs + 1 = 150 KB) stay resident in shared memory; activations stream through a 4-stage ring.
+// then the conv accumulator's kx column groups are added (through shared memory), bias + ReLU applied, g3 written as a
+// K-major fp16 operand into shared memory, and ONE more K = 32 step  LFF accumulator += g3 * Wl[6]  finishes x'.
+// The accumulation order per accumulator is that of conv_igemm_kernel (chunk, ky, k16 step), so the fused and the
+// layer-by-layer results are bit-identical.  All weights (6 x 4 slabs + 1 = 150 KB) stay resident in shared memory.
 //
-// Warp roles (384 threads, 1 CTA/SM, persistent):
-//   warp 0 lane 0 : TMA producer              warp 2 : TMEM allocator
-//   warps 1, 3    : cooperating tcgen05.mma issuers: alternate 8-MMA stage items, one warp's barrier polls overlap
-//                   the other's issue phase
-//   warps 4..7    : epilogue A (conv accumulator -> g3 tile in smem), one TMEM lane quarter each
-//   warps 8..11   : epilogue B (LFF accumulator + bias + residual -> P8 store)
+// Roles (384 threads, 1 CTA/SM, persistent):
+//   warp 0 lane 0 : TMA producer (weights once, then one activation chunk per ring slot)
+//   warpgroup 1+m : tile rows [64 m, 64 m + 64): both accumulators in registers, the g3 rows, the x' stores
 #include <stdio.h>
 #include <stdlib.h>
 
 #include "common.cuh"
 #include "internal.h"
+#include "wgmma.cuh"
 
 namespace binb {
 
-constexpr int kRtTH = 4;                               // output rows per tile (one 128-row accumulator)
+constexpr int kRtTH = 4;                               // output rows per tile (128 GEMM rows)
 constexpr int kRtRows = kRtTH + 2;                     // + 3x3 halo
 constexpr int kRtTW = kTWH - 2;                        // valid output columns per tile
 constexpr int kRtAPlane = kRtRows * kTWH * 16;         // bytes of one 8-channel plane of a stage
 constexpr int kRtABytes = kKPL * kRtAPlane;            // 12 288
-constexpr int kRtN = 96;                               // N of every MMA (3 kx x 32 conv channels, or the 96 LFF channels)
+constexpr int kRtN = 96;                               // N of every wgmma (3 kx x 32 conv channels, or the 96 LFF channels)
 constexpr int kRtSlab = kKPL * kRtN * 16;              // [4 planes][96 rows][16 B] = 6 144
 constexpr int kRtChunks = 6;                           // 192 input channels of the conv
 constexpr int kRtWChunk = 4 * kRtSlab;                 // conv ky = 0,1,2 + LFF slab of the chunk
 constexpr int kRtWBytes = kRtChunks * kRtWChunk + kRtSlab;   // + the LFF slab of the g3 channels
 constexpr int kRtHPlane = 128 * 16;
 constexpr int kRtHBytes = kKPL * kRtHPlane;            // g3 tile: [4 planes][128 pixels][16 B]
-constexpr int kRtStages = 4;                            // even: each MMA warp owns two fixed slots (5 slots were not faster)
-constexpr int kRtCtrl = 1024;                          // barriers + counters (512 B) and the two bias vectors (512 B)
-constexpr int kRtSmem = kRtCtrl + kRtWBytes + 2 * kRtHBytes + kRtStages * kRtABytes;
-constexpr int kRtLffCol0 = 2 * kRtN;                   // TMEM: conv[a] at a*96, lff[l] at 192 + l*96
+constexpr int kRtXPitch = 2 * 32 + 4;                  // kx = 1, 2 column groups of 66 rows, padded pitch (floats)
+constexpr int kRtXBytes = 66 * kRtXPitch * 4;          // per warpgroup
+constexpr int kRtStages = 2;
+constexpr int kRtCtrl = 1024;                          // barriers (512 B) and the two bias vectors (512 B)
+constexpr int kRtSmem = kRtCtrl + kRtWBytes + kRtHBytes + 2 * kRtXBytes + kRtStages * kRtABytes;
 static_assert(kRtSmem <= kSmemMax, "rdb_tail shared memory");
-static_assert(kRtStages % 2 == 0 && kRtChunks % 2 == 0, "slot ownership by parity");
-
-static_assert(kRtWBytes % 1024 == 0 && kRtHBytes % 1024 == 0, "operand alignment");
+static_assert((kRtCtrl + kRtWBytes + kRtHBytes) % 128 == 0 && kRtABytes % 128 == 0, "TMA destinations must be 128-byte aligned");
 
 struct alignas(64) RdbTailParams {
   CUtensorMap tmap0, tmap1;             // x planes, growth planes
@@ -63,745 +58,184 @@ struct alignas(64) RdbTailParams {
   __half* out; int out_planes, out_plane0;
   const __half* res; int res_planes, res_plane0;
   int reverse;                          // walk the tiles last-to-first (zigzag L2 reuse across launches)
-  int polite;                           // producers / epilogue warps sleep between barrier polls
-  int debug; long long* dbg;            // BIN_B200_DEBUG=8: block 0 records clock64 at role milestones (tools only)
 };
-// timeline layout (bin_debug_timeline): [role][iter][4]; role 0 = producer (k 0,1 per stage) and epilogue B (k 2,3 per tile),
-// role 1 = MMA warp 1 (per item it owns: before / after the data wait, after the turn wait, after the issue), role 2 = epilogue A
-__device__ __forceinline__ void rt_rec(const RdbTailParams& p, int role, uint32_t iter, int k) {
-#ifdef BIN_B200_TOOLS       // the product library carries no timeline hooks
-  if ((p.debug & 8) && blockIdx.x == 0 && iter < 1024) p.dbg[role * 4096 + iter * 4 + k] = clock64();
-#endif
-}
 
 struct RtCtrl {
   uint64_t full[kRtStages], empty[kRtStages];
   uint64_t wfull[kRtChunks + 1];
-  uint64_t conv_full[2], conv_empty[2];
-  uint64_t lff_full[3], lff_empty[3];
-  uint64_t h_full[2], h_empty[2];
-  uint32_t tmem_base;
-  volatile uint32_t issued;       // stage items issued so far (hand-off between the two MMA warps)
-  volatile uint32_t issued2[2];   // QUADT: items issued so far per tile stream (hand-off between the stream's two MMA warps)
 };
 static_assert(sizeof(RtCtrl) <= 512, "ctrl block");
 
-__device__ __forceinline__ uint32_t rt_pack_h2(float a, float b) {
+__device__ __forceinline__ uint32_t pack_h2_rt(float a, float b) {
   __half2 h = __floats2half2_rn(a, b);
   return *reinterpret_cast<uint32_t*>(&h);
 }
-__device__ __forceinline__ float2 rt_unpack_h2(uint32_t u) {
+__device__ __forceinline__ float2 unpack_h2_rt(uint32_t u) {
   __half2 h = *reinterpret_cast<__half2*>(&u);
   return __half22float2(h);
 }
 
-// The LFF's centre tap reads the A tile at the x-unshifted start (row offset 32, 512-byte aligned) like the x-stacked
-// conv taps, so its accumulator row p holds output pixel p-1: the g3 tile is stored one row down and epilogue B takes
-// its values from lane+1.  (Shifting the descriptor start by one 16-byte row instead -- no shuffles, but every 8-row
-// core matrix of that operand then straddles two 128-byte shared-memory lines -- measured 1 % slower.)
-//
-// STREAMS: even and odd tiles of a CTA form two independent instruction streams (producer + MMA warp + two ring slots +
-// one conv accumulator each) that share the tensor pipe, the LFF accumulators and the epilogue warps; nothing orders
-// one stream against the other, so one stream's barrier polls and its wait for the g3 tile are covered by the other's
-// MMAs.  !STREAMS: the two MMA warps alternate the items of ONE tile stream through a hand-off counter.
-// QUADT (448 threads, STREAMS only): each tile stream gets TWO MMA warps that alternate the stream's 8-MMA items (warp
-// (Y, P) owns ring slot Y + 2 P and the items of parity P; strict item order through issued2[Y]; the warp of the last
-// item also issues the tile's tail step).  A single warp per stream serialises barrier wait -> data wait -> issue, and
-// a lone issuer sustains only one MMA per ~80 cycles; with two warps per stream one issues while the other already
-// waits for the next slot.  Per-accumulator MMA order is unchanged -> bit-identical results.
-template <bool STREAMS, bool QUADT = false>
-__global__ void __launch_bounds__(QUADT ? 448 : 384, 1) rdb_tail_kernel(const __grid_constant__ RdbTailParams p) {
-  static_assert(!QUADT || STREAMS, "QUADT refines the two-stream scheme");
+__global__ void __launch_bounds__(384, 1) rdb_tail_kernel(const __grid_constant__ RdbTailParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
   RtCtrl* ctrl = reinterpret_cast<RtCtrl*>(smem);
   float* sb_conv = reinterpret_cast<float*>(smem + 512);           // 32 floats
   float* sb_lff = sb_conv + 32;                                    // 96 floats
   uint8_t* res_w = smem + kRtCtrl;
   uint8_t* htile = res_w + kRtWBytes;
-  uint8_t* stage0 = htile + 2 * kRtHBytes;
+  uint8_t* stage0 = htile + kRtHBytes;                            // TMA destinations: 128-byte aligned
+  float* xbuf0 = reinterpret_cast<float*>(stage0 + kRtStages * kRtABytes);
 
-  const int warp = threadIdx.x >> 5;
+  const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);
   const int lane = threadIdx.x & 31;
-
-  if (threadIdx.x == 0) {
-    tma_prefetch_desc(&p.tmap0);
-    tma_prefetch_desc(&p.tmap1);
-    for (int i = 0; i < kRtStages; ++i) { mbar_init(&ctrl->full[i], 1); mbar_init(&ctrl->empty[i], 1); }
-    for (int i = 0; i <= kRtChunks; ++i) mbar_init(&ctrl->wfull[i], 1);
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&ctrl->conv_full[i], (STREAMS && !QUADT) ? 1 : 2);   // tcgen05.commit of the stream's warp / of each MMA warp
-      mbar_init(&ctrl->conv_empty[i], 4);      // the four epilogue-A warps, one arrival per warp (128 threads arriving on
-      mbar_init(&ctrl->h_full[i], 4);          // one mbarrier serialise in the shared-memory atomic unit)
-      mbar_init(&ctrl->h_empty[i], 1);
-    }
-    for (int i = 0; i < 3; ++i) {
-      mbar_init(&ctrl->lff_full[i], QUADT ? 2 : 1);   // QUADT: a commit only tracks the committing thread's MMAs -> both warps commit
-      mbar_init(&ctrl->lff_empty[i], 4);       // the four epilogue-B warps, one arrival per warp
-    }
-    ctrl->issued = 0;
-    ctrl->issued2[0] = ctrl->issued2[1] = 0;
-    fence_barrier_init();
-  }
-  if (threadIdx.x < 32) sb_conv[threadIdx.x] = p.b_conv[threadIdx.x];
-  else if (threadIdx.x < 128) sb_lff[threadIdx.x - 32] = p.b_lff[threadIdx.x - 32];
-  if (warp == 2) {
-    tmem_alloc(&ctrl->tmem_base, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = ctrl->tmem_base;
-
-  if ((warp == 0 || (STREAMS && warp == 2)) && lane == 0) {
-    // ========================================================== TMA producer(s)
-    const uint32_t Y = warp >> 1;
-    if (Y == 0) {
-      for (int c = 0; c < kRtChunks; ++c) {
-        mbar_expect_tx(&ctrl->wfull[c], kRtWChunk);
-        bulk_load_1d(res_w + c * kRtWChunk, p.w_conv + (size_t)c * 3 * kRtSlab, 3 * kRtSlab, &ctrl->wfull[c]);
-        bulk_load_1d(res_w + c * kRtWChunk + 3 * kRtSlab, p.w_lff + (size_t)c * kRtSlab, kRtSlab, &ctrl->wfull[c]);
-      }
-      mbar_expect_tx(&ctrl->wfull[kRtChunks], kRtSlab);
-      bulk_load_1d(res_w + kRtChunks * kRtWChunk, p.w_lff + (size_t)kRtChunks * kRtSlab, kRtSlab, &ctrl->wfull[kRtChunks]);
-    }
-    // STREAMS: stream Y loads tiles Y, Y+2, ... into ring slots Y and Y+2; else one producer fills slots 0..3 in turn
-    uint32_t k = 0;
-    for (uint32_t tl = STREAMS ? Y : 0; (int)(blockIdx.x + tl * gridDim.x) < p.ntiles; tl += STREAMS ? 2 : 1) {
-      int t = blockIdx.x + tl * gridDim.x;
-      if (p.reverse) t = p.ntiles - 1 - t;
-      const int txi = t % p.tiles_x; t /= p.tiles_x;
-      const int tyi = t % p.tiles_y;
-      const int b = p.b0 + t / p.tiles_y;
-      const int x0 = txi * kRtTW - 1, y0 = p.y0 + tyi * kRtTH - 1;
-      for (int c = 0; c < kRtChunks; ++c, ++k) {
-        const uint32_t slot = STREAMS ? Y + 2 * (k & 1) : k % kRtStages;
-        const uint32_t par = STREAMS ? (k >> 1) & 1 : (k / kRtStages) & 1;
-        if (Y == 0) rt_rec(p, 0, k, 0);
-        if (p.polite) mbar_wait_polite(&ctrl->empty[slot], par ^ 1, 200);
-        else mbar_wait(&ctrl->empty[slot], par ^ 1);
-        if (Y == 0) rt_rec(p, 0, k, 1);
-        mbar_expect_tx(&ctrl->full[slot], kRtABytes);
-        const bool seg1 = c >= 3;
-        tma_load_4d(stage0 + (size_t)slot * kRtABytes, seg1 ? (const void*)&p.tmap1 : (const void*)&p.tmap0,
-                    &ctrl->full[slot], x0 * 8, y0, seg1 ? p.plane0_1 + (c - 3) * kKPL : p.plane0_0 + c * kKPL, b);
-      }
-    }
-  } else if (warp == 1 || warp == 3 || (QUADT && warp >= 12)) {
-    // ========================================================== MMA issuers (warp converged, one elected lane)
-    // Measured on B200: an mbarrier poll costs 200-350 cycles even when the phase is complete and the tcgen05 queue is
-    // shallow, so a warp that polls between its 8-MMA items idles the tensor pipe.  Two warps alternate items: stage
-    // item c of a tile belongs to warp c & 1 (6 items per tile, 4 ring slots: a warp always meets the same two slots
-    // and waits only on those), so one warp's barrier poll and descriptor setup overlap the other's issue phase; a
-    // shared-memory counter hands the pipe over in strict item order (deterministic accumulation order).  The
-    // accumulators are zeroed by item 0, so warp A alone waits for them to be free.  The tail of the previous tile
-    // targets an accumulator nobody else touches: warp B issues it after its last item, outside the ordered sequence.
-    // (Tried and slower, see DESIGN.md: one issuing warp fed by a "scout" warp that does all the polling; 16-MMA items;
-    // a 5-slot ring.)
-    const uint32_t Y = (QUADT && warp >= 12) ? (uint32_t)(warp - 12) : (uint32_t)(warp >> 1);   // QUADT: warps 1, 12 -> stream 0; 3, 13 -> stream 1
-    const uint32_t P = (QUADT && warp >= 12) ? 1u : 0u;                            // QUADT: item parity this warp issues
-    constexpr uint32_t idesc = umma_idesc_f16(128, kRtN);
-    constexpr uint32_t D_HI = (128u >> 4) | (1u << 14);                // SBO = 128 B, descriptor version 1
-    constexpr uint32_t A_LBO = ((uint32_t)kRtAPlane >> 4) << 16;
-    constexpr uint32_t B_LBO = ((uint32_t)(kRtN * 16) >> 4) << 16;
-    constexpr uint32_t H_LBO = ((uint32_t)kRtHPlane >> 4) << 16;
-    uint32_t sit = 0, s = 0, ph = 0, tl = 0, dit = 0;
-    auto wait_turn = [&](uint32_t item) {
-      uint32_t spins = 0;
-      while (ctrl->issued < item) {
-        if (++spins > (1u << 26)) {
-          if (lane == 0) printf("bin_b200: rdb_tail hand-off watchdog (block %d item %u)\n", blockIdx.x, item);
-          __trap();
-        }
-      }
-      tc_fence_after();
-    };
-    auto pass_turn = [&](uint32_t item) {
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) ctrl->issued = item + 1;
-    };
-    // tail of local tile pt (warp B): LFF accumulator += g3 tile * Wl[6]
-    auto tail_item = [&](uint32_t pt) {
-      const uint32_t hb = pt & 1, plb = pt % 3;
-      const uint32_t a_lo = ((smem_u32(htile + hb * kRtHBytes) >> 4) & 0x3FFFu) | H_LBO;
-      const uint32_t b_lo = ((smem_u32(res_w + kRtChunks * kRtWChunk) >> 4) & 0x3FFFu) | B_LBO;
-      const uint32_t d = tmem_base + kRtLffCol0 + plb * kRtN;
-      mbar_wait(&ctrl->h_full[hb], (pt >> 1) & 1);
-      if (pt < 2) mbar_wait(&ctrl->wfull[kRtChunks], 0);              // first tail of either MMA warp
-      tc_fence_after();
-      if (elect_one()) {
-#pragma unroll
-        for (int jj = 0; jj < kKC / 16; ++jj) {
-          const uint64_t ad = ((uint64_t)D_HI << 32) | (a_lo + jj * 2 * (kRtHPlane >> 4));
-          const uint64_t bd = ((uint64_t)D_HI << 32) | (b_lo + jj * 2 * kRtN);
-          umma_f16_ss(d, ad, bd, idesc, 1u);
-        }
-        umma_commit(&ctrl->lff_full[plb]);
-        umma_commit(&ctrl->h_empty[hb]);
-      }
-      __syncwarp();
-    };
-    const uint32_t stage_lo = ((smem_u32(stage0) >> 4) & 0x3FFFu) | A_LBO;
-    const uint32_t w_lo = ((smem_u32(res_w) >> 4) & 0x3FFFu) | B_LBO;
-    // one stage item: 3 x 2 conv MMAs + 2 LFF MMAs on ring slot `slot`, chunk c
-    auto issue_item = [&](uint32_t slot, int c, uint32_t d_conv, uint32_t d_lff, bool last, uint32_t as) {
-      const uint32_t a_lo = stage_lo + slot * (kRtABytes >> 4);
-      const uint32_t b_lo = w_lo + c * (kRtWChunk >> 4);
-      const uint32_t first = (c == 0) ? 0u : 1u;
-      if (elect_one()) {
-        // same order per accumulator as conv_igemm.cu (ky outer, k16 step inner): fused and layer-by-layer results
-        // are bit-identical
-#pragma unroll
-        for (int ky = 0; ky < 3; ++ky) {                               // conv: A shifted by ky rows, B = slab ky
-#pragma unroll
-          for (int jj = 0; jj < kKC / 16; ++jj) {
-            const uint64_t ad = ((uint64_t)D_HI << 32) | (a_lo + jj * 2 * (kRtAPlane >> 4) + ky * kTWH);
-            const uint64_t bd = ((uint64_t)D_HI << 32) | (b_lo + jj * 2 * kRtN + ky * (kRtSlab >> 4));
-            umma_f16_ss(d_conv, ad, bd, idesc, (jj == 0 && ky == 0) ? first : 1u);
-          }
-          if (ky == 1) {                                               // LFF: centre row, x-unshifted start, B = slab 3
-#pragma unroll
-            for (int jj = 0; jj < kKC / 16; ++jj) {
-              const uint64_t ad = ((uint64_t)D_HI << 32) | (a_lo + jj * 2 * (kRtAPlane >> 4) + kTWH);
-              const uint64_t bd = ((uint64_t)D_HI << 32) | (b_lo + jj * 2 * kRtN + 3 * (kRtSlab >> 4));
-              umma_f16_ss(d_lff, ad, bd, idesc, jj == 0 ? first : 1u);
-            }
-          }
-        }
-        umma_commit(&ctrl->empty[slot]);                               // frees the smem slot once these MMAs retire
-        if (last) umma_commit(&ctrl->conv_full[as]);
-      }
-      __syncwarp();
-    };
-    if constexpr (STREAMS && QUADT) {
-      uint32_t k = 0, n = 0;
-      for (uint32_t tl2 = Y; (int)(blockIdx.x + tl2 * gridDim.x) < p.ntiles; tl2 += 2, ++n) {
-        const uint32_t lb = tl2 % 3;
-        if (P == 0) {
-          // the warp of item 0 zeroes both accumulators: the rotating LFF accumulator was released three tiles ago, and
-          // conv[Y] is free once epilogue A has read the stream's previous tile (= its g3 tile is written: h_full)
-          mbar_wait(&ctrl->lff_empty[lb], ((tl2 / 3) & 1) ^ 1);
-          if (n > 0) mbar_wait(&ctrl->h_full[Y], (n - 1) & 1);
-        }
-        const uint32_t d_conv = tmem_base + Y * kRtN;
-        const uint32_t d_lff = tmem_base + kRtLffCol0 + lb * kRtN;
-        for (int c = 0; c < kRtChunks; ++c, ++k) {
-          if ((uint32_t)(c & 1) != P) continue;                        // 6 items per tile: item parity = chunk parity
-          const uint32_t slot = Y + 2 * P;                             // this warp's own ring slot
-          if (warp == 1 && lane == 0) rt_rec(p, 1, k >> 1, 0);
-          mbar_wait(&ctrl->full[slot], (k >> 1) & 1);
-          if (n == 0) mbar_wait(&ctrl->wfull[c], 0);
-          if (warp == 1 && lane == 0) rt_rec(p, 1, k >> 1, 1);
-          while (ctrl->issued2[Y] < k) __nanosleep(20);                // item k-1 of this stream has been issued
-          tc_fence_after();
-          if (warp == 1 && lane == 0) rt_rec(p, 1, k >> 1, 2);
-          issue_item(slot, c, d_conv, d_lff, c == kRtChunks - 1, Y);
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) ctrl->issued2[Y] = k + 1;
-          if (warp == 1 && lane == 0) rt_rec(p, 1, k >> 1, 3);
-        }
-        if (P == 0) {                                                  // this warp's share of the tile's MMAs (items 0, 2, 4)
-          if (elect_one()) {
-            umma_commit(&ctrl->conv_full[Y]);
-            umma_commit(&ctrl->lff_full[lb]);
-          }
-          __syncwarp();
-        }
-        if (P == 1) tail_item(tl2);                                    // waits for this tile's g3, then 2 MMAs (+ its commits)
-      }
-    } else if constexpr (STREAMS) {
-      uint32_t k = 0, n = 0;
-      for (uint32_t tl2 = Y; (int)(blockIdx.x + tl2 * gridDim.x) < p.ntiles; tl2 += 2, ++n) {
-        const uint32_t lb = tl2 % 3;
-        // conv[Y] is free: this warp waited for the g3 tile of its previous tile, which epilogue A writes after it
-        // has read the accumulator.  The rotating LFF accumulator was released three tiles ago.
-        mbar_wait(&ctrl->lff_empty[lb], ((tl2 / 3) & 1) ^ 1);
-        const uint32_t d_conv = tmem_base + Y * kRtN;
-        const uint32_t d_lff = tmem_base + kRtLffCol0 + lb * kRtN;
-        for (int c = 0; c < kRtChunks; ++c, ++k) {
-          const uint32_t slot = Y + 2 * (k & 1);
-          if (Y == 0 && lane == 0) rt_rec(p, 1, k, 0);
-          mbar_wait(&ctrl->full[slot], (k >> 1) & 1);
-          if (n == 0) mbar_wait(&ctrl->wfull[c], 0);
-          tc_fence_after();
-          if (Y == 0 && lane == 0) rt_rec(p, 1, k, 1);
-          issue_item(slot, c, d_conv, d_lff, c == kRtChunks - 1, Y);
-          if (Y == 0 && lane == 0) rt_rec(p, 1, k, 3);
-        }
-        tail_item(tl2);                                                // waits for this tile's g3, then 2 MMAs
-      }
-    } else
-    for (int tile = blockIdx.x; tile < p.ntiles; tile += gridDim.x, ++tl) {
-      const uint32_t as = tl & 1, lb = tl % 3;
-      if (Y == 0) {
-        mbar_wait(&ctrl->conv_empty[as], ((tl >> 1) & 1) ^ 1);
-        mbar_wait(&ctrl->lff_empty[lb], ((tl / 3) & 1) ^ 1);
-      }
-      const uint32_t d_conv = tmem_base + as * kRtN;
-      const uint32_t d_lff = tmem_base + kRtLffCol0 + lb * kRtN;
-      for (int c = 0; c < kRtChunks; ++c, ++sit) {
-        if ((uint32_t)(c & 1) == Y) {
-          const uint32_t a_lo = stage_lo + s * (kRtABytes >> 4);
-          const uint32_t b_lo = w_lo + c * (kRtWChunk >> 4);
-          const uint32_t first = (c == 0) ? 0u : 1u;
-          if (Y == 0 && lane == 0) rt_rec(p, 1, dit, 0);
-          mbar_wait(&ctrl->full[s], ph);
-          if (Y == 0 && lane == 0) rt_rec(p, 1, dit, 1);
-          if (tl == 0) mbar_wait(&ctrl->wfull[c], 0);
-          wait_turn(sit);
-          if (Y == 0 && lane == 0) rt_rec(p, 1, dit, 2);
-          if (elect_one()) {
-            // same order per accumulator as conv_igemm.cu (ky outer, k16 step inner): fused and layer-by-layer results
-            // are bit-identical
-#pragma unroll
-            for (int ky = 0; ky < 3; ++ky) {                           // conv: A shifted by ky rows, B = slab ky
-#pragma unroll
-              for (int jj = 0; jj < kKC / 16; ++jj) {
-                const uint64_t ad = ((uint64_t)D_HI << 32) | (a_lo + jj * 2 * (kRtAPlane >> 4) + ky * kTWH);
-                const uint64_t bd = ((uint64_t)D_HI << 32) | (b_lo + jj * 2 * kRtN + ky * (kRtSlab >> 4));
-                umma_f16_ss(d_conv, ad, bd, idesc, (jj == 0 && ky == 0) ? first : 1u);
-              }
-              if (ky == 1) {                                           // LFF: centre tap (ky = 1, kx = 1), B = slab 3
-#pragma unroll
-                for (int jj = 0; jj < kKC / 16; ++jj) {
-                  const uint64_t ad = ((uint64_t)D_HI << 32) | (a_lo + jj * 2 * (kRtAPlane >> 4) + kTWH + 0);
-                  const uint64_t bd = ((uint64_t)D_HI << 32) | (b_lo + jj * 2 * kRtN + 3 * (kRtSlab >> 4));
-                  umma_f16_ss(d_lff, ad, bd, idesc, jj == 0 ? first : 1u);
-                }
-              }
-            }
-            umma_commit(&ctrl->empty[s]);                              // frees the smem stage once these MMAs retire
-          }
-          __syncwarp();
-          pass_turn(sit);
-          if (Y == 0 && lane == 0) rt_rec(p, 1, dit, 3);
-          ++dit;
-        }
-        if (++s == kRtStages) { s = 0; ph ^= 1; }
-      }
-      if (elect_one()) umma_commit(&ctrl->conv_full[as]);              // this warp's share of the tile's conv MMAs
-      __syncwarp();
-      if (Y == 1 && tl > 0) tail_item(tl - 1);
-    }
-    if (!STREAMS && Y == 1 && tl > 0) tail_item(tl - 1);
-  } else if (warp >= 4 && warp < 8) {
-    // ========================================================== epilogue A: conv accumulator -> g3 tile (smem)
-    const int q = warp & 3;
-    uint32_t tl = 0;
-    for (int tile = blockIdx.x; tile < p.ntiles; tile += gridDim.x, ++tl) {
-      const uint32_t as = tl & 1, uph = (tl >> 1) & 1;
-      if (warp == 4 && lane == 0) rt_rec(p, 2, tl, 0);
-      mbar_wait(&ctrl->conv_full[as], uph);
-      if (warp == 4 && lane == 0) rt_rec(p, 2, tl, 1);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + as * kRtN;
-      uint32_t v[96];
-#pragma unroll
-      for (int j = 0; j < 6; ++j) tmem_ld16(taddr + 16 * j, *reinterpret_cast<uint32_t(*)[16]>(&v[16 * j]));
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&ctrl->conv_empty[as]);               // accumulator is in registers: release it now
-      // out[p] = D[p][kx=0] + D[p+1][kx=1] + D[p+2][kx=2]  (p+1, p+2 are lanes +1, +2: one warp = one tile row)
-      uint4 o[4];
-      uint32_t* ow = reinterpret_cast<uint32_t*>(o);
-#pragma unroll
-      for (int i = 0; i < 32; i += 2) {
-        float f[2];
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const float b1 = __shfl_down_sync(0xffffffffu, __uint_as_float(v[32 + i + e]), 1);
-          const float b2 = __shfl_down_sync(0xffffffffu, __uint_as_float(v[64 + i + e]), 2);
-          f[e] = fmaxf(((__uint_as_float(v[i + e]) + b1) + b2) + sb_conv[i + e], 0.f);
-        }
-        ow[i >> 1] = rt_pack_h2(f[0], f[1]);
-      }
-      if (warp == 4 && lane == 0) rt_rec(p, 2, tl, 2);
-      mbar_wait(&ctrl->h_empty[as], uph ^ 1);                          // tail of tile tl-2 has consumed this buffer
-      uint8_t* h = htile + as * kRtHBytes + (q * 32 + lane + 1) * 16;
-      if (lane < 31) {
-#pragma unroll
-        for (int k = 0; k < 4; ++k) *reinterpret_cast<uint4*>(h + k * kRtHPlane) = o[k];
-      }
-      fence_proxy_async();                                             // generic-proxy stores -> visible to tcgen05.mma
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&ctrl->h_full[as]);
-      if (warp == 4 && lane == 0) rt_rec(p, 2, tl, 3);
-    }
-  } else if (warp >= 8 && warp < 12) {
-    // ========================================================== epilogue B: LFF accumulator + bias + x -> x'
-    const int q = warp & 3;
-    uint32_t tl = 0;
-    for (int tile = blockIdx.x; tile < p.ntiles; tile += gridDim.x, ++tl) {
-      int t = p.reverse ? p.ntiles - 1 - tile : tile;
-      const int txi = t % p.tiles_x; t /= p.tiles_x;
-      const int tyi = t % p.tiles_y;
-      const int b = p.b0 + t / p.tiles_y;
-      const int y = p.y0 + tyi * kRtTH + q, x = txi * kRtTW + lane;
-      const bool valid = (lane < kRtTW) && (y < p.y0 + p.ny) && (x < p.W);
-      const uint32_t lb = tl % 3;
-      uint4 rbuf[12];                                                  // residual x (RDN.py:165), fetched before the wait
-#pragma unroll
-      for (int k = 0; k < 12; ++k) {
-        const size_t off = ((((size_t)b * p.res_planes + p.res_plane0 + k) * p.H + y) * p.W + x) * 8;
-        rbuf[k] = valid ? *reinterpret_cast<const uint4*>(p.res + off) : make_uint4(0, 0, 0, 0);
-      }
-      if (warp == 8 && lane == 0) rt_rec(p, 0, tl, 2);
-      if (p.polite) mbar_wait_polite(&ctrl->lff_full[lb], (tl / 3) & 1, 40);
-      else mbar_wait(&ctrl->lff_full[lb], (tl / 3) & 1);
-      if (warp == 8 && lane == 0) rt_rec(p, 0, tl, 3);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + kRtLffCol0 + lb * kRtN;
-#pragma unroll
-      for (int g0 = 0; g0 < kRtN; g0 += 48) {
-        uint32_t v[48];
-#pragma unroll
-        for (int j = 0; j < 3; ++j) tmem_ld16(taddr + g0 + 16 * j, *reinterpret_cast<uint32_t(*)[16]>(&v[16 * j]));
-        tmem_ld_wait();
-        if (g0 == 48) {                                                // all 96 columns are in registers
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&ctrl->lff_empty[lb]);
-        }
-#pragma unroll
-        for (int j = 0; j < 48; ++j) v[j] = __shfl_down_sync(0xffffffffu, v[j], 1);   // accumulator row p holds pixel p-1
-        if (valid) {
-#pragma unroll
-          for (int k = 0; k < 6; ++k) {
-            const uint4 r = rbuf[g0 / 8 + k];
-            const uint32_t rr[4] = {r.x, r.y, r.z, r.w};
-            uint32_t ow[4];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const float2 g = rt_unpack_h2(rr[i]);
-              const int n = g0 + 8 * k + 2 * i;
-              ow[i] = rt_pack_h2((__uint_as_float(v[8 * k + 2 * i]) + sb_lff[n]) + g.x,
-                                 (__uint_as_float(v[8 * k + 2 * i + 1]) + sb_lff[n + 1]) + g.y);
-            }
-            const size_t off = ((((size_t)b * p.out_planes + p.out_plane0 + g0 / 8 + k) * p.H + y) * p.W + x) * 8;
-            *reinterpret_cast<uint4*>(p.out + off) = make_uint4(ow[0], ow[1], ow[2], ow[3]);
-          }
-        }
-      }
-    }
-  }
-
-  // ------------------------------------------------------------ teardown
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
-  }
-}
-
-// ====================================================================================================================
-// CTA-pair version (tcgen05.mma.cta_group::2): the same computation on a (2,1,1) cluster.
-//
-// Why: the single-CTA kernel keeps 150 KB of weights resident, which leaves a 4 x 12 KB activation ring -- 48 KB in
-// flight per SM cannot cover the loaded HBM latency (DESIGN.md 4c: MMA warps wait 300-1200 cycles per 8-MMA item).
-// A CTA pair shares B: each CTA holds 48 of the 96 B rows of every slab (75 KB), runs its OWN 128-pixel tile (A) and
-// its own accumulators / epilogues, and ONE 256 x 96 x 16 MMA issued by the leader feeds both.  That frees room for a
-// 10 x 12 KB ring per CTA (120 KB in flight) and cuts the per-SM operand fetch from 7 KB to 5.5 KB per MMA.
-//
-// Barrier plan (r = cluster rank, leader = rank 0; only the leader's two MMA warps issue):
-//   full[slot]    leader's barrier, 1 arrival (leader's producer, expect_tx 2 x 12 KB); both producers' TMA loads credit it
-//                 (cp.async.bulk.tensor...cta_group::2 with the leader's barrier address from mapa)
-//   empty[slot], conv_full, lff_full, h_empty   one tcgen05.commit...multicast::cluster (mask 0b11) signals the barrier
-//                 at the same offset in BOTH CTAs -> producers and epilogues only ever wait on CTA-local barriers
-//   h_full, lff_empty   leader's barriers counting 8 arrivals: one per epilogue warp of each CTA
-//                 (mbarrier.arrive.release.cluster on the mapa'd address; the MMA warps wait with acquire.cluster)
-//   wready        leader's barrier, 1 arrival from the peer once ITS weight halves have landed
-// Tile pair q = cluster + j * nclusters; CTA r owns tile 2q + r (a cluster with an odd tile count runs a dummy last
-// tile in the peer: valid loads, stores suppressed).  Streams, accumulator rotation and the per-accumulator MMA order
-// are those of rdb_tail_kernel<true>, so the result is bit-identical to it and to the layer-by-layer kernels.
-constexpr int kRpHalf = kRtN / 2;                        // B rows per CTA
-constexpr int kRpSlab = kKPL * kRpHalf * 16;             // [4 planes][48 rows][16 B] = 3 072
-constexpr int kRpPlane = kRpHalf * 16;                   // 768
-constexpr int kRpWChunk = 4 * kRpSlab;                   // conv ky = 0,1,2 + LFF slab halves of a chunk
-constexpr int kRpWBytes = kRtChunks * kRpWChunk + kRpSlab;
-constexpr int kRpR = 5;                                  // ring slots per stream
-constexpr int kRpStages = 2 * kRpR;
-constexpr int kRpSmem = kRtCtrl + kRpWBytes + 2 * kRtHBytes + kRpStages * kRtABytes;
-static_assert(kRpSmem <= kSmemMax, "rdb_tail pair shared memory");
-static_assert(kRpWBytes % 1024 == 0, "operand alignment");
-
-struct RpCtrl {
-  uint64_t full[kRpStages], empty[kRpStages];
-  uint64_t wfull[kRtChunks + 1];
-  uint64_t wready;
-  uint64_t conv_full[2];
-  uint64_t lff_full[3], lff_empty[3];
-  uint64_t h_full[2], h_empty[2];
-  uint32_t tmem_base;
-};
-static_assert(sizeof(RpCtrl) <= 512, "ctrl block");
-
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(384, 1) rdb_tail_pair_kernel(const __grid_constant__ RdbTailParams p) {
-  extern __shared__ __align__(1024) uint8_t smem[];
-  RpCtrl* ctrl = reinterpret_cast<RpCtrl*>(smem);
-  float* sb_conv = reinterpret_cast<float*>(smem + 512);           // 32 floats
-  float* sb_lff = sb_conv + 32;                                    // 96 floats
-  uint8_t* res_w = smem + kRtCtrl;
-  uint8_t* htile = res_w + kRpWBytes;
-  uint8_t* stage0 = htile + 2 * kRtHBytes;
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const uint32_t cluster = blockIdx.x >> 1, nclusters = gridDim.x >> 1;
-  const int npt = (p.ntiles + 1) >> 1;                             // tile pairs
-
-  if (threadIdx.x == 0) {
-    tma_prefetch_desc(&p.tmap0);
-    tma_prefetch_desc(&p.tmap1);
-    for (int i = 0; i < kRpStages; ++i) { mbar_init(&ctrl->full[i], 1); mbar_init(&ctrl->empty[i], 1); }
-    for (int i = 0; i <= kRtChunks; ++i) mbar_init(&ctrl->wfull[i], 1);
-    mbar_init(&ctrl->wready, 1);
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&ctrl->conv_full[i], 1);
-      mbar_init(&ctrl->h_full[i], 8);          // epilogue-A warps of both CTAs, one arrival per warp (used in the leader)
-      mbar_init(&ctrl->h_empty[i], 1);
-    }
-    for (int i = 0; i < 3; ++i) {
-      mbar_init(&ctrl->lff_full[i], 1);
-      mbar_init(&ctrl->lff_empty[i], 8);       // epilogue-B warps of both CTAs, one arrival per warp (used in the leader)
-    }
-    fence_barrier_init();
-  }
-  if (threadIdx.x < 32) sb_conv[threadIdx.x] = p.b_conv[threadIdx.x];
-  else if (threadIdx.x < 128) sb_lff[threadIdx.x - 32] = p.b_lff[threadIdx.x - 32];
-  if (warp == 2) {
-    tmem_alloc_pair(&ctrl->tmem_base, 512);
-    tmem_relinquish_pair();
-  }
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();                                              // both CTAs' barriers are initialised
-  tc_fence_after();
-  const uint32_t tmem_base = ctrl->tmem_base;
-
-  // tile of this CTA in pair q (the peer of an odd tail re-runs the last tile with its stores suppressed)
-  auto tile_of = [&](int q, int& txi, int& tyi, int& b, bool& live) {
-    int t = 2 * q + (int)rank;
-    live = t < p.ntiles;
-    if (!live) t = p.ntiles - 1;
-    if (p.reverse) t = p.ntiles - 1 - t;
+  auto tile_of = [&](int tq, int& txi, int& tyi, int& b) {
+    int t = p.reverse ? p.ntiles - 1 - tq : tq;
     txi = t % p.tiles_x; t /= p.tiles_x;
     tyi = t % p.tiles_y;
     b = p.b0 + t / p.tiles_y;
   };
 
-  if ((warp == 0 || warp == 2) && lane == 0) {
-    // ========================================================== TMA producers (both CTAs; stream Y = warp >> 1)
-    const uint32_t Y = warp >> 1;
-    if (Y == 0) {
-      // this CTA's half (rows 48r .. 48r+47) of every B slab: 768 contiguous bytes per 8-channel plane
-      for (int c = 0; c <= kRtChunks; ++c) {
-        const int nslab = c < kRtChunks ? 4 : 1;
-        mbar_expect_tx(&ctrl->wfull[c], nslab * kRpSlab);
-        for (int sl = 0; sl < nslab; ++sl) {
-          const uint8_t* src = (c < kRtChunks && sl < 3) ? p.w_conv + (size_t)(c * 3 + sl) * kRtSlab
-                                                         : p.w_lff + (size_t)c * kRtSlab;
-          uint8_t* dst = res_w + c * kRpWChunk + sl * kRpSlab;
-          for (int pl = 0; pl < kKPL; ++pl)
-            bulk_load_1d(dst + pl * kRpPlane, src + pl * (kRtN * 16) + rank * kRpPlane, kRpPlane, &ctrl->wfull[c]);
-        }
-      }
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&p.tmap0);
+    tma_prefetch_desc(&p.tmap1);
+    for (int i = 0; i < kRtStages; ++i) { mbar_init(&ctrl->full[i], 1); mbar_init(&ctrl->empty[i], 8); }
+    for (int i = 0; i <= kRtChunks; ++i) mbar_init(&ctrl->wfull[i], 1);
+    fence_barrier_init();
+  }
+  if (threadIdx.x < 32) sb_conv[threadIdx.x] = p.b_conv[threadIdx.x];
+  else if (threadIdx.x < 128) sb_lff[threadIdx.x - 32] = p.b_lff[threadIdx.x - 32];
+  __syncthreads();
+
+  if (warp == 0) {
+    if (lane != 0) return;
+    // ========================================================== TMA producer
+    for (int c = 0; c < kRtChunks; ++c) {
+      mbar_expect_tx(&ctrl->wfull[c], kRtWChunk);
+      bulk_load_1d(res_w + c * kRtWChunk, p.w_conv + (size_t)c * 3 * kRtSlab, 3 * kRtSlab, &ctrl->wfull[c]);
+      bulk_load_1d(res_w + c * kRtWChunk + 3 * kRtSlab, p.w_lff + (size_t)c * kRtSlab, kRtSlab, &ctrl->wfull[c]);
     }
-    const uint32_t full0 = mapa_u32(smem_u32(&ctrl->full[0]), 0);  // the LEADER's full barriers
-    uint32_t k = 0;
-    for (int j = (int)Y; (int)(cluster + j * nclusters) < npt; j += 2) {
-      int txi, tyi, b; bool live;
-      tile_of((int)(cluster + j * nclusters), txi, tyi, b, live);
+    mbar_expect_tx(&ctrl->wfull[kRtChunks], kRtSlab);
+    bulk_load_1d(res_w + kRtChunks * kRtWChunk, p.w_lff + (size_t)kRtChunks * kRtSlab, kRtSlab, &ctrl->wfull[kRtChunks]);
+    uint32_t s = 0, ph = 0;
+    for (int tq = blockIdx.x; tq < p.ntiles; tq += gridDim.x) {
+      int txi, tyi, b;
+      tile_of(tq, txi, tyi, b);
       const int x0 = txi * kRtTW - 1, y0 = p.y0 + tyi * kRtTH - 1;
-      for (int c = 0; c < kRtChunks; ++c, ++k) {
-        const uint32_t slot = Y * kRpR + k % kRpR;
-        const uint32_t par = (k / kRpR) & 1;
-        mbar_wait(&ctrl->empty[slot], par ^ 1);
-        if (rank == 0) mbar_expect_tx(&ctrl->full[slot], 2 * kRtABytes);
+      for (int c = 0; c < kRtChunks; ++c) {
+        mbar_wait(&ctrl->empty[s], ph ^ 1);
+        mbar_expect_tx(&ctrl->full[s], kRtABytes);
         const bool seg1 = c >= 3;
-        tma_load_4d_pair(stage0 + (size_t)slot * kRtABytes, seg1 ? (const void*)&p.tmap1 : (const void*)&p.tmap0,
-                         full0 + slot * 8, x0 * 8, y0, seg1 ? p.plane0_1 + (c - 3) * kKPL : p.plane0_0 + c * kKPL, b);
+        tma_load_4d(stage0 + (size_t)s * kRtABytes, seg1 ? (const void*)&p.tmap1 : (const void*)&p.tmap0, &ctrl->full[s],
+                    x0 * 8, y0, seg1 ? p.plane0_1 + (c - 3) * kKPL : p.plane0_0 + c * kKPL, b);
+        if (++s == kRtStages) { s = 0; ph ^= 1; }
       }
     }
-  } else if (warp == 1 && rank == 1) {
-    // ========================================================== peer: tell the leader when this CTA's B halves have landed
-    for (int c = 0; c <= kRtChunks; ++c) mbar_wait(&ctrl->wfull[c], 0);
-    if (lane == 0) mbar_arrive_cluster(mapa_u32(smem_u32(&ctrl->wready), 0));
-  } else if ((warp == 1 || warp == 3) && rank == 0) {
-    // ========================================================== MMA issuers (leader only; warp converged, one elected lane)
-    const uint32_t Y = warp >> 1;
-    constexpr uint32_t idesc = umma_idesc_f16(256, kRtN);
-    constexpr uint32_t D_HI = (128u >> 4) | (1u << 14);                // SBO = 128 B, descriptor version 1
-    constexpr uint32_t A_LBO = ((uint32_t)kRtAPlane >> 4) << 16;
-    constexpr uint32_t B_LBO = ((uint32_t)kRpPlane >> 4) << 16;
-    constexpr uint32_t H_LBO = ((uint32_t)kRtHPlane >> 4) << 16;
-    const uint32_t stage_lo = ((smem_u32(stage0) >> 4) & 0x3FFFu) | A_LBO;
-    const uint32_t w_lo = ((smem_u32(res_w) >> 4) & 0x3FFFu) | B_LBO;
-    uint32_t k = 0, n = 0;
-    for (int j = (int)Y; (int)(cluster + j * nclusters) < npt; j += 2, ++n) {
-      const uint32_t lb = (uint32_t)j % 3;
-      // conv[Y] is free in BOTH CTAs: this warp waited for the g3 tiles of its previous tile pair (8 warp arrivals), which
-      // the epilogue-A warps write after reading the accumulator.  The rotating LFF accumulator was released three
-      // tile pairs ago (8 arrivals as well).
-      mbar_wait_cluster(&ctrl->lff_empty[lb], (((uint32_t)j / 3) & 1) ^ 1);
-      const uint32_t d_conv = tmem_base + Y * kRtN;
-      const uint32_t d_lff = tmem_base + kRtLffCol0 + lb * kRtN;
-      for (int c = 0; c < kRtChunks; ++c, ++k) {
-        const uint32_t slot = Y * kRpR + k % kRpR;
-        mbar_wait(&ctrl->full[slot], (k / kRpR) & 1);
-        if (n == 0) {
-          mbar_wait(&ctrl->wfull[c], 0);
-          if (c == 0) mbar_wait_cluster(&ctrl->wready, 0);
-        }
-        tc_fence_after();
-        const uint32_t a_lo = stage_lo + slot * (kRtABytes >> 4);
-        const uint32_t b_lo = w_lo + c * (kRpWChunk >> 4);
-        const uint32_t first = (c == 0) ? 0u : 1u;
-        if (elect_one()) {
+    return;
+  }
+  if (warp < 4) return;
+
+  // ============================================================ consumer warpgroups
+  const int m = (warp - 4) >> 2;                 // tile rows [64 m, 64 m + 64)
+  const int wq = warp & 3;
+  const int k4 = lane & 3;
+  float* xbuf = xbuf0 + m * (kRtXBytes / 4);
+  float acc_c[kRtN / 2], acc_l[kRtN / 2];        // fragment: [4 i + 2 h + e] = row 16 wq + lane/4 + 8 h, column 8 i + 2 k4 + e
+  uint32_t s = 0, ph = 0;
+  for (int tq = blockIdx.x; tq < p.ntiles; tq += gridDim.x) {
+    int prev = -1;
+    for (int c = 0; c < kRtChunks; ++c) {
+      mbar_wait(&ctrl->full[s], ph);
+      if (tq == (int)blockIdx.x) mbar_wait(&ctrl->wfull[c], 0);
+      const uint32_t a_base = smem_u32(stage0 + (size_t)s * kRtABytes) + m * 64 * 16;
+      const uint32_t b_base = smem_u32(res_w + c * kRtWChunk);
+      const uint32_t first = c == 0 ? 0u : 1u;
+      wgmma_fence();
 #pragma unroll
-          for (int ky = 0; ky < 3; ++ky) {                               // conv: A shifted by ky rows, B = slab ky
+      for (int ky = 0; ky < 3; ++ky) {                               // conv: A shifted by ky rows, B = slab ky
 #pragma unroll
-            for (int jj = 0; jj < kKC / 16; ++jj) {
-              const uint64_t ad = ((uint64_t)D_HI << 32) | (a_lo + jj * 2 * (kRtAPlane >> 4) + ky * kTWH);
-              const uint64_t bd = ((uint64_t)D_HI << 32) | (b_lo + jj * 2 * kRpHalf + ky * (kRpSlab >> 4));
-              umma_f16_ss_pair(d_conv, ad, bd, idesc, (jj == 0 && ky == 0) ? first : 1u);
-            }
-            if (ky == 1) {                                               // LFF: centre row, x-unshifted start, B = slab 3
-#pragma unroll
-              for (int jj = 0; jj < kKC / 16; ++jj) {
-                const uint64_t ad = ((uint64_t)D_HI << 32) | (a_lo + jj * 2 * (kRtAPlane >> 4) + kTWH);
-                const uint64_t bd = ((uint64_t)D_HI << 32) | (b_lo + jj * 2 * kRpHalf + 3 * (kRpSlab >> 4));
-                umma_f16_ss_pair(d_lff, ad, bd, idesc, jj == 0 ? first : 1u);
-              }
-            }
-          }
-          umma_commit_pair(&ctrl->empty[slot]);                          // frees the slot in both CTAs
-          if (c == kRtChunks - 1) umma_commit_pair(&ctrl->conv_full[Y]);
-        }
-        __syncwarp();
+        for (int jj = 0; jj < kKC / 16; ++jj)
+          Wgmma<kRtN>::mma(acc_c, gmma_desc(a_base + ky * kTWH * 16 + jj * 2 * kRtAPlane, kRtAPlane, 128),
+                           gmma_desc(b_base + ky * kRtSlab + jj * 2 * kRtN * 16, kRtN * 16, 128),
+                           (jj == 0 && ky == 0) ? first : 1u);
       }
-      // tail of this tile pair: LFF accumulator += g3 tile * Wl[6]
-      {
-        const uint32_t hb = Y;
-        const uint32_t a_lo = ((smem_u32(htile + hb * kRtHBytes) >> 4) & 0x3FFFu) | H_LBO;
-        const uint32_t b_lo = w_lo + kRtChunks * (kRpWChunk >> 4);
-        mbar_wait_cluster(&ctrl->h_full[hb], ((uint32_t)j >> 1) & 1);
-        if (n == 0) mbar_wait(&ctrl->wfull[kRtChunks], 0);
-        tc_fence_after();
-        if (elect_one()) {
 #pragma unroll
-          for (int jj = 0; jj < kKC / 16; ++jj) {
-            const uint64_t ad = ((uint64_t)D_HI << 32) | (a_lo + jj * 2 * (kRtHPlane >> 4));
-            const uint64_t bd = ((uint64_t)D_HI << 32) | (b_lo + jj * 2 * kRpHalf);
-            umma_f16_ss_pair(d_lff, ad, bd, idesc, 1u);
-          }
-          umma_commit_pair(&ctrl->lff_full[lb]);
-          umma_commit_pair(&ctrl->h_empty[hb]);
-        }
-        __syncwarp();
-      }
+      for (int jj = 0; jj < kKC / 16; ++jj)                          // LFF: centre row, +1 pixel, B = slab 3
+        Wgmma<kRtN>::mma(acc_l, gmma_desc(a_base + (kTWH + 1) * 16 + jj * 2 * kRtAPlane, kRtAPlane, 128),
+                         gmma_desc(b_base + 3 * kRtSlab + jj * 2 * kRtN * 16, kRtN * 16, 128), jj == 0 ? first : 1u);
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (prev >= 0 && lane == 0) mbar_arrive(&ctrl->empty[prev]);
+      prev = (int)s;
+      if (++s == kRtStages) { s = 0; ph ^= 1; }
     }
-  } else if (warp >= 4 && warp < 8) {
-    // ========================================================== epilogue A: conv accumulator -> g3 tile (smem), both CTAs
-    const int q = warp & 3;
-    const uint32_t hfull0 = mapa_u32(smem_u32(&ctrl->h_full[0]), 0);
-    for (int j = 0; (int)(cluster + j * nclusters) < npt; ++j) {
-      const uint32_t as = (uint32_t)j & 1, uph = ((uint32_t)j >> 1) & 1;
-      mbar_wait(&ctrl->conv_full[as], uph);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + as * kRtN;
-      uint32_t v[96];
+    wgmma_wait<0>();
+    acc_fence(acc_c);
+    acc_fence(acc_l);
+    if (lane == 0) mbar_arrive(&ctrl->empty[prev]);
+
+    // ---------------------------------------------------------- g3 = ReLU(D0[p] + D1[p+1] + D2[p+2] + b) -> smem
 #pragma unroll
-      for (int i = 0; i < 6; ++i) tmem_ld16(taddr + 16 * i, *reinterpret_cast<uint32_t(*)[16]>(&v[16 * i]));
-      tmem_ld_wait();
-      tc_fence_before();
-      uint4 o[4];
-      uint32_t* ow = reinterpret_cast<uint32_t*>(o);
+    for (int i = 4; i < 12; ++i)
 #pragma unroll
-      for (int i = 0; i < 32; i += 2) {
+      for (int h = 0; h < 2; ++h) {
+        const int r = wq * 16 + (lane >> 2) + 8 * h;
+        *reinterpret_cast<float2*>(xbuf + r * kRtXPitch + 8 * i - 32 + 2 * k4) =
+            make_float2(acc_c[4 * i + 2 * h], acc_c[4 * i + 2 * h + 1]);
+      }
+    wg_sync(1 + m);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int r = wq * 16 + (lane >> 2) + 8 * h;
+      uint8_t* hrow = htile + (m * 64 + r) * 16 + 4 * k4;
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
         float f[2];
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
-          const float b1 = __shfl_down_sync(0xffffffffu, __uint_as_float(v[32 + i + e]), 1);
-          const float b2 = __shfl_down_sync(0xffffffffu, __uint_as_float(v[64 + i + e]), 2);
-          f[e] = fmaxf(((__uint_as_float(v[i + e]) + b1) + b2) + sb_conv[i + e], 0.f);
+          const int col = 8 * i + 2 * k4 + e;
+          f[e] = fmaxf(((acc_c[4 * i + 2 * h + e] + xbuf[(r + 1) * kRtXPitch + col]) + xbuf[(r + 2) * kRtXPitch + 32 + col]) +
+                           sb_conv[col], 0.f);
         }
-        ow[i >> 1] = rt_pack_h2(f[0], f[1]);
-      }
-      mbar_wait(&ctrl->h_empty[as], uph ^ 1);                          // tail of tile pair j-2 has consumed this buffer
-      uint8_t* h = htile + as * kRtHBytes + (q * 32 + lane + 1) * 16;
-      if (lane < 31) {
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk) *reinterpret_cast<uint4*>(h + kk * kRtHPlane) = o[kk];
-      }
-      fence_proxy_async();                                             // generic-proxy stores -> visible to tcgen05.mma
-      __syncwarp();
-      if (lane == 0) mbar_arrive_cluster(hfull0 + as * 8);             // the accumulator has been read, the g3 tile is written
-    }
-  } else if (warp >= 8) {
-    // ========================================================== epilogue B: LFF accumulator + bias + x -> x', both CTAs
-    const int q = warp & 3;
-    const uint32_t lffempty0 = mapa_u32(smem_u32(&ctrl->lff_empty[0]), 0);
-    for (int j = 0; (int)(cluster + j * nclusters) < npt; ++j) {
-      int txi, tyi, b; bool live;
-      tile_of((int)(cluster + j * nclusters), txi, tyi, b, live);
-      const int y = p.y0 + tyi * kRtTH + q, x = txi * kRtTW + lane;
-      const bool valid = live && (lane < kRtTW) && (y < p.y0 + p.ny) && (x < p.W);
-      const uint32_t lb = (uint32_t)j % 3;
-      uint4 rbuf[12];                                                  // residual x (RDN.py:165), fetched before the wait
-#pragma unroll
-      for (int kk = 0; kk < 12; ++kk) {
-        const size_t off = ((((size_t)b * p.res_planes + p.res_plane0 + kk) * p.H + y) * p.W + x) * 8;
-        rbuf[kk] = valid ? *reinterpret_cast<const uint4*>(p.res + off) : make_uint4(0, 0, 0, 0);
-      }
-      mbar_wait(&ctrl->lff_full[lb], ((uint32_t)j / 3) & 1);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + kRtLffCol0 + lb * kRtN;
-#pragma unroll
-      for (int g0 = 0; g0 < kRtN; g0 += 48) {
-        uint32_t v[48];
-#pragma unroll
-        for (int i = 0; i < 3; ++i) tmem_ld16(taddr + g0 + 16 * i, *reinterpret_cast<uint32_t(*)[16]>(&v[16 * i]));
-        tmem_ld_wait();
-        if (g0 == 48) {                                                // all 96 columns are in registers
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive_cluster(lffempty0 + lb * 8);
-        }
-#pragma unroll
-        for (int i = 0; i < 48; ++i) v[i] = __shfl_down_sync(0xffffffffu, v[i], 1);   // accumulator row p holds pixel p-1
-        if (valid) {
-#pragma unroll
-          for (int kk = 0; kk < 6; ++kk) {
-            const uint4 rr4 = rbuf[g0 / 8 + kk];
-            const uint32_t rr[4] = {rr4.x, rr4.y, rr4.z, rr4.w};
-            uint32_t ow[4];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const float2 g = rt_unpack_h2(rr[i]);
-              const int nn = g0 + 8 * kk + 2 * i;
-              ow[i] = rt_pack_h2((__uint_as_float(v[8 * kk + 2 * i]) + sb_lff[nn]) + g.x,
-                                 (__uint_as_float(v[8 * kk + 2 * i + 1]) + sb_lff[nn + 1]) + g.y);
-            }
-            const size_t off = ((((size_t)b * p.out_planes + p.out_plane0 + g0 / 8 + kk) * p.H + y) * p.W + x) * 8;
-            *reinterpret_cast<uint4*>(p.out + off) = make_uint4(ow[0], ow[1], ow[2], ow[3]);
-          }
-        }
+        *reinterpret_cast<uint32_t*>(hrow + i * kRtHPlane) = pack_h2_rt(f[0], f[1]);
       }
     }
-  }
+    fence_proxy_async();                                             // generic-proxy stores -> visible to wgmma
+    wg_sync(1 + m);
 
-  // ------------------------------------------------------------ teardown (the leader's MMAs touch the peer's smem / TMEM)
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc_pair(tmem_base, 512);
+    // ---------------------------------------------------------- LFF += g3 * Wl[6]
+    if (tq == (int)blockIdx.x) mbar_wait(&ctrl->wfull[kRtChunks], 0);
+    wgmma_fence();
+    {
+      const uint32_t h_base = smem_u32(htile) + m * 64 * 16;
+      const uint32_t b_base = smem_u32(res_w + kRtChunks * kRtWChunk);
+#pragma unroll
+      for (int jj = 0; jj < kKC / 16; ++jj)
+        Wgmma<kRtN>::mma(acc_l, gmma_desc(h_base + jj * 2 * kRtHPlane, kRtHPlane, 128),
+                         gmma_desc(b_base + jj * 2 * kRtN * 16, kRtN * 16, 128), 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    acc_fence(acc_l);
+
+    // ---------------------------------------------------------- x' = LFF + b + x
+    int txi, tyi, b;
+    tile_of(tq, txi, tyi, b);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int L = m * 64 + wq * 16 + (lane >> 2) + 8 * h;
+      const int y = p.y0 + tyi * kRtTH + (L >> 5), x = txi * kRtTW + (L & 31);
+      if ((L & 31) < kRtTW && y < p.y0 + p.ny && x < p.W) {
+#pragma unroll
+        for (int i = 0; i < kRtN / 8; ++i) {
+          const int n = 8 * i + 2 * k4;
+          const size_t roff = ((((size_t)b * p.res_planes + p.res_plane0 + i) * p.H + y) * p.W + x) * 8 + 2 * k4;
+          const float2 g = unpack_h2_rt(*reinterpret_cast<const uint32_t*>(p.res + roff));
+          const size_t off = ((((size_t)b * p.out_planes + p.out_plane0 + i) * p.H + y) * p.W + x) * 8 + 2 * k4;
+          *reinterpret_cast<uint32_t*>(p.out + off) =
+              pack_h2_rt((acc_l[4 * i + 2 * h] + sb_lff[n]) + g.x, (acc_l[4 * i + 2 * h + 1] + sb_lff[n + 1]) + g.y);
+        }
+      }
+    }
+    wg_sync(1 + m);                                                  // htile / xbuf are rewritten by the next tile
   }
 }
 
@@ -835,39 +269,11 @@ int launch_rdb_tail(const bin_act_t& x, int x_plane0, const bin_act_t& g, int g_
   p.out = reinterpret_cast<__half*>(out.ptr); p.out_planes = out.planes; p.out_plane0 = out_plane0;
   p.res = reinterpret_cast<const __half*>(x.ptr); p.res_planes = x.planes; p.res_plane0 = x_plane0;
   p.reverse = reverse ? 1 : 0;
-  p.polite = options().polite ? 1 : 0;
-  const bool streams = options().tail_streams;
-  p.debug = options().debug;
-#ifdef BIN_B200_TOOLS
-  if (p.debug & 8) {
-    if (!g_dbg) { BIN_CUDA_OK(cudaMalloc(&g_dbg, 3 * 4096 * sizeof(long long))); }
-    BIN_CUDA_OK(cudaMemsetAsync(g_dbg, 0, 3 * 4096 * sizeof(long long), s));
-    p.dbg = g_dbg;
-  }
-#endif
-  if (options().pair) {
-    static std::atomic<unsigned long long> opted_pair{0};   // per device
-    BIN_TRY(ensure_dynamic_smem(rdb_tail_pair_kernel, kRpSmem, opted_pair));
-    const int npt = (p.ntiles + 1) / 2, maxc = num_sms() / 2;
-    const int nclusters = npt < maxc ? npt : maxc;
-    rdb_tail_pair_kernel<<<2 * nclusters, 384, kRpSmem, s>>>(p);
-    BIN_CUDA_OK(cudaGetLastError());
-    return BIN_OK;
-  }
-  if (streams && options().tailq) {
-    static std::atomic<unsigned long long> opted_q{0};   // per device
-    BIN_TRY(ensure_dynamic_smem(rdb_tail_kernel<true, true>, kRtSmem, opted_q));
-    const int sq = num_sms();
-    rdb_tail_kernel<true, true><<<p.ntiles < sq ? p.ntiles : sq, 448, kRtSmem, s>>>(p);
-    BIN_CUDA_OK(cudaGetLastError());
-    return BIN_OK;
-  }
-  auto kern = streams ? rdb_tail_kernel<true> : rdb_tail_kernel<false>;
-  static std::atomic<unsigned long long> opted_streams{0}, opted_handoff{0};   // per device
-  BIN_TRY(ensure_dynamic_smem(kern, kRtSmem, streams ? opted_streams : opted_handoff));
+  static std::atomic<unsigned long long> opted{0};   // per device
+  BIN_TRY(ensure_dynamic_smem(rdb_tail_kernel, kRtSmem, opted));
   const int sms = num_sms();
   const int grid = p.ntiles < sms ? p.ntiles : sms;
-  kern<<<grid, 384, kRtSmem, s>>>(p);
+  rdb_tail_kernel<<<grid, 384, kRtSmem, s>>>(p);
   BIN_CUDA_OK(cudaGetLastError());
   return BIN_OK;
 }

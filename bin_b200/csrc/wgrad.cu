@@ -1,24 +1,25 @@
-// bin_b200 -- weight-gradient GEMM for sm_100a (tcgen05.mma with MN-major operands).
+// bin_b200 -- weight-gradient GEMM for sm_90a (wgmma with MN-major operands).
 //
 // dW[co][ci][ky][kx] += (1/scale) * sum_{b,y,x} dY[b,co,y,x] * X[b,ci,y+ky-pad,x+kx-pad]
 // (the wgrad of every nn.Conv2d of RDN.py; autograd of bin_model.optimize_parameters, bin_model.py:130-141).
 //
 // GEMM view: D_tap[ci][co] = sum_pixels X_tap[pixel][ci] * dY[pixel][co], i.e. M = Cin tile (128),
 // N = Cout, K = pixels.  P8 tiles in shared memory ([plane][row][px][8 ch]) are exactly the canonical
-// MN-major / no-swizzle UMMA layout with K = pixel index: 8 channels contiguous (16 B), 8 consecutive
+// MN-major / no-swizzle wgmma layout with K = pixel index: 8 channels contiguous (16 B), 8 consecutive
 // pixels 16 B apart (one 128-byte core matrix), next 8-pixel group +128 B (LBO), next 8-channel plane
 // +plane stride (SBO).  A tap is again a 16-byte start-address shift of the X halo tile.
-// One MMA = 128(ci) x N(co) x 16 pixels (one 16-pixel tile row); a CTA keeps one fp32 accumulator per
-// tap in TMEM (taps x Cout <= 512 columns; wider layers run several tap groups), walks a slice of the
-// pixel tiles, and finally adds its partial sums into dW with fp32 atomics.
+// One wgmma = 64(ci) x N(co) x 16 pixels (one 16-pixel tile row); each of the two consumer warpgroups keeps one
+// register accumulator per tap for its 64 input channels (taps x N <= 256 columns; wider layers run several tap
+// groups), walks a slice of the pixel tiles, and finally writes its partial sums into a per-CTA slab.
 // SX mode (the Cout=32 RDB convs): dW[ky][kx] = sum_p' dY[p'-(kx-1)] X[p'+(ky-1)*row], so the three kx taps
 // share the SAME X operand when dY is shifted instead: the dY tile is loaded three times at x offsets
-// +1, 0, -1 into consecutive plane groups and becomes one N = 96 operand (8 rows x 3 ky = 24 MMAs per tile
-// instead of 72 N=32 MMAs; the N=32 MMA is operand-fetch bound at 40 % of the math rate).
+// +1, 0, -1 into consecutive plane groups and becomes one N = 96 operand (8 rows x 3 ky = 24 wgmma per tile
+// instead of 72 with N = 32).
 #include <stdio.h>
 
 #include "common.cuh"
 #include "internal.h"
+#include "wgmma.cuh"
 
 namespace binb {
 
@@ -41,26 +42,24 @@ struct alignas(64) WgradParams {
 };
 
 struct WgCtrl {
-  uint64_t full[4], empty[4], done;
-  uint32_t tmem_base;
+  uint64_t full[4], empty[4];
 };
 
-__device__ __forceinline__ uint64_t umma_desc_mnmajor_noswz(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr >> 4) & 0x3FFFu);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;    // stride between 8-element K groups (8 pixels)
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;    // stride between 8-element MN groups (channel planes)
-  d |= (uint64_t)1 << 46;
-  return d;
-}
+template <int N>
+struct WgCfg {
+  static constexpr int TAPS = 256 / N;               // accumulators per thread: TAPS x N / 2 <= 128 registers
+};
 
-__global__ void __launch_bounds__(256, 1) wgrad_kernel(const __grid_constant__ WgradParams p) {
+// Roles (384 threads, 1 CTA/SM): warp 0 lane 0 = TMA producer; warpgroup 1+m = input channels [64 m, 64 m + 64).
+template <int N>
+__global__ void __launch_bounds__(384, 1) wgrad_kernel(const __grid_constant__ WgradParams p) {
+  constexpr int TAPS = WgCfg<N>::TAPS;
   extern __shared__ __align__(1024) uint8_t smem[];
   WgCtrl* ctrl = reinterpret_cast<WgCtrl*>(smem);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
   const int x_plane_bytes = p.rows * p.pw * 16;
   const int x_bytes = 16 * x_plane_bytes;                       // 16 planes = 128 input channels
-  const int y_planes = p.n / 8;                                 // SX: 3 shifted copies of the 4 dY planes
+  const int y_planes = N / 8;                                   // SX: 3 shifted copies of the 4 dY planes
   const int y_plane_bytes = kWgTH * kWgTW * 16;
   const int y_bytes = y_planes * y_plane_bytes;
   const int stage_bytes = x_bytes + y_bytes;
@@ -71,17 +70,13 @@ __global__ void __launch_bounds__(256, 1) wgrad_kernel(const __grid_constant__ W
     tma_prefetch_desc(&p.xmap0);
     if (p.x1_planes > 0) tma_prefetch_desc(&p.xmap1);
     tma_prefetch_desc(&p.ymap);
-    for (int i = 0; i < 4; ++i) { mbar_init(&ctrl->full[i], 1); mbar_init(&ctrl->empty[i], 1); }
-    mbar_init(&ctrl->done, 1);
+    for (int i = 0; i < 4; ++i) { mbar_init(&ctrl->full[i], 1); mbar_init(&ctrl->empty[i], 8); }
     fence_barrier_init();
   }
-  if (warp == 2) { tmem_alloc(&ctrl->tmem_base, 512); tmem_relinquish(); }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = ctrl->tmem_base;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == 0) {
+    if (lane != 0) return;
     // ------------------------------------------------ TMA producer
     uint32_t s = 0, ph = 0;
     for (int tile = blockIdx.x; tile < p.ntiles; tile += gridDim.x) {
@@ -117,61 +112,61 @@ __global__ void __launch_bounds__(256, 1) wgrad_kernel(const __grid_constant__ W
       }
       if (++s == S) { s = 0; ph ^= 1; }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------ MMA issuer: D_tap[ci][co] += X_tap^T * dY
-    const uint32_t idesc = (1u << 4) | (1u << 15) | (1u << 16) | ((uint32_t)(p.n >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-    uint32_t s = 0, ph = 0;
-    bool first = true;
-    for (int tile = blockIdx.x; tile < p.ntiles; tile += gridDim.x) {
-      mbar_wait(&ctrl->full[s], ph);
-      tc_fence_after();
-      const uint32_t xb = smem_u32(stage0 + (size_t)s * stage_bytes);
-      const uint32_t yb = xb + x_bytes;
-      if (elect_one()) {
-        for (int tp = 0; tp < p.ntaps; ++tp) {
-          const int tap = p.tap0 + tp, ky = p.sx ? tp : tap / p.ks, kx = p.sx ? 0 : tap % p.ks;
-          const uint32_t d = tmem_base + tp * p.n;
-          for (int r = 0; r < kWgTH; ++r) {
-            const uint64_t ad = umma_desc_mnmajor_noswz(xb + (uint32_t)((r + ky) * p.pw + kx) * 16, 128, x_plane_bytes);
-            const uint64_t bd = umma_desc_mnmajor_noswz(yb + (uint32_t)(r * kWgTW) * 16, 128, y_plane_bytes);
-            umma_f16_ss(d, ad, bd, idesc, (first && r == 0) ? 0u : 1u);
-          }
-        }
-        umma_commit(&ctrl->empty[s]);
-      }
-      __syncwarp();
-      first = false;
-      if (++s == S) { s = 0; ph ^= 1; }
-    }
-    if (elect_one()) umma_commit(&ctrl->done);
-    __syncwarp();
-  } else if (warp >= 4) {
-    // ------------------------------------------------ flush: TMEM -> this CTA's slab of the partial-sum workspace
-    // (plain 16-byte stores; 36.8 K fp32 atomics per CTA were issue-bound at ~1 lane/clk and took 4x the MMA time;
-    //  wgrad_reduce_kernel sums the slabs afterwards)
-    mbar_wait(&ctrl->done, 0);
-    tc_fence_after();
-    const int q = warp & 3;
-    const int row = q * 32 + lane;                               // accumulator row = input channel within the tile
-    const bool has_tiles = (int)blockIdx.x < p.ntiles;
-    float* slab = p.partial + (size_t)blockIdx.x * p.ntaps * 128 * p.n;
-    for (int tp = 0; tp < p.ntaps; ++tp) {
-      for (int n0 = 0; n0 < p.n; n0 += 16) {
-        uint32_t v[16];
-        tmem_ld16(tmem_base + ((uint32_t)(q * 32) << 16) + tp * p.n + n0, v);
-        tmem_ld_wait();
-        float4* dst = reinterpret_cast<float4*>(slab + ((size_t)tp * 128 + row) * p.n + n0);
+    return;
+  }
+  if (warp < 4) return;
+  // ------------------------------------------------ consumers: D_tap[ci][co] += X_tap^T * dY
+  const int m = (warp - 4) >> 2, wq = warp & 3, k4 = lane & 3;
+  float acc[TAPS][N / 2];
+  uint32_t s = 0, ph = 0;
+  int prev = -1;
+  bool first = true;
+  for (int tile = blockIdx.x; tile < p.ntiles; tile += gridDim.x) {
+    mbar_wait(&ctrl->full[s], ph);
+    const uint32_t xb = smem_u32(stage0 + (size_t)s * stage_bytes) + m * 8 * x_plane_bytes;
+    const uint32_t yb = smem_u32(stage0 + (size_t)s * stage_bytes) + x_bytes;
+    wgmma_fence();
 #pragma unroll
-        for (int i = 0; i < 4; ++i)
-          dst[i] = has_tiles ? make_float4(__uint_as_float(v[4 * i]), __uint_as_float(v[4 * i + 1]), __uint_as_float(v[4 * i + 2]),
-                                           __uint_as_float(v[4 * i + 3]))
-                             : make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int tp = 0; tp < TAPS; ++tp) {
+      if (tp >= p.ntaps) break;
+      const int tap = p.tap0 + tp, ky = p.sx ? tap : tap / p.ks, kx = p.sx ? 0 : tap % p.ks;   // SX: tap = ky
+#pragma unroll
+      for (int r = 0; r < kWgTH; ++r) {
+        const uint64_t ad = gmma_desc(xb + (uint32_t)((r + ky) * p.pw + kx) * 16, 128, x_plane_bytes);
+        const uint64_t bd = gmma_desc(yb + (uint32_t)(r * kWgTW) * 16, 128, y_plane_bytes);
+        Wgmma<N, 1, 1>::mma(acc[tp], ad, bd, (first && r == 0) ? 0u : 1u);
       }
+    }
+    wgmma_commit();
+    if (S > 1) {                         // release the previous stage: this tile's wgmmas overlap the next load
+      wgmma_wait<1>();
+      if (prev >= 0 && lane == 0) mbar_arrive(&ctrl->empty[prev]);
+      prev = (int)s;
+    } else {                             // a one-stage ring (wide Cout x 5x5): the only stage is freed at once, or the
+      wgmma_wait<0>();                   // producer would wait for it while this warpgroup waits for the next load
+      if (lane == 0) mbar_arrive(&ctrl->empty[s]);
+    }
+    first = false;
+    if (++s == S) { s = 0; ph ^= 1; }
+  }
+  wgmma_wait<0>();
+#pragma unroll
+  for (int tp = 0; tp < TAPS; ++tp) acc_fence(acc[tp]);
+  // ------------------------------------------------ flush: this CTA's slab of the partial-sum workspace
+  // (plain stores; wgrad_reduce_kernel sums the slabs afterwards in a fixed order)
+  float* slab = p.partial + (size_t)blockIdx.x * p.ntaps * 128 * N;
+#pragma unroll
+  for (int tp = 0; tp < TAPS; ++tp) {
+    if (tp >= p.ntaps) break;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = m * 64 + wq * 16 + (lane >> 2) + 8 * h;   // accumulator row = input channel within the tile
+#pragma unroll
+      for (int i = 0; i < N / 8; ++i)
+        *reinterpret_cast<float2*>(slab + ((size_t)tp * 128 + row) * N + 8 * i + 2 * k4) =
+            first ? make_float2(0.f, 0.f) : make_float2(acc[tp][4 * i + 2 * h], acc[tp][4 * i + 2 * h + 1]);
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) { tc_fence_after(); tmem_dealloc(tmem_base, 512); }
 }
 
 // dW[co][ci][tap] += (1/scale) * sum over CTAs of partial[cta][tp][ci - ci0][col]   (col = co, or kx*32+co in SX mode)
@@ -203,12 +198,36 @@ __global__ void __launch_bounds__(256) wgrad_reduce_kernel(const float* __restri
     const int col = i % n, row = (i / n) % 128, tp = i / (n * 128);
     const int ci = ci0 + row;
     const int co = sx ? (col & 31) : col;
-    const int tap = sx ? tp * 3 + (col >> 5) : tap0 + tp;
+    const int tap = sx ? (tap0 + tp) * 3 + (col >> 5) : tap0 + tp;
     if (ci < cin && co < cout) dw[((size_t)co * cin + ci) * kk + tap] += acc / scale[0];
   }
 }
 
 int make_p8_tmap_box(CUtensorMap* m, const bin_act_t& t, int box_px, int box_rows, int box_planes);
+
+template <int N>
+static int run_wgrad(WgradParams p, int smem_bytes, int ci_planes, int kk, int ks, cudaStream_t s) {
+  static std::atomic<unsigned long long> smem_opted{0};   // per instantiation, per device
+  BIN_TRY(ensure_dynamic_smem(wgrad_kernel<N>, kSmemMax, smem_opted));
+  const int taps_per_group = WgCfg<N>::TAPS < kk ? WgCfg<N>::TAPS : kk;   // SX: kk = 3, one accumulator per ky
+  const int sms = num_sms();
+  const int grid = p.ntiles < sms ? p.ntiles : sms;
+  if (grid < 1) return BIN_OK;
+  for (int cp = 0; cp < ci_planes; cp += 16) {
+    for (int t0 = 0; t0 < kk; t0 += taps_per_group) {
+      p.ci_tile_plane0 = cp;
+      p.tap0 = t0;
+      p.ntaps = kk - t0 < taps_per_group ? kk - t0 : taps_per_group;
+      wgrad_kernel<N><<<grid, 384, smem_bytes, s>>>(p);
+      BIN_CUDA_OK(cudaGetLastError());
+      const int total = p.ntaps * 128 * N;
+      wgrad_reduce_kernel<<<(total + 63) / 64, 256, 0, s>>>(p.partial, grid, p.ntaps, N, p.sx, t0, cp * 8, p.cout, p.cin,
+                                                           ks * ks, p.scale, p.dw);
+      BIN_CUDA_OK(cudaGetLastError());
+    }
+  }
+  return BIN_OK;
+}
 
 int launch_wgrad_impl(const bin_act_t& x0, int x0_plane0, int x0_planes, const bin_act_t& x1, int x1_plane0, int x1_planes,
                       const bin_act_t& dy, int dy_plane0, int cout, int cin, int ks, const float* scale, float* dw,
@@ -223,6 +242,9 @@ int launch_wgrad_impl(const bin_act_t& x0, int x0_plane0, int x0_planes, const b
   p.pad = ks / 2; p.ks = ks;
   p.sx = (ks == 3 && cout == 32) ? 1 : 0;
   if (p.sx) n = 96;                                   // MMA N = 3 shifted copies of the 32 dY channels
+  // wgmma N of the kernel: the next of 16, 32, 48, 64, 96, 128, 256 (dY planes past Cout are zero-filled by TMA or read
+  // and then dropped by the reduction's co < cout test)
+  n = n <= 64 ? n : n <= 96 ? 96 : n <= 128 ? 128 : 256;
   p.pw = kWgTW + (p.sx ? 0 : 2 * p.pad); p.rows = kWgTH + 2 * p.pad;
   BIN_TRY(make_p8_tmap_box(&p.xmap0, x0, p.pw, p.rows, 4));
   if (x1_planes > 0) BIN_TRY(make_p8_tmap_box(&p.xmap1, x1, p.pw, p.rows, 4));
@@ -239,28 +261,13 @@ int launch_wgrad_impl(const bin_act_t& x0, int x0_plane0, int x0_planes, const b
   if (S < 1) return fail(BIN_ERR_UNSUPPORTED, "wgrad: tile does not fit in shared memory");
   p.nstages = S;
   const int smem_bytes = 1024 + S * (x_bytes + y_bytes);
-  static std::atomic<unsigned long long> smem_opted{0};   // per device
-  BIN_TRY(ensure_dynamic_smem(wgrad_kernel, kSmemMax, smem_opted));
-  const int kk = p.sx ? 3 : ks * ks;                  // SX: one accumulator per ky
-  const int taps_per_group = 512 / n < kk ? 512 / n : kk;
-  const int ci_planes = x0_planes + x1_planes;
-  const int sms = num_sms();
-  int grid = p.ntiles < sms ? p.ntiles : sms;
-  if (grid < 1) return BIN_OK;
-  for (int cp = 0; cp < ci_planes; cp += 16) {
-    for (int t0 = 0; t0 < kk; t0 += taps_per_group) {
-      p.ci_tile_plane0 = cp;
-      p.tap0 = t0;
-      p.ntaps = kk - t0 < taps_per_group ? kk - t0 : taps_per_group;
-      wgrad_kernel<<<grid, 256, smem_bytes, s>>>(p);
-      BIN_CUDA_OK(cudaGetLastError());
-      const int total = p.ntaps * 128 * n;
-      wgrad_reduce_kernel<<<(total + 63) / 64, 256, 0, s>>>(partial_ws, grid, p.ntaps, n, p.sx, t0, cp * 8, cout, cin, ks * ks,
-                                                           scale, dw);
-      BIN_CUDA_OK(cudaGetLastError());
-    }
+  switch (n) {
+#define BIN_WGRAD_N(NN) \
+    case NN: return run_wgrad<NN>(p, smem_bytes, x0_planes + x1_planes, p.sx ? 3 : ks * ks, ks, s);
+    BIN_WGRAD_N(16) BIN_WGRAD_N(32) BIN_WGRAD_N(48) BIN_WGRAD_N(64) BIN_WGRAD_N(96) BIN_WGRAD_N(128) BIN_WGRAD_N(256)
+#undef BIN_WGRAD_N
   }
-  return BIN_OK;
+  return fail(BIN_ERR_UNSUPPORTED, "wgrad: no kernel for this Cout");
 }
 
 }  // namespace binb

@@ -2,7 +2,7 @@
 
 The script slides a window over the 240-fps sharp frames of one video (:99-140): blurry frame w is the float32 mean of
 the `window_size` frames centred on `16 + 8*w`, truncated to uint8 (:117-131).  `blur_average` does every window of a
-clip in one sm_100a launch on uint8 frames already in HBM, bit-exactly.  CUDA only; there is no CPU path."""
+clip in one sm_90a launch on uint8 frames already in HBM, bit-exactly.  CUDA only; there is no CPU path."""
 from __future__ import annotations
 
 import math

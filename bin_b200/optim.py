@@ -4,7 +4,7 @@
 (bin_model.py:97-100) and `optimize_parameters` calls `.step()` after `l_pix.backward()` (:141).  `Adam` below is a
 `torch.optim.Optimizer` with the same constructor, `param_groups` (the reference's schedulers write `group['lr']`,
 lr_scheduler.py / bin_model.py:145) and per-parameter state (`step`, `exp_avg`, `exp_avg_sq` -- state dicts are
-interchangeable with torch.optim.Adam, base_model.save_training_state), whose `step()` is ONE sm_100a launch per
+interchangeable with torch.optim.Adam, base_model.save_training_state), whose `step()` is ONE sm_90a launch per
 parameter group over all tensors (`bin_adam_step`) instead of PyTorch's per-op foreach chain.
 
 CUDA fp32 parameters only; there is no CPU path."""

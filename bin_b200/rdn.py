@@ -1,4 +1,4 @@
-"""Drop-in mirror of the reference's ``models/archs/RDN.py`` (laomao0/BIN) on B200.
+"""Drop-in mirror of the reference's ``models/archs/RDN.py`` (laomao0/BIN) on H100.
 
 Same class names, constructor signatures, forward signatures, 14-tuple return and state_dict
 schema (1 332 keys / 540 unique tensors, SURVEY.md 8b) as the reference file, so that
@@ -7,7 +7,7 @@ schema (1 332 keys / 540 unique tensors, SURVEY.md 8b) as the reference file, so
 keep working unchanged when this module is installed in its place (see INTEGRATION.md).
 
 The nn.Modules here only HOLD the fp32 parameters; no forward does arithmetic in PyTorch.
-Every forward hands device pointers to libbin_b200.so (hand-written sm_100a kernels) through
+Every forward hands device pointers to libbin_b200.so (hand-written sm_90a kernels) through
 the C ABI in include/bin_b200.h and raises if the library or a CUDA device is missing.
 """
 from __future__ import annotations
@@ -39,7 +39,7 @@ def _graphs_enabled() -> bool:
 def _check_frames(frames: Sequence[torch.Tensor]) -> Tuple[int, int, int]:
     f0 = frames[0]
     if not f0.is_cuda:
-        raise BinB200Error("bin_b200 runs on CUDA (sm_100a) only; got a CPU tensor. There is no CPU fallback.")
+        raise BinB200Error("bin_b200 runs on CUDA (sm_90a) only; got a CPU tensor. There is no CPU fallback.")
     B, Cc, H, W = f0.shape
     if Cc != 3 or (H % 2) or (W % 2):
         raise BinB200Error(f"frames must be (B,3,H,W) with even H,W (RDN.py:123-128); got {tuple(f0.shape)}")

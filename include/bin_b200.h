@@ -1,4 +1,4 @@
-/* bin_b200 -- C ABI of the B200-native BIN hot path (libbin_b200.so).
+/* bin_b200 -- C ABI of the Hopper-native (H100, sm_90a) BIN hot path (libbin_b200.so).
  *
  * The reference (laomao0/BIN) has no FFI layer: its boundary for this path is the Python
  * nn.Module contract reached through models/networks.py:9-10 -> models/archs/RDN.py:469-471
@@ -15,7 +15,7 @@
  * Device layouts
  *   frames / outputs : fp32 NCHW, exactly what the reference module takes and returns.
  *   "planar-8" (P8)  : fp16 activations [B][C/8][H][W][8]  (8-channel planes; one pixel of one
- *                      plane = 16 B = one UMMA core-matrix row, so any pixel shift of a smem
+ *                      plane = 16 B = one wgmma core-matrix row, so any pixel shift of a smem
  *                      tile is a 16-byte descriptor offset -> implicit GEMM without im2col).
  *   packed conv W    : fp16 [Cin_pad/32][kh][kw][4][Cout_pad][8]  (K-major B operand, one
  *                      contiguous slab per 32-channel K chunk), + fp32 bias[Cout_pad].
@@ -44,7 +44,7 @@ typedef void* bin_stream_t; /* cudaStream_t */
 
 int bin_abi_version(void);
 const char* bin_last_error(void);
-/* 0 if the current device is sm_100 (B200) and the driver exposes cuTensorMapEncodeTiled. */
+/* 0 if the current device is sm_90 (H100) and the driver exposes cuTensorMapEncodeTiled. */
 int bin_check_device(void);
 
 /* ---- P8 activation tensor view ------------------------------------------------------- */
@@ -77,7 +77,7 @@ size_t bin_packed_weight_bytes(int cout_pad, int cin_pad, int ksize);
 int bin_pack_conv_weight(const float* w_oihw, int cout, int cin, int ksize, int cout_pad, int cin_pad, int variant,
                          void* packed, bin_stream_t s);
 
-/* ---- the implicit-GEMM convolution (tcgen05) ------------------------------------------ */
+/* ---- the implicit-GEMM convolution (wgmma) -------------------------------------------- */
 enum { BIN_EPI_P8 = 0, BIN_EPI_PIXSHUF = 1, BIN_EPI_FINAL = 2 };
 enum { BIN_CONV_DEFAULT = 0, BIN_CONV_PLAIN = 1 };
 /* Precision modes: fp16 storage / fp32 accumulate (<=1e-3 parity), or the split-fp16 "fp32-accurate" mode

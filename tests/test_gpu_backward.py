@@ -1,4 +1,4 @@
-"""Backward parity (BASELINE config 3): gradients from the sm_100a dgrad/wgrad kernels against autograd
+"""Backward parity (BASELINE config 3): gradients from the sm_90a dgrad/wgrad kernels against autograd
 through the fp32 CPU oracle (and the reference's own autograd via tests/golden/window_grad.npz).
 Gradients travel as loss-scaled fp16 -> tolerance 2 % of the tensor's max magnitude."""
 import os
@@ -123,8 +123,18 @@ def test_window_backward_vs_reference_autograd(net, golden_dir):
 @pytest.mark.parametrize("cin,cout,k,split", [(128, 32, 3, 96), (96, 96, 3, None), (224, 96, 1, 96), (36, 96, 5, None),
                                               (96, 256, 3, None), (64, 3, 3, None)])
 def test_single_conv_dgrad_wgrad_exact(cin, cout, k, split):
-    """One conv, no ReLU: dX (same kernel, transposed weights) and dW (MN-major tcgen05 GEMM) against autograd of
+    """One conv, no ReLU: dX (same kernel, transposed weights) and dW (MN-major wgmma GEMM) against autograd of
     F.conv2d on the SAME fp16-rounded operands -> only accumulation-order noise remains (<= 2e-3 of max)."""
+    _single_conv_dgrad_wgrad(cin, cout, k, split, 2, 27, 41)
+
+
+def test_single_conv_wgrad_one_stage_ring():
+    """5x5 with 128 < Cout <= 256 leaves room for only ONE wgrad pipeline stage (N = 256); 2 x 64 x 160 is 160 tiles of
+    8 x 16, more than one per CTA, so the stage must be recycled inside a CTA."""
+    _single_conv_dgrad_wgrad(36, 200, 5, None, 2, 64, 160)
+
+
+def _single_conv_dgrad_wgrad(cin, cout, k, split, B, H, W):
     import ctypes as C
     import torch.nn.functional as F
     from bin_b200 import _lib, ops
@@ -133,7 +143,6 @@ def test_single_conv_dgrad_wgrad_exact(cin, cout, k, split):
     torch.backends.cudnn.allow_tf32 = False          # the fp32 cuDNN reference must not run in TF32
     torch.backends.cuda.matmul.allow_tf32 = False
     dev = "cuda"
-    B, H, W = 2, 27, 41
     x = torch.randn(B, cin, H, W, device=dev).half().float()
     w = (torch.randn(cout, cin, k, k, device=dev) / (cin * k * k) ** 0.5).half().float()
     dy = torch.randn(B, cout, H, W, device=dev).half().float()
@@ -155,7 +164,7 @@ def test_single_conv_dgrad_wgrad_exact(cin, cout, k, split):
     assert (got - gx_ref).abs().max().item() <= 2e-3 * gx_ref.abs().max().item()
     # ---- wgrad
     scale = torch.full((1,), 4.0, device=dev)
-    dys = ops.nchw_to_p8(dy * 4.0, pad_to=16 if cout < 8 else 8)
+    dys = ops.nchw_to_p8(dy * 4.0, pad_to=16)                      # the wgrad reads dY planes up to Cout rounded to 16
     dw = torch.zeros_like(w)
     if split is None:
         x0 = ops.nchw_to_p8(x.detach(), pad_to=32)

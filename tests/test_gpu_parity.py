@@ -1,4 +1,4 @@
-"""Parity of the sm_100a path (through the C ABI / the nn.Module mirror) against
+"""Parity of the sm_90a path (through the C ABI / the nn.Module mirror) against
 (a) the golden fixtures produced by the unmodified reference and (b) the fp32 CPU oracle.
 
 Tolerance (north_star / BASELINE.md §4): fp16 storage + fp32 accumulate -> max-abs <= 1e-3 on the
@@ -293,12 +293,10 @@ def test_fp32_mode_window_vs_oracle(net32, sd):
     assert worst <= TOL_FP32_MODE, worst
 
 
-def test_cta_pair_kernels_bit_identical_to_single_cta():
-    """The cta_group::2 kernels (rdb_tail_pair_kernel, conv_igemm_kernel<...,PAIR>) and the M-split MMA-warp scheme of the
-    conv kernel keep the per-accumulator MMA order of the default kernels: a whole window must hash identically under
-    every combination of BIN_B200_PAIR / BIN_B200_MSPLIT / BIN_B200_QUAD (four MMA warps) / BIN_B200_ZIGZAG (reversed tile
-    order of alternate launches) / BIN_B200_SPREAD / BIN_B200_POLITE; the
-    library reads the switches once per process, hence children.  Shapes: odd tile counts (dummy peer tile), many tiles per cluster."""
+def test_tile_order_and_stage_size_keep_window_bit_identical():
+    """Reversed tile order of alternate RDB launches (BIN_B200_ZIGZAG) and the number of wgmma per pipeline stage
+    (BIN_B200_STAGE_MMAS) do not change the per-accumulator MMA order: a whole window must hash identically under every
+    setting.  The library reads the switches once per process, hence children.  Shapes: partial tiles, many tiles per CTA."""
     import subprocess
     import sys
     code = (
@@ -313,14 +311,9 @@ def test_cta_pair_kernels_bit_identical_to_single_cta():
         "    for o in outs: h.update(o.cpu().numpy().tobytes())\n"
         "print('HASH', h.hexdigest())\n" % ROOT)
     got = {}
-    base = {"BIN_B200_PAIR": "0", "BIN_B200_MSPLIT": "0", "BIN_B200_QUAD": "0", "BIN_B200_ZIGZAG": "0", "BIN_B200_TAILQ": "0",
-            "BIN_B200_SPREAD": "0", "BIN_B200_POLITE": "0"}
-    for tag, over in (("two-warp", {}), ("quad", {"BIN_B200_QUAD": "1"}), ("quad+tailq", {"BIN_B200_QUAD": "1", "BIN_B200_TAILQ": "1"}),
-                      ("tailq", {"BIN_B200_TAILQ": "1"}), ("pair", {"BIN_B200_PAIR": "1"}),
-                      ("msplit", {"BIN_B200_MSPLIT": "1"}), ("pair+msplit", {"BIN_B200_PAIR": "1", "BIN_B200_MSPLIT": "1"}),
-                      ("quad+zigzag", {"BIN_B200_QUAD": "1", "BIN_B200_ZIGZAG": "1"}), ("pair+zigzag", {"BIN_B200_PAIR": "1", "BIN_B200_ZIGZAG": "1"}),
-                      ("quad+tailq+spread+polite", {"BIN_B200_QUAD": "1", "BIN_B200_TAILQ": "1", "BIN_B200_SPREAD": "1", "BIN_B200_POLITE": "1"}),
-                      ("spread+polite", {"BIN_B200_SPREAD": "1", "BIN_B200_POLITE": "1"})):
+    base = {"BIN_B200_ZIGZAG": "0", "BIN_B200_STAGE_MMAS": "12"}
+    for tag, over in (("default", {}), ("zigzag", {"BIN_B200_ZIGZAG": "1"}), ("stage4", {"BIN_B200_STAGE_MMAS": "4"}),
+                      ("stage48+zigzag", {"BIN_B200_STAGE_MMAS": "48", "BIN_B200_ZIGZAG": "1"})):
         env = dict(base, **over)
         r = subprocess.run([sys.executable, "-c", code], env=dict(os.environ, **env), capture_output=True, text=True, timeout=900)
         assert r.returncode == 0, (tag, r.stderr[-2000:])

@@ -72,7 +72,7 @@ def test_library_exports_every_declared_symbol():
         assert hasattr(L, name), f"{name} declared in include/bin_b200.h but not exported"
     assert declared == set(_lib.exported_symbols()), declared ^ set(_lib.exported_symbols())
     assert _lib.lib().bin_abi_version() == _lib.ABI_VERSION == int(re.search(r"#define BIN_ABI_VERSION (\d+)", hdr).group(1))
-    # measurement tooling lives in libbin_b200_tools.so / csrc/tools_abi.h, never in the product library or its header
+    # measurement tooling (microbenchmarks, debug timelines) is never part of the product library or its header
     assert not any(n.startswith(("bin_tools_", "bin_microbench", "bin_debug")) for n in declared)
     assert not hasattr(L, "bin_tools_microbench_mma") and not hasattr(L, "bin_microbench_mma")
 

@@ -1,4 +1,4 @@
-"""compute-sanitizer target: the fused RDB tail kernel (both variants' default = STREAMS) and the x-stacked conv on small
+"""compute-sanitizer target: the fused RDB tail kernel and the x-stacked conv on small
 tensors that still exercise several tiles per CTA (ntiles > #SMs), partial tiles in x and y, and a batch > 1.
 usage: compute-sanitizer --tool {memcheck,racecheck,synccheck} python tools/sanitize_tail.py"""
 import os
