@@ -19,6 +19,7 @@
 #include "common.cuh"
 #include "internal.h"
 #include "wgmma.cuh"
+#include "xstack.cuh"
 
 namespace binb {
 
@@ -42,10 +43,9 @@ struct ConvCfg {
   static constexpr int W_TAP = kKPL * NMMA * 16;         // bytes per tap per chunk
   static constexpr int W_STAGE = TAPS_S * W_TAP;
   static constexpr int W_CHUNK = TAPS_C * W_TAP;
-  // SX: the kx = 1, 2 column groups of a 64-row accumulator block (+2 rows read by the junk columns) go through shared
-  // memory to reach the thread that holds pixel p; pitch padded by 4 words against bank conflicts
-  static constexpr int XPITCH = 2 * NT + 4;
-  static constexpr int XBYTES = SX ? 66 * XPITCH * 4 : 0;   // per consumer warpgroup
+  // SX: xstack_sum exchange buffers, one per warp pair (2 per warpgroup) and 64-row block (2 per accumulator), so the
+  // second block's exchange needs no barrier against the first block's reads
+  static constexpr int XS_BYTES = SX ? kMT * 2 * 2 * kXsFloats<NT> * 4 : 0;
   static_assert(!(SX && ROWSPLIT), "SX is only used for 3x3");
   static_assert(NMMA % 16 == 0 && NMMA <= 256, "invalid wgmma N");
 };
@@ -188,7 +188,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_igemm_kernel(const __grid_co
   const int m = (warp - 4) >> 2;                               // accumulator: tile rows [128 m, 128 m + 128)
   const int wq = warp & 3;                                     // warp within the warpgroup: 16 rows of each 64-row block
   const int k4 = lane & 3;                                     // fragment column pair: columns 8 i + 2 k4, +1
-  float* xbuf = reinterpret_cast<float*>(stage0 + (size_t)S * stage_bytes + m * C::XBYTES);
+  float* xs = reinterpret_cast<float*>(stage0 + (size_t)S * stage_bytes) + (2 * m + (wq >> 1)) * 2 * kXsFloats<NT>;
   float acc[2][NA];
   constexpr float kAcc = X3 ? (1.f / 256.f) : 1.f;            // X3 weights are packed scaled by 2^8
   uint32_t s = 0, ph = 0;
@@ -248,17 +248,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_igemm_kernel(const __grid_co
     const int yend = p.y0 + p.ny;
 #pragma unroll
     for (int mb = 0; mb < 2; ++mb) {
-      if constexpr (SX) {                                      // kx = 1, 2 column groups -> shared memory
-#pragma unroll
-        for (int i = NT / 8; i < C::NMMA / 8; ++i)
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const int r = wq * 16 + (lane >> 2) + 8 * h;
-            *reinterpret_cast<float2*>(xbuf + r * C::XPITCH + 8 * i - NT + 2 * k4) =
-                make_float2(acc[mb][4 * i + 2 * h], acc[mb][4 * i + 2 * h + 1]);
-          }
-        wg_sync(1 + m);
-      }
+      if constexpr (SX) xstack_sum<NT>(acc[mb], xs + mb * kXsFloats<NT>, 3 + 2 * m + (wq >> 1));   // barrier per warp pair
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int r = wq * 16 + (lane >> 2) + 8 * h;           // row within the 64-row block
@@ -266,16 +256,8 @@ __global__ void __launch_bounds__(kThreads, 1) conv_igemm_kernel(const __grid_co
         const int ty = L >> 5, tx = L & 31;
         const int y = p.y0 + tyi * kTH + ty, x = txi * C::TW + tx;
         const bool valid = (tx < C::TW) && (y < yend) && (x < p.W);
-        // value of output channel column 8 i + 2 k4 + e of this pixel (x-stacked: out[p] = D0[p] + D1[p+1] + D2[p+2])
-        auto val = [&](int i, int e) {
-          const float d0 = acc[mb][4 * i + 2 * h + e];
-          if constexpr (SX) {
-            const int col = 8 * i + 2 * k4 + e;
-            return ((d0 + xbuf[(r + 1) * C::XPITCH + col]) + xbuf[(r + 2) * C::XPITCH + NT + col]) * kAcc;
-          } else {
-            return d0 * kAcc;
-          }
-        };
+        // value of output channel column 8 i + 2 k4 + e of this pixel (SX: xstack_sum has added the kx = 1, 2 groups)
+        auto val = [&](int i, int e) { return acc[mb][4 * i + 2 * h + e] * kAcc; };
         if constexpr (EPI == BIN_EPI_P8) {
           if (valid) {
 #pragma unroll
@@ -332,7 +314,6 @@ __global__ void __launch_bounds__(kThreads, 1) conv_igemm_kernel(const __grid_co
           }
         }
       }
-      if constexpr (SX) wg_sync(1 + m);                       // xbuf is rewritten by the next block
     }
   }
 }
@@ -416,7 +397,7 @@ static int launch_inst(const bin_conv_args_t& a, cudaStream_t s, bool reverse) {
   p.ntiles = nb * p.tiles_x * p.tiles_y * p.nh;
   p.relu = a.relu;
   const int nchunks = p.nch0 + p.nch1;
-  const int xbytes = kMT * C::XBYTES;
+  const int xbytes = C::XS_BYTES;
   // keep the whole weight set resident in smem when it leaves room for >= 3 activation stages
   p.resident = (p.nh == 1 && nchunks <= kMaxResidentChunks &&
                 kCtrlBytes + nchunks * C::W_CHUNK + xbytes + 3 * C::A_BYTES + 256 <= kSmemMax) ? 1 : 0;

@@ -8,7 +8,7 @@
 // GEMM view per 128-pixel tile (4 rows x 32-pixel smem pitch, 30 valid columns) and 32-channel chunk c = 0..5:
 //   conv accumulator  (128 x 96, the three kx taps stacked in N as in conv_igemm.cu)  += A(ky) * Wc[c][ky],  ky = 0..2
 //   LFF accumulator   (128 x 96)                                                      += A(centre) * Wl[c]
-// then the conv accumulator's kx column groups are added (through shared memory), bias + ReLU applied, g3 written as a
+// then the conv accumulator's kx column groups are added (xstack_sum), bias + ReLU applied, g3 written as a
 // K-major fp16 operand into shared memory, and ONE more K = 32 step  LFF accumulator += g3 * Wl[6]  finishes x'.
 // The accumulation order per accumulator is that of conv_igemm_kernel (chunk, ky, k16 step), so the fused and the
 // layer-by-layer results are bit-identical.  All weights (6 x 4 slabs + 1 = 150 KB) stay resident in shared memory.
@@ -22,6 +22,7 @@
 #include "common.cuh"
 #include "internal.h"
 #include "wgmma.cuh"
+#include "xstack.cuh"
 
 namespace binb {
 
@@ -37,12 +38,12 @@ constexpr int kRtWChunk = 4 * kRtSlab;                 // conv ky = 0,1,2 + LFF 
 constexpr int kRtWBytes = kRtChunks * kRtWChunk + kRtSlab;   // + the LFF slab of the g3 channels
 constexpr int kRtHPlane = 128 * 16;
 constexpr int kRtHBytes = kKPL * kRtHPlane;            // g3 tile: [4 planes][128 pixels][16 B]
-constexpr int kRtXPitch = 2 * 32 + 4;                  // kx = 1, 2 column groups of 66 rows, padded pitch (floats)
-constexpr int kRtXBytes = 66 * kRtXPitch * 4;          // per warpgroup
-constexpr int kRtStages = 2;
+constexpr int kRtXsBytes = 4 * kXsFloats<32> * 4;      // xstack_sum buffers of the 4 consumer warp pairs
 constexpr int kRtCtrl = 1024;                          // barriers (512 B) and the two bias vectors (512 B)
-constexpr int kRtSmem = kRtCtrl + kRtWBytes + kRtHBytes + 2 * kRtXBytes + kRtStages * kRtABytes;
-static_assert(kRtSmem <= kSmemMax, "rdb_tail shared memory");
+// the activation ring takes all shared memory the resident weights, the g3 tile and the exchange buffers leave
+constexpr int kRtStages = (kSmemMax - kRtCtrl - kRtWBytes - kRtHBytes - kRtXsBytes) / kRtABytes;
+constexpr int kRtSmem = kRtCtrl + kRtWBytes + kRtHBytes + kRtStages * kRtABytes + kRtXsBytes;
+static_assert(kRtStages >= 2 && kRtSmem <= kSmemMax, "rdb_tail shared memory");
 static_assert((kRtCtrl + kRtWBytes + kRtHBytes) % 128 == 0 && kRtABytes % 128 == 0, "TMA destinations must be 128-byte aligned");
 
 struct alignas(64) RdbTailParams {
@@ -83,7 +84,7 @@ __global__ void __launch_bounds__(384, 1) rdb_tail_kernel(const __grid_constant_
   uint8_t* res_w = smem + kRtCtrl;
   uint8_t* htile = res_w + kRtWBytes;
   uint8_t* stage0 = htile + kRtHBytes;                            // TMA destinations: 128-byte aligned
-  float* xbuf0 = reinterpret_cast<float*>(stage0 + kRtStages * kRtABytes);
+  float* xs0 = reinterpret_cast<float*>(stage0 + kRtStages * kRtABytes);
 
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);
   const int lane = threadIdx.x & 31;
@@ -137,7 +138,8 @@ __global__ void __launch_bounds__(384, 1) rdb_tail_kernel(const __grid_constant_
   const int m = (warp - 4) >> 2;                 // tile rows [64 m, 64 m + 64)
   const int wq = warp & 3;
   const int k4 = lane & 3;
-  float* xbuf = xbuf0 + m * (kRtXBytes / 4);
+  float* xs = xs0 + (2 * m + (wq >> 1)) * kXsFloats<32>;
+  const int xs_bar = 3 + 2 * m + (wq >> 1);      // named barrier of the warp pair (1, 2: wg_sync)
   float acc_c[kRtN / 2], acc_l[kRtN / 2];        // fragment: [4 i + 2 h + e] = row 16 wq + lane/4 + 8 h, column 8 i + 2 k4 + e
   uint32_t s = 0, ph = 0;
   for (int tq = blockIdx.x; tq < p.ntiles; tq += gridDim.x) {
@@ -172,16 +174,28 @@ __global__ void __launch_bounds__(384, 1) rdb_tail_kernel(const __grid_constant_
     acc_fence(acc_l);
     if (lane == 0) mbar_arrive(&ctrl->empty[prev]);
 
-    // ---------------------------------------------------------- g3 = ReLU(D0[p] + D1[p+1] + D2[p+2] + b) -> smem
+    // ---------------------------------------------------------- residual x of this thread's pixels
+    // issued before the g3 epilogue so that their latency hides behind it and the g3 LFF wgmma
+    int txi, tyi, b;
+    tile_of(tq, txi, tyi, b);
+    bool valid[2];
+    int y[2], x[2];
+    uint32_t res[2][kRtN / 8];
 #pragma unroll
-    for (int i = 4; i < 12; ++i)
+    for (int h = 0; h < 2; ++h) {
+      const int L = m * 64 + wq * 16 + (lane >> 2) + 8 * h;
+      y[h] = p.y0 + tyi * kRtTH + (L >> 5);
+      x[h] = txi * kRtTW + (L & 31);
+      valid[h] = (L & 31) < kRtTW && y[h] < p.y0 + p.ny && x[h] < p.W;
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int r = wq * 16 + (lane >> 2) + 8 * h;
-        *reinterpret_cast<float2*>(xbuf + r * kRtXPitch + 8 * i - 32 + 2 * k4) =
-            make_float2(acc_c[4 * i + 2 * h], acc_c[4 * i + 2 * h + 1]);
+      for (int i = 0; i < kRtN / 8; ++i) {
+        const size_t roff = ((((size_t)b * p.res_planes + p.res_plane0 + i) * p.H + y[h]) * p.W + x[h]) * 8 + 2 * k4;
+        res[h][i] = valid[h] ? *reinterpret_cast<const uint32_t*>(p.res + roff) : 0u;
       }
-    wg_sync(1 + m);
+    }
+
+    // ---------------------------------------------------------- g3 = ReLU(D0[p] + D1[p+1] + D2[p+2] + b) -> smem
+    xstack_sum<32>(acc_c, xs, xs_bar);
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int r = wq * 16 + (lane >> 2) + 8 * h;
@@ -190,11 +204,7 @@ __global__ void __launch_bounds__(384, 1) rdb_tail_kernel(const __grid_constant_
       for (int i = 0; i < 4; ++i) {
         float f[2];
 #pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int col = 8 * i + 2 * k4 + e;
-          f[e] = fmaxf(((acc_c[4 * i + 2 * h + e] + xbuf[(r + 1) * kRtXPitch + col]) + xbuf[(r + 2) * kRtXPitch + 32 + col]) +
-                           sb_conv[col], 0.f);
-        }
+        for (int e = 0; e < 2; ++e) f[e] = fmaxf(acc_c[4 * i + 2 * h + e] + sb_conv[8 * i + 2 * k4 + e], 0.f);
         *reinterpret_cast<uint32_t*>(hrow + i * kRtHPlane) = pack_h2_rt(f[0], f[1]);
       }
     }
@@ -217,25 +227,20 @@ __global__ void __launch_bounds__(384, 1) rdb_tail_kernel(const __grid_constant_
     acc_fence(acc_l);
 
     // ---------------------------------------------------------- x' = LFF + b + x
-    int txi, tyi, b;
-    tile_of(tq, txi, tyi, b);
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      const int L = m * 64 + wq * 16 + (lane >> 2) + 8 * h;
-      const int y = p.y0 + tyi * kRtTH + (L >> 5), x = txi * kRtTW + (L & 31);
-      if ((L & 31) < kRtTW && y < p.y0 + p.ny && x < p.W) {
+      if (valid[h]) {
 #pragma unroll
         for (int i = 0; i < kRtN / 8; ++i) {
           const int n = 8 * i + 2 * k4;
-          const size_t roff = ((((size_t)b * p.res_planes + p.res_plane0 + i) * p.H + y) * p.W + x) * 8 + 2 * k4;
-          const float2 g = unpack_h2_rt(*reinterpret_cast<const uint32_t*>(p.res + roff));
-          const size_t off = ((((size_t)b * p.out_planes + p.out_plane0 + i) * p.H + y) * p.W + x) * 8 + 2 * k4;
+          const float2 g = unpack_h2_rt(res[h][i]);
+          const size_t off = ((((size_t)b * p.out_planes + p.out_plane0 + i) * p.H + y[h]) * p.W + x[h]) * 8 + 2 * k4;
           *reinterpret_cast<uint32_t*>(p.out + off) =
               pack_h2_rt((acc_l[4 * i + 2 * h] + sb_lff[n]) + g.x, (acc_l[4 * i + 2 * h + 1] + sb_lff[n + 1]) + g.y);
         }
       }
     }
-    wg_sync(1 + m);                                                  // htile / xbuf are rewritten by the next tile
+    wg_sync(1 + m);                                                  // htile / xs are rewritten by the next tile
   }
 }
 
