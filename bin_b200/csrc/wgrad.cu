@@ -234,9 +234,20 @@ int launch_wgrad_impl(const bin_act_t& x0, int x0_plane0, int x0_planes, const b
                       float* partial_ws, cudaStream_t s) {
   if (ks != 1 && ks != 3 && ks != 5) return fail(BIN_ERR_ARG, "wgrad: ksize must be 1, 3 or 5");
   if (!partial_ws) return fail(BIN_ERR_ARG, "wgrad: partial-sum workspace missing");
+  // TMA zero-fills a box that runs past its tensor, so a bad plane range or geometry would silently give wrong
+  // gradients: reject it here, before any tensor map is built
+  if (x0_planes <= 0 || x0_planes % kKPL || x1_planes < 0 || x1_planes % kKPL)
+    return fail(BIN_ERR_ARG, "wgrad: segment plane counts must be multiples of 4 (x0 non-empty)");
+  if (x0_plane0 < 0 || x0_plane0 + x0_planes > x0.planes ||
+      (x1_planes > 0 && (x1_plane0 < 0 || x1_plane0 + x1_planes > x1.planes)))
+    return fail(BIN_ERR_ARG, "wgrad: input plane range exceeds tensor");
+  if ((x1_planes > 0 && (x1.B != x0.B || x1.H != x0.H || x1.W != x0.W)) || dy.B != x0.B || dy.H != x0.H || dy.W != x0.W)
+    return fail(BIN_ERR_ARG, "wgrad: x1 / dY geometry differs from x0");
+  if (cin <= 0 || cout <= 0 || cin > 8 * (x0_planes + x1_planes))
+    return fail(BIN_ERR_ARG, "wgrad: Cin exceeds the input planes provided");
   int n = (cout + 15) / 16 * 16;
   if (n > 256) return fail(BIN_ERR_UNSUPPORTED, "wgrad: Cout > 256");
-  if (dy_plane0 + n / 8 > dy.planes) return fail(BIN_ERR_ARG, "wgrad: dY plane range exceeds tensor");   // (before SX widening)
+  if (dy_plane0 < 0 || dy_plane0 + n / 8 > dy.planes) return fail(BIN_ERR_ARG, "wgrad: dY plane range exceeds tensor");   // (before SX widening)
   WgradParams p;
   memset(&p, 0, sizeof(p));
   p.pad = ks / 2; p.ks = ks;

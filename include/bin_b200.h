@@ -130,7 +130,9 @@ int bin_rdb_tail_fwd(const bin_act_t* x, int x_plane0, const bin_act_t* g, int g
 int bin_pack_conv_weight_t(const float* w_oihw, int cout, int cin, int ksize, int row0, int nrows, int cout_pad_t,
                            int cin_pad_t, void* packed, bin_stream_t s);
 /* Weight gradient of one conv: dw (cout,cin,k,k fp32 OIHW) += (1/ *scale_dev) * sum_px dY[px][co] X[px+tap][ci];
- * X = planes of x0 followed by planes of x1 (like bin_conv_args_t), dY = planes [dy_plane0, +ceil(cout/8)).
+ * X = planes of x0 followed by planes of x1 (like bin_conv_args_t), dY = planes [dy_plane0, +ceil(cout/16)*2).
+ * Segment plane counts are multiples of 4 (x1_planes may be 0), every plane range lies inside its tensor, x1 and dy
+ * have the B/H/W of x0 and cin <= 8 * (x0_planes + x1_planes); anything else fails with BIN_ERR_ARG before any launch.
  * workspace: bin_conv_wgrad_workspace_bytes() bytes (per-CTA partial sums, reduced by a second kernel). */
 size_t bin_conv_wgrad_workspace_bytes(void);
 int bin_conv_wgrad(bin_act_t x0, int x0_plane0, int x0_planes, bin_act_t x1, int x1_plane0, int x1_planes, bin_act_t dy,

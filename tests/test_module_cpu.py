@@ -85,6 +85,39 @@ def test_workspace_queries_are_pure():
     assert 0 < a < L.bin_window_workspace_bytes(1, 128, 128)
 
 
+def test_wgrad_rejects_bad_segments_before_any_launch():
+    """bin_conv_wgrad checks its segments on the host: TMA zero-fills a box that runs past its tensor, so a plane range
+    or geometry error would otherwise come back as quietly wrong gradients.  Every call here is invalid and must fail
+    with BIN_ERR_ARG before a tensor map is built (the tensors are null: nothing reaches a device)."""
+    import ctypes as C
+    from bin_b200 import _lib
+    L = _lib.lib()
+    act = lambda planes, B=2, H=9, W=20: _lib.Act(None, B, planes, H, W)
+    none = _lib.Act(None, 0, 0, 0, 0)
+    ws = (C.c_float * 1)()
+    cases = [  # (x0, x0_plane0, x0_planes, x1, x1_plane0, x1_planes, dy, dy_plane0, cout, cin, ks), error text
+        ((act(12), 0, 0, none, 0, 0, act(4), 0, 32, 96, 3), "plane counts"),
+        ((act(12), 0, 6, none, 0, 0, act(4), 0, 32, 48, 3), "plane counts"),
+        ((act(144), 12, 12, act(192), 16, 6, act(16), 4, 32, 144, 3), "plane counts"),
+        ((act(12), 0, 12, act(16), 0, -4, act(16), 0, 32, 96, 3), "plane counts"),
+        ((act(144), 136, 12, none, 0, 0, act(16), 0, 32, 96, 3), "plane range"),
+        ((act(144), -4, 12, none, 0, 0, act(16), 0, 32, 96, 3), "plane range"),
+        ((act(144), 12, 12, act(192), 180, 16, act(144), 12, 96, 224, 1), "plane range"),
+        ((act(12), 0, 12, act(16, H=8), 0, 16, act(12), 0, 96, 224, 1), "geometry"),
+        ((act(12), 0, 12, act(16, B=3), 0, 16, act(12), 0, 96, 224, 1), "geometry"),
+        ((act(12), 0, 12, none, 0, 0, act(12, W=21), 0, 96, 96, 3), "geometry"),
+        ((act(12), 0, 12, none, 0, 0, act(12, B=1), 0, 96, 96, 3), "geometry"),
+        ((act(144), 12, 12, act(192), 16, 4, act(16), 4, 32, 160, 3), "Cin exceeds"),
+        ((act(4), 0, 4, none, 0, 0, act(12), 0, 96, 36, 5), "Cin exceeds"),
+        ((act(12), 0, 12, none, 0, 0, act(16), 14, 32, 96, 3), "dY plane range"),
+        ((act(12), 0, 12, none, 0, 0, act(16), -1, 32, 96, 3), "dY plane range"),
+    ]
+    for args, text in cases:
+        rc = L.bin_conv_wgrad(*args, None, None, C.addressof(ws), None)
+        err = L.bin_last_error().decode()
+        assert rc == 1 and text in err and err.startswith("wgrad:"), (args[1:3], args[4:6], args[7:], rc, err)
+
+
 def test_training_side_modules_refuse_cpu_tensors():
     """bin_b200.optim / bin_b200.dataprep have no CPU path: they must say so instead of computing something."""
     import torch
