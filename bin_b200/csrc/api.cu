@@ -75,6 +75,9 @@ int launch_adam_step(const bin_adam_tensor_t* table, const int* chunk_prefix, in
                      float bias_correction2, float grad_scale, cudaStream_t s);
 int launch_blur_average_u8(const uint8_t* frames, int T, size_t frame_bytes, int window_size, int first_mid, int stride,
                            int nwin, uint8_t* out, cudaStream_t s);
+size_t metrics_workspace_bytes(int h, int w);
+int launch_image_metrics_u8(const uint8_t* a, const uint8_t* b, int h, int w, int c, double* out4, void* workspace,
+                            size_t workspace_bytes, cudaStream_t s);
 int launch_rdb_tail(const bin_act_t& x, int x_plane0, const bin_act_t& g, int g_plane0, const void* w_conv,
                     const float* b_conv, const void* w_lff, const float* b_lff, const bin_act_t& out, int out_plane0,
                     int b_begin, int b_count, int y_begin, int y_count, cudaStream_t s, bool reverse = false);
@@ -828,6 +831,11 @@ int bin_blur_average_u8(const uint8_t* frames, int T, size_t frame_bytes, int wi
                         int nwin, uint8_t* out, bin_stream_t s) {
   if (!frames || !out) return fail(BIN_ERR_ARG, "blur_average: null argument");
   return launch_blur_average_u8(frames, T, frame_bytes, window_size, first_mid, stride, nwin, out, (cudaStream_t)s);
+}
+size_t bin_image_metrics_workspace_bytes(int h, int w) { return metrics_workspace_bytes(h, w); }
+int bin_image_metrics_u8(const uint8_t* a, const uint8_t* b, int h, int w, int c, double* out4, void* workspace,
+                         size_t workspace_bytes, bin_stream_t s) {
+  return launch_image_metrics_u8(a, b, h, w, c, out4, workspace, workspace_bytes, (cudaStream_t)s);
 }
 
 }  // extern "C"

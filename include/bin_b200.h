@@ -258,6 +258,16 @@ int bin_adam_step(const bin_adam_tensor_t* table_dev, const int* chunk_prefix_de
 int bin_blur_average_u8(const uint8_t* frames, int T, size_t frame_bytes, int window_size, int first_mid, int stride,
                         int nwin, uint8_t* out, bin_stream_t s);
 
+/* ---- evaluation metrics of the caller loop: test.py:404-458 (utils/util.py:201-250, skimage.measure) -------------- */
+/* Bytes of per-tile partial sums for an (h, w) pair (0 if h or w is outside [7, 65535]). */
+size_t bin_image_metrics_workspace_bytes(int h, int w);
+/* a, b: uint8 (h,w,c) contiguous, c = 1 or 3, 7 <= h,w <= 65535, h*w*c < 2^31.  out4 (device fp64[4]) = { sum|a-b|,
+ * sum (a-b)^2, mean Gaussian-11 SSIM (utils/util.py:211-231; NaN if h or w < 11), mean box-7 SSIM (skimage compare_ssim
+ * defaults) }.  Bit-reproducible: the tiling depends only on (h, w) and every sum has a fixed order.  Every argument
+ * is checked (BIN_ERR_ARG) before the first CUDA call. */
+int bin_image_metrics_u8(const uint8_t* a, const uint8_t* b, int h, int w, int c, double* out4,
+                         void* workspace, size_t workspace_bytes, bin_stream_t s);
+
 #ifdef __cplusplus
 }
 #endif
