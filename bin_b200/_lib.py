@@ -11,6 +11,7 @@ LIB_PATH = os.path.join(HERE, "libbin_b200.so")
 BIN_MAX_CALLS = 6
 BIN_MAX_FRAMES = 5
 BIN_BACKBONE_NCONV = 66
+BIN_FLIPX4_MAX_TENSORS = 14
 EPI_P8, EPI_PIXSHUF, EPI_FINAL = 0, 1, 2
 ABI_VERSION = 2
 
@@ -99,6 +100,8 @@ _SIGS = {
     "bin_image_metrics_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int]),
     "bin_image_metrics_u8": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t,
                                        C.c_void_p]),
+    "bin_flipx4_expand": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)] + [C.c_int] * 4 + [C.c_void_p]),
+    "bin_flipx4_mean": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)] + [C.c_int] * 4 + [C.c_void_p]),
 }
 
 _lib = None

@@ -78,6 +78,7 @@ int launch_blur_average_u8(const uint8_t* frames, int T, size_t frame_bytes, int
 size_t metrics_workspace_bytes(int h, int w);
 int launch_image_metrics_u8(const uint8_t* a, const uint8_t* b, int h, int w, int c, double* out4, void* workspace,
                             size_t workspace_bytes, cudaStream_t s);
+int launch_flipx4(int expand, const float* const* src, float* const* dst, int n, int B, int H, int W, cudaStream_t s);
 int launch_rdb_tail(const bin_act_t& x, int x_plane0, const bin_act_t& g, int g_plane0, const void* w_conv,
                     const float* b_conv, const void* w_lff, const float* b_lff, const bin_act_t& out, int out_plane0,
                     int b_begin, int b_count, int y_begin, int y_count, cudaStream_t s, bool reverse = false);
@@ -836,6 +837,12 @@ size_t bin_image_metrics_workspace_bytes(int h, int w) { return metrics_workspac
 int bin_image_metrics_u8(const uint8_t* a, const uint8_t* b, int h, int w, int c, double* out4, void* workspace,
                          size_t workspace_bytes, bin_stream_t s) {
   return launch_image_metrics_u8(a, b, h, w, c, out4, workspace, workspace_bytes, (cudaStream_t)s);
+}
+int bin_flipx4_expand(const float* const* src_host, float* const* dst_host, int n, int B, int H, int W, bin_stream_t s) {
+  return launch_flipx4(1, src_host, dst_host, n, B, H, W, (cudaStream_t)s);
+}
+int bin_flipx4_mean(const float* const* src_host, float* const* dst_host, int n, int B, int H, int W, bin_stream_t s) {
+  return launch_flipx4(0, src_host, dst_host, n, B, H, W, (cudaStream_t)s);
 }
 
 }  // extern "C"

@@ -797,6 +797,75 @@ __global__ void blur_average_u8_kernel(const uint8_t* __restrict__ frames, size_
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------
+// x4 flip self-ensemble (utils/test_util.py:110-132 flipx4_forward) over the tensors of a whole window.  Orientation o:
+// bit 0 flips W, bit 1 flips H.  blockIdx.y = table entry; one thread = 4 consecutive pixels of one row when vec
+// (W % 4 == 0 and 16-byte aligned tensors: a W-flipped float4 is then an aligned float4 with its lanes reversed), else 1.
+// Both kernels are memory-bound copies; indices are 64-bit (a 4B batch at 768x1344 is 12.4 M floats per item).
+struct FlipTable {
+  const float* src[BIN_FLIPX4_MAX_TENSORS];
+  float* dst[BIN_FLIPX4_MAX_TENSORS];
+};
+__device__ __forceinline__ float4 ld4(const float* p, bool rev) {
+  const float4 v = *reinterpret_cast<const float4*>(p);
+  return rev ? make_float4(v.w, v.z, v.y, v.x) : v;
+}
+// src (B,3,H,W) -> dst (4B,3,H,W), item o*B + b = orientation o of item b
+__global__ void __launch_bounds__(256) flipx4_expand_kernel(const __grid_constant__ FlipTable T, int B, int H, int W, int vec) {
+  const float* __restrict__ src = T.src[blockIdx.y];
+  float* __restrict__ dst = T.dst[blockIdx.y];
+  const int per_row = vec ? W >> 2 : W;
+  const size_t orows = (size_t)B * 3 * H;                        // rows of one orientation
+  const size_t total = 4 * orows * per_row;
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const int u = (int)(i % per_row);
+    const size_t r = i / per_row;                                 // dst row ((o*B + b)*3 + c)*H + y
+    const int o = (int)(r / orows);
+    const size_t rr = r - (size_t)o * orows;                      // row (b*3 + c)*H + y of src
+    const int y = (int)(rr % H);
+    const float* s = src + (rr - y + ((o & 2) ? H - 1 - y : y)) * W;
+    float* d = dst + r * W;
+    if (vec) {
+      const int x = 4 * u;
+      *reinterpret_cast<float4*>(d + x) = ld4(s + ((o & 1) ? W - 4 - x : x), o & 1);
+    } else {
+      d[u] = s[(o & 1) ? W - 1 - u : u];
+    }
+  }
+}
+// flipx4_forward's accumulation: ((y0 + flipW(y1)) + flipH(y2)) + flipHW(y3), then / 4, each step rounded on its own
+__device__ __forceinline__ float flipx4_avg(float a, float b, float c, float d) {
+  return __fdiv_rn(__fadd_rn(__fadd_rn(__fadd_rn(a, b), c), d), 4.f);
+}
+// src (4B,3,H,W) as expand lays it out -> dst (B,3,H,W)
+__global__ void __launch_bounds__(256) flipx4_mean_kernel(const __grid_constant__ FlipTable T, int B, int H, int W, int vec) {
+  const float* __restrict__ src = T.src[blockIdx.y];
+  float* __restrict__ dst = T.dst[blockIdx.y];
+  const int per_row = vec ? W >> 2 : W;
+  const size_t orows = (size_t)B * 3 * H;
+  const size_t ostride = orows * W;                               // floats of one orientation
+  const size_t total = orows * per_row;
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const int u = (int)(i % per_row);
+    const size_t r = i / per_row;                                 // row (b*3 + c)*H + y
+    const int y = (int)(r % H);
+    const size_t rf = r - y + (H - 1 - y);                        // the same row, H-flipped
+    const float* s0 = src + r * W;
+    const float* s1 = src + ostride + r * W;
+    const float* s2 = src + 2 * ostride + rf * W;
+    const float* s3 = src + 3 * ostride + rf * W;
+    if (vec) {
+      const int x = 4 * u, xf = W - 4 - x;
+      const float4 a = ld4(s0 + x, false), b = ld4(s1 + xf, true), c = ld4(s2 + x, false), d = ld4(s3 + xf, true);
+      *reinterpret_cast<float4*>(dst + r * W + x) = make_float4(flipx4_avg(a.x, b.x, c.x, d.x), flipx4_avg(a.y, b.y, c.y, d.y),
+                                                                flipx4_avg(a.z, b.z, c.z, d.z), flipx4_avg(a.w, b.w, c.w, d.w));
+    } else {
+      const int xf = W - 1 - u;
+      dst[r * W + u] = flipx4_avg(s0[u], s1[xf], s2[u], s3[xf]);
+    }
+  }
+}
+
 static inline int grid_for(size_t total, int block) {
   size_t g = (total + block - 1) / block;
   const size_t cap = (size_t)num_sms() * 16;
@@ -1082,5 +1151,33 @@ int launch_wgrad(const bin_act_t& x0, int x0_plane0, int x0_planes, const bin_ac
                  float* partial_ws, cudaStream_t s) {
   return launch_wgrad_impl(x0, x0_plane0, x0_planes, x1, x1_plane0, x1_planes, dy, dy_plane0, cout, cin, ks, scale, dw,
                            partial_ws, s);
+}
+// expand = 1: bin_flipx4_expand, 0: bin_flipx4_mean.  Every check runs before the first CUDA call.
+int launch_flipx4(int expand, const float* const* src, float* const* dst, int n, int B, int H, int W, cudaStream_t s) {
+  const std::string who = expand ? "flipx4_expand: " : "flipx4_mean: ";
+  if (!src || !dst) return fail(BIN_ERR_ARG, who + "null table");
+  if (n < 1 || n > BIN_FLIPX4_MAX_TENSORS) return fail(BIN_ERR_ARG, who + "n must be 1..14");
+  if (B < 1 || H < 1 || W < 1) return fail(BIN_ERR_ARG, who + "B, H and W must be >= 1");
+  if ((double)B * H * W * 12 >= 0x1p62) return fail(BIN_ERR_ARG, who + "tensor too large");
+  FlipTable T;
+  memset(&T, 0, sizeof(T));
+  uintptr_t align = 0;
+  for (int i = 0; i < n; ++i) {
+    if (!src[i] || !dst[i]) return fail(BIN_ERR_ARG, who + "null table entry");
+    for (int j = 0; j < n; ++j) {
+      if ((const float*)dst[i] == src[j]) return fail(BIN_ERR_ARG, who + "a dst equals a src (in place would race)");
+      if (j < i && dst[j] == dst[i]) return fail(BIN_ERR_ARG, who + "dst entries must be distinct");
+    }
+    T.src[i] = src[i];
+    T.dst[i] = dst[i];
+    align |= (uintptr_t)src[i] | (uintptr_t)dst[i];
+  }
+  const int vec = (W % 4 == 0) && (align & 15) == 0;
+  const size_t units = (size_t)(expand ? 4 : 1) * B * 3 * H * (vec ? W / 4 : W);
+  const dim3 grid((unsigned)grid_for(units, 256), (unsigned)n);
+  if (expand) flipx4_expand_kernel<<<grid, 256, 0, s>>>(T, B, H, W, vec);
+  else flipx4_mean_kernel<<<grid, 256, 0, s>>>(T, B, H, W, vec);
+  BIN_CUDA_OK(cudaGetLastError());
+  return BIN_OK;
 }
 }  // namespace binb

@@ -147,6 +147,39 @@ def rdb_tail_fwd(x: torch.Tensor, g: torch.Tensor, w_conv: torch.Tensor, b_conv:
     check(lib().bin_rdb_tail_fwd(C.byref(ax), x_plane0, C.byref(ag), g_plane0, w_conv.data_ptr(), b_conv.data_ptr(),
                                  w_lff.data_ptr(), b_lff.data_ptr(), C.byref(ao), out_plane0, *sub, _stream()))
 
+def _flipx4(srcs: Sequence[torch.Tensor], expand: bool) -> List[torch.Tensor]:
+    name = "flipx4_expand" if expand else "flipx4_mean"
+    if not 1 <= len(srcs) <= _lib.BIN_FLIPX4_MAX_TENSORS:
+        raise _lib.BinB200Error(f"{name}: takes 1..{_lib.BIN_FLIPX4_MAX_TENSORS} tensors, got {len(srcs)}")
+    srcs = [_req(t, torch.float32, name) for t in srcs]
+    shape, dev = srcs[0].shape, srcs[0].device
+    if len(shape) != 4 or shape[1] != 3 or (not expand and shape[0] % 4):
+        raise _lib.BinB200Error(f"{name}: expected {'(B' if expand else '(4B'},3,H,W) tensors, got {tuple(shape)}")
+    if any(t.shape != shape or t.device != dev for t in srcs):
+        raise _lib.BinB200Error(f"{name}: all tensors must share shape and device")
+    B = shape[0] if expand else shape[0] // 4
+    H, W = shape[2], shape[3]
+    with torch.cuda.device(dev):
+        dsts = [torch.empty((4 * B if expand else B, 3, H, W), dtype=torch.float32, device=dev) for _ in srcs]
+        sp = (C.c_void_p * len(srcs))(*[t.data_ptr() for t in srcs])
+        dp = (C.c_void_p * len(dsts))(*[t.data_ptr() for t in dsts])
+        fn = lib().bin_flipx4_expand if expand else lib().bin_flipx4_mean
+        check(fn(sp, dp, len(srcs), B, H, W, _stream()))
+    return dsts
+
+
+def flipx4_expand(srcs: Sequence[torch.Tensor]) -> List[torch.Tensor]:
+    """Each (B,3,H,W) tensor -> (4B,3,H,W): items [oB, oB+B) are orientation o = identity, flip W, flip H, flip H and W
+    of utils/test_util.py:110-132 flipx4_forward (one launch for the whole list)."""
+    return _flipx4(srcs, True)
+
+
+def flipx4_mean(srcs: Sequence[torch.Tensor]) -> List[torch.Tensor]:
+    """Each (4B,3,H,W) tensor laid out as flipx4_expand writes it -> (B,3,H,W) =
+    (((y0 + flipW(y1)) + flipH(y2)) + flipHW(y3)) / 4 in fp32, flipx4_forward's order (one launch for the whole list)."""
+    return _flipx4(srcs, False)
+
+
 def convlstm_fwd(x, w, b, state=None):
     """ConvLSTMCell.forward (RDN.py:50-95) -> (h, c)."""
     x = _req(x, torch.float32, "x")

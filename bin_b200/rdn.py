@@ -22,7 +22,7 @@ import torch.nn.init as weight_init
 from . import _lib, ops
 from ._lib import BinB200Error, Net, check, lib
 
-__all__ = ["set_precision", "ConvLSTMCell", "pixel_reshuffle", "RDB_Conv", "RDB", "RDN_residual_interp_2_input",
+__all__ = ["set_precision", "set_self_ensemble", "ConvLSTMCell", "pixel_reshuffle", "RDB_Conv", "RDB", "RDN_residual_interp_2_input",
            "RDN_residual_interp_2_1_input", "RDN_residual_interp_4_1_input", "RDN_residual_interp_5_input",
            "RDN_residual_interp_5_input_ConvLSTM_L", "bin_stage4_lstm"]
 
@@ -391,13 +391,19 @@ class RDN_residual_interp_5_input_ConvLSTM_L(nn.Module):
         """One 6-frame window -> the reference's 14-tuple (RDN.py:461-465): executes 17 unique
         backbone calls of its 20 and the 6 live ConvLSTM calls of its 12 (SURVEY.md App. A)."""
         frames = [B1, B3, B5, B7, B9, B11]
+        ensemble = _ensemble_of(self)
         if torch.is_grad_enabled() and (any(f.requires_grad for f in frames) or
                                         any(p.requires_grad for p in self._all_tensors())):
+            if ensemble is not None:
+                raise BinB200Error(f"self-ensemble {ensemble!r} is inference-only: call the net under torch.no_grad(), "
+                                   "or set_self_ensemble(net, None) to train")
             from .autograd import window_apply
             return window_apply(self, frames)
         frames = [f.contiguous() for f in frames]
         B, H, W = _check_frames(frames)
         dev = frames[0].device
+        if ensemble is not None:
+            return self._forward_flipx4(frames, B, H, W, dev)
         if _graphs_enabled() and not getattr(self, "_is_replica", False) and not torch.cuda.is_current_stream_capturing():
             return self._forward_graphed(frames, B, H, W, dev)
         with torch.cuda.device(dev):
@@ -412,6 +418,16 @@ class RDN_residual_interp_5_input_ConvLSTM_L(nn.Module):
         op = (C.c_void_p * 14)(*[o.data_ptr() for o in outs])
         check(lib().bin_window_fwd_p(C.byref(net), fp, op, B, H, W, ws.data_ptr(), ws.numel(), prec, _stream()))
         return outs, ws
+
+    def _forward_flipx4(self, frames, B, H, W, dev):
+        """x4 flip self-ensemble (utils/test_util.py:110-132 flipx4_forward, applied to all 6 frames and all 14 outputs):
+        the four orientations run as ONE window at batch 4B, then each output is flipped back and averaged.  Eager, not
+        graphed: a graph capture would hold a second batch-4B workspace (about 25 GB at 768x1344) in its private pool."""
+        with torch.cuda.device(dev):
+            big = ops.flipx4_expand(frames)
+            outs, _ = self._launch_window(big, 4 * B, H, W, dev)
+            del big
+            return tuple(ops.flipx4_mean(outs))
 
     def _forward_graphed(self, frames, B, H, W, dev):
         """The ~340 kernel launches of a window are captured once per (shape, weight version) into a
@@ -445,6 +461,8 @@ class RDN_residual_interp_5_input_ConvLSTM_L(nn.Module):
 
     def forward_pyramid3(self, B1, B3, B5, B7):
         """BASELINE config 2a: stages 1-3 on 4 frames -> [I2',I4',I6',I3',I5',I4''] (SURVEY 8d)."""
+        if _ensemble_of(self) is not None:
+            raise BinB200Error("forward_pyramid3 has no self-ensemble mode; set_self_ensemble(net, None) first")
         if torch.is_grad_enabled() and (any(f.requires_grad for f in (B1, B3, B5, B7)) or
                                         self.model.model1_1.SFENet1.weight.requires_grad):
             from .autograd import pyramid3_apply                      # BASELINE config 3a (training on the 4-frame graph)
@@ -465,3 +483,27 @@ class RDN_residual_interp_5_input_ConvLSTM_L(nn.Module):
 def bin_stage4_lstm():
     """Factory with the reference's name and arity (RDN.py:469-471; networks.py:9-10)."""
     return RDN_residual_interp_5_input_ConvLSTM_L()
+
+
+ENSEMBLES = (None, "flipx4")
+
+
+def _ensemble_of(module) -> Optional[str]:
+    mode = getattr(module, "self_ensemble", None)
+    if mode not in ENSEMBLES:
+        raise BinB200Error(f"unknown self-ensemble mode {mode!r}; use None or 'flipx4'")
+    return mode
+
+
+def set_self_ensemble(net: nn.Module, mode: Optional[str]) -> nn.Module:
+    """Turn the x4 flip self-ensemble of utils/test_util.py:110-132 on (mode "flipx4") or off (None) for every window net
+    in `net.modules()` (so a DataParallel wrapper or a model object holding the net works).  Inference only: a
+    grad-enabled call then raises.  It is a plain attribute, not a parameter or buffer: the state_dict is unchanged."""
+    if mode not in ENSEMBLES:
+        raise BinB200Error(f"unknown self-ensemble mode {mode!r}; use None or 'flipx4'")
+    nets = [m for m in net.modules() if isinstance(m, RDN_residual_interp_5_input_ConvLSTM_L)]
+    if not nets:
+        raise BinB200Error("set_self_ensemble: no RDN_residual_interp_5_input_ConvLSTM_L in this module")
+    for m in nets:
+        m.self_ensemble = mode
+    return net

@@ -17,7 +17,7 @@ import torch
 
 from . import ops
 from ._lib import BinB200Error, check, lib
-from .rdn import _LSTM_NAMES, _batched
+from .rdn import _LSTM_NAMES, _batched, _ensemble_of
 
 
 def test_py_padding(h: int, w: int) -> Tuple[int, int, int, int]:
@@ -67,14 +67,19 @@ def tensor2img_u8(t: torch.Tensor, crop: Optional[Tuple[int, int, int, int]] = N
 
 
 class StreamingBIN:
-    """Feed frames one at a time; from the 6th frame on, every push returns the 14-tuple of that window."""
+    """Feed frames one at a time; from the 6th frame on, every push returns the 14-tuple of that window.
+
+    With the net's x4 flip self-ensemble on (rdn.set_self_ensemble), every pushed frame is expanded once into its four
+    orientations (4B items), the stage-1 cache holds 4B outputs, and each window's 14 outputs are flipped back and
+    averaged: the same bits as calling the net per window."""
 
     def __init__(self, net):
         self.net = net
-        self.frames: List[Tuple[int, torch.Tensor]] = []            # (frame id, (B,3,H,W) fp32 device tensor)
+        self.frames: List[Tuple[int, torch.Tensor]] = []            # (frame id, (B,3,H,W) or expanded (4B,3,H,W) tensor)
         self.s1: "OrderedDict[Tuple[int, int], torch.Tensor]" = OrderedDict()   # stage-1 output per adjacent frame pair
         self.next_id = 0
         self.backbone_calls = 0
+        self.key = None                                               # (ensemble mode, pushed frame shape) of the cache
 
     def reset(self):
         self.frames.clear()
@@ -84,9 +89,16 @@ class StreamingBIN:
     def push(self, frame: torch.Tensor):
         if not frame.is_cuda or frame.dtype != torch.float32 or frame.dim() != 4 or frame.shape[1] != 3:
             raise BinB200Error("StreamingBIN.push expects a (B,3,H,W) fp32 CUDA frame (see upload_frame_u8)")
-        if self.frames and self.frames[-1][1].shape != frame.shape:
+        ensemble = _ensemble_of(self.net)
+        key = (ensemble, frame.shape)
+        if self.frames and self.key != key:
             self.reset()
-        self.frames.append((self.next_id, frame.contiguous()))
+        self.key = key
+        frame = frame.contiguous()
+        if ensemble is not None:
+            with torch.cuda.device(frame.device):
+                frame = ops.flipx4_expand([frame])[0]
+        self.frames.append((self.next_id, frame))
         self.next_id += 1
         if len(self.frames) > 6:
             old = self.frames.pop(0)[0]
@@ -123,4 +135,6 @@ class StreamingBIN:
         p6b = lstm(5, o[8])
         o[9], o[13] = _batched(m4, [(o[1], o[1], o[7], o[8], o[2]), (p6b, o[2], t2, o[12], o[3])])
         self.backbone_calls += 12
+        if self.key[0] is not None:
+            return tuple(ops.flipx4_mean(o))
         return tuple(o)

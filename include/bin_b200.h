@@ -268,6 +268,21 @@ size_t bin_image_metrics_workspace_bytes(int h, int w);
 int bin_image_metrics_u8(const uint8_t* a, const uint8_t* b, int h, int w, int c, double* out4,
                          void* workspace, size_t workspace_bytes, bin_stream_t s);
 
+/* ---- x4 flip self-ensemble: utils/test_util.py:110-132 flipx4_forward, for a whole 6-frame window ---------------- */
+/* Orientation o of an image x: 0 = x, 1 = flip W (torch.flip(x, (-1,))), 2 = flip H ((-2,)), 3 = flip H and W ((-2, -1)).
+ * Each flip is its own inverse.  One launch handles a table of n <= BIN_FLIPX4_MAX_TENSORS tensors (the 6 frames or the
+ * 14 outputs of a window).
+ * expand: src[i] (B,3,H,W) fp32 NCHW -> dst[i] (4B,3,H,W), orientation-major: item o*B + b = orientation o of src item b,
+ *         so dst[i] + o*B*3*H*W is a contiguous (B,3,H,W) batch that bin_window_fwd_p takes unchanged.
+ * mean:   src[i] (4B,3,H,W), laid out as expand writes it -> dst[i] (B,3,H,W) =
+ *         (((y0 + flipW(y1)) + flipH(y2)) + flipHW(y3)) / 4 with y_o = items [o*B, o*B+B) of src[i]: flipx4_forward's
+ *         order, every step one correctly rounded fp32 operation (no contraction), so it equals the torch expression.
+ * Fails with BIN_ERR_ARG before the first CUDA call if n is outside 1..BIN_FLIPX4_MAX_TENSORS, B, H or W < 1, a table or
+ * an entry is NULL, or a dst pointer equals a src pointer or another dst pointer (in place would race). */
+#define BIN_FLIPX4_MAX_TENSORS 14
+int bin_flipx4_expand(const float* const* src_host, float* const* dst_host, int n, int B, int H, int W, bin_stream_t s);
+int bin_flipx4_mean(const float* const* src_host, float* const* dst_host, int n, int B, int H, int W, bin_stream_t s);
+
 #ifdef __cplusplus
 }
 #endif
