@@ -12,6 +12,8 @@ BIN_MAX_CALLS = 6
 BIN_MAX_FRAMES = 5
 BIN_BACKBONE_NCONV = 66
 BIN_FLIPX4_MAX_TENSORS = 14
+BIN_TRAIN_MAX_BATCH = 16
+BIN_TRAIN_FRAMES = 17
 EPI_P8, EPI_PIXSHUF, EPI_FINAL = 0, 1, 2
 ABI_VERSION = 2
 
@@ -39,6 +41,11 @@ class ConvArgs(C.Structure):
 
 class Net(C.Structure):
     _fields_ = [("blob", C.c_void_p * 4), ("lstm_w", C.c_void_p * 6), ("lstm_b", C.c_void_p * 6)]
+
+
+class TrainSample(C.Structure):
+    _fields_ = [("src", C.c_void_p * BIN_TRAIN_FRAMES), ("H", C.c_int), ("W", C.c_int),
+                ("top", C.c_int), ("left", C.c_int), ("flip", C.c_int)]
 
 
 class BinB200Error(RuntimeError):
@@ -102,6 +109,7 @@ _SIGS = {
                                        C.c_void_p]),
     "bin_flipx4_expand": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)] + [C.c_int] * 4 + [C.c_void_p]),
     "bin_flipx4_mean": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)] + [C.c_int] * 4 + [C.c_void_p]),
+    "bin_train_batch_u8": (C.c_int, [C.POINTER(TrainSample)] + [C.c_int] * 3 + [C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
 }
 
 _lib = None

@@ -866,6 +866,35 @@ __global__ void __launch_bounds__(256) flipx4_mean_kernel(const __grid_constant_
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------
+// Training batch (data/BIN_dataset.py:62-183 Adobe_BIN_loader + __getitem__ + collation).  grid (row groups, 17 frames,
+// B samples); a block walks rows of one (frame, sample) with its threads along x, so each channel plane is stored
+// coalesced; the 3 bytes of a pixel are read once for its 3 output planes.  Offsets are 64-bit (row pitch 3W of any
+// frame size; a (17,16,3,352,640) batch is 184 M floats).
+struct TrainBatchTable {
+  bin_train_sample_t s[BIN_TRAIN_MAX_BATCH];
+};
+__global__ void __launch_bounds__(256) train_batch_u8_kernel(const __grid_constant__ TrainBatchTable T, int h, int w,
+                                                             float* __restrict__ dst, int dst_B, int b0) {
+  const int f = blockIdx.y, b = blockIdx.z;
+  const bin_train_sample_t& S = T.s[b];
+  const uint8_t* __restrict__ src = S.src[f];
+  const size_t plane = (size_t)h * w;
+  float* __restrict__ out = dst + ((size_t)f * dst_B + b0 + b) * 3 * plane;
+  const size_t pitch = (size_t)S.W * 3;
+  for (int y = blockIdx.x; y < h; y += gridDim.x) {
+    const uint8_t* row = src + (size_t)(S.top + y) * pitch + (size_t)S.left * 3;
+    float* o = out + (size_t)y * w;
+    for (int x = threadIdx.x; x < w; x += blockDim.x) {
+      const uint8_t* p = row + (size_t)(S.flip ? w - 1 - x : x) * 3;
+      const uint8_t bl = p[0], g = p[1], r = p[2];
+      o[x] = __fdiv_rn((float)r, 255.f);
+      o[plane + x] = __fdiv_rn((float)g, 255.f);
+      o[2 * plane + x] = __fdiv_rn((float)bl, 255.f);
+    }
+  }
+}
+
 static inline int grid_for(size_t total, int block) {
   size_t g = (total + block - 1) / block;
   const size_t cap = (size_t)num_sms() * 16;
@@ -1177,6 +1206,36 @@ int launch_flipx4(int expand, const float* const* src, float* const* dst, int n,
   const dim3 grid((unsigned)grid_for(units, 256), (unsigned)n);
   if (expand) flipx4_expand_kernel<<<grid, 256, 0, s>>>(T, B, H, W, vec);
   else flipx4_mean_kernel<<<grid, 256, 0, s>>>(T, B, H, W, vec);
+  BIN_CUDA_OK(cudaGetLastError());
+  return BIN_OK;
+}
+// bin_train_batch_u8.  Every check runs before the first CUDA call.
+int launch_train_batch_u8(const bin_train_sample_t* samples, int B, int h, int w, float* dst, int dst_B, int b0,
+                          cudaStream_t s) {
+  const std::string who = "train_batch_u8: ";
+  if (!samples) return fail(BIN_ERR_ARG, who + "null table");
+  if (B < 1 || B > BIN_TRAIN_MAX_BATCH) return fail(BIN_ERR_ARG, who + "B must be 1..16");
+  if (h < 1 || w < 1) return fail(BIN_ERR_ARG, who + "h and w must be >= 1");
+  if (!dst) return fail(BIN_ERR_ARG, who + "null dst");
+  if (b0 < 0 || (long long)b0 + B > dst_B) return fail(BIN_ERR_ARG, who + "items [b0, b0+B) must lie inside dst_B");
+  if ((double)BIN_TRAIN_FRAMES * dst_B * 3 * h * w * 4 >= 0x1p62) return fail(BIN_ERR_ARG, who + "dst too large");
+  TrainBatchTable T;
+  memset(&T, 0, sizeof(T));
+  for (int i = 0; i < B; ++i) {
+    const bin_train_sample_t& S = samples[i];
+    for (int f = 0; f < BIN_TRAIN_FRAMES; ++f)
+      if (!S.src[f]) return fail(BIN_ERR_ARG, who + "null frame pointer");
+    if (S.flip != 0 && S.flip != 1) return fail(BIN_ERR_ARG, who + "flip must be 0 or 1");
+    if (S.H < 1 || S.W < 1) return fail(BIN_ERR_ARG, who + "source H and W must be >= 1");
+    if ((double)S.H * S.W * 3 >= 0x1p62) return fail(BIN_ERR_ARG, who + "source frame too large");
+    if (S.top < 0 || S.left < 0 || (long long)S.top + h > S.H || (long long)S.left + w > S.W)
+      return fail(BIN_ERR_ARG, who + "crop outside its source frame");
+    T.s[i] = S;
+  }
+  // about 16 blocks per SM in all, each over whole rows of one (frame, sample)
+  const int per = (num_sms() * 16 + BIN_TRAIN_FRAMES * B - 1) / (BIN_TRAIN_FRAMES * B);
+  const dim3 grid((unsigned)(h < per ? h : per), BIN_TRAIN_FRAMES, (unsigned)B);
+  train_batch_u8_kernel<<<grid, 256, 0, s>>>(T, h, w, dst, dst_B, b0);
   BIN_CUDA_OK(cudaGetLastError());
   return BIN_OK;
 }

@@ -6,7 +6,7 @@ computes anything in Python/PyTorch.
 from __future__ import annotations
 
 import ctypes as C
-from typing import List, Optional, Sequence
+from typing import List, Optional, Sequence, Tuple
 
 import torch
 
@@ -178,6 +178,41 @@ def flipx4_mean(srcs: Sequence[torch.Tensor]) -> List[torch.Tensor]:
     """Each (4B,3,H,W) tensor laid out as flipx4_expand writes it -> (B,3,H,W) =
     (((y0 + flipW(y1)) + flipH(y2)) + flipHW(y3)) / 4 in fp32, flipx4_forward's order (one launch for the whole list)."""
     return _flipx4(srcs, False)
+
+
+def train_batch_u8(samples: Sequence[Tuple[Sequence[torch.Tensor], int, int, int]], h: int, w: int) -> torch.Tensor:
+    """Training batch of data/BIN_dataset.py BINDataset as the DataLoader collates it, built on the device.
+
+    samples: (frames, top, left, flip) per item; frames = the 17 contiguous uint8 CUDA (H,W,3) BGR images of the item in
+    output order (6 LQs, 6 GTenh, 5 GTinp), all of one shape.  Returns one fp32 (17,B,3,h,w) tensor with
+    out[f,b,c,y,x] = frames_b[f][top+y, left + (w-1-x if flip else x), 2-c] / 255, one launch per 16 items."""
+    B = len(samples)
+    if B < 1:
+        raise _lib.BinB200Error("train_batch_u8: no samples")
+    dev = samples[0][0][0].device
+    if dev.type != "cuda":
+        raise _lib.BinB200Error("train_batch_u8: expected CUDA frames (bin_b200 has no CPU path)")
+    tab = (_lib.TrainSample * B)()
+    for i, (frames, top, left, flip) in enumerate(samples):
+        if len(frames) != _lib.BIN_TRAIN_FRAMES:
+            raise _lib.BinB200Error(f"train_batch_u8: item {i} has {len(frames)} frames, expected 17")
+        shape = frames[0].shape
+        for t in frames:
+            if t.device != dev or t.dtype != torch.uint8 or t.dim() != 3 or t.shape[2] != 3 or t.shape != shape \
+                    or not t.is_contiguous():
+                raise _lib.BinB200Error(f"train_batch_u8: item {i}: frames must be contiguous uint8 (H,W,3) tensors of "
+                                        f"one shape on {dev}")
+        e = tab[i]
+        for f, t in enumerate(frames):
+            e.src[f] = t.data_ptr()
+        e.H, e.W, e.top, e.left, e.flip = shape[0], shape[1], top, left, int(flip)
+    with torch.cuda.device(dev):
+        out = torch.empty((_lib.BIN_TRAIN_FRAMES, B, 3, h, w), dtype=torch.float32, device=dev)
+        for b0 in range(0, B, _lib.BIN_TRAIN_MAX_BATCH):
+            n = min(_lib.BIN_TRAIN_MAX_BATCH, B - b0)
+            check(lib().bin_train_batch_u8(C.cast(C.byref(tab, b0 * C.sizeof(_lib.TrainSample)), C.POINTER(_lib.TrainSample)),
+                                           n, h, w, out.data_ptr(), B, b0, _stream()))
+    return out
 
 
 def convlstm_fwd(x, w, b, state=None):

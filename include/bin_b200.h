@@ -283,6 +283,27 @@ int bin_image_metrics_u8(const uint8_t* a, const uint8_t* b, int h, int w, int c
 int bin_flipx4_expand(const float* const* src_host, float* const* dst_host, int n, int B, int H, int W, bin_stream_t s);
 int bin_flipx4_mean(const float* const* src_host, float* const* dst_host, int n, int B, int H, int W, bin_stream_t s);
 
+/* ---- training batches: data/BIN_dataset.py:30-54,62-183 BINDataset.__getitem__ + DataLoader collation ------------ */
+/* One sample: its 17 source frames in output order (6 LQs, 6 GTenh, 5 GTinp; the caller applies the order draw), each a
+ * device uint8 (H,W,3) BGR image with row pitch 3W, as cv2.imread returns it; the crop (top, left) and the fliplr draw. */
+#define BIN_TRAIN_MAX_BATCH 16
+#define BIN_TRAIN_FRAMES 17
+typedef struct {
+  const uint8_t* src[BIN_TRAIN_FRAMES];
+  int H, W;
+  int top, left, flip;
+} bin_train_sample_t;
+/* Writes samples[0..B) as items [b0, b0+B) of dst, an fp32 (17, dst_B, 3, h, w) tensor (rows 0-5 LQs, 6-11 GTenh,
+ * 12-16 GTinp; each row is a contiguous (dst_B,3,h,w) batch):
+ *   dst[f][b0+b][c][y][x] = src_f[top+y][left + (flip ? w-1-x : x)][2-c] / 255
+ * as one correctly rounded fp32 division (numpy's float32 `/ 255.`), so the bits equal read_img + the crop, np.fliplr,
+ * BGR->RGB and torch.stack of the reference.  The table travels in the kernel parameters: one launch per call.
+ * Fails with BIN_ERR_ARG before the first CUDA call if B is outside 1..BIN_TRAIN_MAX_BATCH, h or w < 1, the table,
+ * a frame pointer or dst is NULL, [b0, b0+B) is not inside [0, dst_B), flip is not 0 or 1, a crop lies outside its
+ * source frame, or a size overflows. */
+int bin_train_batch_u8(const bin_train_sample_t* samples_host, int B, int h, int w, float* dst, int dst_B, int b0,
+                       bin_stream_t s);
+
 #ifdef __cplusplus
 }
 #endif
