@@ -15,7 +15,7 @@ BIN_FLIPX4_MAX_TENSORS = 14
 BIN_TRAIN_MAX_BATCH = 16
 BIN_TRAIN_FRAMES = 17
 EPI_P8, EPI_PIXSHUF, EPI_FINAL = 0, 1, 2
-ABI_VERSION = 2
+ABI_VERSION = 3
 
 
 class Act(C.Structure):
@@ -80,6 +80,9 @@ _SIGS = {
     "bin_backbone_grad_param_floats": (C.c_size_t, [C.c_int]),
     "bin_backbone_bwd": (C.c_int, [C.c_int, C.c_void_p, C.POINTER(Frames), C.POINTER(Frames), C.c_int, C.c_int, C.c_void_p,
                                    C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "bin_backbone_bwd_recompute": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.POINTER(Frames), C.POINTER(Frames), C.c_int,
+                                             C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p,
+                                             C.c_void_p, C.c_void_p]),
     "bin_grad_scale": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_size_t, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]),
     "bin_rdb_fwd": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
                               C.c_void_p, C.c_size_t, C.c_void_p]),

@@ -36,35 +36,70 @@ def _packed_t(model) -> torch.Tensor:
     return cached[1]
 
 
+def _input_key(model, frames):
+    """What a recomputing backward must find unchanged: the weights and the stage's input frames (pointer, version)."""
+    return tuple((t.data_ptr(), t._version) for t in list(model._conv_params()) + list(frames))
+
+
+def _inference_fwd(model, calls, outs, B, H, W, dev) -> torch.Tensor:
+    """bin_backbone_fwd of one batched stage into the shared per-(device, stream) workspace, which it returns."""
+    from .rdn import _workspace
+    n = model.NFRAMES
+    fr = ops.make_frames(calls, outs)
+    ws = _workspace(dev, lib().bin_backbone_workspace_bytes(n, B * len(calls), H, W))
+    check(lib().bin_backbone_fwd(n, model.packed_blob().data_ptr(), C.byref(fr), H, W, ws.data_ptr(), ws.numel(),
+                                 _stream()))
+    return ws
+
+
 class BackboneStageFn(torch.autograd.Function):
-    """ncalls same-weight backbone calls (RDN.py:210-334) in one launch, with backward."""
+    """ncalls same-weight backbone calls (RDN.py:210-334) in one launch, with backward.
+
+    Default: the forward keeps the stage's whole training workspace (all 12 RDBs' growth maps) until the backward.
+    With set_activation_checkpointing(net, "recompute") it keeps only its input frames: the forward is the inference
+    forward into the shared per-stream workspace, and the backward runs that forward again and rebuilds each RDB's
+    growth maps just before that RDB's backward.  Every kernel sees the same operands in both (DESIGN.md §4e)."""
 
     @staticmethod
     def forward(ctx, model, ncalls: int, *args):
+        from .rdn import _checkpointing_of
         n = model.NFRAMES
         frames = [a.detach().contiguous() for a in args[: ncalls * n]]
         calls = [frames[k * n:(k + 1) * n] for k in range(ncalls)]
         B, _, H, W = frames[0].shape
         dev = frames[0].device
+        recompute = _checkpointing_of(model) == "recompute"
         with torch.cuda.device(dev):
             outs = [torch.empty_like(frames[0]) for _ in range(ncalls)]
-            fr = ops.make_frames(calls, outs)
-            nbytes = lib().bin_backbone_train_workspace_bytes(n, B * ncalls, H, W)
-            save = torch.empty(nbytes, dtype=torch.uint8, device=dev)          # owned by this node until backward
-            check(lib().bin_backbone_fwd_train(n, model.packed_blob().data_ptr(), C.byref(fr), H, W, save.data_ptr(),
-                                               save.numel(), _stream()))
-        ctx.model, ctx.ncalls, ctx.save, ctx.shape = model, ncalls, save, (B, H, W)
+            if recompute:
+                _inference_fwd(model, calls, outs, B, H, W, dev)
+                save = None
+            else:
+                fr = ops.make_frames(calls, outs)
+                nbytes = lib().bin_backbone_train_workspace_bytes(n, B * ncalls, H, W)
+                save = torch.empty(nbytes, dtype=torch.uint8, device=dev)          # owned by this node until backward
+                check(lib().bin_backbone_fwd_train(n, model.packed_blob().data_ptr(), C.byref(fr), H, W, save.data_ptr(),
+                                                   save.numel(), _stream()))
+        ctx.model, ctx.ncalls, ctx.save, ctx.shape, ctx.dev = model, ncalls, save, (B, H, W), dev
+        ctx.recompute_key = _input_key(model, frames) if recompute else None
         ctx.frames_keepalive = frames
         return tuple(outs)
 
     @staticmethod
     def backward(ctx, *gouts):
         model, ncalls, (B, H, W) = ctx.model, ctx.ncalls, ctx.shape
-        if ctx.save is None:
+        recompute = ctx.recompute_key is not None
+        if recompute:
+            # every input of the recomputation is still held (frames_keepalive, the weights), so a second backward
+            # (retain_graph) recomputes the same activations and gives the same gradients
+            if _input_key(model, ctx.frames_keepalive) != ctx.recompute_key:
+                raise BinB200Error("bin_b200: a backbone weight or input frame was modified in place between the forward "
+                                   "and the backward; activation recomputation would give wrong gradients")
+        elif ctx.save is None:
             raise BinB200Error("bin_b200: backward through a backbone stage twice (retain_graph / double backward) is not "
                                "supported: the saved activations are released after the first backward")
         n = model.NFRAMES
-        dev = ctx.save.device
+        dev = ctx.dev
         with torch.cuda.device(dev):
             gouts = [torch.zeros((B, 3, H, W), device=dev) if g is None else g.contiguous().float() for g in gouts]
             sbuf = torch.empty(2, device=dev)                                    # [scale, scratch]; stays on the device
@@ -77,9 +112,19 @@ class BackboneStageFn(torch.autograd.Function):
             dfr = ops.make_frames(dframes, [None] * ncalls)
             gparams = torch.zeros(lib().bin_backbone_grad_param_floats(n), device=dev)
             gws = torch.empty(lib().bin_backbone_grad_workspace_bytes(n, B * ncalls, H, W), dtype=torch.uint8, device=dev)
-            check(lib().bin_backbone_bwd(n, _packed_t(model).data_ptr(), C.byref(dout), C.byref(dfr), H, W,
-                                         ctx.save.data_ptr(), gws.data_ptr(), gws.numel(), gparams.data_ptr(),
-                                         scale.data_ptr(), _stream()))
+            if recompute:
+                frames = ctx.frames_keepalive
+                calls = [frames[k * n:(k + 1) * n] for k in range(ncalls)]
+                scratch = [torch.empty_like(frames[0]) for _ in range(ncalls)]   # the forward's outputs stay untouched
+                ws = _inference_fwd(model, calls, scratch, B, H, W, dev)
+                check(lib().bin_backbone_bwd_recompute(n, model.packed_blob().data_ptr(), _packed_t(model).data_ptr(),
+                                                       C.byref(dout), C.byref(dfr), H, W, ws.data_ptr(), ws.numel(),
+                                                       gws.data_ptr(), gws.numel(), gparams.data_ptr(), scale.data_ptr(),
+                                                       _stream()))
+            else:
+                check(lib().bin_backbone_bwd(n, _packed_t(model).data_ptr(), C.byref(dout), C.byref(dfr), H, W,
+                                             ctx.save.data_ptr(), gws.data_ptr(), gws.numel(), gparams.data_ptr(),
+                                             scale.data_ptr(), _stream()))
         ctx.save = None
         pgrads, off = [], 0
         for p in model._conv_params():

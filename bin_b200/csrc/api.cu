@@ -250,27 +250,36 @@ static std::vector<Band> plan_bands(int Btot, int h, int w) {
 // The last conv and the LFF run as one kernel (rdb_tail.cu) in fp16 inference; training keeps them apart because the
 // backward needs the fourth growth map, and the split-fp16 mode has no fused variant.  BIN_B200_FUSE_LFF=0 disables it.
 static bool fuse_lff_enabled() { return options().fuse_lff; }
+// The first `nconv` growth convs of RDB i over one band (RDN.py:141-147): conv3x3 + ReLU of cat(x, g planes so far)
+// into g planes [g_plane0 + 4c, +4).  The forward runs them in run_rdb; the recomputing backward runs all four again.
+static int run_growth(const void* blob, const BackboneLayout& L, int i, const bin_act_t& xin, int x_plane0,
+                      const bin_act_t& g, int g_plane0, int nconv, const Band& bd, cudaStream_t s, int x3) {
+  const int base = 2 + i * (kCgrow + 1);
+  const int h = xin.H;
+  for (int c = 0; c < nconv; ++c) {
+    bin_conv_args_t a = conv_args(blob, L.conv[base + c], x3);
+    a.in0 = xin; a.in0_plane0 = x_plane0; a.in0_planes = 12;
+    a.in1 = g; a.in1_plane0 = g_plane0; a.in1_planes = 4 * c;
+    a.relu = 1; a.epilogue = BIN_EPI_P8;
+    a.out = g; a.out_plane0 = g_plane0 + 4 * c;
+    const int ext = kCgrow - 1 - c;             // rows still needed by the convs downstream in this band
+    const int lo = bd.y0 - ext < 0 ? 0 : bd.y0 - ext, hi = bd.y1 + ext > h ? h : bd.y1 + ext;
+    a.b_begin = bd.b0; a.b_count = bd.nb; a.y_begin = lo; a.y_count = hi - lo;
+    // zigzag: conv0 forward, conv1 backward, conv2 forward, tail backward -- every launch starts on the tiles its
+    // predecessor touched last, which are the ones still in the 50 MB L2 (the tail ends at tile 0, where the next
+    // RDB's conv0 starts)
+    BIN_TRY(launch_conv(a, s, options().zigzag && (c & 1)));
+  }
+  return BIN_OK;
+}
+
 static int run_rdb(const void* blob, const BackboneLayout& L, int i, const bin_act_t& xin, int x_plane0,
                    const bin_act_t& g, const bin_act_t& out, int out_plane0, const std::vector<Band>& bands,
                    cudaStream_t s, int g_plane0 = 0, int x3 = 0, bool keep_growth = false) {
   const int base = 2 + i * (kCgrow + 1);
-  const int h = xin.H;
   const bool fuse = !x3 && !keep_growth && fuse_lff_enabled();
   for (const Band& bd : bands) {
-    for (int c = 0; c < (fuse ? kCgrow - 1 : kCgrow); ++c) {
-      bin_conv_args_t a = conv_args(blob, L.conv[base + c], x3);
-      a.in0 = xin; a.in0_plane0 = x_plane0; a.in0_planes = 12;
-      a.in1 = g; a.in1_plane0 = g_plane0; a.in1_planes = 4 * c;
-      a.relu = 1; a.epilogue = BIN_EPI_P8;
-      a.out = g; a.out_plane0 = g_plane0 + 4 * c;
-      const int ext = kCgrow - 1 - c;             // rows still needed by the convs downstream in this band
-      const int lo = bd.y0 - ext < 0 ? 0 : bd.y0 - ext, hi = bd.y1 + ext > h ? h : bd.y1 + ext;
-      a.b_begin = bd.b0; a.b_count = bd.nb; a.y_begin = lo; a.y_count = hi - lo;
-      // zigzag: conv0 forward, conv1 backward, conv2 forward, tail backward -- every launch starts on the tiles its
-      // predecessor touched last, which are the ones still in the 50 MB L2 (the tail ends at tile 0, where the next
-      // RDB's conv0 starts)
-      BIN_TRY(launch_conv(a, s, options().zigzag && (c & 1)));
-    }
+    BIN_TRY(run_growth(blob, L, i, xin, x_plane0, g, g_plane0, fuse ? kCgrow - 1 : kCgrow, bd, s, x3));
     if (fuse) {
       const ConvSpec& c3 = L.conv[base + kCgrow - 1];
       const ConvSpec& lf = L.conv[base + kCgrow];
@@ -446,17 +455,27 @@ static GradParamLayout grad_param_layout(int nframes) {
   return g;
 }
 
+// act_ws holds the forward's activations.  recompute_blob == NULL: the saving layout of bin_backbone_fwd_train, with the
+// growth maps of all 12 RDBs (its size is the caller's; act_ws_bytes is not checked).  Otherwise: the inference layout
+// that bin_backbone_fwd left, checked against act_ws_bytes; before RDB i's backward its four growth convs are re-run
+// from cat[i-1] (f2 for RDB 0) with the forward weights in recompute_blob, into growth planes 0..15.  Same inputs, same
+// weights and the same launches as the saving forward, so the rebuilt maps have the same bits, and every launch of the
+// backward reads the same operands in both layouts.
 static int run_backbone_bwd(int nframes, const void* blob_t, const bin_frames_t& dout, const bin_frames_t& dfr, int H,
-                            int W, const void* save_ws, void* gws_ptr, size_t gws_bytes, float* gparams,
-                            const float* scale, cudaStream_t s) {
+                            int W, const void* act_ws, size_t act_ws_bytes, const void* recompute_blob, void* gws_ptr,
+                            size_t gws_bytes, float* gparams, const float* scale, cudaStream_t s) {
   if (!valid_nframes(nframes) || dfr.nframes != nframes) return fail(BIN_ERR_ARG, "backbone_bwd: nframes must be 2, 3 or 5");
   if (dout.ncalls != dfr.ncalls || dout.Bc != dfr.Bc || dout.ncalls < 1 || dout.ncalls > BIN_MAX_CALLS)
     return fail(BIN_ERR_ARG, "backbone_bwd: bad call tables");
   const int Btot = dout.ncalls * dout.Bc;
+  const bool recompute = recompute_blob != nullptr;
+  const BackboneWs ws = backbone_ws(nframes, Btot, H, W, const_cast<void*>(act_ws), !recompute);
+  if (recompute && ws.bytes > act_ws_bytes) return fail(BIN_ERR_WORKSPACE, "backbone_bwd: forward workspace too small");
+  if (recompute && (reinterpret_cast<uintptr_t>(act_ws) & 255) != 0)
+    return fail(BIN_ERR_ARG, "backbone_bwd: forward workspace must be 256-byte aligned");
   const BackboneLayout L = backbone_layout(nframes);
   const BackboneLayoutT T = backbone_layout_t(nframes);
   const GradParamLayout GP = grad_param_layout(nframes);
-  const BackboneWs ws = backbone_ws(nframes, Btot, H, W, const_cast<void*>(save_ws), true);
   const GradWs gw = grad_ws(nframes, Btot, H, W, gws_ptr);
   if (gw.bytes > gws_bytes) return fail(BIN_ERR_WORKSPACE, "backbone_bwd: gradient workspace too small");
   const float* zero_bias = (const float*)((const uint8_t*)blob_t + T.zero_bias_off);
@@ -493,6 +512,7 @@ static int run_backbone_bwd(int nframes, const void* blob_t, const bin_frames_t&
   BIN_TRY(wgrad(62, ws.cat, 0, 12 * kD, none, 0, 0, gw.dt1, 0));                     // GFF.0
   BIN_TRY(dgrad(T.x[62], gw.dt1, 0, 12, gw.dcat, 0, 12 * kD, false));
   BIN_CUDA_OK(cudaMemsetAsync(gw.df2.ptr, 0, (size_t)Btot * 12 * (H / 2) * (W / 2) * 16, s));
+  const std::vector<Band> bands = recompute ? plan_bands(Btot, H / 2, W / 2) : std::vector<Band>();
   for (int i = kD - 1; i >= 0; --i) {
     const int base = 2 + i * (kCgrow + 1);
     const bin_act_t& xin = i == 0 ? ws.f2 : ws.cat;           // forward input of RDB i
@@ -500,13 +520,15 @@ static int run_backbone_bwd(int nframes, const void* blob_t, const bin_frames_t&
     const bin_act_t& dxin = i == 0 ? gw.df2 : gw.dcat;        // its gradient (accumulated)
     const int dxin_p = i == 0 ? 0 : 12 * (i - 1);
     const int dxo_p = 12 * i;                                 // d x_{i+1}, complete at this point
-    BIN_TRY(wgrad(base + kCgrow, xin, xin_p, 12, ws.g, 16 * i, 16, gw.dcat, dxo_p));                 // LFF
+    const int gp0 = recompute ? 0 : 16 * i;                   // growth maps of RDB i
+    for (const Band& bd : bands) BIN_TRY(run_growth(recompute_blob, L, i, xin, xin_p, ws.g, 0, kCgrow, bd, s, 0));
+    BIN_TRY(wgrad(base + kCgrow, xin, xin_p, 12, ws.g, gp0, 16, gw.dcat, dxo_p));                     // LFF
     BIN_TRY(launch_p8_add(dxin, dxin_p, gw.dcat, dxo_p, 12, s));                                      // residual (RDN.py:165)
     BIN_TRY(dgrad(T.x[base + kCgrow], gw.dcat, dxo_p, 12, dxin, dxin_p, 12, true));
     BIN_TRY(dgrad(T.g[base + kCgrow], gw.dcat, dxo_p, 12, gw.dg, 0, 16, false));
     for (int c = kCgrow - 1; c >= 0; --c) {
-      BIN_TRY(launch_relu_mask(gw.dg, 4 * c, ws.g, 16 * i + 4 * c, 4, s));                            // RDN.py:142
-      BIN_TRY(wgrad(base + c, xin, xin_p, 12, ws.g, 16 * i, 4 * c, gw.dg, 4 * c));
+      BIN_TRY(launch_relu_mask(gw.dg, 4 * c, ws.g, gp0 + 4 * c, 4, s));                               // RDN.py:142
+      BIN_TRY(wgrad(base + c, xin, xin_p, 12, ws.g, gp0, 4 * c, gw.dg, 4 * c));
       BIN_TRY(dgrad(T.x[base + c], gw.dg, 4 * c, 4, dxin, dxin_p, 12, true));
       if (c > 0) BIN_TRY(dgrad(T.g[base + c], gw.dg, 4 * c, 4, gw.dg, 0, 4 * c, true));
     }
@@ -702,8 +724,17 @@ int bin_backbone_bwd(int nframes, const void* blob_t, const bin_frames_t* dout, 
                      const float* scale_dev, bin_stream_t s) {
   if (!blob_t || !dout || !dframes || !save_ws || !grad_params || !scale_dev)
     return fail(BIN_ERR_ARG, "backbone_bwd: null argument");
-  return run_backbone_bwd(nframes, blob_t, *dout, *dframes, H, W, save_ws, grad_ws_ptr, grad_ws_bytes, grad_params,
-                          scale_dev, (cudaStream_t)s);
+  return run_backbone_bwd(nframes, blob_t, *dout, *dframes, H, W, save_ws, 0, nullptr, grad_ws_ptr, grad_ws_bytes,
+                          grad_params, scale_dev, (cudaStream_t)s);
+}
+int bin_backbone_bwd_recompute(int nframes, const void* blob, const void* blob_t, const bin_frames_t* dout,
+                               const bin_frames_t* dframes, int H, int W, const void* fwd_ws, size_t fwd_ws_bytes,
+                               void* grad_ws_ptr, size_t grad_ws_bytes, float* grad_params, const float* scale_dev,
+                               bin_stream_t s) {
+  if (!blob || !blob_t || !dout || !dframes || !fwd_ws || !grad_params || !scale_dev)
+    return fail(BIN_ERR_ARG, "backbone_bwd: null argument");
+  return run_backbone_bwd(nframes, blob_t, *dout, *dframes, H, W, fwd_ws, fwd_ws_bytes, blob, grad_ws_ptr, grad_ws_bytes,
+                          grad_params, scale_dev, (cudaStream_t)s);
 }
 
 int bin_grad_scale(const float* const* gouts_host, int n, size_t numel, float target, float* scale_dev, void* tmp4_dev,

@@ -22,7 +22,8 @@ import torch.nn.init as weight_init
 from . import _lib, ops
 from ._lib import BinB200Error, Net, check, lib
 
-__all__ = ["set_precision", "set_self_ensemble", "ConvLSTMCell", "pixel_reshuffle", "RDB_Conv", "RDB", "RDN_residual_interp_2_input",
+__all__ = ["set_precision", "set_self_ensemble", "set_activation_checkpointing", "ConvLSTMCell", "pixel_reshuffle", "RDB_Conv", "RDB",
+           "RDN_residual_interp_2_input",
            "RDN_residual_interp_2_1_input", "RDN_residual_interp_4_1_input", "RDN_residual_interp_5_input",
            "RDN_residual_interp_5_input_ConvLSTM_L", "bin_stage4_lstm"]
 
@@ -264,6 +265,33 @@ def set_precision(net: nn.Module, precision: str) -> nn.Module:
         raise BinB200Error(f"unknown precision {precision!r}; use 'fp16' or 'fp32'")
     for m in net.modules():
         m.precision = precision
+    return net
+
+
+CHECKPOINTING = (None, "recompute")
+
+
+def _checkpointing_of(module) -> Optional[str]:
+    mode = getattr(module, "activation_checkpointing", None)
+    if mode not in CHECKPOINTING:
+        raise BinB200Error(f"unknown activation checkpointing mode {mode!r}; use None or 'recompute'")
+    return mode
+
+
+def set_activation_checkpointing(net: nn.Module, mode: Optional[str]) -> nn.Module:
+    """Choose what a grad-enabled forward keeps for the backward, for every module in `net.modules()` (so a DataParallel
+    wrapper or a module holding the net works).  None (the default): each batched backbone stage keeps its training
+    workspace, growth maps of all 12 RDBs included, until its backward.  "recompute": each stage keeps only its input
+    frames; its backward re-runs the inference forward and rebuilds each RDB's growth maps, so a step holds one stage's
+    activations at a time instead of all of them, at the price of extra forward work.  Every kernel sees the same
+    operands in both modes: outputs, frame gradients and conv weight gradients are bit-identical, and the values that
+    existing kernels sum with float atomics (loss terms, bias and ConvLSTM gradients) vary only in their last bits, as
+    they do from run to run in either mode.  A plain attribute, not a parameter or buffer: the state_dict is
+    unchanged."""
+    if mode not in CHECKPOINTING:
+        raise BinB200Error(f"unknown activation checkpointing mode {mode!r}; use None or 'recompute'")
+    for m in net.modules():
+        m.activation_checkpointing = mode
     return net
 
 

@@ -33,7 +33,7 @@
 extern "C" {
 #endif
 
-#define BIN_ABI_VERSION 2
+#define BIN_ABI_VERSION 3
 #define BIN_MAX_CALLS 6   /* same-weight backbone calls batched along N */
 #define BIN_MAX_FRAMES 5  /* frames per backbone call (2, 3 or 5) */
 #define BIN_MAX_LOSS_PAIRS 20 /* (prediction, target) pairs of one fused loss call */
@@ -176,6 +176,17 @@ size_t bin_backbone_grad_param_floats(int nframes);          /* fp32 [w0,b0,w1,b
 int bin_backbone_bwd(int nframes, const void* blob_t, const bin_frames_t* dout, const bin_frames_t* dframes, int H, int W,
                      const void* save_ws, void* grad_ws, size_t grad_ws_bytes, float* grad_params,
                      const float* scale_dev, bin_stream_t s);
+/* The same backward from the INFERENCE workspace (activation recomputation): fwd_ws (fwd_ws_bytes >=
+ * bin_backbone_workspace_bytes) is what bin_backbone_fwd with `blob` just left for the same frames, which keeps every
+ * activation the backward reads except the growth maps of the 12 RDBs.  Before each RDB's backward its four growth convs
+ * are re-run from its input with `blob`, into the workspace's one RDB of growth scratch.  Every launch then reads the
+ * operands that bin_backbone_bwd reads after bin_backbone_fwd_train, so the frame and weight gradients have the same bits
+ * (the bias gradients are summed with float atomics in both); grad_ws, grad_params and scale_dev are as there.  A NULL pointer, an
+ * undersized or unaligned fwd_ws fail (BIN_ERR_ARG / BIN_ERR_WORKSPACE) before any launch. */
+int bin_backbone_bwd_recompute(int nframes, const void* blob, const void* blob_t, const bin_frames_t* dout,
+                               const bin_frames_t* dframes, int H, int W, const void* fwd_ws, size_t fwd_ws_bytes,
+                               void* grad_ws, size_t grad_ws_bytes, float* grad_params, const float* scale_dev,
+                               bin_stream_t s);
 /* Loss scale for one backbone backward: *scale_dev = 2^floor(log2(target / max_k max|gouts[k]|)) (a power of two, so
  * scaling and un-scaling are exact), computed on the device -- no host synchronisation.  gouts_host: host array of n
  * (<= BIN_MAX_CALLS) device pointers to fp32 tensors of `numel` elements, 16-byte aligned; tmp4_dev: 4 bytes of scratch. */
