@@ -15,7 +15,8 @@ BIN_FLIPX4_MAX_TENSORS = 14
 BIN_TRAIN_MAX_BATCH = 16
 BIN_TRAIN_FRAMES = 17
 EPI_P8, EPI_PIXSHUF, EPI_FINAL = 0, 1, 2
-ABI_VERSION = 3
+BIN_DETERMINISTIC = 1                 # flags bit of the *_ex entry points
+ABI_VERSION = 4
 
 
 class Act(C.Structure):
@@ -68,6 +69,8 @@ _SIGS = {
                                 C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "bin_convlstm_fwd": (C.c_int, [C.c_void_p] * 7 + [C.c_int] * 3 + [C.c_void_p]),
     "bin_convlstm_bwd": (C.c_int, [C.c_void_p] * 13 + [C.c_int] * 3 + [C.c_void_p]),
+    "bin_convlstm_bwd_scratch_bytes": (C.c_size_t, [C.c_int] * 3),
+    "bin_convlstm_bwd_ex": (C.c_int, [C.c_void_p] * 13 + [C.c_int] * 4 + [C.c_void_p, C.c_size_t, C.c_void_p]),
     "bin_backbone_packed_bytes": (C.c_size_t, [C.c_int]),
     "bin_backbone_pack": (C.c_int, [C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_void_p, C.c_void_p]),
     "bin_backbone_workspace_bytes": (C.c_size_t, [C.c_int] * 4),
@@ -83,6 +86,11 @@ _SIGS = {
     "bin_backbone_bwd_recompute": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.POINTER(Frames), C.POINTER(Frames), C.c_int,
                                              C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p,
                                              C.c_void_p, C.c_void_p]),
+    "bin_backbone_bwd_ex": (C.c_int, [C.c_int, C.c_void_p, C.POINTER(Frames), C.POINTER(Frames), C.c_int, C.c_int, C.c_void_p,
+                                      C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
+    "bin_backbone_bwd_recompute_ex": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.POINTER(Frames), C.POINTER(Frames), C.c_int,
+                                                C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p,
+                                                C.c_void_p, C.c_int, C.c_void_p]),
     "bin_grad_scale": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_size_t, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]),
     "bin_rdb_fwd": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
                               C.c_void_p, C.c_size_t, C.c_void_p]),
@@ -99,6 +107,9 @@ _SIGS = {
     "bin_pyramid3_fwd": (C.c_int, [C.POINTER(Net), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_int, C.c_int,
                                    C.c_int, C.c_void_p, C.c_size_t, C.c_void_p]),
     "bin_pixel_loss_fwd": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_int, C.c_size_t, C.c_int, C.c_float, C.c_void_p, C.c_void_p]),
+    "bin_pixel_loss_scratch_bytes": (C.c_size_t, [C.c_int, C.c_size_t]),
+    "bin_pixel_loss_fwd_ex": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_int, C.c_size_t, C.c_int, C.c_float,
+                                        C.c_void_p, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p]),
     "bin_pixel_loss_bwd": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_int,
                                     C.c_size_t, C.c_int, C.c_float, C.c_void_p, C.c_void_p]),
     "bin_tensor2img_u8": (C.c_int, [C.c_void_p] + [C.c_int] * 6 + [C.c_void_p, C.c_void_p]),

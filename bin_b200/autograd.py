@@ -22,6 +22,13 @@ def _stream() -> int:
     return torch.cuda.current_stream().cuda_stream
 
 
+def deterministic_flags() -> int:
+    """BIN_DETERMINISTIC when torch.use_deterministic_algorithms(True) is in force, read at the call that reduces: the loss,
+    bias and ConvLSTM gradient sums then run in a fixed order and the weight gradients on a grid independent of the SM
+    count (DESIGN.md §4f).  0 otherwise: the default atomic sums."""
+    return _lib.BIN_DETERMINISTIC if torch.are_deterministic_algorithms_enabled() else 0
+
+
 def _packed_t(model) -> torch.Tensor:
     ps = model._conv_params()
     key = (ps[0].device.index,) + tuple((p.data_ptr(), p._version) for p in ps)
@@ -100,6 +107,7 @@ class BackboneStageFn(torch.autograd.Function):
                                "supported: the saved activations are released after the first backward")
         n = model.NFRAMES
         dev = ctx.dev
+        flags = deterministic_flags()
         with torch.cuda.device(dev):
             gouts = [torch.zeros((B, 3, H, W), device=dev) if g is None else g.contiguous().float() for g in gouts]
             sbuf = torch.empty(2, device=dev)                                    # [scale, scratch]; stays on the device
@@ -117,14 +125,14 @@ class BackboneStageFn(torch.autograd.Function):
                 calls = [frames[k * n:(k + 1) * n] for k in range(ncalls)]
                 scratch = [torch.empty_like(frames[0]) for _ in range(ncalls)]   # the forward's outputs stay untouched
                 ws = _inference_fwd(model, calls, scratch, B, H, W, dev)
-                check(lib().bin_backbone_bwd_recompute(n, model.packed_blob().data_ptr(), _packed_t(model).data_ptr(),
-                                                       C.byref(dout), C.byref(dfr), H, W, ws.data_ptr(), ws.numel(),
-                                                       gws.data_ptr(), gws.numel(), gparams.data_ptr(), scale.data_ptr(),
-                                                       _stream()))
+                check(lib().bin_backbone_bwd_recompute_ex(n, model.packed_blob().data_ptr(), _packed_t(model).data_ptr(),
+                                                          C.byref(dout), C.byref(dfr), H, W, ws.data_ptr(), ws.numel(),
+                                                          gws.data_ptr(), gws.numel(), gparams.data_ptr(), scale.data_ptr(),
+                                                          flags, _stream()))
             else:
-                check(lib().bin_backbone_bwd(n, _packed_t(model).data_ptr(), C.byref(dout), C.byref(dfr), H, W,
-                                             ctx.save.data_ptr(), gws.data_ptr(), gws.numel(), gparams.data_ptr(),
-                                             scale.data_ptr(), _stream()))
+                check(lib().bin_backbone_bwd_ex(n, _packed_t(model).data_ptr(), C.byref(dout), C.byref(dfr), H, W,
+                                                ctx.save.data_ptr(), gws.data_ptr(), gws.numel(), gparams.data_ptr(),
+                                                scale.data_ptr(), flags, _stream()))
         ctx.save = None
         pgrads, off = [], 0
         for p in model._conv_params():
@@ -173,10 +181,14 @@ class ConvLSTMFn(torch.autograd.Function):
             dhp = torch.empty_like(x) if ctx.has_state else None
             dw = torch.zeros_like(w)
             db = torch.zeros_like(b)
+            flags = deterministic_flags()
+            scratch = (torch.empty(lib().bin_convlstm_bwd_scratch_bytes(B, H, W), dtype=torch.uint8, device=dev)
+                       if flags else None)
             P = lambda t: None if t is None else t.data_ptr()
-            check(lib().bin_convlstm_bwd(x.data_ptr(), P(cp), P(hp), w.data_ptr(), b.data_ptr(), P(dh), P(dc),
-                                         dgates.data_ptr(), dx.data_ptr(), P(dcp), P(dhp), dw.data_ptr(), db.data_ptr(),
-                                         B, H, W, _stream()))
+            check(lib().bin_convlstm_bwd_ex(x.data_ptr(), P(cp), P(hp), w.data_ptr(), b.data_ptr(), P(dh), P(dc),
+                                            dgates.data_ptr(), dx.data_ptr(), P(dcp), P(dhp), dw.data_ptr(), db.data_ptr(),
+                                            B, H, W, flags, P(scratch), 0 if scratch is None else scratch.numel(),
+                                            _stream()))
         return dx, dw, db, dcp, dhp
 
 

@@ -28,6 +28,8 @@ static Options read_options() {
   o.stage_mmas = (e = env("BIN_B200_STAGE_MMAS")) ? atoi(e) : 12;
   if (o.stage_mmas < 1) o.stage_mmas = 12;
   o.band_budget = (e = env("BIN_B200_BAND_BUDGET_KB")) ? (size_t)atoll(e) << 10 : (~(size_t)0 >> 1);
+  o.max_sms = (e = env("BIN_B200_MAX_SMS")) ? atoi(e) : 0;
+  if (o.max_sms < 0) o.max_sms = 0;
   return o;
 }
 const Options& options() {
@@ -43,6 +45,8 @@ int num_sms() {
   if (v == 0) {
     cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
     if (v <= 0) v = 132;
+    const int cap = options().max_sms;          // lowers the grids the library picks, nothing on the device
+    if (cap > 0 && cap < v) v = cap;
     cache[dev & 63].store(v, std::memory_order_relaxed);
   }
   return v;
@@ -66,8 +70,9 @@ int pack_batch_add_bias(void* hb, const float* b, int cout, int cout_pad, float*
 int pack_batch_launch(void* hb, cudaStream_t s);   // launches and frees the batch
 int launch_convlstm(const float* x, const float* c_prev, const float* h_prev, const float* w, const float* b,
                     float* h_out, float* c_out, int B, int H, int W, cudaStream_t s);
+size_t pixel_loss_scratch_bytes(int npairs, size_t n);
 int launch_pixel_loss_fwd(const float* const* a, const float* const* b, int npairs, size_t n, int kind, float eps,
-                          float* pair_loss, cudaStream_t s);
+                          float* pair_loss, cudaStream_t s, int flags, void* scratch, size_t scratch_bytes);
 int launch_pixel_loss_bwd(const float* const* a, const float* const* b, float* const* da, float* const* db, int npairs,
                           size_t n, int kind, float eps, const float* upstream, cudaStream_t s);
 int launch_adam_step(const bin_adam_tensor_t* table, const int* chunk_prefix, int ntensors, int nchunks, float lr,
@@ -86,9 +91,11 @@ int launch_rdb_tail(const bin_act_t& x, int x_plane0, const bin_act_t& g, int g_
                     int b_begin, int b_count, int y_begin, int y_count, cudaStream_t s, bool reverse = false);
 int launch_tensor2img_u8(const float* x, int Hs, int Ws, int top, int left, int h, int w, uint8_t* out, cudaStream_t s);
 int launch_u8_to_frame(const uint8_t* img, int h, int w, int pl, int pr, int pt, int pb, float* out, cudaStream_t s);
+size_t convlstm_bwd_scratch_bytes(int B, int H, int W);
 int launch_convlstm_bwd(const float* x, const float* c_prev, const float* h_prev, const float* w, const float* b,
                         const float* dh, const float* dc, float* dgates_ws, float* dx, float* dc_prev, float* dh_prev,
-                        float* dw, float* db, int B, int H, int W, cudaStream_t s);
+                        float* dw, float* db, int B, int H, int W, cudaStream_t s, int flags, void* scratch,
+                        size_t scratch_bytes);
 
 static inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
@@ -366,11 +373,18 @@ int launch_pixel_unshuffle(const bin_act_t& du, const bin_act_t& dst, cudaStream
 int launch_unpack_frames_grad(const bin_act_t& dx0, const bin_frames_t& dout, const bin_frames_t& dfr, int H, int W,
                               const float* scale, cudaStream_t s);
 int launch_grad_out_to_p8(const bin_frames_t& dout, int H, int W, const bin_act_t& dst, const float* scale, cudaStream_t s);
-int launch_bias_grad(const bin_act_t& dy, int plane0, int C, const float* scale, float* db, cudaStream_t s);
+// partial == NULL: atomic per-block sums; otherwise the deterministic two-launch reduction through `partial`
+size_t bias_grad_partial_floats(int B, int hw, int C);
+int launch_bias_grad(const bin_act_t& dy, int plane0, int C, const float* scale, float* db, cudaStream_t s,
+                     float* partial = nullptr, size_t partial_floats = 0);
 int launch_wgrad(const bin_act_t& x0, int x0_plane0, int x0_planes, const bin_act_t& x1, int x1_plane0, int x1_planes,
                  const bin_act_t& dy, int dy_plane0, int cout, int cin, int ks, const float* scale, float* dw,
-                 float* partial_ws, cudaStream_t s);
-static size_t wgrad_partial_bytes() { return (size_t)num_sms() * 128 * 512 * sizeof(float); }   // per-CTA accumulator slabs (grid = #SMs)
+                 float* partial_ws, cudaStream_t s, bool det = false);
+// per-CTA accumulator slabs: grid = #SMs by default, kDetCtas in deterministic mode
+static size_t wgrad_partial_bytes() {
+  const int ctas = num_sms() > kDetCtas ? num_sms() : kDetCtas;
+  return (size_t)ctas * 128 * 512 * sizeof(float);
+}
 
 struct TSpec {          // one data-gradient conv: output rows [row0,row0+nrows) of the forward conv's Cin axis
   int conv, row0, nrows, cout_pad_t, cin_pad_t, ks;
@@ -413,9 +427,16 @@ static BackboneLayoutT backbone_layout_t(int nframes) {
 
 struct GradWs {
   bin_act_t dout16, du, dup0, dt2, dt1, dcat, df2, dg, dx0;
-  float* wg_partial;
+  float* wg_partial;          // wgrad slabs; in deterministic mode also the bias-gradient partials (stream-ordered reuse)
+  size_t wg_partial_floats;
   size_t bytes;
 };
+// Largest bias-gradient partial array of one backward: UPNet.2 (3 channels, full resolution) or UPNet.0 (256 channels,
+// low resolution).  It fits the wgrad slabs for every shape a card can train; the region grows if it does not.
+static size_t bias_partial_bytes(int Btot, int H, int W) {
+  const size_t a = bias_grad_partial_floats(Btot, H * W, 3), b = bias_grad_partial_floats(Btot, (H / 2) * (W / 2), 256);
+  return (a > b ? a : b) * sizeof(float);
+}
 static GradWs grad_ws(int nframes, int Btot, int H, int W, void* base) {
   GradWs w;
   const int h = H / 2, wd = W / 2;
@@ -437,7 +458,9 @@ static GradWs grad_ws(int nframes, int Btot, int H, int W, void* base) {
   w.dg = carve(16, h, wd);
   w.dx0 = carve((int)align_up(12 * nframes, kKC) / 8, h, wd);
   w.wg_partial = base ? (float*)((uint8_t*)base + off) : nullptr;
-  off = align_up(off + wgrad_partial_bytes(), 256);
+  const size_t wgb = wgrad_partial_bytes(), bb = bias_partial_bytes(Btot, H, W);
+  w.wg_partial_floats = (wgb > bb ? wgb : bb) / sizeof(float);
+  off = align_up(off + w.wg_partial_floats * sizeof(float), 256);
   w.bytes = off;
   return w;
 }
@@ -463,8 +486,10 @@ static GradParamLayout grad_param_layout(int nframes) {
 // backward reads the same operands in both layouts.
 static int run_backbone_bwd(int nframes, const void* blob_t, const bin_frames_t& dout, const bin_frames_t& dfr, int H,
                             int W, const void* act_ws, size_t act_ws_bytes, const void* recompute_blob, void* gws_ptr,
-                            size_t gws_bytes, float* gparams, const float* scale, cudaStream_t s) {
+                            size_t gws_bytes, float* gparams, const float* scale, cudaStream_t s, int flags) {
   if (!valid_nframes(nframes) || dfr.nframes != nframes) return fail(BIN_ERR_ARG, "backbone_bwd: nframes must be 2, 3 or 5");
+  if (flags & ~BIN_DETERMINISTIC) return fail(BIN_ERR_ARG, "backbone_bwd: unknown flags");
+  const bool det = flags & BIN_DETERMINISTIC;
   if (dout.ncalls != dfr.ncalls || dout.Bc != dfr.Bc || dout.ncalls < 1 || dout.ncalls > BIN_MAX_CALLS)
     return fail(BIN_ERR_ARG, "backbone_bwd: bad call tables");
   const int Btot = dout.ncalls * dout.Bc;
@@ -478,6 +503,14 @@ static int run_backbone_bwd(int nframes, const void* blob_t, const bin_frames_t&
   const GradParamLayout GP = grad_param_layout(nframes);
   const GradWs gw = grad_ws(nframes, Btot, H, W, gws_ptr);
   if (gw.bytes > gws_bytes) return fail(BIN_ERR_WORKSPACE, "backbone_bwd: gradient workspace too small");
+  // Deterministic bias partials of every conv must fit the slab region before the first launch (grad_ws sizes it from
+  // bias_partial_bytes; this keeps that invariant explicit should a conv with more partials ever be added).
+  if (det)
+    for (int i = 0; i < BIN_BACKBONE_NCONV; ++i) {
+      const int hw = i == BIN_BACKBONE_NCONV - 1 ? H * W : (H / 2) * (W / 2);   // UPNet.2 runs at full resolution
+      if (bias_grad_partial_floats(Btot, hw, L.conv[i].cout) > gw.wg_partial_floats)
+        return fail(BIN_ERR_WORKSPACE, "backbone_bwd: deterministic bias partials do not fit the gradient workspace");
+    }
   const float* zero_bias = (const float*)((const uint8_t*)blob_t + T.zero_bias_off);
 
   // dX (+)= conv(dY planes [dy_plane0, +dy_planes), V): writes `nstore` planes of `out` at out_plane0
@@ -492,12 +525,15 @@ static int run_backbone_bwd(int nframes, const void* blob_t, const bin_frames_t&
     if (accumulate) { a.res = out; a.res_plane0 = out_plane0; }
     return launch_conv(a, s);
   };
-  // dW += X^T dY, db += sum dY for forward conv `idx`
+  // dW += X^T dY, db += sum dY for forward conv `idx`.  Deterministic mode: the bias partials use the wgrad slabs, which
+  // the stream frees again before the wgrad that follows writes them.
   auto wgrad = [&](int idx, const bin_act_t& x0, int x0p, int x0n, const bin_act_t& x1, int x1p, int x1n,
                    const bin_act_t& dy, int dyp) -> int {
     const ConvSpec& c = L.conv[idx];
-    BIN_TRY(launch_bias_grad(dy, dyp, c.cout, scale, gparams + GP.b[idx], s));
-    return launch_wgrad(x0, x0p, x0n, x1, x1p, x1n, dy, dyp, c.cout, c.cin, c.ks, scale, gparams + GP.w[idx], gw.wg_partial, s);
+    BIN_TRY(launch_bias_grad(dy, dyp, c.cout, scale, gparams + GP.b[idx], s, det ? gw.wg_partial : nullptr,
+                             gw.wg_partial_floats));
+    return launch_wgrad(x0, x0p, x0n, x1, x1p, x1n, dy, dyp, c.cout, c.cin, c.ks, scale, gparams + GP.w[idx], gw.wg_partial,
+                        s, det);
   };
   const bin_act_t none = {nullptr, 0, 0, 0, 0};
 
@@ -623,10 +659,17 @@ int bin_convlstm_fwd(const float* x, const float* c_prev, const float* h_prev, c
   return launch_convlstm(x, c_prev, h_prev, w, b, h_out, c_out, B, H, W, (cudaStream_t)s);
 }
 
+size_t bin_pixel_loss_scratch_bytes(int npairs, size_t n) { return pixel_loss_scratch_bytes(npairs, n); }
+int bin_pixel_loss_fwd_ex(const float* const* a_host, const float* const* b_host, int npairs, size_t n, int kind, float eps,
+                          float* pair_loss, int flags, void* scratch, size_t scratch_bytes, bin_stream_t s) {
+  if (!a_host || !b_host || !pair_loss) return fail(BIN_ERR_ARG, "pixel_loss_fwd: null argument");
+  if (flags & ~BIN_DETERMINISTIC) return fail(BIN_ERR_ARG, "pixel_loss_fwd: unknown flags");
+  return launch_pixel_loss_fwd(a_host, b_host, npairs, n, kind, eps, pair_loss, (cudaStream_t)s, flags, scratch,
+                               scratch_bytes);
+}
 int bin_pixel_loss_fwd(const float* const* a_host, const float* const* b_host, int npairs, size_t n, int kind, float eps,
                        float* pair_loss, bin_stream_t s) {
-  if (!a_host || !b_host || !pair_loss) return fail(BIN_ERR_ARG, "pixel_loss_fwd: null argument");
-  return launch_pixel_loss_fwd(a_host, b_host, npairs, n, kind, eps, pair_loss, (cudaStream_t)s);
+  return bin_pixel_loss_fwd_ex(a_host, b_host, npairs, n, kind, eps, pair_loss, 0, nullptr, 0, s);
 }
 int bin_pixel_loss_bwd(const float* const* a_host, const float* const* b_host, float* const* da_host, float* const* db_host,
                        int npairs, size_t n, int kind, float eps, const float* upstream, bin_stream_t s) {
@@ -641,11 +684,21 @@ int bin_u8_to_frame(const uint8_t* img, int h, int w, int pad_l, int pad_r, int 
   if (!img || !out) return fail(BIN_ERR_ARG, "u8_to_frame: null argument");
   return launch_u8_to_frame(img, h, w, pad_l, pad_r, pad_t, pad_b, out, (cudaStream_t)s);
 }
+size_t bin_convlstm_bwd_scratch_bytes(int B, int H, int W) { return convlstm_bwd_scratch_bytes(B, H, W); }
+int bin_convlstm_bwd_ex(const float* x, const float* c_prev, const float* h_prev, const float* w, const float* b,
+                        const float* dh, const float* dc, float* dgates_ws, float* dx, float* dc_prev, float* dh_prev,
+                        float* dw, float* db, int B, int H, int W, int flags, void* scratch, size_t scratch_bytes,
+                        bin_stream_t s) {
+  if (!x || !w || !b || !dgates_ws || !dx || !dw || !db) return fail(BIN_ERR_ARG, "convlstm_bwd: null argument");
+  if (flags & ~BIN_DETERMINISTIC) return fail(BIN_ERR_ARG, "convlstm_bwd: unknown flags");
+  return launch_convlstm_bwd(x, c_prev, h_prev, w, b, dh, dc, dgates_ws, dx, dc_prev, dh_prev, dw, db, B, H, W,
+                             (cudaStream_t)s, flags, scratch, scratch_bytes);
+}
 int bin_convlstm_bwd(const float* x, const float* c_prev, const float* h_prev, const float* w, const float* b,
                      const float* dh, const float* dc, float* dgates_ws, float* dx, float* dc_prev, float* dh_prev,
                      float* dw, float* db, int B, int H, int W, bin_stream_t s) {
-  if (!x || !w || !b || !dgates_ws || !dx || !dw || !db) return fail(BIN_ERR_ARG, "convlstm_bwd: null argument");
-  return launch_convlstm_bwd(x, c_prev, h_prev, w, b, dh, dc, dgates_ws, dx, dc_prev, dh_prev, dw, db, B, H, W, (cudaStream_t)s);
+  return bin_convlstm_bwd_ex(x, c_prev, h_prev, w, b, dh, dc, dgates_ws, dx, dc_prev, dh_prev, dw, db, B, H, W, 0, nullptr,
+                             0, s);
 }
 
 size_t bin_backbone_packed_bytes(int nframes) { return valid_nframes(nframes) ? backbone_layout(nframes).bytes : 0; }
@@ -719,22 +772,35 @@ size_t bin_backbone_grad_workspace_bytes(int nframes, int Btot, int H, int W) {
   return valid_nframes(nframes) ? grad_ws(nframes, Btot, H, W, nullptr).bytes : 0;
 }
 size_t bin_backbone_grad_param_floats(int nframes) { return valid_nframes(nframes) ? grad_param_layout(nframes).floats : 0; }
-int bin_backbone_bwd(int nframes, const void* blob_t, const bin_frames_t* dout, const bin_frames_t* dframes, int H, int W,
-                     const void* save_ws, void* grad_ws_ptr, size_t grad_ws_bytes, float* grad_params,
-                     const float* scale_dev, bin_stream_t s) {
+int bin_backbone_bwd_ex(int nframes, const void* blob_t, const bin_frames_t* dout, const bin_frames_t* dframes, int H,
+                        int W, const void* save_ws, void* grad_ws_ptr, size_t grad_ws_bytes, float* grad_params,
+                        const float* scale_dev, int flags, bin_stream_t s) {
   if (!blob_t || !dout || !dframes || !save_ws || !grad_params || !scale_dev)
     return fail(BIN_ERR_ARG, "backbone_bwd: null argument");
   return run_backbone_bwd(nframes, blob_t, *dout, *dframes, H, W, save_ws, 0, nullptr, grad_ws_ptr, grad_ws_bytes,
-                          grad_params, scale_dev, (cudaStream_t)s);
+                          grad_params, scale_dev, (cudaStream_t)s, flags);
+}
+int bin_backbone_bwd(int nframes, const void* blob_t, const bin_frames_t* dout, const bin_frames_t* dframes, int H, int W,
+                     const void* save_ws, void* grad_ws_ptr, size_t grad_ws_bytes, float* grad_params,
+                     const float* scale_dev, bin_stream_t s) {
+  return bin_backbone_bwd_ex(nframes, blob_t, dout, dframes, H, W, save_ws, grad_ws_ptr, grad_ws_bytes, grad_params,
+                             scale_dev, 0, s);
+}
+int bin_backbone_bwd_recompute_ex(int nframes, const void* blob, const void* blob_t, const bin_frames_t* dout,
+                                  const bin_frames_t* dframes, int H, int W, const void* fwd_ws, size_t fwd_ws_bytes,
+                                  void* grad_ws_ptr, size_t grad_ws_bytes, float* grad_params, const float* scale_dev,
+                                  int flags, bin_stream_t s) {
+  if (!blob || !blob_t || !dout || !dframes || !fwd_ws || !grad_params || !scale_dev)
+    return fail(BIN_ERR_ARG, "backbone_bwd: null argument");
+  return run_backbone_bwd(nframes, blob_t, *dout, *dframes, H, W, fwd_ws, fwd_ws_bytes, blob, grad_ws_ptr, grad_ws_bytes,
+                          grad_params, scale_dev, (cudaStream_t)s, flags);
 }
 int bin_backbone_bwd_recompute(int nframes, const void* blob, const void* blob_t, const bin_frames_t* dout,
                                const bin_frames_t* dframes, int H, int W, const void* fwd_ws, size_t fwd_ws_bytes,
                                void* grad_ws_ptr, size_t grad_ws_bytes, float* grad_params, const float* scale_dev,
                                bin_stream_t s) {
-  if (!blob || !blob_t || !dout || !dframes || !fwd_ws || !grad_params || !scale_dev)
-    return fail(BIN_ERR_ARG, "backbone_bwd: null argument");
-  return run_backbone_bwd(nframes, blob_t, *dout, *dframes, H, W, fwd_ws, fwd_ws_bytes, blob, grad_ws_ptr, grad_ws_bytes,
-                          grad_params, scale_dev, (cudaStream_t)s);
+  return bin_backbone_bwd_recompute_ex(nframes, blob, blob_t, dout, dframes, H, W, fwd_ws, fwd_ws_bytes, grad_ws_ptr,
+                                       grad_ws_bytes, grad_params, scale_dev, 0, s);
 }
 
 int bin_grad_scale(const float* const* gouts_host, int n, size_t numel, float target, float* scale_dev, void* tmp4_dev,

@@ -284,10 +284,24 @@ __global__ void grad_out_to_p8_kernel(const __grid_constant__ bin_frames_t dout,
     *reinterpret_cast<uint4*>(dst + (((size_t)b * 4 + pl) * hw + px) * 8) = *reinterpret_cast<const uint4*>(v);
   }
 }
+// ---- deterministic reductions (BIN_DETERMINISTIC): a kernel writes one partial per block, a second launch sums them.
+// Warp w of block b owns output 8b + w: lane l adds partials l, l+32, ... in index order, then a fixed xor-shuffle tree
+// adds the 32 lane sums.  Partial i of the output is partial[i * istride].  The order depends only on nparts, which
+// depends only on the shape, never on which block finished first.
+__device__ __forceinline__ float ordered_warp_sum(const float* __restrict__ partial, int nparts, size_t istride) {
+  const int lane = threadIdx.x & 31;
+  float v = 0.f;
+  for (int i = lane; i < nparts; i += 32) v += partial[(size_t)i * istride];
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
 // db[c] += inv_scale * sum over (B, H, W) of dY[c] for P8 planes [plane0, plane0+ceil(C/8)).
-// grid = (pixel groups, planes, batch): no 64-bit div/mod per element, 4 independent 16-byte loads in flight per thread
+// grid = (pixel groups, planes, batch): no 64-bit div/mod per element, 4 independent 16-byte loads in flight per thread.
+// partial == NULL: each block adds its sums with atomicAdd; otherwise it writes them to partial [B][blocks_x][C].
 __global__ void __launch_bounds__(256) p8_bias_grad_kernel(const __half* __restrict__ dy, int planes, int plane0, int C, int hw,
-                                                           const float* __restrict__ scale, float* __restrict__ db) {
+                                                           const float* __restrict__ scale, float* __restrict__ db,
+                                                           float* __restrict__ partial) {
   __shared__ float part[8][8];
   const int pl = blockIdx.y, b = blockIdx.z;
   const __half* base = dy + ((size_t)b * planes + plane0 + pl) * (size_t)hw * 8;
@@ -315,8 +329,19 @@ __global__ void __launch_bounds__(256) p8_bias_grad_kernel(const __half* __restr
     float sum = 0.f;
     for (int wv = 0; wv < 8; ++wv) sum += part[wv][threadIdx.x];
     const int c = pl * 8 + threadIdx.x;
-    if (c < C) atomicAdd(db + c, sum / scale[0]);
+    if (c < C) {
+      if (partial) partial[((size_t)b * gridDim.x + blockIdx.x) * C + c] = sum;        // [B][blocks_x][C]
+      else atomicAdd(db + c, sum / scale[0]);
+    }
   }
+}
+// Deterministic bias gradient: db[c] += (sum of the nparts = B * blocks_x partials of channel c, in index order) / scale.
+__global__ void __launch_bounds__(256) bias_grad_reduce_kernel(const float* __restrict__ partial, int nparts, int C,
+                                                               const float* __restrict__ scale, float* __restrict__ db) {
+  const int c = blockIdx.x * 8 + (threadIdx.x >> 5);
+  if (c >= C) return;
+  const float s = ordered_warp_sum(partial + c, nparts, (size_t)C);
+  if ((threadIdx.x & 31) == 0) db[c] += s / scale[0];
 }
 
 // ---- loss scale of a backbone's backward (autograd.py): scale = 2^floor(log2(target / max|dOut|)), kept on the device
@@ -509,8 +534,11 @@ struct LossPairs {
 __device__ __forceinline__ float loss_term(float d, int kind, float eps) {
   return kind == 0 ? fabsf(d) : (kind == 1 ? d * d : sqrtf(d * d + eps));
 }
+// DET = false: every block adds its sum to pair_loss[k] with atomicAdd (last bits depend on block order).
+// DET = true: block x of pair k writes its sum to partial[k][x]; pixel_loss_reduce_kernel adds them in index order.
+template <bool DET>
 __global__ void pixel_loss_fwd_kernel(const __grid_constant__ LossPairs P, size_t n, int kind, float eps,
-                                      float* __restrict__ pair_loss) {
+                                      float* __restrict__ pair_loss, float* __restrict__ partial) {
   const int k = blockIdx.y;
   const float* a = P.a[k];
   const float* b = P.b[k];
@@ -524,8 +552,16 @@ __global__ void pixel_loss_fwd_kernel(const __grid_constant__ LossPairs P, size_
   if (threadIdx.x == 0) {
     float s = 0.f;
     for (int wv = 0; wv < (int)(blockDim.x >> 5); ++wv) s += part[wv];
-    atomicAdd(pair_loss + k, kind == 2 ? s / (float)n : s);
+    if (DET) partial[(size_t)k * gridDim.x + blockIdx.x] = s;
+    else atomicAdd(pair_loss + k, kind == 2 ? s / (float)n : s);
   }
+}
+__global__ void __launch_bounds__(256) pixel_loss_reduce_kernel(const float* __restrict__ partial, int nparts, int npairs,
+                                                                int kind, size_t n, float* __restrict__ pair_loss) {
+  const int k = blockIdx.x * 8 + (threadIdx.x >> 5);
+  if (k >= npairs) return;
+  const float s = ordered_warp_sum(partial + (size_t)k * nparts, nparts, 1);
+  if ((threadIdx.x & 31) == 0) pair_loss[k] = kind == 2 ? s / (float)n : s;          // the Charbonnier mean: one divide
 }
 // da_k = g * dterm/dd, db_k = -da_k, with g = upstream / npairs (and / n for the Charbonnier mean)
 __global__ void pixel_loss_bwd_kernel(const __grid_constant__ LossPairs P, size_t n, int kind, float eps,
@@ -606,9 +642,13 @@ __global__ void convlstm_bwd_gates_kernel(const float* __restrict__ x, const flo
 // Pass 2: dW[k][c][tap] += sum_p dgates[k][p] * in[c][p+off], db[k] += sum_p dgates[k][p]  (660 outputs).
 // 9 warps per block, warp v owns tap v: 72 register accumulators acc[k][c] (all indices compile-time), lanes
 // stride over pixels; one warp-shuffle reduction + 72 atomics per warp at the end (warp 0 also sums the biases).
+// partial != NULL (deterministic): block x writes its 660 sums to partial[x][660] instead (dw order, then the 12 biases),
+// and convlstm_wgrad_reduce_kernel adds the blocks in index order.
+constexpr int kLstmGradN = 12 * 6 * 9 + 12;
 __global__ void __launch_bounds__(288) convlstm_bwd_weights_kernel(const float* __restrict__ x, const float* __restrict__ h_prev,
                                                                     const float* __restrict__ dgates, float* __restrict__ dw,
-                                                                    float* __restrict__ db, int B, int H, int W) {
+                                                                    float* __restrict__ db, int B, int H, int W,
+                                                                    float* __restrict__ partial) {
   const size_t hw = (size_t)H * W;
   const size_t total = (size_t)B * hw;
   const int tap = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -645,13 +685,29 @@ __global__ void __launch_bounds__(288) convlstm_bwd_weights_kernel(const float* 
     for (int c = 0; c < 6; ++c) {
       float v = acc[k][c];
       for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-      if (lane == 0) atomicAdd(dw + (k * 6 + c) * 9 + tap, v);
+      if (lane == 0) {
+        if (partial) partial[(size_t)blockIdx.x * kLstmGradN + (k * 6 + c) * 9 + tap] = v;
+        else atomicAdd(dw + (k * 6 + c) * 9 + tap, v);
+      }
     }
     if (tap == 0) {
       float v = accb[k];
       for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-      if (lane == 0) atomicAdd(db + k, v);
+      if (lane == 0) {
+        if (partial) partial[(size_t)blockIdx.x * kLstmGradN + 648 + k] = v;
+        else atomicAdd(db + k, v);
+      }
     }
+  }
+}
+__global__ void __launch_bounds__(256) convlstm_wgrad_reduce_kernel(const float* __restrict__ partial, int nparts,
+                                                                    float* __restrict__ dw, float* __restrict__ db) {
+  const int o = blockIdx.x * 8 + (threadIdx.x >> 5);
+  if (o >= kLstmGradN) return;
+  const float s = ordered_warp_sum(partial + o, nparts, (size_t)kLstmGradN);
+  if ((threadIdx.x & 31) == 0) {
+    if (o < 648) dw[o] += s;
+    else db[o - 648] += s;
   }
 }
 // Pass 3: dx[c][q] = sum_{k,tap} W[k][c][tap] * dgates[k][q - off(tap)]  (and dh_prev for c = 3..5).
@@ -1071,11 +1127,20 @@ int launch_grad_out_to_p8(const bin_frames_t& dout, int H, int W, const bin_act_
   BIN_CUDA_OK(cudaGetLastError());
   return BIN_OK;
 }
-int launch_bias_grad(const bin_act_t& dy, int plane0, int C, const float* scale, float* db, cudaStream_t s) {
+size_t bias_grad_partial_floats(int B, int hw, int C) { return (size_t)B * ((hw + 1023) / 1024) * C; }
+int launch_bias_grad(const bin_act_t& dy, int plane0, int C, const float* scale, float* db, cudaStream_t s, float* partial,
+                     size_t partial_floats) {
   const int hw = dy.H * dy.W;
+  // run_backbone_bwd checks every conv's partials against the region before its first launch; this is a backstop
+  if (partial && bias_grad_partial_floats(dy.B, hw, C) > partial_floats)
+    return fail(BIN_ERR_WORKSPACE, "bias_grad: deterministic partial sums do not fit the workspace");
   dim3 grid((unsigned)((hw + 1023) / 1024), (unsigned)((C + 7) / 8), (unsigned)dy.B);
-  p8_bias_grad_kernel<<<grid, 256, 0, s>>>((const __half*)dy.ptr, dy.planes, plane0, C, hw, scale, db);
+  p8_bias_grad_kernel<<<grid, 256, 0, s>>>((const __half*)dy.ptr, dy.planes, plane0, C, hw, scale, db, partial);
   BIN_CUDA_OK(cudaGetLastError());
+  if (partial) {
+    bias_grad_reduce_kernel<<<(C + 7) / 8, 256, 0, s>>>(partial, (int)(grid.x * grid.z), C, scale, db);
+    BIN_CUDA_OK(cudaGetLastError());
+  }
   return BIN_OK;
 }
 int launch_grad_scale(const float* const* gouts, int n, size_t numel, float target, float* scale_dev, unsigned* tmp_dev,
@@ -1133,16 +1198,33 @@ int launch_blur_average_u8(const uint8_t* frames, int T, size_t frame_bytes, int
   BIN_CUDA_OK(cudaGetLastError());
   return BIN_OK;
 }
+static unsigned pixel_loss_blocks(size_t n) {
+  return (unsigned)((n + 256 * 16 - 1) / (256 * 16) < 256 ? (n + 256 * 16 - 1) / (256 * 16) : 256);
+}
+size_t pixel_loss_scratch_bytes(int npairs, size_t n) {
+  if (npairs < 1 || npairs > BIN_MAX_LOSS_PAIRS) return 0;
+  return (size_t)npairs * pixel_loss_blocks(n) * sizeof(float);
+}
 int launch_pixel_loss_fwd(const float* const* a, const float* const* b, int npairs, size_t n, int kind, float eps,
-                          float* pair_loss, cudaStream_t s) {
+                          float* pair_loss, cudaStream_t s, int flags, void* scratch, size_t scratch_bytes) {
   if (npairs < 1 || npairs > BIN_MAX_LOSS_PAIRS || kind < 0 || kind > 2) return fail(BIN_ERR_ARG, "pixel_loss: bad pair count / kind");
+  const bool det = flags & BIN_DETERMINISTIC;
+  if (det && !scratch) return fail(BIN_ERR_ARG, "pixel_loss: BIN_DETERMINISTIC needs a scratch buffer");
+  if (det && scratch_bytes < pixel_loss_scratch_bytes(npairs, n)) return fail(BIN_ERR_WORKSPACE, "pixel_loss: scratch too small");
   LossPairs P;
   memset(&P, 0, sizeof(P));
   P.npairs = npairs;
   for (int k = 0; k < npairs; ++k) { P.a[k] = a[k]; P.b[k] = b[k]; }
+  dim3 grid(pixel_loss_blocks(n), npairs);
+  if (det) {                                        // every pair_loss[k] has one writer: no memset, no atomics
+    pixel_loss_fwd_kernel<true><<<grid, 256, 0, s>>>(P, n, kind, eps, pair_loss, (float*)scratch);
+    BIN_CUDA_OK(cudaGetLastError());
+    pixel_loss_reduce_kernel<<<(npairs + 7) / 8, 256, 0, s>>>((const float*)scratch, (int)grid.x, npairs, kind, n, pair_loss);
+    BIN_CUDA_OK(cudaGetLastError());
+    return BIN_OK;
+  }
   BIN_CUDA_OK(cudaMemsetAsync(pair_loss, 0, npairs * sizeof(float), s));
-  dim3 grid((unsigned)((n + 256 * 16 - 1) / (256 * 16) < 256 ? (n + 256 * 16 - 1) / (256 * 16) : 256), npairs);
-  pixel_loss_fwd_kernel<<<grid, 256, 0, s>>>(P, n, kind, eps, pair_loss);
+  pixel_loss_fwd_kernel<false><<<grid, 256, 0, s>>>(P, n, kind, eps, pair_loss, nullptr);
   BIN_CUDA_OK(cudaGetLastError());
   return BIN_OK;
 }
@@ -1158,28 +1240,41 @@ int launch_pixel_loss_bwd(const float* const* a, const float* const* b, float* c
   BIN_CUDA_OK(cudaGetLastError());
   return BIN_OK;
 }
+static unsigned convlstm_wgrad_blocks(size_t total) { return (unsigned)((total + 31) / 32 < 592 ? (total + 31) / 32 : 592); }
+size_t convlstm_bwd_scratch_bytes(int B, int H, int W) {
+  if (B < 1 || H < 1 || W < 1) return 0;
+  return (size_t)convlstm_wgrad_blocks((size_t)B * H * W) * kLstmGradN * sizeof(float);
+}
 int launch_convlstm_bwd(const float* x, const float* c_prev, const float* h_prev, const float* w, const float* b,
                         const float* dh, const float* dc, float* dgates_ws, float* dx, float* dc_prev, float* dh_prev,
-                        float* dw, float* db, int B, int H, int W, cudaStream_t s) {
+                        float* dw, float* db, int B, int H, int W, cudaStream_t s, int flags, void* scratch,
+                        size_t scratch_bytes) {
   if ((c_prev == nullptr) != (h_prev == nullptr)) return fail(BIN_ERR_ARG, "convlstm_bwd: give both c_prev and h_prev or neither");
+  const bool det = flags & BIN_DETERMINISTIC;
+  if (det && !scratch) return fail(BIN_ERR_ARG, "convlstm_bwd: BIN_DETERMINISTIC needs a scratch buffer");
+  if (det && scratch_bytes < convlstm_bwd_scratch_bytes(B, H, W)) return fail(BIN_ERR_WORKSPACE, "convlstm_bwd: scratch too small");
   const size_t total = (size_t)B * H * W;
   convlstm_bwd_gates_kernel<<<grid_for(total, 128), 128, 0, s>>>(x, c_prev, h_prev, w, b, dh, dc, dgates_ws, dc_prev, B, H, W);
   BIN_CUDA_OK(cudaGetLastError());
-  const unsigned wblocks = (unsigned)((total + 31) / 32 < 592 ? (total + 31) / 32 : 592);
-  convlstm_bwd_weights_kernel<<<wblocks, 288, 0, s>>>(x, h_prev, dgates_ws, dw, db, B, H, W);
+  const unsigned wblocks = convlstm_wgrad_blocks(total);
+  convlstm_bwd_weights_kernel<<<wblocks, 288, 0, s>>>(x, h_prev, dgates_ws, dw, db, B, H, W, det ? (float*)scratch : nullptr);
   BIN_CUDA_OK(cudaGetLastError());
+  if (det) {
+    convlstm_wgrad_reduce_kernel<<<(kLstmGradN + 7) / 8, 256, 0, s>>>((const float*)scratch, (int)wblocks, dw, db);
+    BIN_CUDA_OK(cudaGetLastError());
+  }
   convlstm_bwd_input_kernel<<<grid_for(total, 128), 128, 0, s>>>(dgates_ws, w, dx, dh_prev, B, H, W);
   BIN_CUDA_OK(cudaGetLastError());
   return BIN_OK;
 }
 int launch_wgrad_impl(const bin_act_t& x0, int x0_plane0, int x0_planes, const bin_act_t& x1, int x1_plane0, int x1_planes,
                       const bin_act_t& dy, int dy_plane0, int cout, int cin, int ks, const float* scale, float* dw,
-                      float* partial_ws, cudaStream_t s);
+                      float* partial_ws, cudaStream_t s, bool det);
 int launch_wgrad(const bin_act_t& x0, int x0_plane0, int x0_planes, const bin_act_t& x1, int x1_plane0, int x1_planes,
                  const bin_act_t& dy, int dy_plane0, int cout, int cin, int ks, const float* scale, float* dw,
-                 float* partial_ws, cudaStream_t s) {
+                 float* partial_ws, cudaStream_t s, bool det) {
   return launch_wgrad_impl(x0, x0_plane0, x0_planes, x1, x1_plane0, x1_planes, dy, dy_plane0, cout, cin, ks, scale, dw,
-                           partial_ws, s);
+                           partial_ws, s, det);
 }
 // expand = 1: bin_flipx4_expand, 0: bin_flipx4_mean.  Every check runs before the first CUDA call.
 int launch_flipx4(int expand, const float* const* src, float* const* dst, int n, int B, int H, int W, cudaStream_t s) {

@@ -48,9 +48,13 @@ struct Options {
   bool zigzag;               // BIN_B200_ZIGZAG: consecutive RDB launches walk the tiles in opposite directions (L2 reuse)
   int stage_mmas;            // BIN_B200_STAGE_MMAS: target wgmma instructions per pipeline stage of the conv kernel (default 12)
   size_t band_budget;        // BIN_B200_BAND_BUDGET_KB (L2 band walker; default: one band)
+  int max_sms;               // BIN_B200_MAX_SMS=n: num_sms() reports at most n (grid sizes only; 0 = no cap)
 };
 const Options& options();
-int num_sms();               // SM count of the current device (cached per device)
+int num_sms();               // SM count of the current device (cached per device), capped by BIN_B200_MAX_SMS
+// Grid of the weight-gradient kernel in deterministic mode (BIN_DETERMINISTIC): a constant, so dW does not depend on
+// the SM count.  132 = the SMs of an H100 SXM, where it equals the default grid.
+constexpr int kDetCtas = 132;
 
 // ------------------------------------------------------------------ tile geometry of the conv kernel
 constexpr int kTWH = 32;   // smem row pitch of an activation tile, in pixels (= 4 core-matrix row groups)

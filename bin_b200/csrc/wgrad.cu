@@ -206,11 +206,13 @@ __global__ void __launch_bounds__(256) wgrad_reduce_kernel(const float* __restri
 int make_p8_tmap_box(CUtensorMap* m, const bin_act_t& t, int box_px, int box_rows, int box_planes);
 
 template <int N>
-static int run_wgrad(WgradParams p, int smem_bytes, int ci_planes, int kk, int ks, cudaStream_t s) {
+static int run_wgrad(WgradParams p, int smem_bytes, int ci_planes, int kk, int ks, cudaStream_t s, bool det) {
   static std::atomic<unsigned long long> smem_opted{0};   // per instantiation, per device
   BIN_TRY(ensure_dynamic_smem(wgrad_kernel<N>, kSmemMax, smem_opted));
   const int taps_per_group = WgCfg<N>::TAPS < kk ? WgCfg<N>::TAPS : kk;   // SX: kk = 3, one accumulator per ky
-  const int sms = num_sms();
+  // CTA c sums tiles c, c + grid, ... into its slab, so the grid fixes the bits of dW.  Deterministic mode uses a constant
+  // grid (the SM count of an H100 SXM) so that dW does not depend on the card; on fewer SMs it runs as a second wave.
+  const int sms = det ? kDetCtas : num_sms();
   const int grid = p.ntiles < sms ? p.ntiles : sms;
   if (grid < 1) return BIN_OK;
   for (int cp = 0; cp < ci_planes; cp += 16) {
@@ -231,7 +233,7 @@ static int run_wgrad(WgradParams p, int smem_bytes, int ci_planes, int kk, int k
 
 int launch_wgrad_impl(const bin_act_t& x0, int x0_plane0, int x0_planes, const bin_act_t& x1, int x1_plane0, int x1_planes,
                       const bin_act_t& dy, int dy_plane0, int cout, int cin, int ks, const float* scale, float* dw,
-                      float* partial_ws, cudaStream_t s) {
+                      float* partial_ws, cudaStream_t s, bool det) {
   if (ks != 1 && ks != 3 && ks != 5) return fail(BIN_ERR_ARG, "wgrad: ksize must be 1, 3 or 5");
   if (!partial_ws) return fail(BIN_ERR_ARG, "wgrad: partial-sum workspace missing");
   // TMA zero-fills a box that runs past its tensor, so a bad plane range or geometry would silently give wrong
@@ -274,7 +276,7 @@ int launch_wgrad_impl(const bin_act_t& x0, int x0_plane0, int x0_planes, const b
   const int smem_bytes = 1024 + S * (x_bytes + y_bytes);
   switch (n) {
 #define BIN_WGRAD_N(NN) \
-    case NN: return run_wgrad<NN>(p, smem_bytes, x0_planes + x1_planes, p.sx ? 3 : ks * ks, ks, s);
+    case NN: return run_wgrad<NN>(p, smem_bytes, x0_planes + x1_planes, p.sx ? 3 : ks * ks, ks, s, det);
     BIN_WGRAD_N(16) BIN_WGRAD_N(32) BIN_WGRAD_N(48) BIN_WGRAD_N(64) BIN_WGRAD_N(96) BIN_WGRAD_N(128) BIN_WGRAD_N(256)
 #undef BIN_WGRAD_N
   }

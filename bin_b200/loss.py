@@ -11,6 +11,7 @@ from typing import List, Optional, Sequence, Tuple
 import torch
 
 from ._lib import BinB200Error, check, lib
+from .autograd import deterministic_flags
 
 KINDS = {"l1": 0, "l2": 1, "cb": 2}                   # bin_model.py:54-59
 CYCLE_PAIRS_6V2 = ((1, 7), (5, 9), (2, 8))            # bin_model.py:409-416
@@ -41,11 +42,16 @@ class PixelLossFn(torch.autograd.Function):
             raise BinB200Error("bin_b200.loss runs on CUDA tensors only (no CPU fallback)")
         if any(t.numel() != n or t.device != dev for t in a + b):
             raise BinB200Error("pixel_loss: all tensors must share size and device")
+        flags = deterministic_flags()                 # torch.use_deterministic_algorithms: fixed-order sums
         with torch.cuda.device(dev):
             pair = torch.empty(npairs, device=dev)
+            scratch = (torch.empty(lib().bin_pixel_loss_scratch_bytes(npairs, n), dtype=torch.uint8, device=dev)
+                       if flags else None)
             ap = (C.c_void_p * npairs)(*[t.data_ptr() for t in a])
             bp = (C.c_void_p * npairs)(*[t.data_ptr() for t in b])
-            check(lib().bin_pixel_loss_fwd(ap, bp, npairs, n, kind, eps, pair.data_ptr(), _stream()))
+            check(lib().bin_pixel_loss_fwd_ex(ap, bp, npairs, n, kind, eps, pair.data_ptr(), flags,
+                                              None if scratch is None else scratch.data_ptr(),
+                                              0 if scratch is None else scratch.numel(), _stream()))
         ctx.kind, ctx.eps, ctx.npairs, ctx.n = kind, eps, npairs, n
         ctx.need_b = [t.requires_grad for t in tensors[npairs:]]
         ctx.save_for_backward(*a, *b)

@@ -33,12 +33,19 @@
 extern "C" {
 #endif
 
-#define BIN_ABI_VERSION 3
+#define BIN_ABI_VERSION 4
 #define BIN_MAX_CALLS 6   /* same-weight backbone calls batched along N */
 #define BIN_MAX_FRAMES 5  /* frames per backbone call (2, 3 or 5) */
 #define BIN_MAX_LOSS_PAIRS 20 /* (prediction, target) pairs of one fused loss call */
 
 enum { BIN_OK = 0, BIN_ERR_ARG = 1, BIN_ERR_CUDA = 2, BIN_ERR_UNSUPPORTED = 3, BIN_ERR_WORKSPACE = 4 };
+
+/* `flags` of the *_ex entry points.  BIN_DETERMINISTIC: every cross-block sum (the pixel-loss terms, the backbone bias
+ * gradients, the ConvLSTM weight and bias gradients) writes one partial per block and adds them in index order, and the
+ * backbone weight gradients use a constant grid instead of one CTA per SM, so the result has the same bits from run to
+ * run, on any stream and whatever SM count the device has.  0 = the default: float atomics, grids sized by SM count.
+ * Any other bit fails with BIN_ERR_ARG. */
+#define BIN_DETERMINISTIC 1
 
 typedef void* bin_stream_t; /* cudaStream_t */
 
@@ -150,6 +157,14 @@ int bin_convlstm_fwd(const float* x, const float* c_prev, const float* h_prev, c
 int bin_convlstm_bwd(const float* x, const float* c_prev, const float* h_prev, const float* w, const float* b,
                      const float* dh, const float* dc, float* dgates_ws, float* dx, float* dc_prev, float* dh_prev,
                      float* dw, float* db, int B, int H, int W, bin_stream_t s);
+/* bin_convlstm_bwd with flags (bin_convlstm_bwd = flags 0, scratch NULL).  With BIN_DETERMINISTIC, scratch (device, at
+ * least bin_convlstm_bwd_scratch_bytes(B, H, W) = one 660-float row per weight-gradient block, <= 1.6 MB) receives the
+ * per-block sums; a NULL scratch fails with BIN_ERR_ARG and a small one with BIN_ERR_WORKSPACE, before any launch. */
+size_t bin_convlstm_bwd_scratch_bytes(int B, int H, int W);
+int bin_convlstm_bwd_ex(const float* x, const float* c_prev, const float* h_prev, const float* w, const float* b,
+                        const float* dh, const float* dc, float* dgates_ws, float* dx, float* dc_prev, float* dh_prev,
+                        float* dw, float* db, int B, int H, int W, int flags, void* scratch, size_t scratch_bytes,
+                        bin_stream_t s);
 
 /* ---- one backbone (RDN_residual_interp_{2,2_1,4_1}_input.forward, RDN.py:210-334) ---------- */
 #define BIN_BACKBONE_NCONV 66 /* SFENet1, SFENet2, 12 x (4 conv + LFF), GFF.0, GFF.1, UPNet.0, UPNet.2 */
@@ -180,13 +195,23 @@ int bin_backbone_bwd(int nframes, const void* blob_t, const bin_frames_t* dout, 
  * bin_backbone_workspace_bytes) is what bin_backbone_fwd with `blob` just left for the same frames, which keeps every
  * activation the backward reads except the growth maps of the 12 RDBs.  Before each RDB's backward its four growth convs
  * are re-run from its input with `blob`, into the workspace's one RDB of growth scratch.  Every launch then reads the
- * operands that bin_backbone_bwd reads after bin_backbone_fwd_train, so the frame and weight gradients have the same bits
- * (the bias gradients are summed with float atomics in both); grad_ws, grad_params and scale_dev are as there.  A NULL pointer, an
- * undersized or unaligned fwd_ws fail (BIN_ERR_ARG / BIN_ERR_WORKSPACE) before any launch. */
+ * operands that bin_backbone_bwd reads after bin_backbone_fwd_train, so the frame and weight gradients have the same bits.
+ * The bias gradients are summed with float atomics in both when flags = 0 (their last bits vary from run to run), and in
+ * a fixed order with BIN_DETERMINISTIC (the same bits in both).  grad_ws, grad_params and scale_dev are as there.  A NULL
+ * pointer, an undersized or unaligned fwd_ws fail (BIN_ERR_ARG / BIN_ERR_WORKSPACE) before any launch. */
 int bin_backbone_bwd_recompute(int nframes, const void* blob, const void* blob_t, const bin_frames_t* dout,
                                const bin_frames_t* dframes, int H, int W, const void* fwd_ws, size_t fwd_ws_bytes,
                                void* grad_ws, size_t grad_ws_bytes, float* grad_params, const float* scale_dev,
                                bin_stream_t s);
+/* The two backwards with flags (the calls above = flags 0).  BIN_DETERMINISTIC needs no extra memory: the bias-gradient
+ * partials live in the wgrad region of grad_ws, which bin_backbone_grad_workspace_bytes sizes for both. */
+int bin_backbone_bwd_ex(int nframes, const void* blob_t, const bin_frames_t* dout, const bin_frames_t* dframes, int H,
+                        int W, const void* save_ws, void* grad_ws, size_t grad_ws_bytes, float* grad_params,
+                        const float* scale_dev, int flags, bin_stream_t s);
+int bin_backbone_bwd_recompute_ex(int nframes, const void* blob, const void* blob_t, const bin_frames_t* dout,
+                                  const bin_frames_t* dframes, int H, int W, const void* fwd_ws, size_t fwd_ws_bytes,
+                                  void* grad_ws, size_t grad_ws_bytes, float* grad_params, const float* scale_dev,
+                                  int flags, bin_stream_t s);
 /* Loss scale for one backbone backward: *scale_dev = 2^floor(log2(target / max_k max|gouts[k]|)) (a power of two, so
  * scaling and un-scaling are exact), computed on the device -- no host synchronisation.  gouts_host: host array of n
  * (<= BIN_MAX_CALLS) device pointers to fp32 tensors of `numel` elements, 16-byte aligned; tmp4_dev: 4 bytes of scratch. */
@@ -232,6 +257,13 @@ int bin_pyramid3_fwd(const bin_net_t* net, const float* const* frames_host, floa
 enum { BIN_LOSS_L1_SUM = 0, BIN_LOSS_L2_SUM = 1, BIN_LOSS_CHARBONNIER_MEAN = 2 };
 int bin_pixel_loss_fwd(const float* const* a_host, const float* const* b_host, int npairs, size_t n, int kind, float eps,
                        float* pair_loss, bin_stream_t s);
+/* bin_pixel_loss_fwd with flags (bin_pixel_loss_fwd = flags 0, scratch NULL).  With BIN_DETERMINISTIC each block writes
+ * its partial sum to scratch (device, >= bin_pixel_loss_scratch_bytes(npairs, n) <= 20 KB) and a second launch adds
+ * them in index order (then divides once by n for the Charbonnier mean).  A NULL scratch fails with BIN_ERR_ARG and a
+ * small one with BIN_ERR_WORKSPACE, before any launch. */
+size_t bin_pixel_loss_scratch_bytes(int npairs, size_t n);
+int bin_pixel_loss_fwd_ex(const float* const* a_host, const float* const* b_host, int npairs, size_t n, int kind, float eps,
+                          float* pair_loss, int flags, void* scratch, size_t scratch_bytes, bin_stream_t s);
 /* da_k = (upstream/npairs) * d cri_pix / d a_k, db_k = -da_k (db_host or single entries may be NULL). */
 int bin_pixel_loss_bwd(const float* const* a_host, const float* const* b_host, float* const* da_host, float* const* db_host,
                        int npairs, size_t n, int kind, float eps, const float* upstream, bin_stream_t s);
