@@ -16,7 +16,7 @@ BIN_TRAIN_MAX_BATCH = 16
 BIN_TRAIN_FRAMES = 17
 EPI_P8, EPI_PIXSHUF, EPI_FINAL = 0, 1, 2
 BIN_DETERMINISTIC = 1                 # flags bit of the *_ex entry points
-ABI_VERSION = 4
+ABI_VERSION = 5
 
 
 class Act(C.Structure):
@@ -91,6 +91,12 @@ _SIGS = {
     "bin_backbone_bwd_recompute_ex": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.POINTER(Frames), C.POINTER(Frames), C.c_int,
                                                 C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p,
                                                 C.c_void_p, C.c_int, C.c_void_p]),
+    "bin_backbone_bwd_masked": (C.c_int, [C.c_int, C.c_void_p, C.POINTER(Frames), C.POINTER(Frames), C.c_int, C.c_int,
+                                          C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
+                                          C.c_void_p]),
+    "bin_backbone_bwd_recompute_masked": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.POINTER(Frames), C.POINTER(Frames),
+                                                    C.c_int, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t,
+                                                    C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "bin_grad_scale": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_size_t, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]),
     "bin_rdb_fwd": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
                               C.c_void_p, C.c_size_t, C.c_void_p]),

@@ -48,6 +48,31 @@ def _input_key(model, frames):
     return tuple((t.data_ptr(), t._version) for t in list(model._conv_params()) + list(frames))
 
 
+def grad_plan(needs_input_grad, ncalls: int, nframes: int):
+    """What one BackboneStageFn backward computes, from its ctx.needs_input_grad = (model, ncalls, *frames, *params):
+    (need, frame_needed).  need is the 2 * BIN_BACKBONE_NCONV-byte host mask of bin_backbone_bwd_masked, 1 where a
+    parameter (weight then bias of conv 0..65, the order of _conv_params) wants its gradient; frame_needed[k][f] says
+    whether frame f of call k does (its dframes pointer is NULL when not)."""
+    nf = ncalls * nframes
+    flags = tuple(needs_input_grad)[2:]
+    if len(flags) != nf + 2 * _lib.BIN_BACKBONE_NCONV:
+        raise BinB200Error(f"grad_plan: expected {nf + 2 * _lib.BIN_BACKBONE_NCONV} inputs after (model, ncalls), "
+                           f"got {len(flags)}")
+    frame_needed = [[bool(flags[k * nframes + f]) for f in range(nframes)] for k in range(ncalls)]
+    need = (C.c_ubyte * (2 * _lib.BIN_BACKBONE_NCONV))(*[1 if x else 0 for x in flags[nf:]])
+    return need, frame_needed
+
+
+def _grad_frames(dframes, B: int) -> _lib.Frames:
+    """dframes table of a backward: None entries become NULL pointers (no gradient for that frame)."""
+    fr = _lib.Frames()
+    fr.ncalls, fr.nframes, fr.Bc = len(dframes), len(dframes[0]), B
+    for k, call in enumerate(dframes):
+        for f, t in enumerate(call):
+            fr.frame[k][f] = None if t is None else t.data_ptr()
+    return fr
+
+
 def _inference_fwd(model, calls, outs, B, H, W, dev) -> torch.Tensor:
     """bin_backbone_fwd of one batched stage into the shared per-(device, stream) workspace, which it returns."""
     from .rdn import _workspace
@@ -65,7 +90,11 @@ class BackboneStageFn(torch.autograd.Function):
     Default: the forward keeps the stage's whole training workspace (all 12 RDBs' growth maps) until the backward.
     With set_activation_checkpointing(net, "recompute") it keeps only its input frames: the forward is the inference
     forward into the shared per-stream workspace, and the backward runs that forward again and rebuilds each RDB's
-    growth maps just before that RDB's backward.  Every kernel sees the same operands in both (DESIGN.md §4e)."""
+    growth maps just before that RDB's backward.  Every kernel sees the same operands in both (DESIGN.md §4e).
+
+    Frozen tensors (requires_grad False) get no gradient and cost no work: the backward computes only what
+    ctx.needs_input_grad asks for (DESIGN.md §4g).  A stage none of whose inputs needs a gradient runs the inference
+    forward, with the fused RDB tail, and keeps nothing for a backward."""
 
     @staticmethod
     def forward(ctx, model, ncalls: int, *args):
@@ -75,6 +104,11 @@ class BackboneStageFn(torch.autograd.Function):
         calls = [frames[k * n:(k + 1) * n] for k in range(ncalls)]
         B, _, H, W = frames[0].shape
         dev = frames[0].device
+        if not any(ctx.needs_input_grad[2:]):
+            with torch.cuda.device(dev):
+                outs = [torch.empty_like(frames[0]) for _ in range(ncalls)]
+                _inference_fwd(model, calls, outs, B, H, W, dev)
+            return tuple(outs)
         recompute = _checkpointing_of(model) == "recompute"
         with torch.cuda.device(dev):
             outs = [torch.empty_like(frames[0]) for _ in range(ncalls)]
@@ -115,28 +149,30 @@ class BackboneStageFn(torch.autograd.Function):
             check(lib().bin_grad_scale(gp, ncalls, gouts[0].numel(), LOSS_SCALE_TARGET, sbuf.data_ptr(),
                                        sbuf.data_ptr() + 4, _stream()))
             scale = sbuf[:1]
-            dframes = [[torch.empty((B, 3, H, W), device=dev) for _ in range(n)] for _ in range(ncalls)]
+            need, frame_needed = grad_plan(ctx.needs_input_grad, ncalls, n)
+            dframes = [[torch.empty((B, 3, H, W), device=dev) if want else None for want in call] for call in frame_needed]
             dout = ops.make_frames([[g] * n for g in gouts], gouts)             # only .out / ncalls / Bc are read
-            dfr = ops.make_frames(dframes, [None] * ncalls)
-            gparams = torch.zeros(lib().bin_backbone_grad_param_floats(n), device=dev)
+            dfr = _grad_frames(dframes, B)
+            gparams = torch.zeros(lib().bin_backbone_grad_param_floats(n), device=dev) if any(need) else None
+            gp_ptr = None if gparams is None else gparams.data_ptr()
             gws = torch.empty(lib().bin_backbone_grad_workspace_bytes(n, B * ncalls, H, W), dtype=torch.uint8, device=dev)
             if recompute:
                 frames = ctx.frames_keepalive
                 calls = [frames[k * n:(k + 1) * n] for k in range(ncalls)]
                 scratch = [torch.empty_like(frames[0]) for _ in range(ncalls)]   # the forward's outputs stay untouched
                 ws = _inference_fwd(model, calls, scratch, B, H, W, dev)
-                check(lib().bin_backbone_bwd_recompute_ex(n, model.packed_blob().data_ptr(), _packed_t(model).data_ptr(),
-                                                          C.byref(dout), C.byref(dfr), H, W, ws.data_ptr(), ws.numel(),
-                                                          gws.data_ptr(), gws.numel(), gparams.data_ptr(), scale.data_ptr(),
-                                                          flags, _stream()))
+                check(lib().bin_backbone_bwd_recompute_masked(n, model.packed_blob().data_ptr(),
+                                                              _packed_t(model).data_ptr(), C.byref(dout), C.byref(dfr), H,
+                                                              W, ws.data_ptr(), ws.numel(), gws.data_ptr(), gws.numel(),
+                                                              gp_ptr, scale.data_ptr(), flags, need, _stream()))
             else:
-                check(lib().bin_backbone_bwd_ex(n, _packed_t(model).data_ptr(), C.byref(dout), C.byref(dfr), H, W,
-                                                ctx.save.data_ptr(), gws.data_ptr(), gws.numel(), gparams.data_ptr(),
-                                                scale.data_ptr(), flags, _stream()))
+                check(lib().bin_backbone_bwd_masked(n, _packed_t(model).data_ptr(), C.byref(dout), C.byref(dfr), H, W,
+                                                    ctx.save.data_ptr(), gws.data_ptr(), gws.numel(), gp_ptr,
+                                                    scale.data_ptr(), flags, need, _stream()))
         ctx.save = None
         pgrads, off = [], 0
-        for p in model._conv_params():
-            pgrads.append(gparams[off:off + p.numel()].view_as(p))
+        for p, want in zip(model._conv_params(), need):
+            pgrads.append(gparams[off:off + p.numel()].view_as(p) if want else None)
             off += p.numel()
         flat = [g for call in dframes for g in call]
         return (None, None, *flat, *pgrads)
@@ -175,18 +211,20 @@ class ConvLSTMFn(torch.autograd.Function):
         with torch.cuda.device(dev):
             dh = None if dh is None else dh.contiguous().float()
             dc = None if dc is None else dc.contiguous().float()
+            # a gradient nobody asked for is a NULL output: the library skips the pass that only it needs
+            need_x, need_w, need_b, need_cp, need_hp = ctx.needs_input_grad
             dgates = torch.empty((B, 12, H, W), device=dev)
-            dx = torch.empty_like(x)
-            dcp = torch.empty_like(x) if ctx.has_state else None
-            dhp = torch.empty_like(x) if ctx.has_state else None
-            dw = torch.zeros_like(w)
-            db = torch.zeros_like(b)
+            dx = torch.empty_like(x) if need_x else None
+            dcp = torch.empty_like(x) if ctx.has_state and need_cp else None
+            dhp = torch.empty_like(x) if ctx.has_state and need_hp else None
+            dw = torch.zeros_like(w) if need_w else None
+            db = torch.zeros_like(b) if need_b else None
             flags = deterministic_flags()
             scratch = (torch.empty(lib().bin_convlstm_bwd_scratch_bytes(B, H, W), dtype=torch.uint8, device=dev)
-                       if flags else None)
+                       if flags and (need_w or need_b) else None)
             P = lambda t: None if t is None else t.data_ptr()
             check(lib().bin_convlstm_bwd_ex(x.data_ptr(), P(cp), P(hp), w.data_ptr(), b.data_ptr(), P(dh), P(dc),
-                                            dgates.data_ptr(), dx.data_ptr(), P(dcp), P(dhp), dw.data_ptr(), db.data_ptr(),
+                                            dgates.data_ptr(), P(dx), P(dcp), P(dhp), P(dw), P(db),
                                             B, H, W, flags, P(scratch), 0 if scratch is None else scratch.numel(),
                                             _stream()))
         return dx, dw, db, dcp, dhp

@@ -484,14 +484,34 @@ static GradParamLayout grad_param_layout(int nframes) {
 // from cat[i-1] (f2 for RDB 0) with the forward weights in recompute_blob, into growth planes 0..15.  Same inputs, same
 // weights and the same launches as the saving forward, so the rebuilt maps have the same bits, and every launch of the
 // backward reads the same operands in both layouts.
+//
+// need (host, 2 * BIN_BACKBONE_NCONV bytes, weight then bias of each conv in grad_param_layout order; NULL = all) and the
+// NULL entries of dfr.frame say which gradients the caller reads.  Conv k's input depends on every conv with a lower
+// index, so the gradient with respect to it is needed iff a frame or some tensor of a lower conv needs one: U[k] below.
+// The backward walks the convs from the top; a weight or bias gradient nobody needs is not launched, a data gradient
+// runs only where U holds at the input it feeds, and the walk stops once U is false.  Whatever runs is the launch the full
+// backward makes, on the same operands and in the same order, so every gradient that is kept has the same bits.
 static int run_backbone_bwd(int nframes, const void* blob_t, const bin_frames_t& dout, const bin_frames_t& dfr, int H,
                             int W, const void* act_ws, size_t act_ws_bytes, const void* recompute_blob, void* gws_ptr,
-                            size_t gws_bytes, float* gparams, const float* scale, cudaStream_t s, int flags) {
+                            size_t gws_bytes, float* gparams, const float* scale, cudaStream_t s, int flags,
+                            const unsigned char* need) {
   if (!valid_nframes(nframes) || dfr.nframes != nframes) return fail(BIN_ERR_ARG, "backbone_bwd: nframes must be 2, 3 or 5");
   if (flags & ~BIN_DETERMINISTIC) return fail(BIN_ERR_ARG, "backbone_bwd: unknown flags");
   const bool det = flags & BIN_DETERMINISTIC;
   if (dout.ncalls != dfr.ncalls || dout.Bc != dfr.Bc || dout.ncalls < 1 || dout.ncalls > BIN_MAX_CALLS)
     return fail(BIN_ERR_ARG, "backbone_bwd: bad call tables");
+  bool need_w[BIN_BACKBONE_NCONV], need_b[BIN_BACKBONE_NCONV], U[BIN_BACKBONE_NCONV + 1];
+  bool any_param = false;
+  for (int i = 0; i < BIN_BACKBONE_NCONV; ++i) {
+    need_w[i] = !need || need[2 * i];
+    need_b[i] = !need || need[2 * i + 1];
+    any_param = any_param || need_w[i] || need_b[i];
+  }
+  if (any_param && !gparams) return fail(BIN_ERR_ARG, "backbone_bwd: null argument");
+  U[0] = false;                                                // U[0]: some frame of some call wants its gradient
+  for (int k = 0; k < dfr.ncalls; ++k)
+    for (int f = 0; f < nframes; ++f) U[0] = U[0] || dfr.frame[k][f] != nullptr;
+  for (int i = 0; i < BIN_BACKBONE_NCONV; ++i) U[i + 1] = U[i] || need_w[i] || need_b[i];
   const int Btot = dout.ncalls * dout.Bc;
   const bool recompute = recompute_blob != nullptr;
   const BackboneWs ws = backbone_ws(nframes, Btot, H, W, const_cast<void*>(act_ws), !recompute);
@@ -530,25 +550,35 @@ static int run_backbone_bwd(int nframes, const void* blob_t, const bin_frames_t&
   auto wgrad = [&](int idx, const bin_act_t& x0, int x0p, int x0n, const bin_act_t& x1, int x1p, int x1n,
                    const bin_act_t& dy, int dyp) -> int {
     const ConvSpec& c = L.conv[idx];
-    BIN_TRY(launch_bias_grad(dy, dyp, c.cout, scale, gparams + GP.b[idx], s, det ? gw.wg_partial : nullptr,
-                             gw.wg_partial_floats));
+    if (need_b[idx])
+      BIN_TRY(launch_bias_grad(dy, dyp, c.cout, scale, gparams + GP.b[idx], s, det ? gw.wg_partial : nullptr,
+                               gw.wg_partial_floats));
+    if (!need_w[idx]) return BIN_OK;
     return launch_wgrad(x0, x0p, x0n, x1, x1p, x1n, dy, dyp, c.cout, c.cin, c.ks, scale, gparams + GP.w[idx], gw.wg_partial,
                         s, det);
   };
   const bin_act_t none = {nullptr, 0, 0, 0, 0};
 
+  if (!U[BIN_BACKBONE_NCONV]) return BIN_OK;                                     // nothing asked for
   BIN_TRY(launch_grad_out_to_p8(dout, H, W, gw.dout16, scale, s));
   BIN_TRY(wgrad(65, ws.u, 0, 8, none, 0, 0, gw.dout16, 0));                          // UPNet.2
+  if (!U[65]) return BIN_OK;
   BIN_TRY(dgrad(T.x[65], gw.dout16, 0, 4, gw.du, 0, 8, false));
   BIN_TRY(launch_pixel_unshuffle(gw.du, gw.dup0, s));                               // nn.PixelShuffle backward
   BIN_TRY(wgrad(64, ws.t2, 0, 12, none, 0, 0, gw.dup0, 0));                          // UPNet.0
+  if (!U[64]) return BIN_OK;
   BIN_TRY(dgrad(T.x[64], gw.dup0, 0, 32, gw.dt2, 0, 12, false));
   BIN_TRY(wgrad(63, ws.t1, 0, 12, none, 0, 0, gw.dt2, 0));                           // GFF.1
+  if (!U[63]) return BIN_OK;
   BIN_TRY(dgrad(T.x[63], gw.dt2, 0, 12, gw.dt1, 0, 12, false));                      // dt2 doubles as d f__1 (RDN.py:219)
   BIN_TRY(wgrad(62, ws.cat, 0, 12 * kD, none, 0, 0, gw.dt1, 0));                     // GFF.0
+  if (!U[62]) return BIN_OK;
   BIN_TRY(dgrad(T.x[62], gw.dt1, 0, 12, gw.dcat, 0, 12 * kD, false));
-  BIN_CUDA_OK(cudaMemsetAsync(gw.df2.ptr, 0, (size_t)Btot * 12 * (H / 2) * (W / 2) * 16, s));
+  if (U[2]) BIN_CUDA_OK(cudaMemsetAsync(gw.df2.ptr, 0, (size_t)Btot * 12 * (H / 2) * (W / 2) * 16, s));
   const std::vector<Band> bands = recompute ? plan_bands(Btot, H / 2, W / 2) : std::vector<Band>();
+  // Reaching RDB i means U holds at its output (base + 5).  Inside it, the growth-map gradients dg feed the growth convs
+  // below the current one and the RDB input, so they are needed while U holds at the current conv; the parts that land
+  // in the input gradient dxin (residual, x rows of every conv) are needed iff U holds at the RDB input.
   for (int i = kD - 1; i >= 0; --i) {
     const int base = 2 + i * (kCgrow + 1);
     const bin_act_t& xin = i == 0 ? ws.f2 : ws.cat;           // forward input of RDB i
@@ -557,21 +587,31 @@ static int run_backbone_bwd(int nframes, const void* blob_t, const bin_frames_t&
     const int dxin_p = i == 0 ? 0 : 12 * (i - 1);
     const int dxo_p = 12 * i;                                 // d x_{i+1}, complete at this point
     const int gp0 = recompute ? 0 : 16 * i;                   // growth maps of RDB i
-    for (const Band& bd : bands) BIN_TRY(run_growth(recompute_blob, L, i, xin, xin_p, ws.g, 0, kCgrow, bd, s, 0));
+    const bool dx_in = U[base];
+    // the growth maps are read by the LFF's wgrad and, below it, by the growth-map dgrads and ReLU masks; the LFF's
+    // bias gradient alone reads only dcat
+    if (need_w[base + kCgrow] || U[base + kCgrow])
+      for (const Band& bd : bands) BIN_TRY(run_growth(recompute_blob, L, i, xin, xin_p, ws.g, 0, kCgrow, bd, s, 0));
     BIN_TRY(wgrad(base + kCgrow, xin, xin_p, 12, ws.g, gp0, 16, gw.dcat, dxo_p));                     // LFF
-    BIN_TRY(launch_p8_add(dxin, dxin_p, gw.dcat, dxo_p, 12, s));                                      // residual (RDN.py:165)
-    BIN_TRY(dgrad(T.x[base + kCgrow], gw.dcat, dxo_p, 12, dxin, dxin_p, 12, true));
+    if (!U[base + kCgrow]) return BIN_OK;
+    if (dx_in) {
+      BIN_TRY(launch_p8_add(dxin, dxin_p, gw.dcat, dxo_p, 12, s));                                    // residual (RDN.py:165)
+      BIN_TRY(dgrad(T.x[base + kCgrow], gw.dcat, dxo_p, 12, dxin, dxin_p, 12, true));
+    }
     BIN_TRY(dgrad(T.g[base + kCgrow], gw.dcat, dxo_p, 12, gw.dg, 0, 16, false));
     for (int c = kCgrow - 1; c >= 0; --c) {
       BIN_TRY(launch_relu_mask(gw.dg, 4 * c, ws.g, gp0 + 4 * c, 4, s));                               // RDN.py:142
       BIN_TRY(wgrad(base + c, xin, xin_p, 12, ws.g, gp0, 4 * c, gw.dg, 4 * c));
-      BIN_TRY(dgrad(T.x[base + c], gw.dg, 4 * c, 4, dxin, dxin_p, 12, true));
+      if (!U[base + c]) return BIN_OK;
+      if (dx_in) BIN_TRY(dgrad(T.x[base + c], gw.dg, 4 * c, 4, dxin, dxin_p, 12, true));
       if (c > 0) BIN_TRY(dgrad(T.g[base + c], gw.dg, 4 * c, 4, gw.dg, 0, 4 * c, true));
     }
   }
   BIN_TRY(wgrad(1, ws.f1, 0, 12, none, 0, 0, gw.df2, 0));                            // SFENet2
+  if (!U[1]) return BIN_OK;
   BIN_TRY(dgrad(T.x[1], gw.df2, 0, 12, gw.dt2, 0, 12, true));                        // d f__1 complete
   BIN_TRY(wgrad(0, ws.x0, 0, ws.x0.planes, none, 0, 0, gw.dt2, 0));                  // SFENet1
+  if (!U[0]) return BIN_OK;
   BIN_TRY(dgrad(T.x[0], gw.dt2, 0, 12, gw.dx0, 0, gw.dx0.planes, false));
   return launch_unpack_frames_grad(gw.dx0, dout, dfr, H, W, scale, s);
 }
@@ -689,7 +729,7 @@ int bin_convlstm_bwd_ex(const float* x, const float* c_prev, const float* h_prev
                         const float* dh, const float* dc, float* dgates_ws, float* dx, float* dc_prev, float* dh_prev,
                         float* dw, float* db, int B, int H, int W, int flags, void* scratch, size_t scratch_bytes,
                         bin_stream_t s) {
-  if (!x || !w || !b || !dgates_ws || !dx || !dw || !db) return fail(BIN_ERR_ARG, "convlstm_bwd: null argument");
+  if (!x || !w || !b || !dgates_ws) return fail(BIN_ERR_ARG, "convlstm_bwd: null argument");
   if (flags & ~BIN_DETERMINISTIC) return fail(BIN_ERR_ARG, "convlstm_bwd: unknown flags");
   return launch_convlstm_bwd(x, c_prev, h_prev, w, b, dh, dc, dgates_ws, dx, dc_prev, dh_prev, dw, db, B, H, W,
                              (cudaStream_t)s, flags, scratch, scratch_bytes);
@@ -772,13 +812,18 @@ size_t bin_backbone_grad_workspace_bytes(int nframes, int Btot, int H, int W) {
   return valid_nframes(nframes) ? grad_ws(nframes, Btot, H, W, nullptr).bytes : 0;
 }
 size_t bin_backbone_grad_param_floats(int nframes) { return valid_nframes(nframes) ? grad_param_layout(nframes).floats : 0; }
+int bin_backbone_bwd_masked(int nframes, const void* blob_t, const bin_frames_t* dout, const bin_frames_t* dframes, int H,
+                            int W, const void* save_ws, void* grad_ws_ptr, size_t grad_ws_bytes, float* grad_params,
+                            const float* scale_dev, int flags, const unsigned char* need_host, bin_stream_t s) {
+  if (!blob_t || !dout || !dframes || !save_ws || !scale_dev) return fail(BIN_ERR_ARG, "backbone_bwd: null argument");
+  return run_backbone_bwd(nframes, blob_t, *dout, *dframes, H, W, save_ws, 0, nullptr, grad_ws_ptr, grad_ws_bytes,
+                          grad_params, scale_dev, (cudaStream_t)s, flags, need_host);
+}
 int bin_backbone_bwd_ex(int nframes, const void* blob_t, const bin_frames_t* dout, const bin_frames_t* dframes, int H,
                         int W, const void* save_ws, void* grad_ws_ptr, size_t grad_ws_bytes, float* grad_params,
                         const float* scale_dev, int flags, bin_stream_t s) {
-  if (!blob_t || !dout || !dframes || !save_ws || !grad_params || !scale_dev)
-    return fail(BIN_ERR_ARG, "backbone_bwd: null argument");
-  return run_backbone_bwd(nframes, blob_t, *dout, *dframes, H, W, save_ws, 0, nullptr, grad_ws_ptr, grad_ws_bytes,
-                          grad_params, scale_dev, (cudaStream_t)s, flags);
+  return bin_backbone_bwd_masked(nframes, blob_t, dout, dframes, H, W, save_ws, grad_ws_ptr, grad_ws_bytes, grad_params,
+                                 scale_dev, flags, nullptr, s);
 }
 int bin_backbone_bwd(int nframes, const void* blob_t, const bin_frames_t* dout, const bin_frames_t* dframes, int H, int W,
                      const void* save_ws, void* grad_ws_ptr, size_t grad_ws_bytes, float* grad_params,
@@ -786,14 +831,20 @@ int bin_backbone_bwd(int nframes, const void* blob_t, const bin_frames_t* dout, 
   return bin_backbone_bwd_ex(nframes, blob_t, dout, dframes, H, W, save_ws, grad_ws_ptr, grad_ws_bytes, grad_params,
                              scale_dev, 0, s);
 }
+int bin_backbone_bwd_recompute_masked(int nframes, const void* blob, const void* blob_t, const bin_frames_t* dout,
+                                      const bin_frames_t* dframes, int H, int W, const void* fwd_ws, size_t fwd_ws_bytes,
+                                      void* grad_ws_ptr, size_t grad_ws_bytes, float* grad_params, const float* scale_dev,
+                                      int flags, const unsigned char* need_host, bin_stream_t s) {
+  if (!blob || !blob_t || !dout || !dframes || !fwd_ws || !scale_dev) return fail(BIN_ERR_ARG, "backbone_bwd: null argument");
+  return run_backbone_bwd(nframes, blob_t, *dout, *dframes, H, W, fwd_ws, fwd_ws_bytes, blob, grad_ws_ptr, grad_ws_bytes,
+                          grad_params, scale_dev, (cudaStream_t)s, flags, need_host);
+}
 int bin_backbone_bwd_recompute_ex(int nframes, const void* blob, const void* blob_t, const bin_frames_t* dout,
                                   const bin_frames_t* dframes, int H, int W, const void* fwd_ws, size_t fwd_ws_bytes,
                                   void* grad_ws_ptr, size_t grad_ws_bytes, float* grad_params, const float* scale_dev,
                                   int flags, bin_stream_t s) {
-  if (!blob || !blob_t || !dout || !dframes || !fwd_ws || !grad_params || !scale_dev)
-    return fail(BIN_ERR_ARG, "backbone_bwd: null argument");
-  return run_backbone_bwd(nframes, blob_t, *dout, *dframes, H, W, fwd_ws, fwd_ws_bytes, blob, grad_ws_ptr, grad_ws_bytes,
-                          grad_params, scale_dev, (cudaStream_t)s, flags);
+  return bin_backbone_bwd_recompute_masked(nframes, blob, blob_t, dout, dframes, H, W, fwd_ws, fwd_ws_bytes, grad_ws_ptr,
+                                           grad_ws_bytes, grad_params, scale_dev, flags, nullptr, s);
 }
 int bin_backbone_bwd_recompute(int nframes, const void* blob, const void* blob_t, const bin_frames_t* dout,
                                const bin_frames_t* dframes, int H, int W, const void* fwd_ws, size_t fwd_ws_bytes,

@@ -238,6 +238,7 @@ __global__ void pixel_unshuffle_kernel(const __half* __restrict__ du, __half* __
 }
 // Backward of pack_frames + of the final "+ mean(frames)": for call k, frame f (fp32 NCHW):
 //   dframe = inv_scale * depth_to_space(dX0 channels of frame f) + dOut / nframes
+// A NULL dfr.frame[call][f] is a frame whose gradient nobody asked for: nothing is written for it.
 __global__ void unpack_frames_grad_kernel(const __half* __restrict__ dx0, int planes, const __grid_constant__ bin_frames_t dout,
                                           const __grid_constant__ bin_frames_t dfr, int H, int W, const float* __restrict__ scale) {
   const int h = H / 2, w = W / 2;
@@ -251,6 +252,7 @@ __global__ void unpack_frames_grad_kernel(const __half* __restrict__ dx0, int pl
     const int f = (i / ((size_t)w * h * 3)) % dfr.nframes;
     const int b = i / ((size_t)w * h * 3 * dfr.nframes);
     const int call = b / dfr.Bc, bb = b % dfr.Bc;
+    if (dfr.frame[call][f] == nullptr) continue;
     const int c4 = (f * 3 + rgb) * 4;                 // packed channels c4..c4+3 = (dy,dx) of this (frame,rgb)
     const __half* src = dx0 + ((((size_t)b * planes + (c4 >> 3)) * h + y) * w + x) * 8 + (c4 & 7);
     const float* go = dout.out[call] + (((size_t)bb * 3 + rgb) * H + 2 * y) * W + 2 * x;
@@ -687,7 +689,7 @@ __global__ void __launch_bounds__(288) convlstm_bwd_weights_kernel(const float* 
       for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
       if (lane == 0) {
         if (partial) partial[(size_t)blockIdx.x * kLstmGradN + (k * 6 + c) * 9 + tap] = v;
-        else atomicAdd(dw + (k * 6 + c) * 9 + tap, v);
+        else if (dw) atomicAdd(dw + (k * 6 + c) * 9 + tap, v);
       }
     }
     if (tap == 0) {
@@ -695,7 +697,7 @@ __global__ void __launch_bounds__(288) convlstm_bwd_weights_kernel(const float* 
       for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
       if (lane == 0) {
         if (partial) partial[(size_t)blockIdx.x * kLstmGradN + 648 + k] = v;
-        else atomicAdd(db + k, v);
+        else if (db) atomicAdd(db + k, v);
       }
     }
   }
@@ -706,8 +708,8 @@ __global__ void __launch_bounds__(256) convlstm_wgrad_reduce_kernel(const float*
   if (o >= kLstmGradN) return;
   const float s = ordered_warp_sum(partial + o, nparts, (size_t)kLstmGradN);
   if ((threadIdx.x & 31) == 0) {
-    if (o < 648) dw[o] += s;
-    else db[o - 648] += s;
+    if (o < 648) { if (dw) dw[o] += s; }
+    else if (db) db[o - 648] += s;
   }
 }
 // Pass 3: dx[c][q] = sum_{k,tap} W[k][c][tap] * dgates[k][q - off(tap)]  (and dh_prev for c = 3..5).
@@ -741,7 +743,7 @@ __global__ void convlstm_bwd_input_kernel(const float* __restrict__ dgates, cons
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
       const size_t off = ((size_t)b * 3 + c) * hw + (size_t)y * W + xw;
-      dx[off] = acc[c];
+      if (dx) dx[off] = acc[c];
       if (dh_prev) dh_prev[off] = acc[3 + c];
     }
   }
@@ -1250,21 +1252,29 @@ int launch_convlstm_bwd(const float* x, const float* c_prev, const float* h_prev
                         float* dw, float* db, int B, int H, int W, cudaStream_t s, int flags, void* scratch,
                         size_t scratch_bytes) {
   if ((c_prev == nullptr) != (h_prev == nullptr)) return fail(BIN_ERR_ARG, "convlstm_bwd: give both c_prev and h_prev or neither");
-  const bool det = flags & BIN_DETERMINISTIC;
+  // NULL outputs are not asked for: the weight pass runs when dw or db is wanted, the input pass when dx or dh_prev is,
+  // and the gates pass (which also writes dc_prev) when anything is.  What runs is unchanged, so its bits are too.
+  const bool weights = dw || db, inputs = dx || dh_prev;
+  const bool det = (flags & BIN_DETERMINISTIC) && weights;     // the scratch holds the weight pass's partials only
   if (det && !scratch) return fail(BIN_ERR_ARG, "convlstm_bwd: BIN_DETERMINISTIC needs a scratch buffer");
   if (det && scratch_bytes < convlstm_bwd_scratch_bytes(B, H, W)) return fail(BIN_ERR_WORKSPACE, "convlstm_bwd: scratch too small");
   const size_t total = (size_t)B * H * W;
+  if (!weights && !inputs && !dc_prev) return BIN_OK;
   convlstm_bwd_gates_kernel<<<grid_for(total, 128), 128, 0, s>>>(x, c_prev, h_prev, w, b, dh, dc, dgates_ws, dc_prev, B, H, W);
   BIN_CUDA_OK(cudaGetLastError());
-  const unsigned wblocks = convlstm_wgrad_blocks(total);
-  convlstm_bwd_weights_kernel<<<wblocks, 288, 0, s>>>(x, h_prev, dgates_ws, dw, db, B, H, W, det ? (float*)scratch : nullptr);
-  BIN_CUDA_OK(cudaGetLastError());
-  if (det) {
-    convlstm_wgrad_reduce_kernel<<<(kLstmGradN + 7) / 8, 256, 0, s>>>((const float*)scratch, (int)wblocks, dw, db);
+  if (weights) {
+    const unsigned wblocks = convlstm_wgrad_blocks(total);
+    convlstm_bwd_weights_kernel<<<wblocks, 288, 0, s>>>(x, h_prev, dgates_ws, dw, db, B, H, W, det ? (float*)scratch : nullptr);
+    BIN_CUDA_OK(cudaGetLastError());
+    if (det) {
+      convlstm_wgrad_reduce_kernel<<<(kLstmGradN + 7) / 8, 256, 0, s>>>((const float*)scratch, (int)wblocks, dw, db);
+      BIN_CUDA_OK(cudaGetLastError());
+    }
+  }
+  if (inputs) {
+    convlstm_bwd_input_kernel<<<grid_for(total, 128), 128, 0, s>>>(dgates_ws, w, dx, dh_prev, B, H, W);
     BIN_CUDA_OK(cudaGetLastError());
   }
-  convlstm_bwd_input_kernel<<<grid_for(total, 128), 128, 0, s>>>(dgates_ws, w, dx, dh_prev, B, H, W);
-  BIN_CUDA_OK(cudaGetLastError());
   return BIN_OK;
 }
 int launch_wgrad_impl(const bin_act_t& x0, int x0_plane0, int x0_planes, const bin_act_t& x1, int x1_plane0, int x1_planes,

@@ -50,6 +50,12 @@ def _check_frames(frames: Sequence[torch.Tensor]) -> Tuple[int, int, int]:
     return B, H, W
 
 
+def _needs_grad(tensors) -> bool:
+    """Whether a call takes the autograd path: grad mode is on and some tensor it reads (frames, states, any weight)
+    requires a gradient.  Every tensor counts: a net whose first layer alone is frozen must still train the rest."""
+    return torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in tensors)
+
+
 # --------------------------------------------------------------------------------------------
 # reference RDN.py:9-95
 # --------------------------------------------------------------------------------------------
@@ -68,7 +74,8 @@ class ConvLSTMCell(nn.Module):
         self.Gates.bias.data.zero_()
 
     def forward(self, input_, prev_state):
-        if torch.is_grad_enabled() and (input_.requires_grad or self.Gates.weight.requires_grad):
+        state_ts = () if prev_state is None else (prev_state[0], prev_state[1])
+        if _needs_grad((input_, self.Gates.weight, self.Gates.bias) + state_ts):
             from .autograd import convlstm_apply
             return convlstm_apply(self, input_, prev_state)
         state = None if prev_state is None else (prev_state[0], prev_state[1])     # (c, h), RDN.py:71
@@ -209,7 +216,7 @@ class _Backbone(nn.Module):
     def _forward_frames(self, *frames):
         if len(frames) != self.NFRAMES:
             raise BinB200Error(f"{type(self).__name__} takes {self.NFRAMES} frames")
-        if torch.is_grad_enabled() and (any(f.requires_grad for f in frames) or self.SFENet1.weight.requires_grad):
+        if _needs_grad(list(frames) + self._conv_params()):
             from .autograd import backbone_apply
             return backbone_apply(self, frames)
         frames = [f.contiguous() for f in frames]
@@ -341,8 +348,9 @@ class RDN_residual_interp_5_input(nn.Module):
     def forward(self, B1, B3, B5, B7, B9, previous_input=None):
         """10 backbone calls of RDN.py:367-405, issued as 4 batched launches (same-weight calls
         ride along the batch dimension)."""
-        if torch.is_grad_enabled() and (any(t.requires_grad for t in (B1, B3, B5, B7, B9)) or
-                                        self.model1_1.SFENet1.weight.requires_grad):
+        prev = list(previous_input) if previous_input is not None and previous_input[0] is not None else []
+        if _needs_grad([B1, B3, B5, B7, B9] + prev + [p for m in (self.model1_1, self.model2_1, self.model3_1,
+                                                                   self.model4_1) for p in m._conv_params()]):
             from .autograd import pyramid_apply
             return pyramid_apply(self, B1, B3, B5, B7, B9, previous_input)
         m1, m2, m3, m4 = self.model1_1, self.model2_1, self.model3_1, self.model4_1
@@ -491,8 +499,8 @@ class RDN_residual_interp_5_input_ConvLSTM_L(nn.Module):
         """BASELINE config 2a: stages 1-3 on 4 frames -> [I2',I4',I6',I3',I5',I4''] (SURVEY 8d)."""
         if _ensemble_of(self) is not None:
             raise BinB200Error("forward_pyramid3 has no self-ensemble mode; set_self_ensemble(net, None) first")
-        if torch.is_grad_enabled() and (any(f.requires_grad for f in (B1, B3, B5, B7)) or
-                                        self.model.model1_1.SFENet1.weight.requires_grad):
+        pyr = self.model
+        if _needs_grad([B1, B3, B5, B7] + [p for m in (pyr.model1_1, pyr.model2_1, pyr.model3_1) for p in m._conv_params()]):
             from .autograd import pyramid3_apply                      # BASELINE config 3a (training on the 4-frame graph)
             return pyramid3_apply(self, (B1, B3, B5, B7))
         frames = [f.contiguous() for f in (B1, B3, B5, B7)]

@@ -33,7 +33,7 @@
 extern "C" {
 #endif
 
-#define BIN_ABI_VERSION 4
+#define BIN_ABI_VERSION 5
 #define BIN_MAX_CALLS 6   /* same-weight backbone calls batched along N */
 #define BIN_MAX_FRAMES 5  /* frames per backbone call (2, 3 or 5) */
 #define BIN_MAX_LOSS_PAIRS 20 /* (prediction, target) pairs of one fused loss call */
@@ -153,7 +153,9 @@ int bin_convlstm_fwd(const float* x, const float* c_prev, const float* h_prev, c
                      float* h_out, float* c_out, int B, int H, int W, bin_stream_t s);
 
 /* Backward of the cell: dh/dc = gradients of the two outputs (either may be NULL = zero); dgates_ws = scratch
- * (B,12,H,W) fp32; writes dx (and dc_prev/dh_prev when a state was given), ACCUMULATES into dw (12,6,3,3) and db (12). */
+ * (B,12,H,W) fp32; writes dx (and dc_prev/dh_prev when a state was given), ACCUMULATES into dw (12,6,3,3) and db (12).
+ * Any of dx, dc_prev, dh_prev, dw, db may be NULL: that gradient is not computed (no dw and no db skips the weight
+ * pass, no dx and no dh_prev the input pass; the others are unchanged). */
 int bin_convlstm_bwd(const float* x, const float* c_prev, const float* h_prev, const float* w, const float* b,
                      const float* dh, const float* dc, float* dgates_ws, float* dx, float* dc_prev, float* dh_prev,
                      float* dw, float* db, int B, int H, int W, bin_stream_t s);
@@ -212,6 +214,20 @@ int bin_backbone_bwd_recompute_ex(int nframes, const void* blob, const void* blo
                                   const bin_frames_t* dframes, int H, int W, const void* fwd_ws, size_t fwd_ws_bytes,
                                   void* grad_ws, size_t grad_ws_bytes, float* grad_params, const float* scale_dev,
                                   int flags, bin_stream_t s);
+/* The two backwards for a partly frozen network (the _ex calls above = need_host NULL).  need_host: host array of
+ * 2 * BIN_BACKBONE_NCONV bytes, nonzero where a gradient is wanted: weight then bias of conv 0..65, the order of
+ * grad_params; NULL = all.  A NULL dframes->frame[k][f] = no gradient for that frame.  Gradients not asked for are not
+ * computed and their grad_params entries are left untouched; grad_params may be NULL when need_host asks for none.  The
+ * data gradient of conv k's input is computed only if a frame or a tensor of a lower-index conv wants a gradient, and
+ * the walk stops once none does.  Everything that is computed runs the launches of the full backward on the same
+ * operands in the same order, so the gradients that are kept have its bits. */
+int bin_backbone_bwd_masked(int nframes, const void* blob_t, const bin_frames_t* dout, const bin_frames_t* dframes, int H,
+                            int W, const void* save_ws, void* grad_ws, size_t grad_ws_bytes, float* grad_params,
+                            const float* scale_dev, int flags, const unsigned char* need_host, bin_stream_t s);
+int bin_backbone_bwd_recompute_masked(int nframes, const void* blob, const void* blob_t, const bin_frames_t* dout,
+                                      const bin_frames_t* dframes, int H, int W, const void* fwd_ws, size_t fwd_ws_bytes,
+                                      void* grad_ws, size_t grad_ws_bytes, float* grad_params, const float* scale_dev,
+                                      int flags, const unsigned char* need_host, bin_stream_t s);
 /* Loss scale for one backbone backward: *scale_dev = 2^floor(log2(target / max_k max|gouts[k]|)) (a power of two, so
  * scaling and un-scaling are exact), computed on the device -- no host synchronisation.  gouts_host: host array of n
  * (<= BIN_MAX_CALLS) device pointers to fp32 tensors of `numel` elements, 16-byte aligned; tmp4_dev: 4 bytes of scratch. */
