@@ -14,6 +14,7 @@ BIN_BACKBONE_NCONV = 66
 BIN_FLIPX4_MAX_TENSORS = 14
 BIN_TRAIN_MAX_BATCH = 16
 BIN_TRAIN_FRAMES = 17
+BIN_PNG_MAX_BATCH = 16
 EPI_P8, EPI_PIXSHUF, EPI_FINAL = 0, 1, 2
 BIN_DETERMINISTIC = 1                 # flags bit of the *_ex entry points
 ABI_VERSION = 5
@@ -130,6 +131,10 @@ _SIGS = {
     "bin_flipx4_expand": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)] + [C.c_int] * 4 + [C.c_void_p]),
     "bin_flipx4_mean": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)] + [C.c_int] * 4 + [C.c_void_p]),
     "bin_train_batch_u8": (C.c_int, [C.POINTER(TrainSample)] + [C.c_int] * 3 + [C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
+    "bin_png_max_bytes": (C.c_size_t, [C.c_int, C.c_int]),
+    "bin_png_workspace_bytes": (C.c_size_t, [C.c_int] * 3),
+    "bin_png_encode_u8": (C.c_int, [C.POINTER(C.c_void_p)] + [C.c_int] * 3 + [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p,
+                                                                               C.c_size_t, C.c_void_p]),
 }
 
 _lib = None

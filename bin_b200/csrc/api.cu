@@ -86,6 +86,10 @@ int launch_image_metrics_u8(const uint8_t* a, const uint8_t* b, int h, int w, in
 int launch_flipx4(int expand, const float* const* src, float* const* dst, int n, int B, int H, int W, cudaStream_t s);
 int launch_train_batch_u8(const bin_train_sample_t* samples, int B, int h, int w, float* dst, int dst_B, int b0,
                           cudaStream_t s);
+size_t png_max_bytes(int h, int w);
+size_t png_workspace_bytes(int n, int h, int w);
+int launch_png_encode_u8(const uint8_t* const* imgs_host, int n, int h, int w, uint8_t* out, size_t out_stride,
+                         int64_t* sizes, void* workspace, size_t workspace_bytes, cudaStream_t s);
 int launch_rdb_tail(const bin_act_t& x, int x_plane0, const bin_act_t& g, int g_plane0, const void* w_conv,
                     const float* b_conv, const void* w_lff, const float* b_lff, const bin_act_t& out, int out_plane0,
                     int b_begin, int b_count, int y_begin, int y_count, cudaStream_t s, bool reverse = false);
@@ -997,6 +1001,12 @@ int bin_flipx4_mean(const float* const* src_host, float* const* dst_host, int n,
 int bin_train_batch_u8(const bin_train_sample_t* samples_host, int B, int h, int w, float* dst, int dst_B, int b0,
                        bin_stream_t s) {
   return launch_train_batch_u8(samples_host, B, h, w, dst, dst_B, b0, (cudaStream_t)s);
+}
+size_t bin_png_max_bytes(int h, int w) { return png_max_bytes(h, w); }
+size_t bin_png_workspace_bytes(int n, int h, int w) { return png_workspace_bytes(n, h, w); }
+int bin_png_encode_u8(const uint8_t* const* imgs_host, int n, int h, int w, uint8_t* out, size_t out_stride,
+                      int64_t* sizes, void* workspace, size_t workspace_bytes, bin_stream_t s) {
+  return launch_png_encode_u8(imgs_host, n, h, w, out, out_stride, sizes, workspace, workspace_bytes, (cudaStream_t)s);
 }
 
 }  // extern "C"

@@ -363,6 +363,23 @@ typedef struct {
 int bin_train_batch_u8(const bin_train_sample_t* samples_host, int B, int h, int w, float* dst, int dst_B, int b0,
                        bin_stream_t s);
 
+/* ---- PNG output of the caller loop: test.py / demo.py cv2.imwrite(path.png, uint8 BGR image) ------------------- */
+/* Each file holds IHDR (8-bit truecolour), 8192-byte IDAT chunks and IEND; its inflated payload is the one cv2.imwrite
+ * writes (RGB; filter type 1, Sub, on every row, 0 when w = 1; deflate with literals and distance-1 matches as zlib's
+ * Z_RLE parses them), so any decoder returns the same pixels.  The bytes depend only on the pixels and (h, w). */
+#define BIN_PNG_MAX_BATCH 16
+/* Exact worst-case file size (every deflate block stored); 0 if (h, w) is out of range. */
+size_t bin_png_max_bytes(int h, int w);
+size_t bin_png_workspace_bytes(int n, int h, int w);   /* 0 if n, h or w is out of range */
+/* imgs_host: n device pointers to uint8 (h,w,3) BGR, row pitch 3w (what bin_tensor2img_u8 writes and cv2.imwrite
+ * takes).  out: device, n slots of out_stride >= bin_png_max_bytes(h,w) bytes; slot i receives a complete PNG file
+ * and sizes[i] (device int64) its length.  1 <= n <= BIN_PNG_MAX_BATCH, 1 <= h,w <= 65535, h*(3w+1) < 2^31.
+ * workspace: 256-byte aligned.  A null pointer, a bad n, h or w, an undersized or overflowing stride fail with
+ * BIN_ERR_ARG and a small workspace with BIN_ERR_WORKSPACE, before the first CUDA call.  Nothing outside
+ * [out, out + n*out_stride), sizes[0..n) and the workspace is written. */
+int bin_png_encode_u8(const uint8_t* const* imgs_host, int n, int h, int w, uint8_t* out, size_t out_stride,
+                      int64_t* sizes, void* workspace, size_t workspace_bytes, bin_stream_t s);
+
 #ifdef __cplusplus
 }
 #endif
