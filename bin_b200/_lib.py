@@ -63,6 +63,8 @@ _SIGS = {
     "bin_pack_frames": (C.c_int, [C.POINTER(Frames), C.c_int, C.c_int, Act, C.c_void_p]),
     "bin_packed_weight_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int]),
     "bin_pack_conv_weight": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "bin_pack_frames_p": (C.c_int, [C.POINTER(Frames), C.c_int, C.c_int, Act, C.c_int, C.c_void_p]),
+    "bin_pack_conv_weight_p": (C.c_int, [C.c_void_p] + [C.c_int] * 7 + [C.c_void_p, C.c_void_p]),
     "bin_conv_fwd": (C.c_int, [C.POINTER(ConvArgs), C.c_void_p]),
     "bin_pack_conv_weight_t": (C.c_int, [C.c_void_p] + [C.c_int] * 7 + [C.c_void_p, C.c_void_p]),
     "bin_conv_wgrad_workspace_bytes": (C.c_size_t, []),

@@ -683,6 +683,17 @@ int bin_pack_conv_weight(const float* w_oihw, int cout, int cin, int ksize, int 
                          void* packed, bin_stream_t s) {
   return launch_pack_weight(w_oihw, cout, cin, ksize, cout_pad, cin_pad, variant, packed, (cudaStream_t)s);
 }
+int bin_pack_frames_p(const bin_frames_t* fr, int H, int W, bin_act_t dst, int prec, bin_stream_t s) {
+  if (!fr) return fail(BIN_ERR_ARG, "pack_frames: null frame table");
+  if (prec != BIN_PREC_F16 && prec != BIN_PREC_F32X3) return fail(BIN_ERR_ARG, "pack_frames: unknown precision");
+  return launch_pack_frames(*fr, H, W, dst, (cudaStream_t)s, prec == BIN_PREC_F32X3);
+}
+int bin_pack_conv_weight_p(const float* w_oihw, int cout, int cin, int ksize, int cout_pad, int cin_pad, int variant,
+                           int prec, void* packed, bin_stream_t s) {
+  if (prec != BIN_PREC_F16 && prec != BIN_PREC_F32X3) return fail(BIN_ERR_ARG, "pack_conv_weight: unknown precision");
+  return launch_pack_weight(w_oihw, cout, cin, ksize, cout_pad, cin_pad, variant, packed, (cudaStream_t)s,
+                            prec == BIN_PREC_F32X3);
+}
 int bin_pack_conv_weight_t(const float* w_oihw, int cout, int cin, int ksize, int row0, int nrows, int cout_pad_t,
                            int cin_pad_t, void* packed, bin_stream_t s) {
   return launch_pack_weight_t(w_oihw, cout, cin, ksize, row0, nrows, cout_pad_t, cin_pad_t, packed, (cudaStream_t)s);
@@ -970,8 +981,7 @@ int bin_pyramid3_fwd(const bin_net_t* net, const float* const* F, float* const* 
 int bin_rdb_tail_fwd(const bin_act_t* x, int x_plane0, const bin_act_t* g, int g_plane0, const void* w_conv,
                      const float* b_conv, const void* w_lff, const float* b_lff, const bin_act_t* out, int out_plane0,
                      int b_begin, int b_count, int y_begin, int y_count, bin_stream_t s) {
-  if (!x || !g || !out || !x->ptr || !g->ptr || !out->ptr || !w_conv || !b_conv || !w_lff || !b_lff)
-    return fail(BIN_ERR_ARG, "rdb_tail_fwd: null argument");
+  if (!x || !g || !out) return fail(BIN_ERR_ARG, "rdb_tail_fwd: null argument");
   return launch_rdb_tail(*x, x_plane0, *g, g_plane0, w_conv, b_conv, w_lff, b_lff, *out, out_plane0, b_begin, b_count,
                          y_begin, y_count, (cudaStream_t)s);
 }

@@ -68,9 +68,11 @@ __device__ __forceinline__ float2 unpack_h2(uint32_t u) {
 
 constexpr int kThreads = 384;   // warpgroup 0: TMA producer (one thread); warpgroups 1, 2: wgmma + epilogue
 
-// X3 ("fp32-accurate" mode, 1e-5 parity bar): every value is carried as an fp16 pair hi + lo (22 significant bits).
+// X3 ("fp32-accurate" mode, 1e-5 parity bar): every value is carried as an fp16 pair hi = fp16(x), lo = fp16(x - hi).
+// The pair is within 2^-22 |x| of x while lo is a normal fp16 number; below |x| ~ 2^-3 lo is subnormal and the pair
+// carries an absolute 2^-25 instead (the fp16 subnormal half-spacing), which is what tests/test_gpu_forward_fuzz.py bars.
 // Tensors hold, per 32-channel chunk, 4 planes of hi followed by 4 planes of lo; a logical K chunk becomes three
-// physical chunks  x_hi*W_hi + x_lo*W_hi + x_hi*W_lo  (the lo*lo term is below 2^-22), the weights are packed
+// physical chunks  x_hi*W_hi + x_lo*W_hi + x_hi*W_lo  (the lo*lo term is below 2^-22 |x w|), the weights are packed
 // pre-scaled by 2^8 so that W_lo stays a normal fp16 number, and the epilogue un-scales the fp32 accumulator and
 // splits its result into (hi, lo) again.  Same kernel, same descriptors: 3x the MMAs, 2x the activation bytes.
 __device__ __forceinline__ int x3_plane(int logical_plane) { return 2 * (logical_plane & ~3) + (logical_plane & 3); }
@@ -369,17 +371,14 @@ int make_p8_tmap_box(CUtensorMap* m, const bin_act_t& t, int box_px, int box_row
   return BIN_OK;
 }
 
+// Every argument check of a conv launch runs before the first tensor map is encoded (launch_conv_t, then the
+// shared-memory fit here), so a rejected call has touched neither the driver nor the device.
 template <int NT, int KS, int EPI, bool SX, bool X3>
 static int launch_inst(const bin_conv_args_t& a, cudaStream_t s, bool reverse) {
   using C = ConvCfg<NT, KS, SX>;
   ConvParams p;
   memset(&p, 0, sizeof(p));
   const int H = a.in0.H, W = a.in0.W, B = a.in0.B;
-  BIN_TRY(make_p8_tmap(&p.tmap0, a.in0, C::ROWS));
-  if (a.in1_planes > 0) {
-    if (a.in1.H != H || a.in1.W != W || a.in1.B != B) return fail(BIN_ERR_ARG, "in1 geometry differs from in0");
-    BIN_TRY(make_p8_tmap(&p.tmap1, a.in1, C::ROWS));
-  }
   // X3: plane indices are LOGICAL (the tensors hold 2x the planes: hi/lo groups of 4), K has 3 chunks per logical chunk
   p.plane0_0 = a.in0_plane0; p.nch0l = a.in0_planes / kKPL; p.nch0 = (X3 ? 3 : 1) * p.nch0l;
   p.plane0_1 = a.in1_plane0; p.nch1 = (X3 ? 3 : 1) * (a.in1_planes / kKPL);
@@ -388,9 +387,7 @@ static int launch_inst(const bin_conv_args_t& a, cudaStream_t s, bool reverse) {
   p.H = H; p.W = W; p.Btot = B;
   p.b0 = a.b_begin; p.y0 = a.y_begin;
   const int nb = a.b_count > 0 ? a.b_count : B - a.b_begin;
-  p.ny = a.y_count > 0 ? a.y_count : H - a.y_begin;
-  if (p.b0 < 0 || p.y0 < 0 || nb < 1 || p.ny < 1 || p.b0 + nb > B || p.y0 + p.ny > H)
-    return fail(BIN_ERR_ARG, "conv: batch/row sub-range outside the tensor");
+  p.ny = a.y_count > 0 ? a.y_count : H - a.y_begin;   // launch_conv_t has checked the sub-range
   p.tiles_x = (W + C::TW - 1) / C::TW;
   p.tiles_y = (p.ny + kTH - 1) / kTH;
   p.nh = a.cout_pad / NT;
@@ -422,6 +419,8 @@ static int launch_inst(const bin_conv_args_t& a, cudaStream_t s, bool reverse) {
   p.res = reinterpret_cast<const __half*>(a.res.ptr); p.res_planes = a.res.planes; p.res_plane0 = a.res_plane0;
   p.fr = a.fr;
   p.reverse = (reverse && EPI == BIN_EPI_P8) ? 1 : 0;
+  BIN_TRY(make_p8_tmap(&p.tmap0, a.in0, C::ROWS));
+  if (a.in1_planes > 0) BIN_TRY(make_p8_tmap(&p.tmap1, a.in1, C::ROWS));
   auto kern = conv_igemm_kernel<NT, KS, EPI, SX, X3>;
   static std::atomic<unsigned long long> smem_opted{0};   // per instantiation, per device
   BIN_TRY(ensure_dynamic_smem(kern, kSmemMax, smem_opted));
@@ -445,38 +444,70 @@ static int launch_inst(const bin_conv_args_t& a, cudaStream_t s, bool reverse) {
 template <bool X3>
 static int launch_conv_t(const bin_conv_args_t& a, cudaStream_t s, bool reverse) {
   constexpr int f = X3 ? 2 : 1;      // X3 tensors hold hi+lo: twice the planes of their logical channel count
-  if (a.in0_planes % kKPL || a.in1_planes % kKPL || a.in0_planes <= 0)
-    return fail(BIN_ERR_ARG, "input plane counts must be positive multiples of 4 (32 channels)");
+  // one past the last PHYSICAL plane that logical planes [plane0, plane0 + n) occupy (X3: the lo plane of the last one)
+  auto plane_end = [](int plane0, int n) { return X3 ? 2 * ((plane0 + n - 1) & ~3) + ((plane0 + n - 1) & 3) + 5 : plane0 + n; };
+  auto misaligned = [](const void* ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15) != 0; };
+  const bool has_in1 = a.in1_planes > 0;
+  const int H = a.in0.H, W = a.in0.W, B = a.in0.B;
+  // ---- geometry: plane counts, offsets and ranges, shapes, sub-range, epilogue options
+  if (a.in0_planes % kKPL || a.in1_planes % kKPL || a.in0_planes <= 0 || a.in1_planes < 0)
+    return fail(BIN_ERR_ARG, "conv: input plane counts must be positive multiples of 4 (32 channels)");
+  if (a.in0_plane0 < 0 || (has_in1 && a.in1_plane0 < 0) || a.out_plane0 < 0 || (a.res.ptr && a.res_plane0 < 0) ||
+      a.store_planes < 0)
+    return fail(BIN_ERR_ARG, "conv: negative plane offset or store_planes");
   if (X3 && ((a.in0_plane0 | a.in1_plane0 | a.out_plane0 | a.res_plane0) & 3))
-    return fail(BIN_ERR_ARG, "x3 mode: plane offsets must be multiples of 4");
-  if (f * (a.in0_plane0 + a.in0_planes) > a.in0.planes || (a.in1_planes > 0 && f * (a.in1_plane0 + a.in1_planes) > a.in1.planes))
-    return fail(BIN_ERR_ARG, "input plane range exceeds tensor");
+    return fail(BIN_ERR_ARG, "conv: x3 mode: plane offsets must be multiples of 4");
+  if (f * (a.in0_plane0 + a.in0_planes) > a.in0.planes || (has_in1 && f * (a.in1_plane0 + a.in1_planes) > a.in1.planes))
+    return fail(BIN_ERR_ARG, "conv: input plane range exceeds tensor");
+  if (has_in1 && (a.in1.H != H || a.in1.W != W || a.in1.B != B)) return fail(BIN_ERR_ARG, "conv: in1 geometry differs from in0");
+  const int nb = a.b_count > 0 ? a.b_count : B - a.b_begin;
+  const int ny = a.y_count > 0 ? a.y_count : H - a.y_begin;
+  if (a.b_begin < 0 || a.y_begin < 0 || a.b_count < 0 || a.y_count < 0 || nb < 1 || ny < 1 || a.b_begin + nb > B ||
+      a.y_begin + ny > H)
+    return fail(BIN_ERR_ARG, "conv: batch/row sub-range outside the tensor");
+  if (a.epilogue != BIN_EPI_P8 && (a.relu || a.res.ptr))
+    return fail(BIN_ERR_ARG, "conv: the pixel-shuffle and final epilogues take no ReLU and no residual");
+  const bool sx = a.ksize == 3 && a.cout_pad == 32 && a.variant == BIN_CONV_DEFAULT;
   if (a.epilogue == BIN_EPI_P8) {
     const int nstore = a.store_planes > 0 ? a.store_planes : a.cout_pad / 8;
-    if (a.out.H != a.in0.H || a.out.W != a.in0.W || a.out.B != a.in0.B || nstore > a.cout_pad / 8 ||
-        f * (a.out_plane0 + nstore) > a.out.planes + (X3 ? 4 : 0))
-      return fail(BIN_ERR_ARG, "output tensor geometry mismatch");
-    if (a.res.ptr && (a.res.H != a.in0.H || a.res.W != a.in0.W || a.res.B != a.in0.B ||
-                      f * (a.res_plane0 + nstore) > a.res.planes + (X3 ? 4 : 0)))
-      return fail(BIN_ERR_ARG, "residual tensor geometry mismatch");
-    if (a.ksize == 3 && a.cout_pad == 32 && a.variant == 0) return launch_inst<32, 3, BIN_EPI_P8, true, X3>(a, s, reverse);
-    if (a.ksize == 3 && a.cout_pad == 32 && a.variant == 1 && !X3) return launch_inst<32, 3, BIN_EPI_P8, false, false>(a, s, reverse);
+    if (a.out.H != H || a.out.W != W || a.out.B != B || nstore > a.cout_pad / 8 || plane_end(a.out_plane0, nstore) > a.out.planes)
+      return fail(BIN_ERR_ARG, "conv: output tensor geometry mismatch");
+    if (a.res.ptr && (a.res.H != H || a.res.W != W || a.res.B != B || plane_end(a.res_plane0, nstore) > a.res.planes))
+      return fail(BIN_ERR_ARG, "conv: residual tensor geometry mismatch");
+    if (sx && a.res.ptr) return fail(BIN_ERR_ARG, "conv: the x-stacked 3x3 / Cout 32 kernel takes no residual");
+  } else if (a.epilogue == BIN_EPI_PIXSHUF) {
+    if (a.out.H != 2 * H || a.out.W != 2 * W || a.out.B != B || plane_end(a.out_plane0, a.cout_pad / 32) > a.out.planes)
+      return fail(BIN_ERR_ARG, "conv: pixel-shuffle output geometry mismatch");
+  } else if (a.epilogue == BIN_EPI_FINAL) {
+    if (a.fr.ncalls < 1 || a.fr.ncalls > BIN_MAX_CALLS || a.fr.nframes < 1 || a.fr.nframes > BIN_MAX_FRAMES ||
+        a.fr.Bc < 1 || a.fr.ncalls * a.fr.Bc != B)
+      return fail(BIN_ERR_ARG, "conv: frame table does not match the batch");
+  }
+  // ---- pointers
+  if (!a.in0.ptr || (has_in1 && !a.in1.ptr)) return fail(BIN_ERR_ARG, "conv: null input tensor");
+  if (misaligned(a.in0.ptr) || (has_in1 && misaligned(a.in1.ptr))) return fail(BIN_ERR_ARG, "conv: P8 tensor not 16-byte aligned");
+  if (!a.w_packed || !a.bias) return fail(BIN_ERR_ARG, "conv: null weights or bias");
+  if (a.epilogue != BIN_EPI_FINAL && !a.out.ptr) return fail(BIN_ERR_ARG, "conv: null output tensor");
+  if (a.epilogue == BIN_EPI_FINAL)
+    for (int k = 0; k < a.fr.ncalls; ++k) {
+      bool ok = a.fr.out[k] != nullptr;
+      for (int fi = 0; fi < a.fr.nframes; ++fi) ok = ok && a.fr.frame[k][fi] != nullptr;
+      if (!ok) return fail(BIN_ERR_ARG, "conv: null frame or output pointer in the frame table");
+    }
+  // ---- the instantiation
+  if (a.epilogue == BIN_EPI_P8) {
+    if (sx) return launch_inst<32, 3, BIN_EPI_P8, true, X3>(a, s, reverse);
+    if (a.ksize == 3 && a.cout_pad == 32 && a.variant == BIN_CONV_PLAIN && !X3) return launch_inst<32, 3, BIN_EPI_P8, false, false>(a, s, reverse);
     if (a.ksize == 3 && a.cout_pad % 96 == 0) return launch_inst<96, 3, BIN_EPI_P8, false, X3>(a, s, reverse);
     if (a.ksize == 5 && a.cout_pad == 96) return launch_inst<96, 5, BIN_EPI_P8, false, X3>(a, s, reverse);
     if (a.ksize == 1 && a.cout_pad % 96 == 0) return launch_inst<96, 1, BIN_EPI_P8, false, X3>(a, s, reverse);
   } else if (a.epilogue == BIN_EPI_PIXSHUF) {
-    if (a.out.H != 2 * a.in0.H || a.out.W != 2 * a.in0.W || a.out.B != a.in0.B ||
-        f * (a.out_plane0 + a.cout_pad / 32) > a.out.planes)
-      return fail(BIN_ERR_ARG, "pixel-shuffle output geometry mismatch");
     if (a.ksize == 3 && a.cout_pad == 256) return launch_inst<128, 3, BIN_EPI_PIXSHUF, false, X3>(a, s, reverse);
   } else if (a.epilogue == BIN_EPI_FINAL) {
-    if (a.fr.ncalls < 1 || a.fr.ncalls > BIN_MAX_CALLS || a.fr.nframes < 1 || a.fr.nframes > BIN_MAX_FRAMES ||
-        a.fr.ncalls * a.fr.Bc != a.in0.B)
-      return fail(BIN_ERR_ARG, "frame table does not match the batch");
-    if (a.ksize == 3 && a.cout_pad == 16 && a.variant == 0) return launch_inst<16, 3, BIN_EPI_FINAL, true, X3>(a, s, reverse);
-    if (a.ksize == 3 && a.cout_pad == 16 && a.variant == 1 && !X3) return launch_inst<16, 3, BIN_EPI_FINAL, false, false>(a, s, reverse);
+    if (a.ksize == 3 && a.cout_pad == 16 && a.variant == BIN_CONV_DEFAULT) return launch_inst<16, 3, BIN_EPI_FINAL, true, X3>(a, s, reverse);
+    if (a.ksize == 3 && a.cout_pad == 16 && a.variant == BIN_CONV_PLAIN && !X3) return launch_inst<16, 3, BIN_EPI_FINAL, false, false>(a, s, reverse);
   }
-  return fail(BIN_ERR_UNSUPPORTED, "no kernel instantiation for this conv (ksize/cout_pad/epilogue/precision)");
+  return fail(BIN_ERR_UNSUPPORTED, "conv: no kernel instantiation for this conv (ksize/cout_pad/epilogue/precision)");
 }
 
 int launch_conv(const bin_conv_args_t& a, cudaStream_t s, bool reverse) {

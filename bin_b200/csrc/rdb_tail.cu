@@ -253,12 +253,11 @@ int launch_rdb_tail(const bin_act_t& x, int x_plane0, const bin_act_t& g, int g_
   const int H = x.H, W = x.W, B = x.B;
   if (g.H != H || g.W != W || g.B != B || out.H != H || out.W != W || out.B != B)
     return fail(BIN_ERR_ARG, "rdb_tail: tensor geometry mismatch");
-  if (x_plane0 + 12 > x.planes || g_plane0 + 12 > g.planes || out_plane0 + 12 > out.planes)
+  if (x_plane0 < 0 || g_plane0 < 0 || out_plane0 < 0 || x_plane0 + 12 > x.planes || g_plane0 + 12 > g.planes ||
+      out_plane0 + 12 > out.planes)
     return fail(BIN_ERR_ARG, "rdb_tail: plane range exceeds tensor");
   RdbTailParams p;
   memset(&p, 0, sizeof(p));
-  BIN_TRY(make_p8_tmap(&p.tmap0, x, kRtRows));
-  BIN_TRY(make_p8_tmap(&p.tmap1, g, kRtRows));
   p.plane0_0 = x_plane0; p.plane0_1 = g_plane0;
   p.w_conv = reinterpret_cast<const uint8_t*>(w_conv); p.w_lff = reinterpret_cast<const uint8_t*>(w_lff);
   p.b_conv = b_conv; p.b_lff = b_lff;
@@ -268,12 +267,15 @@ int launch_rdb_tail(const bin_act_t& x, int x_plane0, const bin_act_t& g, int g_
   p.ny = y_count > 0 ? y_count : H - y_begin;
   if (p.b0 < 0 || p.y0 < 0 || nb < 1 || p.ny < 1 || p.b0 + nb > B || p.y0 + p.ny > H)
     return fail(BIN_ERR_ARG, "rdb_tail: batch/row sub-range outside the tensor");
+  if (!x.ptr || !g.ptr || !out.ptr || !w_conv || !b_conv || !w_lff || !b_lff) return fail(BIN_ERR_ARG, "rdb_tail_fwd: null argument");
   p.tiles_x = (W + kRtTW - 1) / kRtTW;
   p.tiles_y = (p.ny + kRtTH - 1) / kRtTH;
   p.ntiles = nb * p.tiles_x * p.tiles_y;
   p.out = reinterpret_cast<__half*>(out.ptr); p.out_planes = out.planes; p.out_plane0 = out_plane0;
   p.res = reinterpret_cast<const __half*>(x.ptr); p.res_planes = x.planes; p.res_plane0 = x_plane0;
   p.reverse = reverse ? 1 : 0;
+  BIN_TRY(make_p8_tmap(&p.tmap0, x, kRtRows));                // every argument is checked before the first tensor map
+  BIN_TRY(make_p8_tmap(&p.tmap1, g, kRtRows));
   static std::atomic<unsigned long long> opted{0};   // per device
   BIN_TRY(ensure_dynamic_smem(rdb_tail_kernel, kRtSmem, opted));
   const int sms = num_sms();

@@ -84,21 +84,25 @@ def make_frames(calls: Sequence[Sequence[torch.Tensor]], outs: Sequence[Optional
     return fr
 
 
-def pack_frames(calls: Sequence[Sequence[torch.Tensor]]) -> torch.Tensor:
-    """RDN.py:211 + 107-132: concat + space-to-depth + fp16 cast, batched over calls."""
+def pack_frames(calls: Sequence[Sequence[torch.Tensor]], prec: int = 0) -> torch.Tensor:
+    """RDN.py:211 + 107-132: concat + space-to-depth + fp16 cast, batched over calls.  prec=1 (BIN_PREC_F32X3): (hi, lo)
+    fp16 pairs, 4 hi planes then 4 lo planes per 32-channel chunk, so the result has twice the planes."""
     fr = make_frames(calls, [None] * len(calls))
     B, _, H, W = calls[0][0].shape
     cin_pad = (12 * fr.nframes + 31) // 32 * 32
-    dst = empty_p8(fr.ncalls * B, cin_pad // 8, H // 2, W // 2, calls[0][0].device)
-    check(lib().bin_pack_frames(C.byref(fr), H, W, act_view(dst), _stream()))
+    dst = empty_p8(fr.ncalls * B, cin_pad // 8 * (2 if prec else 1), H // 2, W // 2, calls[0][0].device)
+    check(lib().bin_pack_frames_p(C.byref(fr), H, W, act_view(dst), prec, _stream()))
     return dst
 
 
-def pack_conv_weight(w: torch.Tensor, cout_pad: int, cin_pad: int, variant: int = 0) -> torch.Tensor:
+def pack_conv_weight(w: torch.Tensor, cout_pad: int, cin_pad: int, variant: int = 0, prec: int = 0) -> torch.Tensor:
+    """prec=1 (BIN_PREC_F32X3): the three-slab split pack the x3 conv reads (3x the fp16 pack's size)."""
     w = _req(w, torch.float32, "weight")
     cout, cin, k, _ = w.shape
-    out = torch.empty(lib().bin_packed_weight_bytes(cout_pad, cin_pad, k) // 2, dtype=torch.float16, device=w.device)
-    check(lib().bin_pack_conv_weight(w.data_ptr(), cout, cin, k, cout_pad, cin_pad, variant, out.data_ptr(), _stream()))
+    n = lib().bin_packed_weight_bytes(cout_pad, cin_pad, k) // 2 * (3 if prec else 1)
+    out = torch.empty(n, dtype=torch.float16, device=w.device)
+    check(lib().bin_pack_conv_weight_p(w.data_ptr(), cout, cin, k, cout_pad, cin_pad, variant, prec, out.data_ptr(),
+                                       _stream()))
     return out
 
 
@@ -114,11 +118,15 @@ def conv_fwd(in0: torch.Tensor, w_packed: torch.Tensor, bias_pad: torch.Tensor, 
              relu: bool = False, epilogue: int = _lib.EPI_P8,
              out: Optional[torch.Tensor] = None, out_plane0: int = 0,
              res: Optional[torch.Tensor] = None, res_plane0: int = 0,
-             frames: Optional[Frames] = None, variant: int = 0, sub=None, store_planes: int = 0) -> None:
+             frames: Optional[Frames] = None, variant: int = 0, sub=None, store_planes: int = 0,
+             x3: bool = False) -> None:
+    """bin_conv_fwd.  x3=True runs the split-fp16 kernel: tensors hold (hi, lo) pairs (twice the planes), every plane
+    offset and count stays logical, and w_packed must come from pack_conv_weight(..., prec=1)."""
     a = ConvArgs()
     a.in0 = act_view(in0)
     a.in0_plane0 = in0_plane0
-    a.in0_planes = in0.shape[1] - in0_plane0 if in0_planes is None else in0_planes
+    a.in0_planes = in0.shape[1] // (2 if x3 else 1) - in0_plane0 if in0_planes is None else in0_planes
+    a.x3 = int(x3)
     if in1 is not None and in1_planes > 0:
         a.in1 = act_view(in1)
         a.in1_plane0, a.in1_planes = in1_plane0, in1_planes

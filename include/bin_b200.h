@@ -83,6 +83,14 @@ size_t bin_packed_weight_bytes(int cout_pad, int cin_pad, int ksize);
 /* variant: BIN_CONV_DEFAULT, or BIN_CONV_PLAIN to force the un-stacked layout for 3x3/Cout=32. */
 int bin_pack_conv_weight(const float* w_oihw, int cout, int cin, int ksize, int cout_pad, int cin_pad, int variant,
                          void* packed, bin_stream_t s);
+/* Precision-parameterised twins of bin_pack_frames / bin_pack_conv_weight (prec = BIN_PREC_F16 | BIN_PREC_F32X3; the
+ * enum is below), for unit-level use of the x3 conv.  F32X3: bin_pack_frames_p writes (hi, lo) = (fp16(v), fp16(v - hi))
+ * per 32-channel chunk, 4 hi planes then 4 lo planes, so dst.planes is twice the logical count (a multiple of 8);
+ * bin_pack_conv_weight_p writes three slabs per 32-channel K chunk, hi, hi and lo of (w * 2^8), so `packed` needs
+ * 3 * bin_packed_weight_bytes.  Any other prec fails with BIN_ERR_ARG. */
+int bin_pack_frames_p(const bin_frames_t* fr, int H, int W, bin_act_t dst, int prec, bin_stream_t s);
+int bin_pack_conv_weight_p(const float* w_oihw, int cout, int cin, int ksize, int cout_pad, int cin_pad, int variant,
+                           int prec, void* packed, bin_stream_t s);
 
 /* ---- the implicit-GEMM convolution (wgmma) -------------------------------------------- */
 enum { BIN_EPI_P8 = 0, BIN_EPI_PIXSHUF = 1, BIN_EPI_FINAL = 2 };
@@ -112,21 +120,29 @@ typedef struct {
    * 4 planes of lo, so bin_act_t.planes is twice the logical plane count while every *_plane0 / *_planes field
    * stays LOGICAL (multiples of 4); weights must have been packed with BIN_PREC_F32X3. */
   int x3;
-  /* BIN_EPI_P8: out planes [out_plane0, +cout_pad/8), optional residual (RDN.py:165, :219) */
+  /* BIN_EPI_P8: out planes [out_plane0, +cout_pad/8), optional residual (RDN.py:165, :219), except for the x-stacked
+   * 3x3 / cout_pad 32 kernel (variant BIN_CONV_DEFAULT), which takes none */
   bin_act_t out; int out_plane0;
   bin_act_t res; int res_plane0; /* res.ptr = NULL -> none */
   /* BIN_EPI_PIXSHUF (RDN.py:206): cout_pad=256 -> out is P8 (B, 8 planes, 2H, 2W) */
   /* BIN_EPI_FINAL (RDN.py:207 + :221/:279/:333): cout_pad=16 (3 used); out = conv + bias +
-   * mean(frames) written as fp32 NCHW to fr.out[call] */
+   * mean(frames) written as fp32 NCHW to fr.out[call] (call = b / fr.Bc, item b % fr.Bc) */
   bin_frames_t fr;
 } bin_conv_args_t;
+/* Fails with BIN_ERR_ARG, before any tensor map is built or anything is launched, on: a NULL in0 / in1 (when used) /
+ * w_packed / bias, or out for the P8 and pixel-shuffle epilogues, or a NULL frame or output pointer of the final one;
+ * a negative plane offset or store_planes; an input, output or residual plane range that runs past its tensor (x3: up
+ * to the lo plane of the last logical plane); a residual for the x-stacked kernel; relu or a residual with the
+ * pixel-shuffle or final epilogue (neither applies them); a batch/row sub-range outside the tensor. */
 int bin_conv_fwd(const bin_conv_args_t* a, bin_stream_t s);
 
 /* Fused tail of one RDB (RDN.py:141-147 for the 4th RDB_Conv, :162-165): g3 = ReLU(conv3x3(cat(x, g0..g2))) and
  * out = LFF(cat(x, g0..g3)) + x in one kernel; g3 is never written.  x: 12 planes from x_plane0, g: the 12 planes of
  * g0..g2 from g_plane0, out: 12 planes from out_plane0 (may be other planes of x's tensor).  w_conv / w_lff are the
  * bin_pack_conv_weight outputs of the (32,192,3,3) conv (variant BIN_CONV_DEFAULT) and the (96,224,1,1) LFF; b_conv
- * has 32 floats, b_lff 96.  b/y sub-ranges as in the conv arguments: a count of 0 means "to the end".  fp16 mode only. */
+ * has 32 floats, b_lff 96.  b/y sub-ranges as in the conv arguments: a count of 0 means "to the end".  fp16 mode only.
+ * A NULL argument, a negative plane offset, a plane range past its tensor or a bad sub-range fails with BIN_ERR_ARG
+ * before any tensor map is built. */
 int bin_rdb_tail_fwd(const bin_act_t* x, int x_plane0, const bin_act_t* g, int g_plane0, const void* w_conv,
                      const float* b_conv, const void* w_lff, const float* b_lff, const bin_act_t* out, int out_plane0,
                      int b_begin, int b_count, int y_begin, int y_count, bin_stream_t s);

@@ -118,6 +118,138 @@ def test_wgrad_rejects_bad_segments_before_any_launch():
         assert rc == 1 and text in err and err.startswith("wgrad:"), (args[1:3], args[4:6], args[7:], rc, err)
 
 
+def test_conv_fwd_rejects_bad_arguments_before_any_launch():
+    """bin_conv_fwd checks every argument on the host before it builds a tensor map: a plane range past a tensor would
+    otherwise be zero-filled by TMA (reads) or written past its end (stores), and an option the selected kernel does not
+    apply would be dropped without a word.  Every call here is invalid and must fail with BIN_ERR_ARG.  The geometry
+    cases pass null pointers only; the pointer cases point the non-null arguments at a small host buffer, and each of
+    them still has a null pointer, so nothing reaches a device."""
+    import ctypes as C
+    from bin_b200 import _lib
+    L = _lib.lib()
+    buf = (C.c_double * 8)()                        # host memory, never dereferenced
+    hp = (C.addressof(buf) + 15) & ~15
+    act = lambda planes, B=2, H=9, W=20, ptr=None: _lib.Act(ptr, B, planes, H, W)
+    res = lambda planes, B=2: act(planes, B=B, ptr=hp)   # a residual is present iff its pointer is set
+
+    def args(**kw):
+        a = _lib.ConvArgs()
+        a.in0, a.in0_planes, a.ksize, a.cout_pad, a.epilogue = act(12), 12, 1, 96, _lib.EPI_P8
+        a.out = act(12)
+        for k, v in kw.items():
+            setattr(a, k, v)
+        return a
+    x3 = dict(x3=1)
+    cases = [  # (fields, error text)
+        # plane counts, negative offsets, x3 alignment
+        (dict(in0_planes=0), "plane counts"),
+        (dict(in0_planes=6), "plane counts"),
+        (dict(in1=act(16), in1_planes=-4), "plane counts"),
+        (dict(in0=act(24), in0_plane0=-4), "negative plane offset"),
+        (dict(in1=act(16), in1_plane0=-4, in1_planes=4), "negative plane offset"),
+        (dict(out=act(24), out_plane0=-12), "negative plane offset"),
+        (dict(res=res(24), res_plane0=-12), "negative plane offset"),
+        (dict(store_planes=-1), "negative plane offset"),
+        (dict(epilogue=_lib.EPI_PIXSHUF, ksize=3, cout_pad=256, out=act(8, H=18, W=40), out_plane0=-4), "negative plane offset"),
+        (dict(in0=act(24), in0_plane0=2, **x3), "multiples of 4"),
+        # input ranges and geometry
+        (dict(in0=act(12), in0_plane0=4), "input plane range"),
+        (dict(in0=act(20), in0_planes=12, **x3), "input plane range"),
+        (dict(in1=act(16), in1_plane0=8, in1_planes=12), "input plane range"),
+        (dict(in1=act(16, H=8), in1_planes=16), "in1 geometry"),
+        (dict(in1=act(16, B=3), in1_planes=4), "in1 geometry"),
+        # sub-ranges
+        (dict(b_begin=2), "sub-range"),
+        (dict(b_begin=1, b_count=2), "sub-range"),
+        (dict(y_begin=-1), "sub-range"),
+        (dict(y_begin=5, y_count=5), "sub-range"),
+        (dict(b_count=-1), "sub-range"),
+        # output / residual ranges; x3: the last logical plane's lo half must lie inside the tensor
+        (dict(out=act(11)), "output tensor geometry"),
+        (dict(out=act(24), out_plane0=13), "output tensor geometry"),
+        (dict(out=act(12, W=21)), "output tensor geometry"),
+        (dict(store_planes=13), "output tensor geometry"),
+        (dict(in0=act(24), out=act(20), **x3), "output tensor geometry"),                       # 4 planes short
+        (dict(in0=act(24), out=act(28), out_plane0=12, store_planes=1, **x3), "output tensor geometry"),   # needs 29
+        (dict(in0=act(24), out=act(24), res=res(20), **x3), "residual tensor geometry"),
+        (dict(in0=act(24), out=act(24), res=res(284), res_plane0=132, **x3), "residual tensor geometry"),
+        (dict(res=res(24), res_plane0=13), "residual tensor geometry"),
+        (dict(res=res(12, B=1)), "residual tensor geometry"),
+        (dict(epilogue=_lib.EPI_PIXSHUF, ksize=3, cout_pad=256, out=act(7, H=18, W=40)), "pixel-shuffle output"),
+        (dict(epilogue=_lib.EPI_PIXSHUF, ksize=3, cout_pad=256, out=act(8, H=9, W=40)), "pixel-shuffle output"),
+        (dict(epilogue=_lib.EPI_PIXSHUF, ksize=3, cout_pad=256, in0=act(24), out=act(12, H=18, W=40), **x3),
+         "pixel-shuffle output"),
+        # options the selected kernel would drop
+        (dict(ksize=3, cout_pad=32, out=act(4), res=res(4), relu=1), "takes no residual"),
+        (dict(ksize=3, cout_pad=32, in0=act(24), out=act(8), res=res(8), **x3), "takes no residual"),
+        (dict(epilogue=_lib.EPI_PIXSHUF, ksize=3, cout_pad=256, out=act(8, H=18, W=40), relu=1), "no ReLU and no residual"),
+        (dict(epilogue=_lib.EPI_PIXSHUF, ksize=3, cout_pad=256, out=act(8, H=18, W=40), res=res(12)), "no ReLU and no residual"),
+        (dict(epilogue=_lib.EPI_FINAL, ksize=3, cout_pad=16, relu=1), "no ReLU and no residual"),
+        (dict(epilogue=_lib.EPI_FINAL, ksize=3, cout_pad=16, res=res(12)), "no ReLU and no residual"),
+        # the final epilogue's frame table
+        (dict(epilogue=_lib.EPI_FINAL, ksize=3, cout_pad=16), "frame table"),
+        # null pointers, once every shape is right
+        (dict(), "null input tensor"),
+        (dict(in0=act(12, ptr=hp), in1=act(16), in1_planes=16), "null input tensor"),
+        (dict(in0=act(12, ptr=hp + 8)), "16-byte aligned"),
+        (dict(in0=act(12, ptr=hp)), "null weights or bias"),
+        (dict(in0=act(12, ptr=hp), w_packed=hp), "null weights or bias"),
+        (dict(in0=act(12, ptr=hp), bias=hp), "null weights or bias"),
+        (dict(in0=act(12, ptr=hp), w_packed=hp, bias=hp), "null output tensor"),
+        (dict(epilogue=_lib.EPI_PIXSHUF, ksize=3, cout_pad=256, in0=act(12, ptr=hp), w_packed=hp, bias=hp,
+              out=act(8, H=18, W=40)), "null output tensor"),
+    ]
+    for fields, text in cases:
+        a = args(**fields)
+        rc = L.bin_conv_fwd(C.byref(a), None)
+        err = L.bin_last_error().decode()
+        assert rc == 1 and text in err and err.startswith("conv:"), (fields, rc, err)
+    # FINAL: a frame table that matches the batch but holds a null frame or output pointer
+    for null_out in (False, True):
+        a = args(epilogue=_lib.EPI_FINAL, ksize=3, cout_pad=16, in0=act(12, ptr=hp), w_packed=hp, bias=hp)
+        a.fr.ncalls, a.fr.nframes, a.fr.Bc = 2, 3, 1
+        for k in range(2):
+            a.fr.out[k] = None if (null_out and k == 1) else hp
+            for f in range(3):
+                a.fr.frame[k][f] = None if (not null_out and (k, f) == (1, 2)) else hp
+        rc = L.bin_conv_fwd(C.byref(a), None)
+        err = L.bin_last_error().decode()
+        assert rc == 1 and "null frame or output" in err, (null_out, rc, err)
+
+
+def test_rdb_tail_rejects_bad_planes_before_any_launch():
+    """bin_rdb_tail_fwd: negative plane offsets and ranges past a tensor fail with BIN_ERR_ARG (null pointers only)."""
+    import ctypes as C
+    from bin_b200 import _lib
+    L = _lib.lib()
+    act = lambda planes, B=2, H=9, W=20: _lib.Act(None, B, planes, H, W)
+    cases = [  # (x, x_plane0, g, g_plane0, out, out_plane0, sub), error text
+        ((act(144), -12, act(192), 0, act(144), 0, (0, 0, 0, 0)), "plane range"),
+        ((act(144), 0, act(192), -16, act(144), 12, (0, 0, 0, 0)), "plane range"),
+        ((act(144), 0, act(192), 0, act(144), -12, (0, 0, 0, 0)), "plane range"),
+        ((act(144), 133, act(192), 0, act(144), 0, (0, 0, 0, 0)), "plane range"),
+        ((act(144), 0, act(192), 181, act(144), 12, (0, 0, 0, 0)), "plane range"),
+        ((act(144), 0, act(192), 0, act(144, H=8), 12, (0, 0, 0, 0)), "geometry"),
+        ((act(144), 0, act(192), 0, act(144), 12, (0, 0, 9, 0)), "sub-range"),
+        ((act(144), 0, act(192), 0, act(144), 12, (0, 0, 0, 0)), "null argument"),
+    ]
+    for (x, xp, g, gp, out, op, sub), text in cases:
+        rc = L.bin_rdb_tail_fwd(C.byref(x), xp, C.byref(g), gp, None, None, None, None, C.byref(out), op, *sub, None)
+        err = L.bin_last_error().decode()
+        assert rc == 1 and text in err and err.startswith("rdb_tail"), (xp, gp, op, sub, rc, err)
+
+
+def test_precision_pack_entry_points_check_prec():
+    import ctypes as C
+    from bin_b200 import _lib
+    L = _lib.lib()
+    fr = _lib.Frames()
+    assert L.bin_pack_frames_p(C.byref(fr), 4, 4, _lib.Act(None, 1, 8, 2, 2), 2, None) == 1
+    assert "precision" in L.bin_last_error().decode()
+    assert L.bin_pack_conv_weight_p(None, 96, 96, 3, 96, 96, 0, -1, None, None) == 1
+    assert "precision" in L.bin_last_error().decode()
+
+
 def test_training_side_modules_refuse_cpu_tensors():
     """bin_b200.optim / bin_b200.dataprep have no CPU path: they must say so instead of computing something."""
     import torch
