@@ -14,12 +14,10 @@ import torch
 
 from . import _lib, ops
 from ._lib import BinB200Error, check, lib
+from .ops import _stream
+from .rdn import _LSTM_NAMES, _check_frames, _checkpointing_of, _launch_stage, _pyramid_schedule, _window_schedule
 
 LOSS_SCALE_TARGET = 2048.0    # max|dOut| * scale after loss scaling (fp16: 32x headroom to 65504; deep-layer gradients stay normal)
-
-
-def _stream() -> int:
-    return torch.cuda.current_stream().cuda_stream
 
 
 def deterministic_flags() -> int:
@@ -27,20 +25,6 @@ def deterministic_flags() -> int:
     bias and ConvLSTM gradient sums then run in a fixed order and the weight gradients on a grid independent of the SM
     count (DESIGN.md §4f).  0 otherwise: the default atomic sums."""
     return _lib.BIN_DETERMINISTIC if torch.are_deterministic_algorithms_enabled() else 0
-
-
-def _packed_t(model) -> torch.Tensor:
-    ps = model._conv_params()
-    key = (ps[0].device.index,) + tuple((p.data_ptr(), p._version) for p in ps)
-    cached = model.__dict__.get("_packed_t")
-    if cached is None or cached[0] != key:
-        dev = ps[0].device
-        blob = torch.empty(lib().bin_backbone_packed_t_bytes(model.NFRAMES), dtype=torch.uint8, device=dev)
-        wp = (C.c_void_p * _lib.BIN_BACKBONE_NCONV)(*[p.data_ptr() for p in ps[0::2]])
-        check(lib().bin_backbone_pack_t(model.NFRAMES, wp, blob.data_ptr(), _stream()))
-        model.__dict__["_packed_t"] = (key, blob)
-        cached = model.__dict__["_packed_t"]
-    return cached[1]
 
 
 def _input_key(model, frames):
@@ -73,17 +57,6 @@ def _grad_frames(dframes, B: int) -> _lib.Frames:
     return fr
 
 
-def _inference_fwd(model, calls, outs, B, H, W, dev) -> torch.Tensor:
-    """bin_backbone_fwd of one batched stage into the shared per-(device, stream) workspace, which it returns."""
-    from .rdn import _workspace
-    n = model.NFRAMES
-    fr = ops.make_frames(calls, outs)
-    ws = _workspace(dev, lib().bin_backbone_workspace_bytes(n, B * len(calls), H, W))
-    check(lib().bin_backbone_fwd(n, model.packed_blob().data_ptr(), C.byref(fr), H, W, ws.data_ptr(), ws.numel(),
-                                 _stream()))
-    return ws
-
-
 class BackboneStageFn(torch.autograd.Function):
     """ncalls same-weight backbone calls (RDN.py:210-334) in one launch, with backward.
 
@@ -98,22 +71,22 @@ class BackboneStageFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, model, ncalls: int, *args):
-        from .rdn import _checkpointing_of
         n = model.NFRAMES
         frames = [a.detach().contiguous() for a in args[: ncalls * n]]
         calls = [frames[k * n:(k + 1) * n] for k in range(ncalls)]
         B, _, H, W = frames[0].shape
         dev = frames[0].device
+        # training runs in fp16 whatever set_precision says: the backward kernels have no fp32 (x3) mode
         if not any(ctx.needs_input_grad[2:]):
             with torch.cuda.device(dev):
                 outs = [torch.empty_like(frames[0]) for _ in range(ncalls)]
-                _inference_fwd(model, calls, outs, B, H, W, dev)
+                _launch_stage(model, calls, outs, prec=0)
             return tuple(outs)
         recompute = _checkpointing_of(model) == "recompute"
         with torch.cuda.device(dev):
             outs = [torch.empty_like(frames[0]) for _ in range(ncalls)]
             if recompute:
-                _inference_fwd(model, calls, outs, B, H, W, dev)
+                _launch_stage(model, calls, outs, prec=0)
                 save = None
             else:
                 fr = ops.make_frames(calls, outs)
@@ -160,13 +133,14 @@ class BackboneStageFn(torch.autograd.Function):
                 frames = ctx.frames_keepalive
                 calls = [frames[k * n:(k + 1) * n] for k in range(ncalls)]
                 scratch = [torch.empty_like(frames[0]) for _ in range(ncalls)]   # the forward's outputs stay untouched
-                ws = _inference_fwd(model, calls, scratch, B, H, W, dev)
+                ws = _launch_stage(model, calls, scratch, prec=0)                  # fp16, as in the forward
                 check(lib().bin_backbone_bwd_recompute_masked(n, model.packed_blob().data_ptr(),
-                                                              _packed_t(model).data_ptr(), C.byref(dout), C.byref(dfr), H,
-                                                              W, ws.data_ptr(), ws.numel(), gws.data_ptr(), gws.numel(),
-                                                              gp_ptr, scale.data_ptr(), flags, need, _stream()))
+                                                              model._cached_pack("t").data_ptr(), C.byref(dout),
+                                                              C.byref(dfr), H, W, ws.data_ptr(), ws.numel(),
+                                                              gws.data_ptr(), gws.numel(), gp_ptr, scale.data_ptr(),
+                                                              flags, need, _stream()))
             else:
-                check(lib().bin_backbone_bwd_masked(n, _packed_t(model).data_ptr(), C.byref(dout), C.byref(dfr), H, W,
+                check(lib().bin_backbone_bwd_masked(n, model._cached_pack("t").data_ptr(), C.byref(dout), C.byref(dfr), H, W,
                                                     ctx.save.data_ptr(), gws.data_ptr(), gws.numel(), gp_ptr,
                                                     scale.data_ptr(), flags, need, _stream()))
         ctx.save = None
@@ -238,18 +212,7 @@ def convlstm_apply(module, x, state):
 
 def pyramid_apply(pyr, B1, B3, B5, B7, B9, previous_input=None):
     """RDN_residual_interp_5_input.forward (RDN.py:367-405) with autograd, 4 batched stage launches."""
-    m1, m2, m3, m4 = pyr.model1_1, pyr.model2_1, pyr.model3_1, pyr.model4_1
-    I2, I4, I6, I8 = backbone_stage(m1, [(B1, B3), (B3, B5), (B5, B7), (B7, B9)])
-    if previous_input is not None and previous_input[0] is not None:
-        p4, p6, p8, p5, p7, p6b = previous_input
-        I3, I5, I7 = backbone_stage(m2, [(p4, I2, I4), (p6, I4, I6), (p8, I6, I8)])
-        I4b, I6b = backbone_stage(m3, [(p5, B3, I3, I5, B5), (p7, B5, I5, I7, B7)])
-        (I5c,) = backbone_stage(m4, [(p6b, I4, I4b, I6b, I6)])
-    else:
-        I3, I5, I7 = backbone_stage(m2, [(I2, I2, I4), (I4, I4, I6), (I6, I6, I8)])
-        I4b, I6b = backbone_stage(m3, [(I3, B3, I3, I5, B5), (I5, B5, I5, I7, B7)])
-        (I5c,) = backbone_stage(m4, [(I4, I4, I4b, I6b, I6)])
-    return I2, I4, I6, I8, I3, I5, I7, I4b, I6b, I5c
+    return _pyramid_schedule(backbone_stage, pyr, B1, B3, B5, B7, B9, previous_input)
 
 
 def pyramid3_apply(module, F):
@@ -264,21 +227,9 @@ def pyramid3_apply(module, F):
 def window_apply(module, F):
     """Grad-enabled RDN_residual_interp_5_input_ConvLSTM_L.forward (RDN.py:422-465): the same 17 unique
     backbone calls / 6 live ConvLSTM calls as bin_window_fwd (SURVEY App. A), each batched stage an autograd node."""
-    from .rdn import _LSTM_NAMES, _check_frames
     F = [f.contiguous() for f in F]
     _check_frames(F)
     pyr = module.model
-    m1, m2, m3, m4 = pyr.model1_1, pyr.model2_1, pyr.model3_1, pyr.model4_1
     cells = [getattr(module, n) for n in _LSTM_NAMES]
-    lstm = lambda k, x: convlstm_apply(cells[k], x, None)[0]
-    o = [None] * 14
-    o[0], o[1], o[2], o[3], o[10] = backbone_stage(m1, [(F[0], F[1]), (F[1], F[2]), (F[2], F[3]), (F[3], F[4]), (F[4], F[5])])
-    p4, p6, p8 = lstm(0, o[1]), lstm(1, o[2]), lstm(2, o[3])
-    o[4], o[5], o[6], t0, t1, o[11] = backbone_stage(m2, [(o[0], o[0], o[1]), (o[1], o[1], o[2]), (o[2], o[2], o[3]),
-                                                          (p4, o[1], o[2]), (p6, o[2], o[3]), (p8, o[3], o[10])])
-    p5, p7 = lstm(3, o[5]), lstm(4, o[6])
-    o[7], o[8], t2, o[12] = backbone_stage(m3, [(o[4], F[1], o[4], o[5], F[2]), (o[5], F[2], o[5], o[6], F[3]),
-                                              (p5, F[2], t0, t1, F[3]), (p7, F[3], t1, o[11], F[4])])
-    p6b = lstm(5, o[8])
-    o[9], o[13] = backbone_stage(m4, [(o[1], o[1], o[7], o[8], o[2]), (p6b, o[2], t2, o[12], o[3])])
-    return tuple(o)
+    s1 = backbone_stage(pyr.model1_1, [(F[0], F[1]), (F[1], F[2]), (F[2], F[3]), (F[3], F[4]), (F[4], F[5])])
+    return _window_schedule(backbone_stage, lambda k, x: convlstm_apply(cells[k], x, None)[0], pyr, F, s1)

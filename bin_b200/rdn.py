@@ -28,10 +28,6 @@ __all__ = ["set_precision", "set_self_ensemble", "set_activation_checkpointing",
            "RDN_residual_interp_5_input_ConvLSTM_L", "bin_stage4_lstm"]
 
 
-def _stream() -> int:
-    return torch.cuda.current_stream().cuda_stream
-
-
 def _graphs_enabled() -> bool:
     import os
     return os.environ.get("BIN_B200_GRAPH", "1") != "0"
@@ -158,8 +154,6 @@ class _Backbone(nn.Module):
         self.GFF = nn.Sequential(nn.Conv2d(D * G0, G0, 1, padding=0, stride=1), nn.Conv2d(G0, G0, k, padding=1, stride=1))
         self.UPNet = nn.Sequential(nn.Conv2d(G0, 256, k, padding=1, stride=1), nn.PixelShuffle(2),
                                    nn.Conv2d(64, 3, k, padding=1, stride=1))
-        self._packed: Optional[torch.Tensor] = None
-        self._packed_key = None
 
     # -- packed weights (cached per parameter version / device) ---------------------------------
     def _conv_modules(self) -> List[nn.Conv2d]:
@@ -183,35 +177,40 @@ class _Backbone(nn.Module):
 
     def packed_blob(self, prec: int = 0) -> torch.Tensor:
         """Packed weights for BIN_PREC_F16 (0) or BIN_PREC_F32X3 (1), cached per parameter version."""
+        return self._cached_pack("x3" if prec else "f16")
+
+    def _cached_pack(self, kind: str) -> torch.Tensor:
+        """Packed weights of one kind, cached per device and parameter version: "f16" and "x3" feed the forward in
+        BIN_PREC_F16 and BIN_PREC_F32X3, "t" (transposed, tap-flipped) the backward's data gradients.  Each kind is its
+        own __dict__ slot, assigned whole: replicate() gives an nn.DataParallel replica a shallow copy of the master's
+        __dict__, so a replica packing its own weights (in its own worker thread) never writes into the master's cache."""
         ps = self._conv_params()
-        key = (prec, ps[0].device.index) + tuple((p.data_ptr(), p._version) for p in ps)
-        if prec:
-            cached = self.__dict__.get("_packed_x3")
-            if cached is None or cached[0] != key:
-                dev = ps[0].device
-                if dev.type != "cuda":
-                    raise BinB200Error("bin_b200: parameters must live on a CUDA device (call .to('cuda')); no CPU fallback")
-                with torch.cuda.device(dev):
-                    blob = torch.empty(lib().bin_backbone_packed_bytes_p(self.NFRAMES, prec), dtype=torch.uint8, device=dev)
-                    wp = (C.c_void_p * _lib.BIN_BACKBONE_NCONV)(*[p.data_ptr() for p in ps[0::2]])
-                    bp = (C.c_void_p * _lib.BIN_BACKBONE_NCONV)(*[p.data_ptr() for p in ps[1::2]])
-                    check(lib().bin_backbone_pack_p(self.NFRAMES, wp, bp, blob.data_ptr(), prec, _stream()))
-                self.__dict__["_packed_x3"] = cached = (key, blob)
+        key = (kind, ps[0].device.index) + tuple((p.data_ptr(), p._version) for p in ps)
+        slot = "_pack_" + kind
+        cached = self.__dict__.get(slot)
+        if cached is not None and cached[0] == key:
             return cached[1]
-        if self._packed is None or key != self._packed_key:
-            dev = ps[0].device
-            if dev.type != "cuda":
-                raise BinB200Error("bin_b200: parameters must live on a CUDA device (call .to('cuda')); no CPU fallback")
-            for p in ps:
-                if p.dtype != torch.float32 or not p.is_contiguous():
-                    raise BinB200Error("bin_b200: parameters must be contiguous fp32")
-            with torch.cuda.device(dev):
-                blob = torch.empty(lib().bin_backbone_packed_bytes(self.NFRAMES), dtype=torch.uint8, device=dev)
-                wp = (C.c_void_p * _lib.BIN_BACKBONE_NCONV)(*[p.data_ptr() for p in ps[0::2]])
-                bp = (C.c_void_p * _lib.BIN_BACKBONE_NCONV)(*[p.data_ptr() for p in ps[1::2]])
-                check(lib().bin_backbone_pack(self.NFRAMES, wp, bp, blob.data_ptr(), _stream()))
-            self._packed, self._packed_key = blob, key
-        return self._packed
+        dev = ps[0].device
+        if dev.type != "cuda":
+            raise BinB200Error("bin_b200: parameters must live on a CUDA device (call .to('cuda')); no CPU fallback")
+        for p in ps:
+            if p.dtype != torch.float32 or not p.is_contiguous():
+                raise BinB200Error("bin_b200: parameters must be contiguous fp32")
+        n, L = self.NFRAMES, lib()
+        wp = (C.c_void_p * _lib.BIN_BACKBONE_NCONV)(*[p.data_ptr() for p in ps[0::2]])
+        bp = (C.c_void_p * _lib.BIN_BACKBONE_NCONV)(*[p.data_ptr() for p in ps[1::2]])
+        with torch.cuda.device(dev):
+            if kind == "t":
+                blob = torch.empty(L.bin_backbone_packed_t_bytes(n), dtype=torch.uint8, device=dev)
+                check(L.bin_backbone_pack_t(n, wp, blob.data_ptr(), ops._stream()))
+            elif kind == "x3":
+                blob = torch.empty(L.bin_backbone_packed_bytes_p(n, 1), dtype=torch.uint8, device=dev)
+                check(L.bin_backbone_pack_p(n, wp, bp, blob.data_ptr(), 1, ops._stream()))
+            else:
+                blob = torch.empty(L.bin_backbone_packed_bytes(n), dtype=torch.uint8, device=dev)
+                check(L.bin_backbone_pack(n, wp, bp, blob.data_ptr(), ops._stream()))
+        self.__dict__[slot] = (key, blob)
+        return blob
 
     def _forward_frames(self, *frames):
         if len(frames) != self.NFRAMES:
@@ -219,18 +218,7 @@ class _Backbone(nn.Module):
         if _needs_grad(list(frames) + self._conv_params()):
             from .autograd import backbone_apply
             return backbone_apply(self, frames)
-        frames = [f.contiguous() for f in frames]
-        B, H, W = _check_frames(frames)
-        dev = frames[0].device
-        with torch.cuda.device(dev):
-            out = torch.empty_like(frames[0])
-            fr = ops.make_frames([frames], [out])
-            prec = _prec_of(self)
-            nbytes = lib().bin_backbone_workspace_bytes_p(self.NFRAMES, B, H, W, prec)
-            ws = _workspace(dev, nbytes)
-            check(lib().bin_backbone_fwd_p(self.NFRAMES, self.packed_blob(prec).data_ptr(), C.byref(fr), H, W, ws.data_ptr(),
-                                           ws.numel(), prec, _stream()))
-        return out
+        return _batched(self, [frames])[0]
 
 
 class RDN_residual_interp_2_input(_Backbone):       # RDN.py:167-222
@@ -353,32 +341,43 @@ class RDN_residual_interp_5_input(nn.Module):
                                                                    self.model4_1) for p in m._conv_params()]):
             from .autograd import pyramid_apply
             return pyramid_apply(self, B1, B3, B5, B7, B9, previous_input)
-        m1, m2, m3, m4 = self.model1_1, self.model2_1, self.model3_1, self.model4_1
-        I2, I4, I6, I8 = _batched(m1, [(B1, B3), (B3, B5), (B5, B7), (B7, B9)])
-        if previous_input is not None and previous_input[0] is not None:
-            p4, p6, p8, p5, p7, p6b = previous_input
-            I3, I5, I7 = _batched(m2, [(p4, I2, I4), (p6, I4, I6), (p8, I6, I8)])
-            I4b, I6b = _batched(m3, [(p5, B3, I3, I5, B5), (p7, B5, I5, I7, B7)])
-            (I5c,) = _batched(m4, [(p6b, I4, I4b, I6b, I6)])
-        else:
-            I3, I5, I7 = _batched(m2, [(I2, I2, I4), (I4, I4, I6), (I6, I6, I8)])
-            I4b, I6b = _batched(m3, [(I3, B3, I3, I5, B5), (I5, B5, I5, I7, B7)])
-            (I5c,) = _batched(m4, [(I4, I4, I4b, I6b, I6)])
-        return I2, I4, I6, I8, I3, I5, I7, I4b, I6b, I5c
+        return _pyramid_schedule(_batched, self, B1, B3, B5, B7, B9, previous_input)
+
+
+def _pyramid_schedule(stage, pyr, B1, B3, B5, B7, B9, previous_input):
+    """The 10 backbone calls of RDN.py:367-405 as 4 batched stages; stage(model, calls) runs one and returns its outputs.
+    Without previous_input (the first step) the recurrent inputs p4, p6, p8, p5, p7, p6b are this step's own
+    I2, I4, I6, I3, I5, I4."""
+    m1, m2, m3, m4 = pyr.model1_1, pyr.model2_1, pyr.model3_1, pyr.model4_1
+    first = previous_input is None or previous_input[0] is None
+    I2, I4, I6, I8 = stage(m1, [(B1, B3), (B3, B5), (B5, B7), (B7, B9)])
+    p4, p6, p8, p5, p7, p6b = (I2, I4, I6, None, None, I4) if first else previous_input
+    I3, I5, I7 = stage(m2, [(p4, I2, I4), (p6, I4, I6), (p8, I6, I8)])
+    if first:
+        p5, p7 = I3, I5
+    I4b, I6b = stage(m3, [(p5, B3, I3, I5, B5), (p7, B5, I5, I7, B7)])
+    (I5c,) = stage(m4, [(p6b, I4, I4b, I6b, I6)])
+    return I2, I4, I6, I8, I3, I5, I7, I4b, I6b, I5c
+
+
+def _launch_stage(model: _Backbone, calls, outs, prec: int) -> torch.Tensor:
+    """One batched backbone stage (same-weight calls riding along the batch) in precision `prec`, on the current device,
+    into the shared per-(device, stream) workspace, which it returns: a recomputing backward reads what it left there."""
+    B, _, H, W = calls[0][0].shape
+    fr = ops.make_frames(calls, outs)
+    ws = _workspace(calls[0][0].device, lib().bin_backbone_workspace_bytes_p(model.NFRAMES, B * len(calls), H, W, prec))
+    check(lib().bin_backbone_fwd_p(model.NFRAMES, model.packed_blob(prec).data_ptr(), C.byref(fr), H, W, ws.data_ptr(),
+                                   ws.numel(), prec, ops._stream()))
+    return ws
 
 
 def _batched(model: _Backbone, calls):
+    """Inference of one batched stage in the net's precision (set_precision)."""
     calls = [[t.contiguous() for t in c] for c in calls]
-    B, H, W = _check_frames([t for c in calls for t in c])
-    dev = calls[0][0].device
-    with torch.cuda.device(dev):
+    _check_frames([t for c in calls for t in c])
+    with torch.cuda.device(calls[0][0].device):
         outs = [torch.empty_like(calls[0][0]) for _ in calls]
-        fr = ops.make_frames(calls, outs)
-        prec = _prec_of(model)
-        nbytes = lib().bin_backbone_workspace_bytes_p(model.NFRAMES, B * len(calls), H, W, prec)
-        ws = _workspace(dev, nbytes)
-        check(lib().bin_backbone_fwd_p(model.NFRAMES, model.packed_blob(prec).data_ptr(), C.byref(fr), H, W, ws.data_ptr(),
-                                       ws.numel(), prec, _stream()))
+        _launch_stage(model, calls, outs, _prec_of(model))
     return outs
 
 
@@ -387,6 +386,25 @@ def _batched(model: _Backbone, calls):
 # --------------------------------------------------------------------------------------------
 _LSTM_NAMES = ["clstm_4_prime", "clstm_6_prime", "clstm_8_prime", "clstm_5_prime_prime", "clstm_7_prime_prime",
                "clstm_6_prime_prime_prime"]
+
+
+def _window_schedule(stage, lstm, pyr, F, s1):
+    """Stages 2-4 of the six-frame window (RDN.py:422-465) -> the 14-tuple: the unique backbone calls of both
+    recurrent steps and the 6 live ConvLSTM calls, in the order bin_window_fwd issues them (SURVEY App. A).
+    stage(model, calls) runs one batched backbone stage and returns its outputs, lstm(k, x) returns h of ConvLSTM cell k
+    (the order of _LSTM_NAMES) from no state, and s1 holds the stage-1 outputs o[0..3], o[10] of the frame pairs."""
+    m2, m3, m4 = pyr.model2_1, pyr.model3_1, pyr.model4_1
+    o = [None] * 14
+    o[0], o[1], o[2], o[3], o[10] = s1
+    p4, p6, p8 = lstm(0, o[1]), lstm(1, o[2]), lstm(2, o[3])
+    o[4], o[5], o[6], t0, t1, o[11] = stage(m2, [(o[0], o[0], o[1]), (o[1], o[1], o[2]), (o[2], o[2], o[3]),
+                                                 (p4, o[1], o[2]), (p6, o[2], o[3]), (p8, o[3], o[10])])
+    p5, p7 = lstm(3, o[5]), lstm(4, o[6])
+    o[7], o[8], t2, o[12] = stage(m3, [(o[4], F[1], o[4], o[5], F[2]), (o[5], F[2], o[5], o[6], F[3]),
+                                       (p5, F[2], t0, t1, F[3]), (p7, F[3], t1, o[11], F[4])])
+    p6b = lstm(5, o[8])
+    o[9], o[13] = stage(m4, [(o[1], o[1], o[7], o[8], o[2]), (p6b, o[2], t2, o[12], o[3])])
+    return tuple(o)
 
 
 class RDN_residual_interp_5_input_ConvLSTM_L(nn.Module):
@@ -428,8 +446,7 @@ class RDN_residual_interp_5_input_ConvLSTM_L(nn.Module):
         backbone calls of its 20 and the 6 live ConvLSTM calls of its 12 (SURVEY.md App. A)."""
         frames = [B1, B3, B5, B7, B9, B11]
         ensemble = _ensemble_of(self)
-        if torch.is_grad_enabled() and (any(f.requires_grad for f in frames) or
-                                        any(p.requires_grad for p in self._all_tensors())):
+        if _needs_grad(frames + self._all_tensors()):
             if ensemble is not None:
                 raise BinB200Error(f"self-ensemble {ensemble!r} is inference-only: call the net under torch.no_grad(), "
                                    "or set_self_ensemble(net, None) to train")
@@ -452,7 +469,7 @@ class RDN_residual_interp_5_input_ConvLSTM_L(nn.Module):
         ws = _workspace(dev, lib().bin_window_workspace_bytes_p(B, H, W, prec))
         fp = (C.c_void_p * 6)(*[f.data_ptr() for f in frames])
         op = (C.c_void_p * 14)(*[o.data_ptr() for o in outs])
-        check(lib().bin_window_fwd_p(C.byref(net), fp, op, B, H, W, ws.data_ptr(), ws.numel(), prec, _stream()))
+        check(lib().bin_window_fwd_p(C.byref(net), fp, op, B, H, W, ws.data_ptr(), ws.numel(), prec, ops._stream()))
         return outs, ws
 
     def _forward_flipx4(self, frames, B, H, W, dev):
@@ -512,7 +529,7 @@ class RDN_residual_interp_5_input_ConvLSTM_L(nn.Module):
             ws = _workspace(dev, lib().bin_window_workspace_bytes(B, H, W))
             fp = (C.c_void_p * 4)(*[f.data_ptr() for f in frames])
             op = (C.c_void_p * 6)(*[o.data_ptr() for o in outs])
-            check(lib().bin_pyramid3_fwd(C.byref(net), fp, op, B, H, W, ws.data_ptr(), ws.numel(), _stream()))
+            check(lib().bin_pyramid3_fwd(C.byref(net), fp, op, B, H, W, ws.data_ptr(), ws.numel(), ops._stream()))
         return tuple(outs)
 
 

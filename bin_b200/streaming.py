@@ -17,7 +17,7 @@ import torch
 
 from . import ops
 from ._lib import BinB200Error, check, lib
-from .rdn import _LSTM_NAMES, _batched, _ensemble_of
+from .rdn import _LSTM_NAMES, _batched, _ensemble_of, _window_schedule
 
 
 def test_py_padding(h: int, w: int) -> Tuple[int, int, int, int]:
@@ -48,7 +48,7 @@ def upload_frame_u8(img_u8: torch.Tensor, pad: Tuple[int, int, int, int], device
     with torch.cuda.device(dev):
         d = img_u8.contiguous().to(dev, non_blocking=True)
         out = torch.empty((1, 3, h + pt + pb, w + pl + pr), dtype=torch.float32, device=dev)
-        check(lib().bin_u8_to_frame(d.data_ptr(), h, w, pl, pr, pt, pb, out.data_ptr(), torch.cuda.current_stream().cuda_stream))
+        check(lib().bin_u8_to_frame(d.data_ptr(), h, w, pl, pr, pt, pb, out.data_ptr(), ops._stream()))
     return out
 
 
@@ -62,7 +62,7 @@ def tensor2img_u8(t: torch.Tensor, crop: Optional[Tuple[int, int, int, int]] = N
     top, left, h, w = crop if crop is not None else (0, 0, Hs, Ws)
     with torch.cuda.device(x.device):
         out = torch.empty((h, w, 3), dtype=torch.uint8, device=x.device)
-        check(lib().bin_tensor2img_u8(x.data_ptr(), Hs, Ws, top, left, h, w, out.data_ptr(), torch.cuda.current_stream().cuda_stream))
+        check(lib().bin_tensor2img_u8(x.data_ptr(), Hs, Ws, top, left, h, w, out.data_ptr(), ops._stream()))
     return out
 
 
@@ -110,31 +110,20 @@ class StreamingBIN:
 
     def _window(self):
         net = self.net
-        pyr = net.model
-        m1, m2, m3, m4 = pyr.model1_1, pyr.model2_1, pyr.model3_1, pyr.model4_1
         ids = [i for i, _ in self.frames]
         F = [f for _, f in self.frames]
         # ---- stage 1: only the frame pairs not seen before (1 per window in steady state, 5 for the first)
         need = [(a, b) for a, b in zip(range(5), range(1, 6)) if (ids[a], ids[b]) not in self.s1]
         if need:
-            outs = _batched(m1, [(F[a], F[b]) for a, b in need])
+            outs = _batched(net.model.model1_1, [(F[a], F[b]) for a, b in need])
             for (a, b), o in zip(need, outs):
                 self.s1[(ids[a], ids[b])] = o
             self.backbone_calls += len(need)
         s1 = [self.s1[(ids[k], ids[k + 1])] for k in range(5)]
-        o: List[Optional[torch.Tensor]] = [None] * 14
-        o[0], o[1], o[2], o[3], o[10] = s1
         cells = [getattr(net, n) for n in _LSTM_NAMES]
         lstm = lambda k, x: ops.convlstm_fwd(x, cells[k].Gates.weight.detach(), cells[k].Gates.bias.detach(), None)[0]
-        p4, p6, p8 = lstm(0, o[1]), lstm(1, o[2]), lstm(2, o[3])
-        o[4], o[5], o[6], t0, t1, o[11] = _batched(m2, [(o[0], o[0], o[1]), (o[1], o[1], o[2]), (o[2], o[2], o[3]),
-                                                        (p4, o[1], o[2]), (p6, o[2], o[3]), (p8, o[3], o[10])])
-        p5, p7 = lstm(3, o[5]), lstm(4, o[6])
-        o[7], o[8], t2, o[12] = _batched(m3, [(o[4], F[1], o[4], o[5], F[2]), (o[5], F[2], o[5], o[6], F[3]),
-                                              (p5, F[2], t0, t1, F[3]), (p7, F[3], t1, o[11], F[4])])
-        p6b = lstm(5, o[8])
-        o[9], o[13] = _batched(m4, [(o[1], o[1], o[7], o[8], o[2]), (p6b, o[2], t2, o[12], o[3])])
+        o = _window_schedule(_batched, lstm, net.model, F, s1)
         self.backbone_calls += 12
         if self.key[0] is not None:
             return tuple(ops.flipx4_mean(o))
-        return tuple(o)
+        return o

@@ -212,6 +212,29 @@ def test_dataparallel_wrapper_like_bin_model(net):
     assert dp.module is net
 
 
+def test_replica_packs_leave_the_masters_cache_alone(net):
+    """An nn.DataParallel replica (bin_model.py:42) starts from a shallow copy of the master's __dict__, packed-weight
+    caches included, and holds other weight tensors: packing those must cache on the replica only, so the master's next
+    call still returns its own blob, in both precisions."""
+    bb = net.model.model3_1
+    blobs = [bb.packed_blob(prec) for prec in (0, 1)]
+    # what replicate() does to one module tree, as in test_module_cpu's weight-walk test: copy every module, drop
+    # _parameters, set plain tensor attributes
+    mods = list(bb.modules())
+    copies = {id(m): m._replicate_for_data_parallel() for m in mods}
+    for m in mods:
+        r = copies[id(m)]
+        for key, child in m._modules.items():
+            setattr(r, key, copies[id(child)])
+        for key, p in m._parameters.items():
+            setattr(r, key, p.detach() * 2.0)
+    rep = copies[id(bb)]
+    for prec, blob in zip((0, 1), blobs):
+        rblob = rep.packed_blob(prec)
+        assert rblob is not blob and rep.packed_blob(prec) is rblob
+        assert bb.packed_blob(prec) is blob
+
+
 def test_inputs_not_mutated_and_outputs_fresh(net):
     fr = [f.cuda() for f in O.synth_frames(6, 1, 32, 32, seed=2)]
     keep = [f.clone() for f in fr]
