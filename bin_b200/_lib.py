@@ -126,6 +126,10 @@ _SIGS = {
     "bin_rdb_tail_fwd": (C.c_int, [C.POINTER(Act), C.c_int, C.POINTER(Act), C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                    C.POINTER(Act), C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "bin_adam_step": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int] + [C.c_float] * 8 + [C.c_void_p]),
+    "bin_grad_audit_scratch_bytes": (C.c_size_t, [C.c_int]),
+    "bin_grad_audit": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_float, C.c_void_p, C.c_size_t,
+                                 C.c_void_p, C.c_void_p]),
+    "bin_adam_step_guarded": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int] + [C.c_float] * 8 + [C.c_void_p, C.c_void_p]),
     "bin_blur_average_u8": (C.c_int, [C.c_void_p, C.c_int, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "bin_image_metrics_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int]),
     "bin_image_metrics_u8": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t,

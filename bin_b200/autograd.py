@@ -18,6 +18,22 @@ from .ops import _stream
 from .rdn import _LSTM_NAMES, _check_frames, _checkpointing_of, _launch_stage, _pyramid_schedule, _window_schedule
 
 LOSS_SCALE_TARGET = 2048.0    # max|dOut| * scale after loss scaling (fp16: 32x headroom to 65504; deep-layer gradients stay normal)
+_loss_scale_target = LOSS_SCALE_TARGET
+
+
+def loss_scale_target() -> float:
+    """What each backbone backward scales max|dOut| to.  LOSS_SCALE_TARGET unless set_loss_scale_target, or
+    bin_b200.optim.Adam(loss_scale_backoff=True) after a skipped step, has lowered it."""
+    return _loss_scale_target
+
+
+def set_loss_scale_target(x: float) -> None:
+    """A smaller target leaves more of fp16's range above the scaled gradients and pushes the small ones towards the
+    subnormals.  Takes effect at the next backward; 1 <= x <= LOSS_SCALE_TARGET."""
+    global _loss_scale_target
+    if not 1.0 <= x <= LOSS_SCALE_TARGET:
+        raise ValueError(f"loss-scale target must lie in [1, {LOSS_SCALE_TARGET:g}]")
+    _loss_scale_target = float(x)
 
 
 def deterministic_flags() -> int:
@@ -119,7 +135,7 @@ class BackboneStageFn(torch.autograd.Function):
             gouts = [torch.zeros((B, 3, H, W), device=dev) if g is None else g.contiguous().float() for g in gouts]
             sbuf = torch.empty(2, device=dev)                                    # [scale, scratch]; stays on the device
             gp = (C.c_void_p * ncalls)(*[g.data_ptr() for g in gouts])
-            check(lib().bin_grad_scale(gp, ncalls, gouts[0].numel(), LOSS_SCALE_TARGET, sbuf.data_ptr(),
+            check(lib().bin_grad_scale(gp, ncalls, gouts[0].numel(), loss_scale_target(), sbuf.data_ptr(),
                                        sbuf.data_ptr() + 4, _stream()))
             scale = sbuf[:1]
             need, frame_needed = grad_plan(ctx.needs_input_grad, ncalls, n)

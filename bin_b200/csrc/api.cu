@@ -1,6 +1,7 @@
 // bin_b200 -- extern "C" entry points (include/bin_b200.h) and the host-side orchestration of
 // one backbone / one 6-frame window.  Host code only: every arithmetic step is a kernel in
 // conv_igemm.cu / aux_kernels.cu.
+#include <math.h>
 #include <stdlib.h>
 #include <string.h>
 
@@ -77,7 +78,10 @@ int launch_pixel_loss_bwd(const float* const* a, const float* const* b, float* c
                           size_t n, int kind, float eps, const float* upstream, cudaStream_t s);
 int launch_adam_step(const bin_adam_tensor_t* table, const int* chunk_prefix, int ntensors, int nchunks, float lr,
                      float beta1, float beta2, float eps, float weight_decay, float bias_correction1,
-                     float bias_correction2, float grad_scale, cudaStream_t s);
+                     float bias_correction2, float grad_scale, const bin_grad_audit_t* audit, cudaStream_t s);   // audit: NULL = unguarded
+size_t grad_audit_scratch_bytes(int nchunks);
+int launch_grad_audit(const bin_adam_tensor_t* table, const int* chunk_prefix, int ntensors, int nchunks, float grad_scale,
+                      float max_norm, void* scratch, bin_grad_audit_t* audit, cudaStream_t s);
 int launch_blur_average_u8(const uint8_t* frames, int T, size_t frame_bytes, int window_size, int first_mid, int stride,
                            int nwin, uint8_t* out, cudaStream_t s);
 size_t metrics_workspace_bytes(int h, int w);
@@ -990,7 +994,29 @@ int bin_adam_step(const bin_adam_tensor_t* table_dev, const int* chunk_prefix_de
                   float bias_correction2, float grad_scale, bin_stream_t s) {
   if (!table_dev || !chunk_prefix_dev) return fail(BIN_ERR_ARG, "adam_step: null argument");
   return launch_adam_step(table_dev, chunk_prefix_dev, ntensors, nchunks, lr, beta1, beta2, eps, weight_decay,
-                          bias_correction1, bias_correction2, grad_scale, (cudaStream_t)s);
+                          bias_correction1, bias_correction2, grad_scale, nullptr, (cudaStream_t)s);
+}
+int bin_adam_step_guarded(const bin_adam_tensor_t* table_dev, const int* chunk_prefix_dev, int ntensors, int nchunks,
+                          float lr, float beta1, float beta2, float eps, float weight_decay, float bias_correction1,
+                          float bias_correction2, float grad_scale, const bin_grad_audit_t* audit_dev, bin_stream_t s) {
+  if (!table_dev || !chunk_prefix_dev || !audit_dev) return fail(BIN_ERR_ARG, "adam_step_guarded: null argument");
+  if (reinterpret_cast<uintptr_t>(audit_dev) & 7) return fail(BIN_ERR_ARG, "adam_step_guarded: audit record not 8-byte aligned");
+  return launch_adam_step(table_dev, chunk_prefix_dev, ntensors, nchunks, lr, beta1, beta2, eps, weight_decay,
+                          bias_correction1, bias_correction2, grad_scale, audit_dev, (cudaStream_t)s);
+}
+size_t bin_grad_audit_scratch_bytes(int nchunks) { return grad_audit_scratch_bytes(nchunks); }
+int bin_grad_audit(const bin_adam_tensor_t* table_dev, const int* chunk_prefix_dev, int ntensors, int nchunks,
+                   float grad_scale, float max_norm, void* scratch, size_t scratch_bytes, bin_grad_audit_t* audit_dev,
+                   bin_stream_t s) {
+  if (!table_dev || !chunk_prefix_dev || !scratch || !audit_dev) return fail(BIN_ERR_ARG, "grad_audit: null argument");
+  if (ntensors < 1 || nchunks < 1) return fail(BIN_ERR_ARG, "grad_audit: empty table");
+  if (!(max_norm > 0.f) || !isfinite(grad_scale))
+    return fail(BIN_ERR_ARG, "grad_audit: max_norm must be positive (INFINITY = no clipping) and grad_scale finite");
+  if ((reinterpret_cast<uintptr_t>(scratch) & 15) || (reinterpret_cast<uintptr_t>(audit_dev) & 7))
+    return fail(BIN_ERR_ARG, "grad_audit: scratch must be 16-byte and the record 8-byte aligned");
+  if (scratch_bytes < grad_audit_scratch_bytes(nchunks)) return fail(BIN_ERR_WORKSPACE, "grad_audit: scratch too small");
+  return launch_grad_audit(table_dev, chunk_prefix_dev, ntensors, nchunks, grad_scale, max_norm, scratch, audit_dev,
+                           (cudaStream_t)s);
 }
 int bin_blur_average_u8(const uint8_t* frames, int T, size_t frame_bytes, int window_size, int first_mid, int stride,
                         int nwin, uint8_t* out, bin_stream_t s) {

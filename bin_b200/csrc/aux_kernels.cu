@@ -1,5 +1,7 @@
 // bin_b200 -- memory-bound helper kernels: layout conversion, input packer (space-to-depth),
 // weight packer, ConvLSTM cell.
+#include <climits>
+
 #include "common.cuh"
 #include "internal.h"
 
@@ -765,9 +767,17 @@ __device__ __forceinline__ void adam_one(float& p, float g, float& m, float& v, 
   const float denom = sqrtf(v) * inv_sqrt_bc2 + eps;   // (exp_avg_sq.sqrt() / sqrt(bias_correction2)).add_(eps)
   p = p - lr_bc1 * (m / denom);                        // param.addcdiv_(exp_avg, denom, value=-lr / bias_correction1)
 }
+// kGuard: the step obeys the record grad_audit_reduce_kernel left in `audit` (DESIGN 4i).  A block of a skipped step
+// returns before it loads anything else; an applied one scales the gradient by grad_scale * coef, which is grad_scale
+// itself when coef == 1, so an unclipped guarded step writes the plain step's bits.
+template <bool kGuard>
 __global__ void adam_step_kernel(const bin_adam_tensor_t* __restrict__ table, const int* __restrict__ chunk_prefix,
                                  int ntensors, float lr_bc1, float b1, float b2, float eps, float wd,
-                                 float inv_sqrt_bc2, float gscale) {
+                                 float inv_sqrt_bc2, float gscale, const bin_grad_audit_t* __restrict__ audit) {
+  if (kGuard) {
+    if (audit->skip) return;
+    gscale = gscale * audit->coef;
+  }
   __shared__ int s_t;
   if (threadIdx.x == 0) {
     int lo = 0, hi = ntensors - 1;                     // chunk_prefix[0] == 0 <= blockIdx.x
@@ -812,6 +822,117 @@ __global__ void adam_step_kernel(const bin_adam_tensor_t* __restrict__ table, co
       adam_one(p, G[i], m, v, lr_bc1, b1, b2, eps, wd, inv_sqrt_bc2, gscale);
       P[i] = p; M[i] = m; V[i] = v;
     }
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// Gradient audit of the guarded optimizer step (DESIGN 4i).  grad_audit_kernel walks the Adam table with the Adam
+// grid: block b reads its chunk of g once, sums g^2 of the finite elements in fp64 and counts the others, and writes one
+// 16-byte partial.  grad_audit_reduce_kernel adds the partials in index order and writes the record the guarded step
+// reads.  fp64 because an fp32 sum of squares overflows at |g| ~ 1.8e19, where the gradients are still finite.  Every
+// sum has a fixed order (strided per thread, shuffle tree, warp order) and the grids depend on the tensor shapes alone,
+// so the record's bytes do not depend on the SM count.  No float atomics.
+struct GradAuditPartial {
+  double sumsq;
+  unsigned nonfinite;
+  int first_bad;                                       // this block's tensor if it saw a non-finite element, else INT_MAX
+};
+static_assert(sizeof(GradAuditPartial) == 16, "bin_grad_audit_scratch_bytes assumes 16-byte partials");
+constexpr int kAuditThreads = 256;
+
+__device__ __forceinline__ void audit_one(float g, double& ss, unsigned& bad) {
+  if ((__float_as_uint(g) & 0x7f800000u) == 0x7f800000u) {
+    ++bad;
+  } else {
+    const double d = (double)g;
+    ss = fma(d, d, ss);
+  }
+}
+// Block sum of (ss, bad) and block minimum of tb in a fixed tree; the result is valid in thread 0.
+__device__ __forceinline__ void audit_block_reduce(double& ss, unsigned long long& bad, int& tb) {
+  __shared__ double s_ss[kAuditThreads / 32];
+  __shared__ unsigned long long s_bad[kAuditThreads / 32];
+  __shared__ int s_tb[kAuditThreads / 32];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    ss += __shfl_down_sync(0xffffffffu, ss, o);
+    bad += __shfl_down_sync(0xffffffffu, bad, o);
+    tb = min(tb, __shfl_down_sync(0xffffffffu, tb, o));
+  }
+  if ((threadIdx.x & 31) == 0) {
+    s_ss[threadIdx.x >> 5] = ss;
+    s_bad[threadIdx.x >> 5] = bad;
+    s_tb[threadIdx.x >> 5] = tb;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int w = 1; w < kAuditThreads / 32; ++w) {
+      ss += s_ss[w];
+      bad += s_bad[w];
+      tb = min(tb, s_tb[w]);
+    }
+  }
+}
+__global__ void __launch_bounds__(kAuditThreads)
+grad_audit_kernel(const bin_adam_tensor_t* __restrict__ table, const int* __restrict__ chunk_prefix, int ntensors,
+                  GradAuditPartial* __restrict__ partial) {
+  __shared__ int s_t;
+  if (threadIdx.x == 0) {
+    int lo = 0, hi = ntensors - 1;                     // as adam_step_kernel
+    while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if (chunk_prefix[mid] <= (int)blockIdx.x) lo = mid; else hi = mid - 1;
+    }
+    s_t = lo;
+  }
+  __syncthreads();
+  const int t = s_t;
+  const float* __restrict__ G = table[t].g;
+  const size_t n = (size_t)table[t].n;
+  const size_t base = (size_t)((int)blockIdx.x - chunk_prefix[t]) * kAdamChunk;
+  const size_t end = (base + kAdamChunk < n) ? base + kAdamChunk : n;
+  double ss = 0.0;
+  unsigned nbad = 0;
+  size_t tail = base;                                  // first element the scalar loop reads
+  if ((((uintptr_t)G) & 15u) == 0) {                   // base is a multiple of 4 elements
+    tail = base + ((end - base) & ~(size_t)3);
+    for (size_t i = base + threadIdx.x * 4; i < tail; i += kAuditThreads * 4) {
+      const float4 g = *reinterpret_cast<const float4*>(G + i);
+      audit_one(g.x, ss, nbad);
+      audit_one(g.y, ss, nbad);
+      audit_one(g.z, ss, nbad);
+      audit_one(g.w, ss, nbad);
+    }
+  }
+  for (size_t i = tail + threadIdx.x; i < end; i += kAuditThreads) audit_one(G[i], ss, nbad);
+  unsigned long long bad = nbad;
+  int tb = nbad ? t : INT_MAX;
+  audit_block_reduce(ss, bad, tb);
+  if (threadIdx.x == 0) partial[blockIdx.x] = GradAuditPartial{ss, (unsigned)bad, tb};
+}
+__global__ void __launch_bounds__(kAuditThreads)
+grad_audit_reduce_kernel(const GradAuditPartial* __restrict__ partial, int nchunks, float grad_scale, float max_norm,
+                         bin_grad_audit_t* __restrict__ audit) {
+  double ss = 0.0;
+  unsigned long long bad = 0;
+  int tb = INT_MAX;
+  for (int i = threadIdx.x; i < nchunks; i += kAuditThreads) {
+    const GradAuditPartial p = partial[i];
+    ss += p.sumsq;
+    bad += p.nonfinite;
+    tb = min(tb, p.first_bad);
+  }
+  audit_block_reduce(ss, bad, tb);
+  if (threadIdx.x == 0) {
+    const float norm = (float)(fabs((double)grad_scale) * sqrt(ss));
+    // torch.nn.utils.clip_grad_norm_: clip_coef = max_norm / (total_norm + 1e-6), clamped to 1
+    const float coef = isinf(max_norm) ? 1.f : fminf(1.f, __fdiv_rn(max_norm, norm + 1e-6f));
+    audit->sumsq = ss;
+    audit->nonfinite = bad;
+    audit->first_bad = bad ? tb : -1;
+    audit->skip = bad != 0;
+    audit->norm = norm;
+    audit->coef = coef;
   }
 }
 
@@ -1178,11 +1299,26 @@ int launch_u8_to_frame(const uint8_t* img, int h, int w, int pl, int pr, int pt,
 }
 int launch_adam_step(const bin_adam_tensor_t* table, const int* chunk_prefix, int ntensors, int nchunks, float lr,
                      float beta1, float beta2, float eps, float weight_decay, float bias_correction1,
-                     float bias_correction2, float grad_scale, cudaStream_t s) {
+                     float bias_correction2, float grad_scale, const bin_grad_audit_t* audit, cudaStream_t s) {
   if (ntensors < 1 || nchunks < 1 || !(bias_correction1 > 0.f) || !(bias_correction2 > 0.f))
     return fail(BIN_ERR_ARG, "adam_step: empty table or non-positive bias correction");
-  adam_step_kernel<<<nchunks, 256, 0, s>>>(table, chunk_prefix, ntensors, lr / bias_correction1, beta1, beta2, eps,
-                                           weight_decay, 1.f / sqrtf(bias_correction2), grad_scale);
+  const float lr_bc1 = lr / bias_correction1, inv_sqrt_bc2 = 1.f / sqrtf(bias_correction2);
+  if (audit)
+    adam_step_kernel<true><<<nchunks, 256, 0, s>>>(table, chunk_prefix, ntensors, lr_bc1, beta1, beta2, eps, weight_decay,
+                                                   inv_sqrt_bc2, grad_scale, audit);
+  else
+    adam_step_kernel<false><<<nchunks, 256, 0, s>>>(table, chunk_prefix, ntensors, lr_bc1, beta1, beta2, eps,
+                                                    weight_decay, inv_sqrt_bc2, grad_scale, nullptr);
+  BIN_CUDA_OK(cudaGetLastError());
+  return BIN_OK;
+}
+size_t grad_audit_scratch_bytes(int nchunks) { return nchunks < 1 ? 0 : (size_t)nchunks * sizeof(GradAuditPartial); }
+int launch_grad_audit(const bin_adam_tensor_t* table, const int* chunk_prefix, int ntensors, int nchunks, float grad_scale,
+                      float max_norm, void* scratch, bin_grad_audit_t* audit, cudaStream_t s) {
+  grad_audit_kernel<<<nchunks, kAuditThreads, 0, s>>>(table, chunk_prefix, ntensors, (GradAuditPartial*)scratch);
+  BIN_CUDA_OK(cudaGetLastError());
+  grad_audit_reduce_kernel<<<1, kAuditThreads, 0, s>>>((const GradAuditPartial*)scratch, nchunks, grad_scale, max_norm,
+                                                       audit);
   BIN_CUDA_OK(cudaGetLastError());
   return BIN_OK;
 }

@@ -326,6 +326,32 @@ int bin_adam_step(const bin_adam_tensor_t* table_dev, const int* chunk_prefix_de
                   float beta1, float beta2, float eps, float weight_decay, float bias_correction1,
                   float bias_correction2, float grad_scale, bin_stream_t s);
 
+/* ---- guarded optimizer step: a device-side audit of all gradients, then an Adam step that obeys it --------------- */
+/* bin_grad_audit makes one pass over the g column of an Adam table (two launches: one block per chunk, then one block)
+ * and leaves this record on the device.  Every sum is fp64 in a fixed order and the grids depend on the tensor shapes
+ * alone, so the record's bytes are reproducible.  sumsq and norm cover the finite elements. */
+typedef struct {
+  double sumsq;                 /* sum of g^2 over every finite element of every tensor                              */
+  unsigned long long nonfinite; /* elements that are inf or NaN                                                     */
+  int first_bad;                /* lowest table index of a tensor with such an element, -1 if none                  */
+  int skip;                     /* nonfinite != 0: bin_adam_step_guarded writes nothing                              */
+  float norm;                   /* |grad_scale| * sqrt(sumsq): the global L2 norm of the gradients Adam would see    */
+  float coef;                   /* min(1, max_norm / (norm + 1e-6)) as torch's clip_grad_norm_; 1 if max_norm is inf  */
+} bin_grad_audit_t;
+/* Bytes of per-chunk partial sums (device, 16-byte aligned); 0 if nchunks < 1. */
+size_t bin_grad_audit_scratch_bytes(int nchunks);
+/* table / chunk_prefix as bin_adam_step takes them; one table may span every parameter group, so that one record
+ * decides for the whole optimizer.  max_norm > 0, INFINITY for no clipping.  NULL, misaligned or empty arguments fail
+ * with BIN_ERR_ARG and a small scratch with BIN_ERR_WORKSPACE, before any launch. */
+int bin_grad_audit(const bin_adam_tensor_t* table_dev, const int* chunk_prefix_dev, int ntensors, int nchunks,
+                   float grad_scale, float max_norm, void* scratch, size_t scratch_bytes, bin_grad_audit_t* audit_dev,
+                   bin_stream_t s);
+/* bin_adam_step that reads audit_dev on the device: if skip, p, m and v keep their bits; otherwise the step runs with
+ * grad_scale * coef in place of grad_scale (coef == 1 gives bin_adam_step's bits).  No host synchronisation. */
+int bin_adam_step_guarded(const bin_adam_tensor_t* table_dev, const int* chunk_prefix_dev, int ntensors, int nchunks,
+                          float lr, float beta1, float beta2, float eps, float weight_decay, float bias_correction1,
+                          float bias_correction2, float grad_scale, const bin_grad_audit_t* audit_dev, bin_stream_t s);
+
 /* ---- training-data synthesis (SURVEY 8f rank 4): create_dataset_blur_N_frames_average.py:108-134 ------------------ */
 /* frames: device uint8 [T][frame_bytes] (consecutive sharp frames, any pixel layout); out: [nwin][frame_bytes].
  * out[w] = uint8( sum_{j=-r..r} float32(frames[first_mid + w*stride + j]) / float32(2r+1) ), r = (window_size-1)/2
