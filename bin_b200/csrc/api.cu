@@ -897,6 +897,29 @@ int bin_rdb_fwd(const void* blob, int nframes, int index, const float* x, float*
   return launch_p8_to_nchw(out, 0, kG0, y, (cudaStream_t)s);
 }
 
+// The window's dataflow (SURVEY App. A), one row per backbone call in issue order.  A node is an output o[0..13], one of
+// the 9 workspace images (the ConvLSTM images p*, then the step-1 intermediates t*; tmp[node - 14]) or an input frame.
+enum { P4 = 14, P6, P8, P5, P7, P6B, T0, T1, T2, WIN_NODES, FR = 32 };
+struct WinCall { int dst, in[BIN_MAX_FRAMES]; };
+static const WinCall kWinCalls[17] = {
+    // Stage 1 (RDN.py:371-374): 4 calls of step 0 + the one stage-1 call of step 1 that is not a repeat.
+    {0, {FR + 0, FR + 1}}, {1, {FR + 1, FR + 2}}, {2, {FR + 2, FR + 3}}, {3, {FR + 3, FR + 4}},
+    {10, {FR + 4, FR + 5}},
+    // Stage 2: step 0 (RDN.py:384-386, "prev" slot duplicated) + step 1 (RDN.py:377-379) in ONE launch of 6 calls:
+    // the step-1 calls only need stage-1 outputs and their ConvLSTM images, not step-0's stage 2.
+    {4, {0, 0, 1}}, {5, {1, 1, 2}}, {6, {2, 2, 3}}, {T0, {P4, 1, 2}}, {T1, {P6, 2, 3}}, {11, {P8, 3, 10}},
+    // Stage 3: step 0 (RDN.py:387-388) + step 1 (RDN.py:380-381)
+    {7, {4, FR + 1, 4, 5, FR + 2}}, {8, {5, FR + 2, 5, 6, FR + 3}}, {T2, {P5, FR + 2, T0, T1, FR + 3}},
+    {12, {P7, FR + 3, T1, 11, FR + 4}},
+    // Stage 4: step 0 (RDN.py:389) + step 1 (RDN.py:382)
+    {9, {1, 1, 7, 8, 2}}, {13, {P6B, 2, T2, 12, 3}}};
+static const int kStageFrames[4] = {2, 3, 5, 5};
+static const int kStageRow0[5] = {0, 5, 11, 15, 17};            // rows of stage k: kStageRow0[k] .. kStageRow0[k + 1] - 1
+// ConvLSTM cell k writes image P4 + k from output kCellSrc[k]; the cells of one recurrent hand-off (RDN.py:451-453,
+// 454-455, 456) run before stage kCellStage[k] and are independent: one launch for all of them (grid.z = cell).
+static const int kCellSrc[6] = {1, 2, 3, 5, 6, 8};
+static const int kCellStage[6] = {1, 1, 1, 2, 2, 3};
+
 static int window_fwd_impl(const bin_net_t* net, const float* const* F, float* const* o, int B, int H, int W, void* workspace,
                            size_t workspace_bytes, bin_stream_t s_, int x3) {
   if (!net || !F || !o) return fail(BIN_ERR_ARG, "window_fwd: null argument");
@@ -905,42 +928,58 @@ static int window_fwd_impl(const bin_net_t* net, const float* const* F, float* c
   if (workspace_bytes < need) return fail(BIN_ERR_WORKSPACE, "window_fwd: workspace too small");
   const size_t fbytes = align_up((size_t)B * 3 * H * W * sizeof(float), 256);
   uint8_t* base = (uint8_t*)workspace;
-  float* tmp[9];
-  for (int i = 0; i < 9; ++i) tmp[i] = (float*)(base + i * fbytes);
+  float* node[WIN_NODES];
+  for (int i = 0; i < 14; ++i) node[i] = o[i];
+  for (int i = 14; i < WIN_NODES; ++i) node[i] = (float*)(base + (i - 14) * fbytes);
   void* bws = base + 9 * fbytes;
   const size_t bws_bytes = workspace_bytes - 9 * fbytes;
-  float *p4 = tmp[0], *p6 = tmp[1], *p8 = tmp[2], *p5 = tmp[3], *p7 = tmp[4], *p6b = tmp[5];
-  float *t0 = tmp[6], *t1 = tmp[7], *t2 = tmp[8];
-  // the cells of one recurrent hand-off are independent: one launch for all of them (grid.z = cell)
-  auto lstm = [&](int k0, int n, std::initializer_list<const float*> xs, std::initializer_list<float*> hs) {
-    LstmCells c;
-    memset(&c, 0, sizeof(c));
-    int i = 0;
-    for (const float* x : xs) c.x[i++] = x;
-    i = 0;
-    for (float* h : hs) c.h_out[i++] = h;
-    for (i = 0; i < n; ++i) { c.w[i] = net->lstm_w[k0 + i]; c.b[i] = net->lstm_b[k0 + i]; }
-    return launch_convlstm_multi(c, n, B, H, W, s);
+  // A NULL o[i] means "do not compute output i".  for_out[n] >= 0 when node n is computed: n itself for a non-NULL
+  // output, and for a workspace image the output its first reader serves (the stages are walked last to first, so a
+  // node's readers are seen before its writer).  The caller passes a closed set: no computed node reads a NULL output.
+  int for_out[WIN_NODES], nout = 0;
+  for (int i = 0; i < WIN_NODES; ++i) for_out[i] = (i < 14 && o[i]) ? i : -1;
+  for (int i = 0; i < 14; ++i) nout += o[i] != nullptr;
+  if (!nout) return fail(BIN_ERR_ARG, "window_fwd: every output pointer is NULL");
+  auto reads = [&](int src, int reader) -> int {
+    if (src >= FR) return BIN_OK;
+    if (src < 14 && !o[src])
+      return fail(BIN_ERR_ARG, "window_fwd: output " + std::to_string(for_out[reader]) + " depends on output " +
+                                   std::to_string(src) + ", whose pointer is NULL");
+    if (for_out[src] < 0) for_out[src] = for_out[reader];
+    return BIN_OK;
   };
-  // Stage 1 (RDN.py:371-374): 4 calls of step 0 + the one stage-1 call of step 1 that is not a repeat.
-  BIN_TRY(run_stage(net, 0, 2, {{{F[0], F[1]}, o[0]}, {{F[1], F[2]}, o[1]}, {{F[2], F[3]}, o[2]},
-                               {{F[3], F[4]}, o[3]}, {{F[4], F[5]}, o[10]}}, B, H, W, bws, bws_bytes, s, x3));
-  // recurrent hand-off for the stage-1 outputs (RDN.py:451-453)
-  BIN_TRY(lstm(0, 3, {o[1], o[2], o[3]}, {p4, p6, p8}));
-  // Stage 2: step 0 (RDN.py:384-386, "prev" slot duplicated) + step 1 (RDN.py:377-379) in ONE launch of 6 calls:
-  // the step-1 calls only need stage-1 outputs and their ConvLSTM images, not step-0's stage 2.
-  BIN_TRY(run_stage(net, 1, 3, {{{o[0], o[0], o[1]}, o[4]}, {{o[1], o[1], o[2]}, o[5]}, {{o[2], o[2], o[3]}, o[6]},
-                               {{p4, o[1], o[2]}, t0}, {{p6, o[2], o[3]}, t1}, {{p8, o[3], o[10]}, o[11]}},
-                    B, H, W, bws, bws_bytes, s, x3));
-  BIN_TRY(lstm(3, 2, {o[5], o[6]}, {p5, p7}));                                    // RDN.py:454-455
-  // Stage 3: step 0 (RDN.py:387-388) + step 1 (RDN.py:380-381)
-  BIN_TRY(run_stage(net, 2, 5, {{{o[4], F[1], o[4], o[5], F[2]}, o[7]}, {{o[5], F[2], o[5], o[6], F[3]}, o[8]},
-                               {{p5, F[2], t0, t1, F[3]}, t2}, {{p7, F[3], t1, o[11], F[4]}, o[12]}},
-                    B, H, W, bws, bws_bytes, s, x3));
-  BIN_TRY(lstm(5, 1, {o[8]}, {p6b}));                                             // RDN.py:456
-  // Stage 4: step 0 (RDN.py:389) + step 1 (RDN.py:382)
-  BIN_TRY(run_stage(net, 3, 5, {{{o[1], o[1], o[7], o[8], o[2]}, o[9]}, {{p6b, o[2], t2, o[12], o[3]}, o[13]}},
-                    B, H, W, bws, bws_bytes, s, x3));
+  for (int stage = 3; stage >= 0; --stage) {
+    for (int c = kStageRow0[stage]; c < kStageRow0[stage + 1]; ++c) {
+      const WinCall& wc = kWinCalls[c];
+      if (for_out[wc.dst] < 0) continue;
+      for (int f = 0; f < kStageFrames[stage]; ++f) BIN_TRY(reads(wc.in[f], wc.dst));
+    }
+    for (int k = 0; k < 6; ++k)
+      if (kCellStage[k] == stage && for_out[P4 + k] >= 0) BIN_TRY(reads(kCellSrc[k], P4 + k));
+  }
+  for (int stage = 0; stage < 4; ++stage) {
+    LstmCells cells;
+    memset(&cells, 0, sizeof(cells));
+    int ncells = 0;
+    for (int k = 0; k < 6; ++k) {
+      if (kCellStage[k] != stage || for_out[P4 + k] < 0) continue;
+      cells.x[ncells] = node[kCellSrc[k]]; cells.h_out[ncells] = node[P4 + k];
+      cells.w[ncells] = net->lstm_w[k]; cells.b[ncells] = net->lstm_b[k];
+      ++ncells;
+    }
+    if (ncells) BIN_TRY(launch_convlstm_multi(cells, ncells, B, H, W, s));
+    std::vector<Call> calls;
+    for (int c = kStageRow0[stage]; c < kStageRow0[stage + 1]; ++c) {
+      const WinCall& wc = kWinCalls[c];
+      if (for_out[wc.dst] < 0) continue;
+      Call call;
+      memset(&call, 0, sizeof(call));
+      for (int f = 0; f < kStageFrames[stage]; ++f) call.in[f] = wc.in[f] >= FR ? F[wc.in[f] - FR] : node[wc.in[f]];
+      call.out = node[wc.dst];
+      calls.push_back(call);
+    }
+    if (!calls.empty()) BIN_TRY(run_stage(net, stage, kStageFrames[stage], calls, B, H, W, bws, bws_bytes, s, x3));
+  }
   return BIN_OK;
 }
 

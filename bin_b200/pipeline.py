@@ -13,6 +13,9 @@ import torch
 
 
 class WindowPipeline:
+    """Copies back the window outputs `out_indices`; call rdn.set_outputs(net, out_indices) first so that the net
+    computes only those."""
+
     def __init__(self, net: torch.nn.Module, device, out_indices: Sequence[int] = (13, 8, 12), slots: int = 2):
         self.net, self.dev, self.out_idx = net, torch.device(device), tuple(out_indices)
         self.s_in, self.s_out = torch.cuda.Stream(self.dev), torch.cuda.Stream(self.dev)

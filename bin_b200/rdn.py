@@ -22,7 +22,7 @@ import torch.nn.init as weight_init
 from . import _lib, ops
 from ._lib import BinB200Error, Net, check, lib
 
-__all__ = ["set_precision", "set_self_ensemble", "set_activation_checkpointing", "ConvLSTMCell", "pixel_reshuffle", "RDB_Conv", "RDB",
+__all__ = ["set_precision", "set_self_ensemble", "set_activation_checkpointing", "set_outputs", "ConvLSTMCell", "pixel_reshuffle", "RDB_Conv", "RDB",
            "RDN_residual_interp_2_input",
            "RDN_residual_interp_2_1_input", "RDN_residual_interp_4_1_input", "RDN_residual_interp_5_input",
            "RDN_residual_interp_5_input_ConvLSTM_L", "bin_stage4_lstm"]
@@ -388,23 +388,72 @@ _LSTM_NAMES = ["clstm_4_prime", "clstm_6_prime", "clstm_8_prime", "clstm_5_prime
                "clstm_6_prime_prime_prime"]
 
 
-def _window_schedule(stage, lstm, pyr, F, s1):
+def _window_schedule(stage, lstm, pyr, F, s1, live=None):
     """Stages 2-4 of the six-frame window (RDN.py:422-465) -> the 14-tuple: the unique backbone calls of both
     recurrent steps and the 6 live ConvLSTM calls, in the order bin_window_fwd issues them (SURVEY App. A).
     stage(model, calls) runs one batched backbone stage and returns its outputs, lstm(k, x) returns h of ConvLSTM cell k
-    (the order of _LSTM_NAMES) from no state, and s1 holds the stage-1 outputs o[0..3], o[10] of the frame pairs."""
+    (the order of _LSTM_NAMES) from no state, and s1 holds the stage-1 outputs o[0..3], o[10] of the frame pairs.
+    With `live` (a node set from _window_live) only the calls and cells in it run, each stage with its shortened call
+    list, and every other result, s1 entries included, is None."""
     m2, m3, m4 = pyr.model2_1, pyr.model3_1, pyr.model4_1
+
+    def run(n, model, calls):
+        keep = [i for i in range(len(calls)) if live is None or (n, i) in live]
+        outs = [None] * len(calls)
+        if keep:
+            for i, out in zip(keep, stage(model, [calls[i] for i in keep])):
+                outs[i] = out
+        return outs
+
+    def cell(k, x):
+        return lstm(k, x) if live is None or ("lstm", k) in live else None
+
     o = [None] * 14
     o[0], o[1], o[2], o[3], o[10] = s1
-    p4, p6, p8 = lstm(0, o[1]), lstm(1, o[2]), lstm(2, o[3])
-    o[4], o[5], o[6], t0, t1, o[11] = stage(m2, [(o[0], o[0], o[1]), (o[1], o[1], o[2]), (o[2], o[2], o[3]),
-                                                 (p4, o[1], o[2]), (p6, o[2], o[3]), (p8, o[3], o[10])])
-    p5, p7 = lstm(3, o[5]), lstm(4, o[6])
-    o[7], o[8], t2, o[12] = stage(m3, [(o[4], F[1], o[4], o[5], F[2]), (o[5], F[2], o[5], o[6], F[3]),
-                                       (p5, F[2], t0, t1, F[3]), (p7, F[3], t1, o[11], F[4])])
-    p6b = lstm(5, o[8])
-    o[9], o[13] = stage(m4, [(o[1], o[1], o[7], o[8], o[2]), (p6b, o[2], t2, o[12], o[3])])
+    p4, p6, p8 = cell(0, o[1]), cell(1, o[2]), cell(2, o[3])
+    o[4], o[5], o[6], t0, t1, o[11] = run(2, m2, [(o[0], o[0], o[1]), (o[1], o[1], o[2]), (o[2], o[2], o[3]),
+                                                  (p4, o[1], o[2]), (p6, o[2], o[3]), (p8, o[3], o[10])])
+    p5, p7 = cell(3, o[5]), cell(4, o[6])
+    o[7], o[8], t2, o[12] = run(3, m3, [(o[4], F[1], o[4], o[5], F[2]), (o[5], F[2], o[5], o[6], F[3]),
+                                        (p5, F[2], t0, t1, F[3]), (p7, F[3], t1, o[11], F[4])])
+    p6b = cell(5, o[8])
+    o[9], o[13] = run(4, m4, [(o[1], o[1], o[7], o[8], o[2]), (p6b, o[2], t2, o[12], o[3])])
     return tuple(o)
+
+
+def _record_window():
+    """The window's dependency graph, read off _window_schedule itself: the schedule runs on symbolic nodes, named
+    (stage, position in the stage's full call list) for a backbone call and ("lstm", k) for a ConvLSTM image.
+    -> (the node of each of the 14 outputs, {node: the nodes it reads})."""
+    from types import SimpleNamespace
+    reads = {(1, i): set() for i in range(5)}
+
+    def stage(n, calls):
+        for i, call in enumerate(calls):
+            reads[(n, i)] = {x for x in call if x is not None}
+        return [(n, i) for i in range(len(calls))]
+
+    def lstm(k, x):
+        reads[("lstm", k)] = {x}
+        return ("lstm", k)
+
+    outs = _window_schedule(stage, lstm, SimpleNamespace(model2_1=2, model3_1=3, model4_1=4), [None] * 6, list(reads))
+    return outs, reads
+
+
+_OUT_NODE, _NODE_READS = _record_window()
+
+
+def _window_live(wanted) -> frozenset:
+    """Every node (see _record_window) a window must compute so that the outputs `wanted` (indices 0..13) come out: the
+    backward closure of their nodes over the schedule's own dataflow."""
+    live, todo = set(), [_OUT_NODE[i] for i in wanted]
+    while todo:
+        n = todo.pop()
+        if n not in live:
+            live.add(n)
+            todo += _NODE_READS[n]
+    return frozenset(live)
 
 
 class RDN_residual_interp_5_input_ConvLSTM_L(nn.Module):
@@ -443,50 +492,63 @@ class RDN_residual_interp_5_input_ConvLSTM_L(nn.Module):
 
     def forward(self, B1, B3, B5, B7, B9, B11):
         """One 6-frame window -> the reference's 14-tuple (RDN.py:461-465): executes 17 unique
-        backbone calls of its 20 and the 6 live ConvLSTM calls of its 12 (SURVEY.md App. A)."""
+        backbone calls of its 20 and the 6 live ConvLSTM calls of its 12 (SURVEY.md App. A), or, with set_outputs,
+        only the calls the wanted outputs depend on."""
         frames = [B1, B3, B5, B7, B9, B11]
         ensemble = _ensemble_of(self)
+        sel = _outputs_of(self)
         if _needs_grad(frames + self._all_tensors()):
             if ensemble is not None:
                 raise BinB200Error(f"self-ensemble {ensemble!r} is inference-only: call the net under torch.no_grad(), "
                                    "or set_self_ensemble(net, None) to train")
+            if sel is not None:
+                raise BinB200Error(f"output selection {sel[0]} is inference-only: call the net under torch.no_grad(), "
+                                   "or set_outputs(net, None) to train")
             from .autograd import window_apply
             return window_apply(self, frames)
         frames = [f.contiguous() for f in frames]
         B, H, W = _check_frames(frames)
         dev = frames[0].device
+        wanted = range(14) if sel is None else sel[0]
+        live = range(14) if sel is None else _live_outputs(wanted)
         if ensemble is not None:
-            return self._forward_flipx4(frames, B, H, W, dev)
-        if _graphs_enabled() and not getattr(self, "_is_replica", False) and not torch.cuda.is_current_stream_capturing():
-            return self._forward_graphed(frames, B, H, W, dev)
-        with torch.cuda.device(dev):
-            return tuple(self._launch_window(frames, B, H, W, dev)[0])
+            outs = self._forward_flipx4(frames, B, H, W, dev, live, wanted)
+        elif _graphs_enabled() and not getattr(self, "_is_replica", False) and not torch.cuda.is_current_stream_capturing():
+            outs = self._forward_graphed(frames, B, H, W, dev, live, wanted)
+        else:
+            with torch.cuda.device(dev):
+                outs = self._launch_window(frames, B, H, W, dev, live)[0]
+        return tuple(outs) if sel is None else _selected(outs, sel)
 
-    def _launch_window(self, frames, B, H, W, dev):
-        outs = [torch.empty_like(frames[0]) for _ in range(14)]
+    def _launch_window(self, frames, B, H, W, dev, live=range(14)):
+        """One bin_window_fwd_p call computing the outputs `live` (a set closed under the window's dataflow); the other
+        positions of the returned list are None and reach the library as NULL pointers."""
+        outs = [torch.empty_like(frames[0]) if i in live else None for i in range(14)]
         prec = _prec_of(self)
         net = self._net(prec)
         ws = _workspace(dev, lib().bin_window_workspace_bytes_p(B, H, W, prec))
         fp = (C.c_void_p * 6)(*[f.data_ptr() for f in frames])
-        op = (C.c_void_p * 14)(*[o.data_ptr() for o in outs])
+        op = (C.c_void_p * 14)(*[None if o is None else o.data_ptr() for o in outs])
         check(lib().bin_window_fwd_p(C.byref(net), fp, op, B, H, W, ws.data_ptr(), ws.numel(), prec, ops._stream()))
         return outs, ws
 
-    def _forward_flipx4(self, frames, B, H, W, dev):
-        """x4 flip self-ensemble (utils/test_util.py:110-132 flipx4_forward, applied to all 6 frames and all 14 outputs):
-        the four orientations run as ONE window at batch 4B, then each output is flipped back and averaged.  Eager, not
-        graphed: a graph capture would hold a second batch-4B workspace (about 25 GB at 768x1344) in its private pool."""
+    def _forward_flipx4(self, frames, B, H, W, dev, live, wanted):
+        """x4 flip self-ensemble (utils/test_util.py:110-132 flipx4_forward, applied to all 6 frames and the wanted
+        outputs): the four orientations run as ONE window at batch 4B, then each output is flipped back and averaged.
+        Eager, not graphed: a graph capture would hold a second batch-4B workspace (about 25 GB at 768x1344) in its
+        private pool."""
         with torch.cuda.device(dev):
             big = ops.flipx4_expand(frames)
-            outs, _ = self._launch_window(big, 4 * B, H, W, dev)
+            outs, _ = self._launch_window(big, 4 * B, H, W, dev, live)
             del big
-            return tuple(ops.flipx4_mean(outs))
+            return _flipx4_mean_at(outs, wanted)
 
-    def _forward_graphed(self, frames, B, H, W, dev):
-        """The ~340 kernel launches of a window are captured once per (shape, weight version) into a
+    def _forward_graphed(self, frames, B, H, W, dev, live, wanted):
+        """The ~340 kernel launches of a window are captured once per (shape, weight version, live outputs) into a
         CUDA graph and replayed: removes ~10 % of host launch overhead at 720p.  Inputs are copied
-        into the graph's static buffers, outputs are returned as fresh tensors (SURVEY 8b)."""
-        key = (dev.index, B, H, W, _prec_of(self), tuple((p.data_ptr(), p._version) for p in self._all_tensors()))
+        into the graph's static buffers, the wanted outputs are returned as fresh tensors (SURVEY 8b)."""
+        key = (dev.index, B, H, W, _prec_of(self), tuple(live),
+               tuple((p.data_ptr(), p._version) for p in self._all_tensors()))
         ent = self.__dict__.get("_graph_entry")
         with torch.cuda.device(dev):
             if ent is None or ent["key"] != key:
@@ -497,12 +559,12 @@ class RDN_residual_interp_5_input_ConvLSTM_L(nn.Module):
                 side = torch.cuda.Stream()
                 side.wait_stream(torch.cuda.current_stream())
                 with torch.cuda.stream(side):                       # warm-up: packs weights, opts kernels into their smem
-                    self._launch_window(static_in, B, H, W, dev)
+                    self._launch_window(static_in, B, H, W, dev, live)
                     _WS.pop(_ws_key(dev), None)                     # the side stream's scratch buffer is not needed again
                 torch.cuda.current_stream().wait_stream(side)
                 graph = torch.cuda.CUDAGraph()
                 with torch.cuda.graph(graph):
-                    static_out, ws = self._launch_window(static_in, B, H, W, dev)
+                    static_out, ws = self._launch_window(static_in, B, H, W, dev, live)
                     _WS.pop(_ws_key(dev), None)                     # owned by this entry (graph-private memory pool)
                 ent = {"key": key, "graph": graph, "in": static_in, "out": static_out, "ws": ws}
                 self.__dict__["_graph_entry"] = ent
@@ -510,7 +572,7 @@ class RDN_residual_interp_5_input_ConvLSTM_L(nn.Module):
                 for d, f in zip(ent["in"], frames):
                     d.copy_(f)
             ent["graph"].replay()
-            return tuple(o.clone() for o in ent["out"])
+            return [ent["out"][i].clone() if i in wanted else None for i in range(14)]
 
     def forward_pyramid3(self, B1, B3, B5, B7):
         """BASELINE config 2a: stages 1-3 on 4 frames -> [I2',I4',I6',I3',I5',I4''] (SURVEY 8d)."""
@@ -559,4 +621,72 @@ def set_self_ensemble(net: nn.Module, mode: Optional[str]) -> nn.Module:
         raise BinB200Error("set_self_ensemble: no RDN_residual_interp_5_input_ConvLSTM_L in this module")
     for m in nets:
         m.self_ensemble = mode
+    return net
+
+
+UNWANTED = ("none", "zeros")
+
+
+def _outputs_of(module) -> Optional[Tuple[Tuple[int, ...], str]]:
+    """`module.outputs`: None (all 14 outputs) or (the wanted indices in ascending order, "none" | "zeros")."""
+    sel = getattr(module, "outputs", None)
+    if sel is None:
+        return None
+    ok = (isinstance(sel, tuple) and len(sel) == 2 and isinstance(sel[0], tuple) and sel[0] and sel[1] in UNWANTED
+          and all(type(i) is int and 0 <= i < 14 for i in sel[0]) and list(sel[0]) == sorted(set(sel[0])))
+    if not ok:
+        raise BinB200Error(f"unknown output selection {sel!r}; set it with set_outputs(net, indices, unwanted)")
+    return sel
+
+
+def _live_outputs(wanted) -> Tuple[int, ...]:
+    """The outputs a window must compute for `wanted`: the wanted ones and those they are computed from."""
+    live = _window_live(wanted)
+    return tuple(i for i in range(14) if _OUT_NODE[i] in live)
+
+
+def _flipx4_mean_at(outs, wanted) -> list:
+    """ops.flipx4_mean of the outputs `wanted` of a batch-4B window, at their positions of a 14-list; None elsewhere."""
+    means = [None] * 14
+    for i, m in zip(wanted, ops.flipx4_mean([outs[i] for i in wanted])):
+        means[i] = m
+    return means
+
+
+def _selected(outs, sel) -> tuple:
+    """The 14-tuple a net with the selection `sel` returns: outs[i] at the wanted positions; elsewhere None, or with
+    unwanted="zeros" one shared all-zero view of an output's shape, backed by a single element."""
+    wanted, unwanted = sel
+    like = outs[wanted[0]]
+    rest = torch.zeros((), device=like.device).expand(like.shape) if unwanted == "zeros" else None
+    return tuple(outs[i] if i in wanted else rest for i in range(14))
+
+
+def set_outputs(net: nn.Module, indices, unwanted: str = "none") -> nn.Module:
+    """Compute only the outputs a caller reads, for every window net in `net.modules()` (so a DataParallel wrapper or a
+    model object holding the net works).  `indices`: distinct positions 0..13 of the 14-tuple, or None for all 14 (the
+    default).  A call still returns a 14-tuple: the wanted positions hold the same bits as without a selection, and the
+    backbone calls and ConvLSTM cells that no wanted output depends on do not run (13 of the 17 calls for (13, 8, 12),
+    the three images test.py writes).  The other positions hold None (unwanted="none"), so a wrong index fails loudly,
+    or one shared all-zero (B,3,H,W) view of a single element (unwanted="zeros"), for test.py and demo.py run unchanged:
+    they convert Ft_p[7] and Ft_p[9] to images they never use.  StreamingBIN follows the selection.  Inference only: a
+    grad-enabled call then raises.  It is a plain attribute, not a parameter or buffer: the state_dict is unchanged."""
+    if unwanted not in UNWANTED:
+        raise BinB200Error(f"unknown unwanted mode {unwanted!r}; use 'none' or 'zeros'")
+    sel = None
+    if indices is not None:
+        try:
+            idx = list(indices)
+        except TypeError:
+            raise BinB200Error(f"set_outputs: indices must be an iterable of ints in 0..13 or None; got {indices!r}") from None
+        if not idx:
+            raise BinB200Error("set_outputs: the selection is empty; pass None for all 14 outputs")
+        if any(type(i) is not int or not 0 <= i < 14 for i in idx) or len(set(idx)) != len(idx):
+            raise BinB200Error(f"set_outputs: indices must be distinct ints in 0..13; got {indices!r}")
+        sel = (tuple(sorted(idx)), unwanted)
+    nets = [m for m in net.modules() if isinstance(m, RDN_residual_interp_5_input_ConvLSTM_L)]
+    if not nets:
+        raise BinB200Error("set_outputs: no RDN_residual_interp_5_input_ConvLSTM_L in this module")
+    for m in nets:
+        m.outputs = sel
     return net

@@ -17,7 +17,8 @@ import torch
 
 from . import ops
 from ._lib import BinB200Error, check, lib
-from .rdn import _LSTM_NAMES, _batched, _ensemble_of, _window_schedule
+from .rdn import (_LSTM_NAMES, _batched, _ensemble_of, _flipx4_mean_at, _outputs_of, _selected, _window_live,
+                  _window_schedule)
 
 
 def test_py_padding(h: int, w: int) -> Tuple[int, int, int, int]:
@@ -71,7 +72,11 @@ class StreamingBIN:
 
     With the net's x4 flip self-ensemble on (rdn.set_self_ensemble), every pushed frame is expanded once into its four
     orientations (4B items), the stage-1 cache holds 4B outputs, and each window's 14 outputs are flipped back and
-    averaged: the same bits as calling the net per window."""
+    averaged: the same bits as calling the net per window.
+
+    With an output selection on the net (rdn.set_outputs) a window runs only the backbone calls its wanted outputs depend
+    on, and returns what the net would: for (13, 8, 12) the pair of the two oldest frames is never evaluated, so the
+    first window costs 13 calls and every later one 10."""
 
     def __init__(self, net):
         self.net = net
@@ -79,7 +84,7 @@ class StreamingBIN:
         self.s1: "OrderedDict[Tuple[int, int], torch.Tensor]" = OrderedDict()   # stage-1 output per adjacent frame pair
         self.next_id = 0
         self.backbone_calls = 0
-        self.key = None                                               # (ensemble mode, pushed frame shape) of the cache
+        self.key = None                                # (ensemble mode, output selection, frame shape) of the cache
 
     def reset(self):
         self.frames.clear()
@@ -90,7 +95,7 @@ class StreamingBIN:
         if not frame.is_cuda or frame.dtype != torch.float32 or frame.dim() != 4 or frame.shape[1] != 3:
             raise BinB200Error("StreamingBIN.push expects a (B,3,H,W) fp32 CUDA frame (see upload_frame_u8)")
         ensemble = _ensemble_of(self.net)
-        key = (ensemble, frame.shape)
+        key = (ensemble, _outputs_of(self.net), frame.shape)
         if self.frames and self.key != key:
             self.reset()
         self.key = key
@@ -112,18 +117,20 @@ class StreamingBIN:
         net = self.net
         ids = [i for i, _ in self.frames]
         F = [f for _, f in self.frames]
-        # ---- stage 1: only the frame pairs not seen before (1 per window in steady state, 5 for the first)
-        need = [(a, b) for a, b in zip(range(5), range(1, 6)) if (ids[a], ids[b]) not in self.s1]
+        sel = self.key[1]
+        wanted = range(14) if sel is None else sel[0]
+        live = _window_live(wanted)
+        # ---- stage 1: only the live frame pairs not seen before (1 per window in steady state, 5 for the first)
+        need = [(a, a + 1) for a in range(5) if (1, a) in live and (ids[a], ids[a + 1]) not in self.s1]
         if need:
             outs = _batched(net.model.model1_1, [(F[a], F[b]) for a, b in need])
             for (a, b), o in zip(need, outs):
                 self.s1[(ids[a], ids[b])] = o
-            self.backbone_calls += len(need)
-        s1 = [self.s1[(ids[k], ids[k + 1])] for k in range(5)]
+        s1 = [self.s1.get((ids[k], ids[k + 1])) for k in range(5)]
         cells = [getattr(net, n) for n in _LSTM_NAMES]
         lstm = lambda k, x: ops.convlstm_fwd(x, cells[k].Gates.weight.detach(), cells[k].Gates.bias.detach(), None)[0]
-        o = _window_schedule(_batched, lstm, net.model, F, s1)
-        self.backbone_calls += 12
+        o = _window_schedule(_batched, lstm, net.model, F, s1, live)
+        self.backbone_calls += len(need) + sum(1 for n in live if n[0] in (2, 3, 4))
         if self.key[0] is not None:
-            return tuple(ops.flipx4_mean(o))
-        return o
+            o = tuple(_flipx4_mean_at(o, wanted))
+        return o if sel is None else _selected(o, sel)

@@ -263,7 +263,13 @@ typedef struct {
 size_t bin_window_workspace_bytes(int B, int H, int W);
 /* frames[6], outs[14]: (B,3,H,W) fp32 NCHW device tensors.  Executes the 17 unique backbone
  * calls of the reference's 20 (the 3 repeated stage-1 calls are bit-identical) and the 6 live
- * ConvLSTM calls of its 12 (SURVEY.md Appendix A). */
+ * ConvLSTM calls of its 12 (SURVEY.md Appendix A).
+ * A NULL outs_host[i] means "do not compute output i": its backbone call is dropped from its stage's launch, and a
+ * stage, a ConvLSTM cell or a workspace image that then has no reader left is dropped too (outputs 13, 8, 12 alone need
+ * 13 of the 17 calls).  The non-NULL outputs hold the same bits as with all 14 present.  The non-NULL set must be closed
+ * under the window's dataflow: if a computed output reads a NULL one the call returns BIN_ERR_ARG before launching
+ * anything, and bin_last_error() names both indices.  All-NULL is BIN_ERR_ARG too.  The workspace size and layout do not
+ * depend on which outputs are NULL. */
 int bin_window_fwd(const bin_net_t* net, const float* const* frames_host, float* const* outs_host, int B, int H,
                    int W, void* workspace, size_t workspace_bytes, bin_stream_t s);
 /* Precision-parameterised twins of the calls above (prec = BIN_PREC_F16 | BIN_PREC_F32X3).  In BIN_PREC_F32X3 the
