@@ -389,7 +389,7 @@ __device__ __forceinline__ float fast_sigmoid(float v) { return __frcp_rn(1.f + 
 __device__ __forceinline__ float fast_tanh(float v) { return 2.f * __frcp_rn(1.f + __expf(-2.f * v)) - 1.f; }
 
 template <bool STATE>
-__global__ void __launch_bounds__(256, 3) convlstm_kernel(const __grid_constant__ LstmCells P, int B, int H, int W, int tiles_x,
+__global__ void __launch_bounds__(256, STATE ? 2 : 3) convlstm_kernel(const __grid_constant__ LstmCells P, int B, int H, int W, int tiles_x,
                                                        int tiles_y) {
   constexpr int C = STATE ? 6 : 3;
   __shared__ __align__(16) float sin_[C][kLsTH + 2][kLsPitch];
@@ -441,7 +441,7 @@ __global__ void __launch_bounds__(256, 3) convlstm_kernel(const __grid_constant_
   for (int px = 0; px < 4; ++px)
 #pragma unroll
     for (int k = 0; k < 12; ++k) acc[px][k] = sb[k];
-#pragma unroll
+#pragma unroll 1
   for (int c = 0; c < C; ++c) {
 #pragma unroll
     for (int ky = 0; ky < 3; ++ky) {
@@ -469,7 +469,10 @@ __global__ void __launch_bounds__(256, 3) convlstm_kernel(const __grid_constant_
     float cp[4] = {0.f, 0.f, 0.f, 0.f};
     if (STATE) {
       if (vec) { const float4 q = *reinterpret_cast<const float4*>(P.c_prev[cell] + off); cp[0] = q.x; cp[1] = q.y; cp[2] = q.z; cp[3] = q.w; }
-      else { for (int px = 0; px < 4; ++px) if (x + px < W) cp[px] = P.c_prev[cell][off + px]; }
+      else {
+#pragma unroll
+        for (int px = 0; px < 4; ++px) if (x + px < W) cp[px] = P.c_prev[cell][off + px];
+      }
     }
     float hn[4], cn[4];
 #pragma unroll
@@ -483,6 +486,7 @@ __global__ void __launch_bounds__(256, 3) convlstm_kernel(const __grid_constant_
       *reinterpret_cast<float4*>(P.h_out[cell] + off) = make_float4(hn[0], hn[1], hn[2], hn[3]);
       if (P.c_out[cell]) *reinterpret_cast<float4*>(P.c_out[cell] + off) = make_float4(cn[0], cn[1], cn[2], cn[3]);
     } else {
+#pragma unroll
       for (int px = 0; px < 4; ++px)
         if (x + px < W) {
           P.h_out[cell][off + px] = hn[px];

@@ -68,6 +68,14 @@ __device__ __forceinline__ float2 unpack_h2(uint32_t u) {
 
 constexpr int kThreads = 384;   // warpgroup 0: TMA producer (one thread); warpgroups 1, 2: wgmma + epilogue
 
+// PixelShuffle epilogue staging buffer of one consumer warp: one accumulator row set (8 low-res pixels x 128 channels)
+// as [plane q][pixel r][sub-pixel s][8 channels] fp16, each pixel's 4 sub-pixels padded by 16 bytes so that the
+// 2-byte writes of a warp spread over the banks (2-way conflicts instead of 4-way); X3 adds a second part for lo.
+constexpr int kPsRowBytes = 4 * 16 + 16;
+constexpr int kPsPartBytes = 4 * 8 * kPsRowBytes;
+template <bool X3>
+constexpr int kPsWarpBytes = (X3 ? 2 : 1) * kPsPartBytes;
+
 // X3 ("fp32-accurate" mode, 1e-5 parity bar): every value is carried as an fp16 pair hi = fp16(x), lo = fp16(x - hi).
 // The pair is within 2^-22 |x| of x while lo is a normal fp16 number; below |x| ~ 2^-3 lo is subnormal and the pair
 // carries an absolute 2^-25 instead (the fp16 subnormal half-spacing), which is what tests/test_gpu_forward_fuzz.py bars.
@@ -88,12 +96,6 @@ __device__ __forceinline__ void store_pair(__half* p, size_t lo_off, float a, fl
     *reinterpret_cast<uint32_t*>(p) = pack_h2(a, b);
   }
 }
-template <bool X3>
-__device__ __forceinline__ void store_one(__half* p, size_t lo_off, float a) {
-  const __half h = __float2half_rn(a);
-  *p = h;
-  if constexpr (X3) p[lo_off] = __float2half_rn(a - __half2float(h));
-}
 
 // Roles (384 threads, 1 CTA/SM, persistent over tiles):
 //   warp 0 lane 0 : TMA producer (activation box + weight slab per stage, mbarrier ring)
@@ -105,6 +107,7 @@ __device__ __forceinline__ void store_one(__half* p, size_t lo_off, float a) {
 template <int NT, int KS, int EPI, bool SX, bool X3>
 __global__ void __launch_bounds__(kThreads, 1) conv_igemm_kernel(const __grid_constant__ ConvParams p) {
   using C = ConvCfg<NT, KS, SX>;
+  static_assert(EPI != BIN_EPI_PIXSHUF || NT == 128, "the PixelShuffle staging buffer holds 4 output planes");
   constexpr int NA = C::NMMA / 2;                              // accumulator registers per thread and 64-row block
   auto tile_at = [&](int tq) { return p.reverse ? p.ntiles - 1 - tq : tq; };
   extern __shared__ __align__(1024) uint8_t smem[];
@@ -191,10 +194,51 @@ __global__ void __launch_bounds__(kThreads, 1) conv_igemm_kernel(const __grid_co
   const int wq = warp & 3;                                     // warp within the warpgroup: 16 rows of each 64-row block
   const int k4 = lane & 3;                                     // fragment column pair: columns 8 i + 2 k4, +1
   float* xs = reinterpret_cast<float*>(stage0 + (size_t)S * stage_bytes) + (2 * m + (wq >> 1)) * 2 * kXsFloats<NT>;
+  uint8_t* psbuf = stage0 + (size_t)S * stage_bytes + (warp - 4) * kPsWarpBytes<X3>;   // PIXSHUF staging buffer
   float acc[2][NA];
   constexpr float kAcc = X3 ? (1.f / 256.f) : 1.f;            // X3 weights are packed scaled by 2^8
   uint32_t s = 0, ph = 0;
+  // tile tq -> (cout block nh, tile column txi, tile row tyi, image b)
+  auto tile_coords = [&](int tq, int& nh, int& txi, int& tyi, int& b) {
+    int t = tile_at(tq);
+    nh = t % p.nh; t /= p.nh;
+    txi = t % p.tiles_x; t /= p.tiles_x;
+    tyi = t % p.tiles_y;
+    b = p.b0 + t / p.tiles_y;
+  };
+  // fragment of a 64-row block: acc[mb][4 i + 2 h + e] = row 16 wq + lane/4 + 8 h, column 8 i + 2 k4 + e
+  auto pixel = [&](int txi, int tyi, int mb, int h, int& y, int& x) {
+    const int L = m * 128 + mb * 64 + wq * 16 + (lane >> 2) + 8 * h;
+    const int ty = L >> 5, tx = L & 31;
+    y = p.y0 + tyi * kTH + ty; x = txi * C::TW + tx;
+    return (tx < C::TW) && (y < p.y0 + p.ny) && (x < p.W);
+  };
   for (int tq = blockIdx.x; tq < p.ntiles; tq += gridDim.x) {
+    // BIN_EPI_FINAL: the input frames this thread's outputs add are loaded here, so their latency hides behind the
+    // main loop; the epilogue sums them.
+    constexpr int NFR = EPI == BIN_EPI_FINAL ? BIN_MAX_FRAMES : 1;
+    float fpre[2][2][2][NFR];                                   // [mb][h][e][frame]
+    if constexpr (EPI == BIN_EPI_FINAL) {
+      int nh, txi, tyi, b;
+      tile_coords(tq, nh, txi, tyi, b);
+      const int call = b / p.fr.Bc, bb = b % p.fr.Bc;
+      const size_t hw = (size_t)p.H * p.W;
+#pragma unroll
+      for (int mb = 0; mb < 2; ++mb)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          int y, x;
+          const bool valid = pixel(txi, tyi, mb, h, y, x);
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int c = 2 * k4 + e;
+            const size_t off = ((size_t)bb * 3 + c) * hw + (size_t)y * p.W + x;
+#pragma unroll
+            for (int fi = 0; fi < NFR; ++fi)
+              fpre[mb][h][e][fi] = (valid && c < 3 && fi < p.fr.nframes) ? __ldg(p.fr.frame[call][fi] + off) : 0.f;
+          }
+        }
+    }
     // ---------------------------------------------------------- main loop: K = chunks x taps
     int unit = 0, prev = -1;
     for (int j = 0; j < spt; ++j) {
@@ -241,27 +285,34 @@ __global__ void __launch_bounds__(kThreads, 1) conv_igemm_kernel(const __grid_co
     if (lane == 0) mbar_arrive(&ctrl->empty[prev]);
 
     // ---------------------------------------------------------- epilogue from the accumulator fragments
-    // fragment of a 64-row block: acc[mb][4 i + 2 h + e] = row 16 wq + lane/4 + 8 h, column 8 i + 2 k4 + e
-    int t = tile_at(tq);
-    const int nh = t % p.nh; t /= p.nh;
-    const int txi = t % p.tiles_x; t /= p.tiles_x;
-    const int tyi = t % p.tiles_y;
-    const int b = p.b0 + t / p.tiles_y;
-    const int yend = p.y0 + p.ny;
+    int nh, txi, tyi, b;
+    tile_coords(tq, nh, txi, tyi, b);
 #pragma unroll
     for (int mb = 0; mb < 2; ++mb) {
       if constexpr (SX) xstack_sum<NT>(acc[mb], xs + mb * kXsFloats<NT>, 3 + 2 * m + (wq >> 1));   // barrier per warp pair
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        const int r = wq * 16 + (lane >> 2) + 8 * h;           // row within the 64-row block
-        const int L = m * 128 + mb * 64 + r;
-        const int ty = L >> 5, tx = L & 31;
-        const int y = p.y0 + tyi * kTH + ty, x = txi * C::TW + tx;
-        const bool valid = (tx < C::TW) && (y < yend) && (x < p.W);
+        int y, x;
+        const bool valid = pixel(txi, tyi, mb, h, y, x);
         // value of output channel column 8 i + 2 k4 + e of this pixel (SX: xstack_sum has added the kx = 1, 2 groups)
         auto val = [&](int i, int e) { return acc[mb][4 * i + 2 * h + e] * kAcc; };
         if constexpr (EPI == BIN_EPI_P8) {
           if (valid) {
+            // the row's residual values are all loaded before its first store: a store to p.out may alias p.res, so
+            // loads issued between the stores would each wait for a memory round trip of their own
+            constexpr int NR = SX ? 1 : NT / 8;
+            uint32_t rres[NR][X3 ? 2 : 1];
+            if (!SX && p.res != nullptr) {
+#pragma unroll
+              for (int i = 0; i < NR; ++i) {
+                const int rel = (nh * NT) / 8 + i;
+                if (rel >= p.store_planes) continue;
+                const int lp = p.res_plane0 + rel;
+                const size_t off = ((((size_t)b * p.res_planes + (X3 ? x3_plane(lp) : lp)) * p.H + y) * p.W + x) * 8 + 2 * k4;
+                rres[i][0] = *reinterpret_cast<const uint32_t*>(p.res + off);
+                if constexpr (X3) rres[i][X3 ? 1 : 0] = *reinterpret_cast<const uint32_t*>(p.res + off + (size_t)4 * p.H * p.W * 8);
+              }
+            }
 #pragma unroll
             for (int i = 0; i < NT / 8; ++i) {
               const int rel = (nh * NT) / 8 + i;                // channel plane relative to out_plane0
@@ -270,12 +321,10 @@ __global__ void __launch_bounds__(kThreads, 1) conv_igemm_kernel(const __grid_co
               float f0 = val(i, 0) + bsrc[n], f1 = val(i, 1) + bsrc[n + 1];
               if (p.relu) { f0 = fmaxf(f0, 0.f); f1 = fmaxf(f1, 0.f); }
               if (!SX && p.res != nullptr) {
-                const int lp = p.res_plane0 + rel;
-                const size_t off = ((((size_t)b * p.res_planes + (X3 ? x3_plane(lp) : lp)) * p.H + y) * p.W + x) * 8 + 2 * k4;
-                const float2 g = unpack_h2(*reinterpret_cast<const uint32_t*>(p.res + off));
+                const float2 g = unpack_h2(rres[SX ? 0 : i][0]);
                 f0 += g.x; f1 += g.y;
                 if constexpr (X3) {
-                  const float2 g2 = unpack_h2(*reinterpret_cast<const uint32_t*>(p.res + off + (size_t)4 * p.H * p.W * 8));
+                  const float2 g2 = unpack_h2(rres[SX ? 0 : i][X3 ? 1 : 0]);
                   f0 += g2.x; f1 += g2.y;
                 }
               }
@@ -285,21 +334,40 @@ __global__ void __launch_bounds__(kThreads, 1) conv_igemm_kernel(const __grid_co
             }
           }
         } else if constexpr (EPI == BIN_EPI_PIXSHUF) {
-          // out[c, 2y+i, 2x+j] = conv[4c+2i+j, y, x]   (nn.PixelShuffle(2), RDN.py:206)
-          if (valid) {
-            const int H2 = 2 * p.H, W2 = 2 * p.W;
+          // out[c, 2y+i, 2x+j] = conv[4c+2i+j, y, x]   (nn.PixelShuffle(2), RDN.py:206).  Column 8 (4 q + m) + 2 k4 + e
+          // of this row is channel 2 m + k4/2 of output plane nh NT/32 + q at full-res pixel (2y + (k4 & 1), 2x + e).
+          // The warp writes the fp16 values into its staging buffer in P8 order, then each lane reads back whole
+          // 16-byte pixels (lane = row r, sub-pixel s = 2 dy + dx; its row is its own fragment row) and stores them:
+          // a warp store covers two full-res rows of 256 contiguous bytes instead of 4 bytes in each of 16 sectors.
+          const int r = lane >> 2;
 #pragma unroll
-            for (int i = 0; i < NT / 8; ++i) {
+          for (int i = 0; i < NT / 8; ++i) {
 #pragma unroll
-              for (int e = 0; e < 2; ++e) {
-                const int n = nh * NT + 8 * i + 2 * k4 + e;
-                const int c = n >> 2, yy = 2 * y + ((n >> 1) & 1), xx = 2 * x + (n & 1);
-                const int op = p.out_plane0 + (c >> 3);
-                const size_t off = ((((size_t)b * p.out_planes + (X3 ? x3_plane(op) : op)) * H2 + yy) * W2 + xx) * 8 + (c & 7);
-                store_one<X3>(p.out + off, (size_t)4 * H2 * W2 * 8, val(i, e) + sbias[n]);
-              }
+            for (int e = 0; e < 2; ++e) {
+              const int n = nh * NT + 8 * i + 2 * k4 + e;
+              const float a = val(i, e) + sbias[n];
+              const __half hi = __float2half_rn(a);
+              __half* dst = reinterpret_cast<__half*>(psbuf + ((i >> 2) * 8 + r) * kPsRowBytes + (2 * (k4 & 1) + e) * 16) +
+                            2 * (i & 3) + (k4 >> 1);
+              dst[0] = hi;
+              if constexpr (X3) dst[kPsPartBytes / 2] = __float2half_rn(a - __half2float(hi));
             }
           }
+          __syncwarp();
+          if (valid) {
+            const int H2 = 2 * p.H, W2 = 2 * p.W;
+            const int yy = 2 * y + (k4 >> 1), xx = 2 * x + (k4 & 1);
+#pragma unroll
+            for (int q = 0; q < NT / 32; ++q) {
+              const int op = p.out_plane0 + nh * (NT / 32) + q;
+              const size_t off = ((((size_t)b * p.out_planes + (X3 ? x3_plane(op) : op)) * H2 + yy) * W2 + xx) * 8;
+#pragma unroll
+              for (int part = 0; part < (X3 ? 2 : 1); ++part)
+                *reinterpret_cast<uint4*>(p.out + off + (size_t)part * 4 * H2 * W2 * 8) =
+                    *reinterpret_cast<const uint4*>(psbuf + part * kPsPartBytes + (q * 8 + r) * kPsRowBytes + k4 * 16);
+            }
+          }
+          __syncwarp();                                        // the buffer is rewritten by the next row
         } else {  // BIN_EPI_FINAL: fp32 NCHW = conv + bias + mean(frames) (RDN.py:221/279/333); channels 0..2
           if (valid && k4 < 2) {
             const int call = b / p.fr.Bc, bb = b % p.fr.Bc;
@@ -309,8 +377,10 @@ __global__ void __launch_bounds__(kThreads, 1) conv_igemm_kernel(const __grid_co
               const int c = 2 * k4 + e;
               if (c >= 3) continue;
               const size_t off = ((size_t)bb * 3 + c) * hw + (size_t)y * p.W + x;
-              float fm = __ldg(p.fr.frame[call][0] + off);
-              for (int fi = 1; fi < p.fr.nframes; ++fi) fm += __ldg(p.fr.frame[call][fi] + off);   // left to right
+              float fm = fpre[mb][h][e][0];
+#pragma unroll
+              for (int fi = 1; fi < NFR; ++fi)
+                if (fi < p.fr.nframes) fm += fpre[mb][h][e][fi];   // left to right
               p.fr.out[call][off] = (val(0, e) + sbias[c]) + fm / (float)p.fr.nframes;
             }
           }
@@ -394,7 +464,7 @@ static int launch_inst(const bin_conv_args_t& a, cudaStream_t s, bool reverse) {
   p.ntiles = nb * p.tiles_x * p.tiles_y * p.nh;
   p.relu = a.relu;
   const int nchunks = p.nch0 + p.nch1;
-  const int xbytes = C::XS_BYTES;
+  const int xbytes = C::XS_BYTES + (EPI == BIN_EPI_PIXSHUF ? 8 * kPsWarpBytes<X3> : 0);   // + the consumer warps' staging
   // keep the whole weight set resident in smem when it leaves room for >= 3 activation stages
   p.resident = (p.nh == 1 && nchunks <= kMaxResidentChunks &&
                 kCtrlBytes + nchunks * C::W_CHUNK + xbytes + 3 * C::A_BYTES + 256 <= kSmemMax) ? 1 : 0;
@@ -478,6 +548,7 @@ static int launch_conv_t(const bin_conv_args_t& a, cudaStream_t s, bool reverse)
   } else if (a.epilogue == BIN_EPI_PIXSHUF) {
     if (a.out.H != 2 * H || a.out.W != 2 * W || a.out.B != B || plane_end(a.out_plane0, a.cout_pad / 32) > a.out.planes)
       return fail(BIN_ERR_ARG, "conv: pixel-shuffle output geometry mismatch");
+    if (misaligned(a.out.ptr)) return fail(BIN_ERR_ARG, "conv: P8 tensor not 16-byte aligned");   // 16-byte pixel stores
   } else if (a.epilogue == BIN_EPI_FINAL) {
     if (a.fr.ncalls < 1 || a.fr.ncalls > BIN_MAX_CALLS || a.fr.nframes < 1 || a.fr.nframes > BIN_MAX_FRAMES ||
         a.fr.Bc < 1 || a.fr.ncalls * a.fr.Bc != B)
