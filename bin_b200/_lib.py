@@ -17,7 +17,7 @@ BIN_TRAIN_FRAMES = 17
 BIN_PNG_MAX_BATCH = 16
 EPI_P8, EPI_PIXSHUF, EPI_FINAL = 0, 1, 2
 BIN_DETERMINISTIC = 1                 # flags bit of the *_ex entry points
-ABI_VERSION = 5
+ABI_VERSION = 6
 
 
 class Act(C.Structure):
@@ -41,8 +41,9 @@ class ConvArgs(C.Structure):
                 ("fr", Frames)]
 
 
-class Net(C.Structure):
-    _fields_ = [("blob", C.c_void_p * 4), ("lstm_w", C.c_void_p * 6), ("lstm_b", C.c_void_p * 6)]
+class LstmCell(C.Structure):
+    _fields_ = [("x", C.c_void_p), ("c_prev", C.c_void_p), ("h_prev", C.c_void_p), ("w", C.c_void_p), ("b", C.c_void_p),
+                ("h_out", C.c_void_p), ("c_out", C.c_void_p)]
 
 
 class TrainSample(C.Structure):
@@ -70,7 +71,7 @@ _SIGS = {
     "bin_conv_wgrad_workspace_bytes": (C.c_size_t, []),
     "bin_conv_wgrad": (C.c_int, [Act, C.c_int, C.c_int, Act, C.c_int, C.c_int, Act, C.c_int, C.c_int, C.c_int, C.c_int,
                                 C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
-    "bin_convlstm_fwd": (C.c_int, [C.c_void_p] * 7 + [C.c_int] * 3 + [C.c_void_p]),
+    "bin_convlstm_fwd": (C.c_int, [C.POINTER(LstmCell)] + [C.c_int] * 4 + [C.c_void_p]),
     "bin_convlstm_bwd": (C.c_int, [C.c_void_p] * 13 + [C.c_int] * 3 + [C.c_void_p]),
     "bin_convlstm_bwd_scratch_bytes": (C.c_size_t, [C.c_int] * 3),
     "bin_convlstm_bwd_ex": (C.c_int, [C.c_void_p] * 13 + [C.c_int] * 4 + [C.c_void_p, C.c_size_t, C.c_void_p]),
@@ -103,18 +104,10 @@ _SIGS = {
     "bin_grad_scale": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_size_t, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]),
     "bin_rdb_fwd": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
                               C.c_void_p, C.c_size_t, C.c_void_p]),
-    "bin_window_workspace_bytes": (C.c_size_t, [C.c_int] * 3),
-    "bin_window_fwd": (C.c_int, [C.POINTER(Net), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_int, C.c_int,
-                                 C.c_int, C.c_void_p, C.c_size_t, C.c_void_p]),
     "bin_backbone_packed_bytes_p": (C.c_size_t, [C.c_int, C.c_int]),
     "bin_backbone_pack_p": (C.c_int, [C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_void_p, C.c_int, C.c_void_p]),
     "bin_backbone_workspace_bytes_p": (C.c_size_t, [C.c_int] * 5),
     "bin_backbone_fwd_p": (C.c_int, [C.c_int, C.c_void_p, C.POINTER(Frames), C.c_int, C.c_int, C.c_void_p, C.c_size_t, C.c_int, C.c_void_p]),
-    "bin_window_workspace_bytes_p": (C.c_size_t, [C.c_int] * 4),
-    "bin_window_fwd_p": (C.c_int, [C.POINTER(Net), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_int, C.c_int,
-                                   C.c_int, C.c_void_p, C.c_size_t, C.c_int, C.c_void_p]),
-    "bin_pyramid3_fwd": (C.c_int, [C.POINTER(Net), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_int, C.c_int,
-                                   C.c_int, C.c_void_p, C.c_size_t, C.c_void_p]),
     "bin_pixel_loss_fwd": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_int, C.c_size_t, C.c_int, C.c_float, C.c_void_p, C.c_void_p]),
     "bin_pixel_loss_scratch_bytes": (C.c_size_t, [C.c_int, C.c_size_t]),
     "bin_pixel_loss_fwd_ex": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_int, C.c_size_t, C.c_int, C.c_float,

@@ -15,7 +15,8 @@ import torch
 from . import _lib, ops
 from ._lib import BinB200Error, check, lib
 from .ops import _stream
-from .rdn import _LSTM_NAMES, _check_frames, _checkpointing_of, _launch_stage, _pyramid_schedule, _window_schedule
+from .rdn import (_LSTM_NAMES, _check_frames, _checkpointing_of, _launch_stage, _pyramid3_schedule, _pyramid_schedule,
+                  _window_schedule)
 
 LOSS_SCALE_TARGET = 2048.0    # max|dOut| * scale after loss scaling (fp16: 32x headroom to 65504; deep-layer gradients stay normal)
 _loss_scale_target = LOSS_SCALE_TARGET
@@ -233,19 +234,17 @@ def pyramid_apply(pyr, B1, B3, B5, B7, B9, previous_input=None):
 
 def pyramid3_apply(module, F):
     """Stages 1-3 on 4 frames with autograd (BASELINE config 2a/3a; pattern of RDN.py:383-387)."""
-    pyr = module.model
-    o0, o1, o2 = backbone_stage(pyr.model1_1, [(F[0], F[1]), (F[1], F[2]), (F[2], F[3])])
-    o3, o4 = backbone_stage(pyr.model2_1, [(o0, o0, o1), (o1, o1, o2)])
-    (o5,) = backbone_stage(pyr.model3_1, [(o3, F[1], o3, o4, F[2])])
-    return o0, o1, o2, o3, o4, o5
+    return _pyramid3_schedule(backbone_stage, module.model, F)
 
 
 def window_apply(module, F):
     """Grad-enabled RDN_residual_interp_5_input_ConvLSTM_L.forward (RDN.py:422-465): the same 17 unique
-    backbone calls / 6 live ConvLSTM calls as bin_window_fwd (SURVEY App. A), each batched stage an autograd node."""
+    backbone calls / 6 live ConvLSTM calls as the inference window (SURVEY App. A), each batched stage an autograd node
+    and each ConvLSTM cell its own."""
     F = [f.contiguous() for f in F]
     _check_frames(F)
     pyr = module.model
     cells = [getattr(module, n) for n in _LSTM_NAMES]
     s1 = backbone_stage(pyr.model1_1, [(F[0], F[1]), (F[1], F[2]), (F[2], F[3]), (F[3], F[4]), (F[4], F[5])])
-    return _window_schedule(backbone_stage, lambda k, x: convlstm_apply(cells[k], x, None)[0], pyr, F, s1)
+    lstm = lambda group: [convlstm_apply(cells[k], x, None)[0] for k, x in group]
+    return _window_schedule(backbone_stage, lstm, pyr, F, s1)

@@ -1,11 +1,10 @@
 // bin_b200 -- extern "C" entry points (include/bin_b200.h) and the host-side orchestration of
-// one backbone / one 6-frame window.  Host code only: every arithmetic step is a kernel in
-// conv_igemm.cu / aux_kernels.cu.
+// one batched backbone stage.  Host code only: every arithmetic step is a kernel in
+// conv_igemm.cu / aux_kernels.cu.  The six-frame window and the pyramids are scheduled in bin_b200/rdn.py.
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
 
-#include <initializer_list>
 #include <string>
 #include <vector>
 
@@ -69,8 +68,6 @@ int pack_batch_add_weight_t(void* hb, const float* w, int cout, int cin, int ks,
                             int cin_pad_t, void* packed);
 int pack_batch_add_bias(void* hb, const float* b, int cout, int cout_pad, float* dst);
 int pack_batch_launch(void* hb, cudaStream_t s);   // launches and frees the batch
-int launch_convlstm(const float* x, const float* c_prev, const float* h_prev, const float* w, const float* b,
-                    float* h_out, float* c_out, int B, int H, int W, cudaStream_t s);
 size_t pixel_loss_scratch_bytes(int npairs, size_t n);
 int launch_pixel_loss_fwd(const float* const* a, const float* const* b, int npairs, size_t n, int kind, float eps,
                           float* pair_loss, cudaStream_t s, int flags, void* scratch, size_t scratch_bytes);
@@ -624,33 +621,6 @@ static int run_backbone_bwd(int nframes, const void* blob_t, const bin_frames_t&
   return launch_unpack_frames_grad(gw.dx0, dout, dfr, H, W, scale, s);
 }
 
-// ------------------------------------------------------------------ window orchestration
-struct Call {
-  const float* in[BIN_MAX_FRAMES];
-  float* out;
-};
-static int run_stage(const bin_net_t* net, int which, int nframes, const std::vector<Call>& calls, int B, int H, int W,
-                     void* ws, size_t ws_bytes, cudaStream_t s, int x3 = 0) {
-  bin_frames_t fr;
-  memset(&fr, 0, sizeof(fr));
-  fr.ncalls = (int)calls.size(); fr.nframes = nframes; fr.Bc = B;
-  for (int k = 0; k < fr.ncalls; ++k) {
-    for (int f = 0; f < nframes; ++f) fr.frame[k][f] = calls[k].in[f];
-    fr.out[k] = calls[k].out;
-  }
-  return run_backbone(nframes, net->blob[which], fr, H, W, ws, ws_bytes, s, false, x3);
-}
-
-static size_t window_ws_bytes(int B, int H, int W, int max_calls, int ntemp, int x3 = 0) {
-  size_t bb = 0;
-  const int nf[3] = {2, 3, 5};
-  for (int i = 0; i < 3; ++i) {
-    size_t v = backbone_ws(nf[i], max_calls * B, H, W, nullptr, false, x3).bytes;
-    bb = v > bb ? v : bb;
-  }
-  return bb + (size_t)ntemp * align_up((size_t)B * 3 * H * W * sizeof(float), 256);
-}
-
 }  // namespace binb
 
 using namespace binb;
@@ -713,9 +683,17 @@ int bin_conv_fwd(const bin_conv_args_t* a, bin_stream_t s) {
   if (!a) return fail(BIN_ERR_ARG, "conv: null args");
   return launch_conv(*a, (cudaStream_t)s);
 }
-int bin_convlstm_fwd(const float* x, const float* c_prev, const float* h_prev, const float* w, const float* b,
-                     float* h_out, float* c_out, int B, int H, int W, bin_stream_t s) {
-  return launch_convlstm(x, c_prev, h_prev, w, b, h_out, c_out, B, H, W, (cudaStream_t)s);
+int bin_convlstm_fwd(const bin_lstm_cell_t* cells_host, int ncells, int B, int H, int W, bin_stream_t s) {
+  if (!cells_host) return fail(BIN_ERR_ARG, "convlstm: null cell table");
+  if (ncells < 1 || ncells > 3) return fail(BIN_ERR_ARG, "convlstm: 1..3 cells per launch");
+  LstmCells c;
+  memset(&c, 0, sizeof(c));
+  for (int i = 0; i < ncells; ++i) {
+    const bin_lstm_cell_t& e = cells_host[i];
+    c.x[i] = e.x; c.c_prev[i] = e.c_prev; c.h_prev[i] = e.h_prev; c.w[i] = e.w; c.b[i] = e.b;
+    c.h_out[i] = e.h_out; c.c_out[i] = e.c_out;
+  }
+  return launch_convlstm_multi(c, ncells, B, H, W, (cudaStream_t)s);
 }
 
 size_t bin_pixel_loss_scratch_bytes(int npairs, size_t n) { return pixel_loss_scratch_bytes(npairs, n); }
@@ -897,103 +875,7 @@ int bin_rdb_fwd(const void* blob, int nframes, int index, const float* x, float*
   return launch_p8_to_nchw(out, 0, kG0, y, (cudaStream_t)s);
 }
 
-// The window's dataflow (SURVEY App. A), one row per backbone call in issue order.  A node is an output o[0..13], one of
-// the 9 workspace images (the ConvLSTM images p*, then the step-1 intermediates t*; tmp[node - 14]) or an input frame.
-enum { P4 = 14, P6, P8, P5, P7, P6B, T0, T1, T2, WIN_NODES, FR = 32 };
-struct WinCall { int dst, in[BIN_MAX_FRAMES]; };
-static const WinCall kWinCalls[17] = {
-    // Stage 1 (RDN.py:371-374): 4 calls of step 0 + the one stage-1 call of step 1 that is not a repeat.
-    {0, {FR + 0, FR + 1}}, {1, {FR + 1, FR + 2}}, {2, {FR + 2, FR + 3}}, {3, {FR + 3, FR + 4}},
-    {10, {FR + 4, FR + 5}},
-    // Stage 2: step 0 (RDN.py:384-386, "prev" slot duplicated) + step 1 (RDN.py:377-379) in ONE launch of 6 calls:
-    // the step-1 calls only need stage-1 outputs and their ConvLSTM images, not step-0's stage 2.
-    {4, {0, 0, 1}}, {5, {1, 1, 2}}, {6, {2, 2, 3}}, {T0, {P4, 1, 2}}, {T1, {P6, 2, 3}}, {11, {P8, 3, 10}},
-    // Stage 3: step 0 (RDN.py:387-388) + step 1 (RDN.py:380-381)
-    {7, {4, FR + 1, 4, 5, FR + 2}}, {8, {5, FR + 2, 5, 6, FR + 3}}, {T2, {P5, FR + 2, T0, T1, FR + 3}},
-    {12, {P7, FR + 3, T1, 11, FR + 4}},
-    // Stage 4: step 0 (RDN.py:389) + step 1 (RDN.py:382)
-    {9, {1, 1, 7, 8, 2}}, {13, {P6B, 2, T2, 12, 3}}};
-static const int kStageFrames[4] = {2, 3, 5, 5};
-static const int kStageRow0[5] = {0, 5, 11, 15, 17};            // rows of stage k: kStageRow0[k] .. kStageRow0[k + 1] - 1
-// ConvLSTM cell k writes image P4 + k from output kCellSrc[k]; the cells of one recurrent hand-off (RDN.py:451-453,
-// 454-455, 456) run before stage kCellStage[k] and are independent: one launch for all of them (grid.z = cell).
-static const int kCellSrc[6] = {1, 2, 3, 5, 6, 8};
-static const int kCellStage[6] = {1, 1, 1, 2, 2, 3};
-
-static int window_fwd_impl(const bin_net_t* net, const float* const* F, float* const* o, int B, int H, int W, void* workspace,
-                           size_t workspace_bytes, bin_stream_t s_, int x3) {
-  if (!net || !F || !o) return fail(BIN_ERR_ARG, "window_fwd: null argument");
-  cudaStream_t s = (cudaStream_t)s_;
-  const size_t need = window_ws_bytes(B, H, W, BIN_MAX_CALLS, 9, x3);
-  if (workspace_bytes < need) return fail(BIN_ERR_WORKSPACE, "window_fwd: workspace too small");
-  const size_t fbytes = align_up((size_t)B * 3 * H * W * sizeof(float), 256);
-  uint8_t* base = (uint8_t*)workspace;
-  float* node[WIN_NODES];
-  for (int i = 0; i < 14; ++i) node[i] = o[i];
-  for (int i = 14; i < WIN_NODES; ++i) node[i] = (float*)(base + (i - 14) * fbytes);
-  void* bws = base + 9 * fbytes;
-  const size_t bws_bytes = workspace_bytes - 9 * fbytes;
-  // A NULL o[i] means "do not compute output i".  for_out[n] >= 0 when node n is computed: n itself for a non-NULL
-  // output, and for a workspace image the output its first reader serves (the stages are walked last to first, so a
-  // node's readers are seen before its writer).  The caller passes a closed set: no computed node reads a NULL output.
-  int for_out[WIN_NODES], nout = 0;
-  for (int i = 0; i < WIN_NODES; ++i) for_out[i] = (i < 14 && o[i]) ? i : -1;
-  for (int i = 0; i < 14; ++i) nout += o[i] != nullptr;
-  if (!nout) return fail(BIN_ERR_ARG, "window_fwd: every output pointer is NULL");
-  auto reads = [&](int src, int reader) -> int {
-    if (src >= FR) return BIN_OK;
-    if (src < 14 && !o[src])
-      return fail(BIN_ERR_ARG, "window_fwd: output " + std::to_string(for_out[reader]) + " depends on output " +
-                                   std::to_string(src) + ", whose pointer is NULL");
-    if (for_out[src] < 0) for_out[src] = for_out[reader];
-    return BIN_OK;
-  };
-  for (int stage = 3; stage >= 0; --stage) {
-    for (int c = kStageRow0[stage]; c < kStageRow0[stage + 1]; ++c) {
-      const WinCall& wc = kWinCalls[c];
-      if (for_out[wc.dst] < 0) continue;
-      for (int f = 0; f < kStageFrames[stage]; ++f) BIN_TRY(reads(wc.in[f], wc.dst));
-    }
-    for (int k = 0; k < 6; ++k)
-      if (kCellStage[k] == stage && for_out[P4 + k] >= 0) BIN_TRY(reads(kCellSrc[k], P4 + k));
-  }
-  for (int stage = 0; stage < 4; ++stage) {
-    LstmCells cells;
-    memset(&cells, 0, sizeof(cells));
-    int ncells = 0;
-    for (int k = 0; k < 6; ++k) {
-      if (kCellStage[k] != stage || for_out[P4 + k] < 0) continue;
-      cells.x[ncells] = node[kCellSrc[k]]; cells.h_out[ncells] = node[P4 + k];
-      cells.w[ncells] = net->lstm_w[k]; cells.b[ncells] = net->lstm_b[k];
-      ++ncells;
-    }
-    if (ncells) BIN_TRY(launch_convlstm_multi(cells, ncells, B, H, W, s));
-    std::vector<Call> calls;
-    for (int c = kStageRow0[stage]; c < kStageRow0[stage + 1]; ++c) {
-      const WinCall& wc = kWinCalls[c];
-      if (for_out[wc.dst] < 0) continue;
-      Call call;
-      memset(&call, 0, sizeof(call));
-      for (int f = 0; f < kStageFrames[stage]; ++f) call.in[f] = wc.in[f] >= FR ? F[wc.in[f] - FR] : node[wc.in[f]];
-      call.out = node[wc.dst];
-      calls.push_back(call);
-    }
-    if (!calls.empty()) BIN_TRY(run_stage(net, stage, kStageFrames[stage], calls, B, H, W, bws, bws_bytes, s, x3));
-  }
-  return BIN_OK;
-}
-
-size_t bin_window_workspace_bytes(int B, int H, int W) { return window_ws_bytes(B, H, W, BIN_MAX_CALLS, 9); }
-int bin_window_fwd(const bin_net_t* net, const float* const* F, float* const* o, int B, int H, int W, void* workspace,
-                   size_t workspace_bytes, bin_stream_t s) {
-  return window_fwd_impl(net, F, o, B, H, W, workspace, workspace_bytes, s, 0);
-}
 /* precision-parameterised twins (BIN_PREC_*) */
-size_t bin_window_workspace_bytes_p(int B, int H, int W, int prec) { return window_ws_bytes(B, H, W, BIN_MAX_CALLS, 9, prec ? 1 : 0); }
-int bin_window_fwd_p(const bin_net_t* net, const float* const* F, float* const* o, int B, int H, int W, void* workspace,
-                     size_t workspace_bytes, int prec, bin_stream_t s) {
-  return window_fwd_impl(net, F, o, B, H, W, workspace, workspace_bytes, s, prec ? 1 : 0);
-}
 size_t bin_backbone_packed_bytes_p(int nframes, int prec) { return valid_nframes(nframes) ? backbone_layout(nframes, prec ? 1 : 0).bytes : 0; }
 int bin_backbone_pack_p(int nframes, const float* const* w_host, const float* const* b_host, void* blob, int prec,
                         bin_stream_t s) {
@@ -1007,18 +889,6 @@ int bin_backbone_fwd_p(int nframes, const void* blob, const bin_frames_t* fr, in
                        size_t workspace_bytes, int prec, bin_stream_t s) {
   if (!fr || !blob) return fail(BIN_ERR_ARG, "backbone_fwd: null argument");
   return run_backbone(nframes, blob, *fr, H, W, workspace, workspace_bytes, (cudaStream_t)s, false, prec ? 1 : 0);
-}
-
-int bin_pyramid3_fwd(const bin_net_t* net, const float* const* F, float* const* o, int B, int H, int W,
-                     void* workspace, size_t workspace_bytes, bin_stream_t s_) {
-  if (!net || !F || !o) return fail(BIN_ERR_ARG, "pyramid3_fwd: null argument");
-  cudaStream_t s = (cudaStream_t)s_;
-  if (workspace_bytes < window_ws_bytes(B, H, W, BIN_MAX_CALLS, 9)) return fail(BIN_ERR_WORKSPACE, "pyramid3_fwd: workspace too small");
-  BIN_TRY(run_stage(net, 0, 2, {{{F[0], F[1]}, o[0]}, {{F[1], F[2]}, o[1]}, {{F[2], F[3]}, o[2]}}, B, H, W, workspace,
-                    workspace_bytes, s));
-  BIN_TRY(run_stage(net, 1, 3, {{{o[0], o[0], o[1]}, o[3]}, {{o[1], o[1], o[2]}, o[4]}}, B, H, W, workspace,
-                    workspace_bytes, s));
-  return run_stage(net, 2, 5, {{{o[3], F[1], o[3], o[4], F[2]}, o[5]}}, B, H, W, workspace, workspace_bytes, s);
 }
 
 int bin_rdb_tail_fwd(const bin_act_t* x, int x_plane0, const bin_act_t* g, int g_plane0, const void* w_conv,

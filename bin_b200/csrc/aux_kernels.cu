@@ -1215,13 +1215,6 @@ int launch_convlstm_multi(const LstmCells& cells, int ncells, int B, int H, int 
   BIN_CUDA_OK(cudaGetLastError());
   return BIN_OK;
 }
-int launch_convlstm(const float* x, const float* c_prev, const float* h_prev, const float* w, const float* b,
-                    float* h_out, float* c_out, int B, int H, int W, cudaStream_t s) {
-  LstmCells c;
-  memset(&c, 0, sizeof(c));
-  c.x[0] = x; c.c_prev[0] = c_prev; c.h_prev[0] = h_prev; c.w[0] = w; c.b[0] = b; c.h_out[0] = h_out; c.c_out[0] = c_out;
-  return launch_convlstm_multi(c, 1, B, H, W, s);
-}
 int launch_p8_add(const bin_act_t& dst, int dplane0, const bin_act_t& src, int splane0, int nplanes, cudaStream_t s) {
   const int hw = dst.H * dst.W;
   const dim3 grid((unsigned)((hw + 511) / 512), (unsigned)nplanes, (unsigned)dst.B);

@@ -232,6 +232,22 @@ def convlstm_fwd(x, w, b, state=None):
     cp = hp = None
     if state is not None:
         cp, hp = (_req(t, torch.float32, "state") for t in state)
-    check(lib().bin_convlstm_fwd(x.data_ptr(), _ptr(cp), _ptr(hp), _req(w, torch.float32, "w").data_ptr(),
-                                 _req(b, torch.float32, "b").data_ptr(), h.data_ptr(), c.data_ptr(), B, H, W, _stream()))
+    w, b = _req(w, torch.float32, "w"), _req(b, torch.float32, "b")
+    cell = _lib.LstmCell(x.data_ptr(), _ptr(cp), _ptr(hp), w.data_ptr(), b.data_ptr(), h.data_ptr(), c.data_ptr())
+    check(lib().bin_convlstm_fwd(C.byref(cell), 1, B, H, W, _stream()))
     return h, c
+
+
+def convlstm_group(cells: Sequence[Tuple[torch.Tensor, torch.Tensor, torch.Tensor]]) -> List[torch.Tensor]:
+    """1..3 ConvLSTM cells [(x, w, b), ...] from no state (RDN.py:57-68), one (B,3,H,W) shape, in one launch -> their h;
+    c is not written.  The cells of one recurrent hand-off of the window (RDN.py:451-456) run this way."""
+    xs = [_req(x, torch.float32, "x") for x, _, _ in cells]
+    ws = [(_req(w, torch.float32, "w"), _req(b, torch.float32, "b")) for _, w, b in cells]
+    if any(x.shape != xs[0].shape for x in xs):
+        raise _lib.BinB200Error("convlstm_group: the cells of one launch must share their (B,3,H,W) shape")
+    hs = [torch.empty_like(x) for x in xs]
+    tab = (_lib.LstmCell * len(xs))(*[_lib.LstmCell(x.data_ptr(), None, None, w.data_ptr(), b.data_ptr(), h.data_ptr(), None)
+                                      for x, (w, b), h in zip(xs, ws, hs)])
+    B, _, H, W = xs[0].shape
+    check(lib().bin_convlstm_fwd(tab, len(xs), B, H, W, _stream()))
+    return hs

@@ -20,7 +20,7 @@ import torch.nn as nn
 import torch.nn.init as weight_init
 
 from . import _lib, ops
-from ._lib import BinB200Error, Net, check, lib
+from ._lib import BinB200Error, check, lib
 
 __all__ = ["set_precision", "set_self_ensemble", "set_activation_checkpointing", "set_outputs", "ConvLSTMCell", "pixel_reshuffle", "RDB_Conv", "RDB",
            "RDN_residual_interp_2_input",
@@ -360,6 +360,15 @@ def _pyramid_schedule(stage, pyr, B1, B3, B5, B7, B9, previous_input):
     return I2, I4, I6, I8, I3, I5, I7, I4b, I6b, I5c
 
 
+def _pyramid3_schedule(stage, pyr, F):
+    """BASELINE config 2a: stages 1-3 of the pyramid on the 4 frames F (pattern of RDN.py:383-387) as 3 batched stages
+    -> [I2', I4', I6', I3', I5', I4''] (SURVEY 8d); stage(model, calls) runs one and returns its outputs."""
+    o0, o1, o2 = stage(pyr.model1_1, [(F[0], F[1]), (F[1], F[2]), (F[2], F[3])])
+    o3, o4 = stage(pyr.model2_1, [(o0, o0, o1), (o1, o1, o2)])
+    (o5,) = stage(pyr.model3_1, [(o3, F[1], o3, o4, F[2])])
+    return o0, o1, o2, o3, o4, o5
+
+
 def _launch_stage(model: _Backbone, calls, outs, prec: int) -> torch.Tensor:
     """One batched backbone stage (same-weight calls riding along the batch) in precision `prec`, on the current device,
     into the shared per-(device, stream) workspace, which it returns: a recomputing backward reads what it left there."""
@@ -371,13 +380,13 @@ def _launch_stage(model: _Backbone, calls, outs, prec: int) -> torch.Tensor:
     return ws
 
 
-def _batched(model: _Backbone, calls):
-    """Inference of one batched stage in the net's precision (set_precision)."""
+def _batched(model: _Backbone, calls, prec: Optional[int] = None):
+    """Inference of one batched stage in precision `prec`, by default the net's (set_precision)."""
     calls = [[t.contiguous() for t in c] for c in calls]
     _check_frames([t for c in calls for t in c])
     with torch.cuda.device(calls[0][0].device):
         outs = [torch.empty_like(calls[0][0]) for _ in calls]
-        _launch_stage(model, calls, outs, _prec_of(model))
+        _launch_stage(model, calls, outs, _prec_of(model) if prec is None else prec)
     return outs
 
 
@@ -390,11 +399,12 @@ _LSTM_NAMES = ["clstm_4_prime", "clstm_6_prime", "clstm_8_prime", "clstm_5_prime
 
 def _window_schedule(stage, lstm, pyr, F, s1, live=None):
     """Stages 2-4 of the six-frame window (RDN.py:422-465) -> the 14-tuple: the unique backbone calls of both
-    recurrent steps and the 6 live ConvLSTM calls, in the order bin_window_fwd issues them (SURVEY App. A).
-    stage(model, calls) runs one batched backbone stage and returns its outputs, lstm(k, x) returns h of ConvLSTM cell k
-    (the order of _LSTM_NAMES) from no state, and s1 holds the stage-1 outputs o[0..3], o[10] of the frame pairs.
-    With `live` (a node set from _window_live) only the calls and cells in it run, each stage with its shortened call
-    list, and every other result, s1 entries included, is None."""
+    recurrent steps and the 6 live ConvLSTM calls, in issue order (SURVEY App. A).  stage(model, calls) runs one
+    batched backbone stage and returns its outputs; lstm(group) runs the cells of one recurrent hand-off, a list of
+    (k, x) for ConvLSTM cell k (the order of _LSTM_NAMES) on input x from no state, and returns their h in that order;
+    s1 holds the stage-1 outputs o[0..3], o[10] of the frame pairs.  With `live` (a node set from _window_live) only
+    the calls and cells in it run, each stage with its shortened call list and each hand-off with its live cells (none
+    left: lstm is not called), and every other result, s1 entries included, is None."""
     m2, m3, m4 = pyr.model2_1, pyr.model3_1, pyr.model4_1
 
     def run(n, model, calls):
@@ -405,18 +415,22 @@ def _window_schedule(stage, lstm, pyr, F, s1, live=None):
                 outs[i] = out
         return outs
 
-    def cell(k, x):
-        return lstm(k, x) if live is None or ("lstm", k) in live else None
+    def cells(*group):
+        todo = [(k, x) for k, x in group if live is None or ("lstm", k) in live]
+        hs = dict(zip([k for k, _ in todo], lstm(todo) if todo else []))
+        return [hs.get(k) for k, _ in group]
 
     o = [None] * 14
     o[0], o[1], o[2], o[3], o[10] = s1
-    p4, p6, p8 = cell(0, o[1]), cell(1, o[2]), cell(2, o[3])
+    p4, p6, p8 = cells((0, o[1]), (1, o[2]), (2, o[3]))
     o[4], o[5], o[6], t0, t1, o[11] = run(2, m2, [(o[0], o[0], o[1]), (o[1], o[1], o[2]), (o[2], o[2], o[3]),
                                                   (p4, o[1], o[2]), (p6, o[2], o[3]), (p8, o[3], o[10])])
-    p5, p7 = cell(3, o[5]), cell(4, o[6])
+    del p4, p6, p8                      # no later call reads them: in inference their memory serves the next images
+    p5, p7 = cells((3, o[5]), (4, o[6]))
     o[7], o[8], t2, o[12] = run(3, m3, [(o[4], F[1], o[4], o[5], F[2]), (o[5], F[2], o[5], o[6], F[3]),
                                         (p5, F[2], t0, t1, F[3]), (p7, F[3], t1, o[11], F[4])])
-    p6b = cell(5, o[8])
+    del p5, p7, t0, t1
+    (p6b,) = cells((5, o[8]))
     o[9], o[13] = run(4, m4, [(o[1], o[1], o[7], o[8], o[2]), (p6b, o[2], t2, o[12], o[3])])
     return tuple(o)
 
@@ -433,9 +447,10 @@ def _record_window():
             reads[(n, i)] = {x for x in call if x is not None}
         return [(n, i) for i in range(len(calls))]
 
-    def lstm(k, x):
-        reads[("lstm", k)] = {x}
-        return ("lstm", k)
+    def lstm(group):
+        for k, x in group:
+            reads[("lstm", k)] = {x}
+        return [("lstm", k) for k, _ in group]
 
     outs = _window_schedule(stage, lstm, SimpleNamespace(model2_1=2, model3_1=3, model4_1=4), [None] * 6, list(reads))
     return outs, reads
@@ -454,6 +469,31 @@ def _window_live(wanted) -> frozenset:
             live.add(n)
             todo += _NODE_READS[n]
     return frozenset(live)
+
+
+def _window_fwd(net, F, live, s1=None) -> tuple:
+    """Inference of the window's nodes `live` (a set from _window_live) on the six contiguous frames F -> the 14 outputs,
+    None where not computed.  s1: the stage-1 outputs a caller already holds (StreamingBIN's cache), None where it has
+    none; the live stage-1 pairs without one run as one batched stage.  Stages 2-4 follow _window_schedule, every stage
+    in the net's precision, and the live cells of each recurrent hand-off run as one ConvLSTM launch."""
+    pyr = net.model
+    s1 = [None] * 5 if s1 is None else list(s1)
+    need = [a for a in range(5) if (1, a) in live and s1[a] is None]
+    B, _, H, W = F[0].shape
+    prec = _prec_of(net)
+    with torch.cuda.device(F[0].device):
+        # the shared workspace grows once, to the largest stage, before the first stage runs (also inside a graph capture)
+        ncalls = [(pyr.model1_1, len(need))] + [(m, sum(1 for n in live if n[0] == st))
+                                                 for st, m in ((2, pyr.model2_1), (3, pyr.model3_1), (4, pyr.model4_1))]
+        _workspace(F[0].device, max([lib().bin_backbone_workspace_bytes_p(m.NFRAMES, B * k, H, W, prec)
+                                     for m, k in ncalls if k], default=0))
+        stage = lambda model, calls: _batched(model, calls, prec)
+        if need:
+            for a, out in zip(need, stage(pyr.model1_1, [(F[a], F[a + 1]) for a in need])):
+                s1[a] = out
+        gates = [getattr(net, n).Gates for n in _LSTM_NAMES]
+        lstm = lambda group: ops.convlstm_group([(x, gates[k].weight.detach(), gates[k].bias.detach()) for k, x in group])
+        return _window_schedule(stage, lstm, pyr, F, s1, live)
 
 
 class RDN_residual_interp_5_input_ConvLSTM_L(nn.Module):
@@ -479,17 +519,6 @@ class RDN_residual_interp_5_input_ConvLSTM_L(nn.Module):
             ts += [g.weight, g.bias]
         return ts
 
-    def _net(self, prec: int = 0) -> Net:
-        net = Net()
-        pyr = self.model
-        for k, m in enumerate((pyr.model1_1, pyr.model2_1, pyr.model3_1, pyr.model4_1)):
-            net.blob[k] = m.packed_blob(prec).data_ptr()
-        for k, n in enumerate(_LSTM_NAMES):
-            cell = getattr(self, n)
-            net.lstm_w[k] = cell.Gates.weight.data_ptr()
-            net.lstm_b[k] = cell.Gates.bias.data_ptr()
-        return net
-
     def forward(self, B1, B3, B5, B7, B9, B11):
         """One 6-frame window -> the reference's 14-tuple (RDN.py:461-465): executes 17 unique
         backbone calls of its 20 and the 6 live ConvLSTM calls of its 12 (SURVEY.md App. A), or, with set_outputs,
@@ -507,47 +536,34 @@ class RDN_residual_interp_5_input_ConvLSTM_L(nn.Module):
             from .autograd import window_apply
             return window_apply(self, frames)
         frames = [f.contiguous() for f in frames]
-        B, H, W = _check_frames(frames)
-        dev = frames[0].device
+        _check_frames(frames)
         wanted = range(14) if sel is None else sel[0]
-        live = range(14) if sel is None else _live_outputs(wanted)
+        live = _window_live(wanted)
         if ensemble is not None:
-            outs = self._forward_flipx4(frames, B, H, W, dev, live, wanted)
+            outs = self._forward_flipx4(frames, live, wanted)
         elif _graphs_enabled() and not getattr(self, "_is_replica", False) and not torch.cuda.is_current_stream_capturing():
-            outs = self._forward_graphed(frames, B, H, W, dev, live, wanted)
+            outs = self._forward_graphed(frames, live, wanted)
         else:
-            with torch.cuda.device(dev):
-                outs = self._launch_window(frames, B, H, W, dev, live)[0]
+            outs = _window_fwd(self, frames, live)
         return tuple(outs) if sel is None else _selected(outs, sel)
 
-    def _launch_window(self, frames, B, H, W, dev, live=range(14)):
-        """One bin_window_fwd_p call computing the outputs `live` (a set closed under the window's dataflow); the other
-        positions of the returned list are None and reach the library as NULL pointers."""
-        outs = [torch.empty_like(frames[0]) if i in live else None for i in range(14)]
-        prec = _prec_of(self)
-        net = self._net(prec)
-        ws = _workspace(dev, lib().bin_window_workspace_bytes_p(B, H, W, prec))
-        fp = (C.c_void_p * 6)(*[f.data_ptr() for f in frames])
-        op = (C.c_void_p * 14)(*[None if o is None else o.data_ptr() for o in outs])
-        check(lib().bin_window_fwd_p(C.byref(net), fp, op, B, H, W, ws.data_ptr(), ws.numel(), prec, ops._stream()))
-        return outs, ws
-
-    def _forward_flipx4(self, frames, B, H, W, dev, live, wanted):
+    def _forward_flipx4(self, frames, live, wanted):
         """x4 flip self-ensemble (utils/test_util.py:110-132 flipx4_forward, applied to all 6 frames and the wanted
         outputs): the four orientations run as ONE window at batch 4B, then each output is flipped back and averaged.
         Eager, not graphed: a graph capture would hold a second batch-4B workspace (about 25 GB at 768x1344) in its
         private pool."""
-        with torch.cuda.device(dev):
+        with torch.cuda.device(frames[0].device):
             big = ops.flipx4_expand(frames)
-            outs, _ = self._launch_window(big, 4 * B, H, W, dev, live)
+            outs = _window_fwd(self, big, live)
             del big
             return _flipx4_mean_at(outs, wanted)
 
-    def _forward_graphed(self, frames, B, H, W, dev, live, wanted):
-        """The ~340 kernel launches of a window are captured once per (shape, weight version, live outputs) into a
+    def _forward_graphed(self, frames, live, wanted):
+        """The ~340 kernel launches of a window are captured once per (shape, weight version, live nodes) into a
         CUDA graph and replayed: removes ~10 % of host launch overhead at 720p.  Inputs are copied
         into the graph's static buffers, the wanted outputs are returned as fresh tensors (SURVEY 8b)."""
-        key = (dev.index, B, H, W, _prec_of(self), tuple(live),
+        dev = frames[0].device
+        key = (dev.index, tuple(frames[0].shape), _prec_of(self), live,
                tuple((p.data_ptr(), p._version) for p in self._all_tensors()))
         ent = self.__dict__.get("_graph_entry")
         with torch.cuda.device(dev):
@@ -559,13 +575,13 @@ class RDN_residual_interp_5_input_ConvLSTM_L(nn.Module):
                 side = torch.cuda.Stream()
                 side.wait_stream(torch.cuda.current_stream())
                 with torch.cuda.stream(side):                       # warm-up: packs weights, opts kernels into their smem
-                    self._launch_window(static_in, B, H, W, dev, live)
+                    _window_fwd(self, static_in, live)
                     _WS.pop(_ws_key(dev), None)                     # the side stream's scratch buffer is not needed again
                 torch.cuda.current_stream().wait_stream(side)
                 graph = torch.cuda.CUDAGraph()
                 with torch.cuda.graph(graph):
-                    static_out, ws = self._launch_window(static_in, B, H, W, dev, live)
-                    _WS.pop(_ws_key(dev), None)                     # owned by this entry (graph-private memory pool)
+                    static_out = _window_fwd(self, static_in, live)
+                    ws = _WS.pop(_ws_key(dev), None)                # owned by this entry (graph-private memory pool)
                 ent = {"key": key, "graph": graph, "in": static_in, "out": static_out, "ws": ws}
                 self.__dict__["_graph_entry"] = ent
             else:
@@ -582,17 +598,8 @@ class RDN_residual_interp_5_input_ConvLSTM_L(nn.Module):
         if _needs_grad([B1, B3, B5, B7] + [p for m in (pyr.model1_1, pyr.model2_1, pyr.model3_1) for p in m._conv_params()]):
             from .autograd import pyramid3_apply                      # BASELINE config 3a (training on the 4-frame graph)
             return pyramid3_apply(self, (B1, B3, B5, B7))
-        frames = [f.contiguous() for f in (B1, B3, B5, B7)]
-        B, H, W = _check_frames(frames)
-        dev = frames[0].device
-        with torch.cuda.device(dev):
-            outs = [torch.empty_like(frames[0]) for _ in range(6)]
-            net = self._net()
-            ws = _workspace(dev, lib().bin_window_workspace_bytes(B, H, W))
-            fp = (C.c_void_p * 4)(*[f.data_ptr() for f in frames])
-            op = (C.c_void_p * 6)(*[o.data_ptr() for o in outs])
-            check(lib().bin_pyramid3_fwd(C.byref(net), fp, op, B, H, W, ws.data_ptr(), ws.numel(), ops._stream()))
-        return tuple(outs)
+        # every stage in fp16, whatever set_precision says
+        return _pyramid3_schedule(lambda m, calls: _batched(m, calls, prec=0), pyr, (B1, B3, B5, B7))
 
 
 def bin_stage4_lstm():
@@ -637,12 +644,6 @@ def _outputs_of(module) -> Optional[Tuple[Tuple[int, ...], str]]:
     if not ok:
         raise BinB200Error(f"unknown output selection {sel!r}; set it with set_outputs(net, indices, unwanted)")
     return sel
-
-
-def _live_outputs(wanted) -> Tuple[int, ...]:
-    """The outputs a window must compute for `wanted`: the wanted ones and those they are computed from."""
-    live = _window_live(wanted)
-    return tuple(i for i in range(14) if _OUT_NODE[i] in live)
 
 
 def _flipx4_mean_at(outs, wanted) -> list:

@@ -17,8 +17,7 @@ import torch
 
 from . import ops
 from ._lib import BinB200Error, check, lib
-from .rdn import (_LSTM_NAMES, _batched, _ensemble_of, _flipx4_mean_at, _outputs_of, _selected, _window_live,
-                  _window_schedule)
+from .rdn import _OUT_NODE, _ensemble_of, _flipx4_mean_at, _outputs_of, _selected, _window_fwd, _window_live
 
 
 def test_py_padding(h: int, w: int) -> Tuple[int, int, int, int]:
@@ -120,17 +119,15 @@ class StreamingBIN:
         sel = self.key[1]
         wanted = range(14) if sel is None else sel[0]
         live = _window_live(wanted)
-        # ---- stage 1: only the live frame pairs not seen before (1 per window in steady state, 5 for the first)
-        need = [(a, a + 1) for a in range(5) if (1, a) in live and (ids[a], ids[a + 1]) not in self.s1]
-        if need:
-            outs = _batched(net.model.model1_1, [(F[a], F[b]) for a, b in need])
-            for (a, b), o in zip(need, outs):
-                self.s1[(ids[a], ids[b])] = o
-        s1 = [self.s1.get((ids[k], ids[k + 1])) for k in range(5)]
-        cells = [getattr(net, n) for n in _LSTM_NAMES]
-        lstm = lambda k, x: ops.convlstm_fwd(x, cells[k].Gates.weight.detach(), cells[k].Gates.bias.detach(), None)[0]
-        o = _window_schedule(_batched, lstm, net.model, F, s1, live)
-        self.backbone_calls += len(need) + sum(1 for n in live if n[0] in (2, 3, 4))
+        # stage 1 runs only the live frame pairs not seen before (1 per window in steady state, 5 for the first)
+        pairs = [(ids[a], ids[a + 1]) for a in range(5)]
+        s1 = [self.s1.get(p) for p in pairs]
+        fresh = sum(1 for a in range(5) if (1, a) in live and s1[a] is None)
+        o = _window_fwd(net, F, live, s1)
+        self.backbone_calls += fresh + sum(1 for n in live if n[0] in (2, 3, 4))
+        for i, n in enumerate(_OUT_NODE):
+            if n[0] == 1 and o[i] is not None:
+                self.s1[pairs[n[1]]] = o[i]
         if self.key[0] is not None:
             o = tuple(_flipx4_mean_at(o, wanted))
         return o if sel is None else _selected(o, sel)

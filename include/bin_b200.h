@@ -33,7 +33,7 @@
 extern "C" {
 #endif
 
-#define BIN_ABI_VERSION 5
+#define BIN_ABI_VERSION 6
 #define BIN_MAX_CALLS 6   /* same-weight backbone calls batched along N */
 #define BIN_MAX_FRAMES 5  /* frames per backbone call (2, 3 or 5) */
 #define BIN_MAX_LOSS_PAIRS 20 /* (prediction, target) pairs of one fused loss call */
@@ -163,10 +163,17 @@ int bin_conv_wgrad(bin_act_t x0, int x0_plane0, int x0_planes, bin_act_t x1, int
                    bin_stream_t s);
 
 /* ---- ConvLSTMCell.forward, RDN.py:50-95 ------------------------------------------------ */
-/* x,(c_prev,h_prev): (B,3,H,W) fp32; c_prev/h_prev NULL = zeros (RDN.py:57-68);
- * w: (12,6,3,3), b: (12); writes h_out and (optionally) c_out. */
-int bin_convlstm_fwd(const float* x, const float* c_prev, const float* h_prev, const float* w, const float* b,
-                     float* h_out, float* c_out, int B, int H, int W, bin_stream_t s);
+/* One cell: x,(c_prev,h_prev): (B,3,H,W) fp32; c_prev/h_prev NULL = zeros (RDN.py:57-68);
+ * w: (12,6,3,3), b: (12); writes h_out and (optionally, c_out NULL = not written) c_out. */
+typedef struct {
+  const float *x, *c_prev, *h_prev, *w, *b;
+  float *h_out, *c_out;
+} bin_lstm_cell_t;
+/* ncells (1..3) independent cells of one (B,3,H,W) shape in one launch (the cells of one recurrent hand-off of the
+ * window, RDN.py:451-456); each cell's results have the bits of its own one-cell launch.  cells_host: host array.
+ * A NULL table or x / w / b / h_out, a count outside 1..3, half a state, or cells that do not all have (or all lack) a
+ * state fail with BIN_ERR_ARG before the launch. */
+int bin_convlstm_fwd(const bin_lstm_cell_t* cells_host, int ncells, int B, int H, int W, bin_stream_t s);
 
 /* Backward of the cell: dh/dc = gradients of the two outputs (either may be NULL = zero); dgates_ws = scratch
  * (B,12,H,W) fp32; writes dx (and dc_prev/dh_prev when a state was given), ACCUMULATES into dw (12,6,3,3) and db (12).
@@ -254,25 +261,7 @@ int bin_grad_scale(const float* const* gouts_host, int n, size_t numel, float ta
 int bin_rdb_fwd(const void* blob, int nframes, int index, const float* x, float* y, int B, int h, int w,
                 void* workspace, size_t workspace_bytes, bin_stream_t s);
 
-/* ---- whole 6-frame window (RDN_residual_interp_5_input_ConvLSTM_L.forward, RDN.py:422-465) */
-typedef struct {
-  const void* blob[4];      /* packed model1_1, model2_1, model3_1, model4_1 */
-  const float* lstm_w[6];   /* clstm_{4',6',8',5'',7'',6'''}.Gates.weight (12,6,3,3) */
-  const float* lstm_b[6];
-} bin_net_t;
-size_t bin_window_workspace_bytes(int B, int H, int W);
-/* frames[6], outs[14]: (B,3,H,W) fp32 NCHW device tensors.  Executes the 17 unique backbone
- * calls of the reference's 20 (the 3 repeated stage-1 calls are bit-identical) and the 6 live
- * ConvLSTM calls of its 12 (SURVEY.md Appendix A).
- * A NULL outs_host[i] means "do not compute output i": its backbone call is dropped from its stage's launch, and a
- * stage, a ConvLSTM cell or a workspace image that then has no reader left is dropped too (outputs 13, 8, 12 alone need
- * 13 of the 17 calls).  The non-NULL outputs hold the same bits as with all 14 present.  The non-NULL set must be closed
- * under the window's dataflow: if a computed output reads a NULL one the call returns BIN_ERR_ARG before launching
- * anything, and bin_last_error() names both indices.  All-NULL is BIN_ERR_ARG too.  The workspace size and layout do not
- * depend on which outputs are NULL. */
-int bin_window_fwd(const bin_net_t* net, const float* const* frames_host, float* const* outs_host, int B, int H,
-                   int W, void* workspace, size_t workspace_bytes, bin_stream_t s);
-/* Precision-parameterised twins of the calls above (prec = BIN_PREC_F16 | BIN_PREC_F32X3).  In BIN_PREC_F32X3 the
+/* Precision-parameterised twins of the backbone calls (prec = BIN_PREC_F16 | BIN_PREC_F32X3).  In BIN_PREC_F32X3 the
  * packed blob is 3x and the workspace 2x as large; results match the fp32 reference to <=1e-5. */
 size_t bin_backbone_packed_bytes_p(int nframes, int prec);
 int bin_backbone_pack_p(int nframes, const float* const* w_host, const float* const* b_host, void* blob, int prec,
@@ -280,13 +269,6 @@ int bin_backbone_pack_p(int nframes, const float* const* w_host, const float* co
 size_t bin_backbone_workspace_bytes_p(int nframes, int Btot, int H, int W, int prec);
 int bin_backbone_fwd_p(int nframes, const void* blob, const bin_frames_t* fr, int H, int W, void* workspace,
                        size_t workspace_bytes, int prec, bin_stream_t s);
-size_t bin_window_workspace_bytes_p(int B, int H, int W, int prec);
-int bin_window_fwd_p(const bin_net_t* net, const float* const* frames_host, float* const* outs_host, int B, int H,
-                     int W, void* workspace, size_t workspace_bytes, int prec, bin_stream_t s);
-
-/* BASELINE config 2a/3a: stages 1-3 on 4 frames -> 6 outputs [I2',I4',I6',I3',I5',I4'']. */
-int bin_pyramid3_fwd(const bin_net_t* net, const float* const* frames_host, float* const* outs_host, int B, int H,
-                     int W, void* workspace, size_t workspace_bytes, bin_stream_t s);
 
 /* ---- fused pixel loss (SURVEY 8f rank 3): bin_model.get_loss, bin_model.py:395-425 ---------------------- */
 /* kind: 0 = nn.L1Loss(reduction='sum') (bin_model.py:55), 1 = nn.MSELoss(reduction='sum') (:57),
@@ -380,7 +362,7 @@ int bin_image_metrics_u8(const uint8_t* a, const uint8_t* b, int h, int w, int c
  * Each flip is its own inverse.  One launch handles a table of n <= BIN_FLIPX4_MAX_TENSORS tensors (the 6 frames or the
  * 14 outputs of a window).
  * expand: src[i] (B,3,H,W) fp32 NCHW -> dst[i] (4B,3,H,W), orientation-major: item o*B + b = orientation o of src item b,
- *         so dst[i] + o*B*3*H*W is a contiguous (B,3,H,W) batch that bin_window_fwd_p takes unchanged.
+ *         so dst[i] + o*B*3*H*W is a contiguous (B,3,H,W) batch.
  * mean:   src[i] (4B,3,H,W), laid out as expand writes it -> dst[i] (B,3,H,W) =
  *         (((y0 + flipW(y1)) + flipH(y2)) + flipHW(y3)) / 4 with y_o = items [o*B, o*B+B) of src[i]: flipx4_forward's
  *         order, every step one correctly rounded fp32 operation (no contraction), so it equals the torch expression.

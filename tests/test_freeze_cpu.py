@@ -14,7 +14,7 @@ NCONV = 66
 @pytest.fixture(scope="module")
 def L():
     from bin_b200 import _lib
-    assert _lib.ABI_VERSION == 5
+    assert _lib.ABI_VERSION == 6
     return _lib.lib()
 
 

@@ -8,7 +8,8 @@ tile remainders, more tiles than SMs, both weight paths (resident in shared memo
 activation magnitudes.  Every plane of every tensor outside a call's ranges holds NaN, every output element the call must
 not write holds a sentinel, and both keep their bits.  The first 36 cases are the draws of the earlier conv fuzz.
 Part 2 holds bin_rdb_tail_fwd to fp64 at the backbone's plane offsets, part 3 bin_pack_frames(_p) bit for bit to a torch
-restatement, part 4 bin_convlstm_fwd to fp64.
+restatement, part 4 bin_convlstm_fwd to fp64 with 1, 2 and 3 cells per launch, each cell of a group bit for bit to its
+own one-cell launch.
 
 Bars (u = 2^-24, the fp32 unit roundoff; A = sum |x||w| + |b| + |res| of the element, an fp64 conv of absolute values):
   fp16 P8 / PIXSHUF   |got - ref| <= ulp16(ref) + C_F16 u A          ref: fp64 on the same fp16 operands
@@ -653,50 +654,67 @@ def test_pack_frames_bit_exact(idx, x3):
 # --------------------------------------------------------------------------------------------------------------------
 # part 4: the ConvLSTM cell against fp64
 # --------------------------------------------------------------------------------------------------------------------
+def _convlstm_launch(cells, B, H, W, write_c):
+    """One bin_convlstm_fwd launch over the cell table [(x, w, b, c_prev, h_prev), ...] -> ([h], [c]), both NaN-filled
+    beforehand; write_c False passes c_out NULL."""
+    from bin_b200 import _lib
+    P = lambda t: None if t is None else t.data_ptr()
+    hs = [torch.full((B, 3, H, W), NAN, device=DEV) for _ in cells]
+    cs = [torch.full((B, 3, H, W), NAN, device=DEV) for _ in cells]
+    tab = (_lib.LstmCell * len(cells))(*[_lib.LstmCell(x.data_ptr(), P(cp), P(hp), w.data_ptr(), b.data_ptr(), h.data_ptr(),
+                                                       c.data_ptr() if write_c else None)
+                                         for (x, w, b, cp, hp), h, c in zip(cells, hs, cs)])
+    _lib.check(_lib.lib().bin_convlstm_fwd(tab, len(cells), B, H, W, torch.cuda.current_stream().cuda_stream))
+    torch.cuda.synchronize()
+    return hs, cs
+
+
+@pytest.mark.parametrize("ncells", [1, 2, 3])
 @pytest.mark.parametrize("W", [1, 2, 3, 4, 5, 63, 64, 65, 67, 128, 130])
-def test_convlstm_vs_fp64(W):
-    import ctypes as C
-    from bin_b200._lib import check, lib
+def test_convlstm_vs_fp64(W, ncells):
+    """ncells cells in one launch, each with its own inputs and weights: every cell against fp64, and with more than one
+    cell every cell with the bits of its own one-cell launch."""
     gen = torch.Generator(device=DEV).manual_seed(500 + W)
     worst = 0.0
     for hi_, H in enumerate([1, 2, 15, 16, 17, 33]):
         for mode in ("none", "state", "state_no_c"):
             B = 1 + (hi_ + len(mode)) % 3
-            x = torch.randn((B, 3, H, W), generator=gen, device=DEV) * 3
-            w = torch.randn((12, 6, 3, 3), generator=gen, device=DEV) * 2      # gate sums reach +-30 and beyond
-            b = torch.randn((12,), generator=gen, device=DEV)
             state = mode != "none"
-            cp = (torch.rand((B, 3, H, W), generator=gen, device=DEV) * 100 - 50) if state else None
-            hp = (torch.rand((B, 3, H, W), generator=gen, device=DEV) * 2 - 1) if state else None
-            h = torch.full((B, 3, H, W), NAN, device=DEV)
-            c = torch.full((B, 3, H, W), NAN, device=DEV)
-            P = lambda t: None if t is None else t.data_ptr()
-            check(lib().bin_convlstm_fwd(x.data_ptr(), P(cp), P(hp), w.data_ptr(), b.data_ptr(), h.data_ptr(),
-                                         None if mode == "state_no_c" else c.data_ptr(), B, H, W,
-                                         torch.cuda.current_stream().cuda_stream))
-            torch.cuda.synchronize()
-            c0 = cp.double() if state else torch.zeros((B, 3, H, W), dtype=torch.float64, device=DEV)
-            h0 = hp.double() if state else torch.zeros_like(c0)
-            xh = torch.cat((x.double(), h0), 1)
-            gsum = F.conv2d(xh, w.double(), b.double(), padding=1)
-            G = F.conv2d(xh.abs(), w.double().abs(), b.double().abs(), padding=1)
-            gi, gj, gf, go = gsum.chunk(4, 1)
-            Gi, Gj, Gf, Go = G.chunk(4, 1)
-            si, tj, sf, so = torch.sigmoid(gi), torch.tanh(gj), torch.sigmoid(gf + 1.0), torch.sigmoid(go)
-            c_ref = c0 * sf + si * tj
-            h_ref = torch.tanh(c_ref) * so
-            e_i, e_f, e_o = (0.25 * K_LSTM * U * G_ + T_LSTM for G_ in (Gi, Gf + 1.0, Go))
-            e_j = K_LSTM * U * Gj + T_LSTM
-            e_c = c0.abs() * e_f + tj.abs() * e_i + si.abs() * e_j + 3 * U * (c0 * sf).abs() + 3 * U * (si * tj).abs()
-            e_h = so.abs() * (e_c + T_LSTM) + torch.tanh(c_ref).abs() * e_o + U * h_ref.abs()
-            rh = ((h.double() - h_ref).abs() / e_h).max().item()
-            worst = max(worst, rh)
-            assert rh <= 1.0, (mode, B, H, W, rh)
-            if mode == "state_no_c":
-                assert torch.isnan(c).all()                           # c_out NULL: nothing written
-            else:
-                rc = ((c.double() - c_ref).abs() / e_c).max().item()
-                worst = max(worst, rc)
-                assert rc <= 1.0, (mode, B, H, W, rc)
+            cells = []
+            for _ in range(ncells):
+                x = torch.randn((B, 3, H, W), generator=gen, device=DEV) * 3
+                w = torch.randn((12, 6, 3, 3), generator=gen, device=DEV) * 2      # gate sums reach +-30 and beyond
+                b = torch.randn((12,), generator=gen, device=DEV)
+                cp = (torch.rand((B, 3, H, W), generator=gen, device=DEV) * 100 - 50) if state else None
+                hp = (torch.rand((B, 3, H, W), generator=gen, device=DEV) * 2 - 1) if state else None
+                cells.append((x, w, b, cp, hp))
+            hs, cs = _convlstm_launch(cells, B, H, W, mode != "state_no_c")
+            for k, ((x, w, b, cp, hp), h, c) in enumerate(zip(cells, hs, cs)):
+                c0 = cp.double() if state else torch.zeros((B, 3, H, W), dtype=torch.float64, device=DEV)
+                h0 = hp.double() if state else torch.zeros_like(c0)
+                xh = torch.cat((x.double(), h0), 1)
+                gsum = F.conv2d(xh, w.double(), b.double(), padding=1)
+                G = F.conv2d(xh.abs(), w.double().abs(), b.double().abs(), padding=1)
+                gi, gj, gf, go = gsum.chunk(4, 1)
+                Gi, Gj, Gf, Go = G.chunk(4, 1)
+                si, tj, sf, so = torch.sigmoid(gi), torch.tanh(gj), torch.sigmoid(gf + 1.0), torch.sigmoid(go)
+                c_ref = c0 * sf + si * tj
+                h_ref = torch.tanh(c_ref) * so
+                e_i, e_f, e_o = (0.25 * K_LSTM * U * G_ + T_LSTM for G_ in (Gi, Gf + 1.0, Go))
+                e_j = K_LSTM * U * Gj + T_LSTM
+                e_c = c0.abs() * e_f + tj.abs() * e_i + si.abs() * e_j + 3 * U * (c0 * sf).abs() + 3 * U * (si * tj).abs()
+                e_h = so.abs() * (e_c + T_LSTM) + torch.tanh(c_ref).abs() * e_o + U * h_ref.abs()
+                rh = ((h.double() - h_ref).abs() / e_h).max().item()
+                worst = max(worst, rh)
+                assert rh <= 1.0, (mode, B, H, W, k, rh)
+                if mode == "state_no_c":
+                    assert torch.isnan(c).all()                           # c_out NULL: nothing written
+                else:
+                    rc = ((c.double() - c_ref).abs() / e_c).max().item()
+                    worst = max(worst, rc)
+                    assert rc <= 1.0, (mode, B, H, W, k, rc)
+                if ncells > 1:
+                    (h1,), (c1,) = _convlstm_launch([cells[k]], B, H, W, mode != "state_no_c")
+                    assert torch.equal(_bits(h), _bits(h1)) and torch.equal(_bits(c), _bits(c1)), (mode, B, H, W, k)
     _record("convlstm", "f32", worst)
-    print(f"[fwd fuzz] convlstm W={W}: worst err/bar {worst:.3f}")
+    print(f"[fwd fuzz] convlstm W={W} cells={ncells}: worst err/bar {worst:.3f}")

@@ -1,7 +1,6 @@
 """The output selection (rdn.set_outputs) on the GPU: wanted outputs bit-identical to the full window's on the eager and
-the graphed path in both precisions, the stage launches a selection issues, the C entry's NULL convention, streaming,
-the self-ensemble, the refusals, and the test.py caller sequence with the three images it writes."""
-import ctypes as C
+the graphed path in both precisions, the stage launches a selection issues, streaming, the self-ensemble, the refusals,
+and the test.py caller sequence with the three images it writes."""
 from contextlib import contextmanager
 
 import numpy as np
@@ -101,7 +100,8 @@ def _profiled_launches(fn):
 
 @pytest.mark.parametrize("wanted", [None] + SELECTIONS, ids=str)
 def test_library_window_issues_one_packer_launch_per_live_stage(net, monkeypatch, wanted):
-    """The module's window is one bin_window_fwd_p call: the frame packer runs once per stage that is left."""
+    """The module's window runs each stage that is left as one batched backbone launch, so the frame packer runs once per
+    such stage, and the live cells of each recurrent hand-off as one ConvLSTM launch."""
     monkeypatch.setenv("BIN_B200_GRAPH", "0")
     frames = [f.cuda() for f in O.synth_frames(6, 1, 32, 48, seed=8)]
     with torch.no_grad(), selection(net, wanted):
@@ -153,12 +153,12 @@ def test_streaming_stage_counts_for_a_step0_selection(net, monkeypatch):
     """(9,) needs frames 0..4 only: stage 1 runs its four step-0 pairs, then 3, 2 and 1 calls, and no ConvLSTM cell."""
     from bin_b200 import ops, rdn
     from bin_b200.streaming import StreamingBIN
-    stages, real = [], rdn._launch_stage
-    monkeypatch.setattr(rdn, "_launch_stage", lambda m, calls, outs, prec: stages.append(len(calls)) or real(m, calls, outs, prec))
-    monkeypatch.setattr(ops, "convlstm_fwd", lambda *a, **k: pytest.fail("a ConvLSTM cell ran"))
     video = [f.cuda() for f in O.synth_frames(6, 1, 32, 48, seed=12)]
     with torch.no_grad():
         full = net(*video)
+    stages, real = [], rdn._launch_stage
+    monkeypatch.setattr(rdn, "_launch_stage", lambda m, calls, outs, prec: stages.append(len(calls)) or real(m, calls, outs, prec))
+    monkeypatch.setattr(ops, "convlstm_group", lambda *a, **k: pytest.fail("a ConvLSTM cell ran"))
     with selection(net, (9,), unwanted="zeros"):
         st = StreamingBIN(net)
         got = [st.push(f) for f in video][-1]
@@ -200,44 +200,6 @@ def test_grad_enabled_call_raises(net):
             net(*frames)                                  # parameters require grad
         with pytest.raises(BinB200Error, match="set_outputs"):
             net(*[f.clone().requires_grad_(True) for f in frames])
-
-
-def _window_call(net, frames, present, prec=0):
-    """bin_window_fwd_p with NULL at every output not in `present` -> (return code, error text, output tensors)."""
-    from bin_b200 import _lib, ops, rdn
-    L = _lib.lib()
-    B, _, H, W = frames[0].shape
-    outs = [torch.full_like(frames[0], -7.0) if i in present else None for i in range(14)]
-    ws = torch.empty(L.bin_window_workspace_bytes_p(B, H, W, prec), dtype=torch.uint8, device="cuda")
-    cnet = net._net(prec)
-    fp = (C.c_void_p * 6)(*[f.data_ptr() for f in frames])
-    op = (C.c_void_p * 14)(*[None if o is None else o.data_ptr() for o in outs])
-    rc = L.bin_window_fwd_p(C.byref(cnet), fp, op, B, H, W, ws.data_ptr(), ws.numel(), prec, ops._stream())
-    err = L.bin_last_error().decode()
-    torch.cuda.synchronize()
-    return rc, err, outs
-
-
-def test_library_null_convention(net):
-    """A closed NULL pattern computes the present outputs; an open one is an argument error, returned before any launch:
-    the output buffers keep their fill value."""
-    from bin_b200 import rdn
-    frames = [f.cuda() for f in O.synth_frames(6, 1, 32, 48, seed=8)]
-    with torch.no_grad():
-        full = net(*frames)
-    for wanted in SELECTIONS:
-        present = rdn._live_outputs(wanted)
-        rc, err, outs = _window_call(net, frames, present)
-        assert rc == 0, err
-        assert all(torch.equal(outs[i], full[i]) for i in present), wanted
-    for present, reader, missing in [((1, 2, 3, 5, 6, 8, 11, 12, 13), 11, 10), ((1, 2, 3, 5, 6, 10, 11, 12, 13), 13, 8),
-                                     ((0, 1, 2, 3, 4, 5, 6, 8, 9), 9, 7)]:
-        from torch.profiler import ProfilerActivity, profile
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            rc, err, outs = _window_call(net, frames, present)
-        assert rc == 1 and err == f"window_fwd: output {reader} depends on output {missing}, whose pointer is NULL"
-        assert all(bool((outs[i] == -7.0).all()) for i in present)
-        assert not any("binb::" in ev.name for ev in prof.events())
 
 
 def test_caller_sequence_writes_the_same_three_images():

@@ -8,7 +8,8 @@
   final     UPNet.2 <16,3> + mean(frames): the frames are loaded before the main loop.  2, 3 and 5 frames, 1-3 calls,
             shared frame pools, both kernel variants, both precisions for the x-stacked one.
   convlstm  the forward cell at a vector-path (W % 4 == 0) and a scalar-path width, with and without state, at sizes
-            with many more blocks than SMs.
+            with many more blocks than SMs; 1, 2 and 3 cells per launch, each cell of a group with the bits of its own
+            one-cell launch.
 
 Every tensor plane a call does not read holds NaN, every output element it must not write holds a sentinel, and both
 keep their bits.  Bars as in test_gpu_forward_fuzz.py (u = 2^-24, A = fp64 conv of absolute values):
@@ -264,34 +265,51 @@ def test_final_vs_fp64(idx):
 K_LSTM, T_LSTM = 56.0, 3e-7
 
 
+def _convlstm_launch(cells, B, H, W):
+    """One bin_convlstm_fwd launch over the cell table [(x, w, b, c_prev, h_prev), ...] -> ([h], [c]), NaN-filled first."""
+    from bin_b200 import _lib
+    P = lambda t: None if t is None else t.data_ptr()
+    hs = [torch.full((B, 3, H, W), NAN, device=DEV) for _ in cells]
+    cs = [torch.full((B, 3, H, W), NAN, device=DEV) for _ in cells]
+    tab = (_lib.LstmCell * len(cells))(*[_lib.LstmCell(x.data_ptr(), P(cp), P(hp), w.data_ptr(), b.data_ptr(), h.data_ptr(),
+                                                       c.data_ptr()) for (x, w, b, cp, hp), h, c in zip(cells, hs, cs)])
+    _lib.check(_lib.lib().bin_convlstm_fwd(tab, len(cells), B, H, W, torch.cuda.current_stream().cuda_stream))
+    torch.cuda.synchronize()
+    return hs, cs
+
+
+@pytest.mark.parametrize("ncells", [1, 2, 3])
 @pytest.mark.parametrize("state", [False, True])
 @pytest.mark.parametrize("W", [1280, 1283])
-def test_convlstm_large_vs_fp64(W, state):
-    from bin_b200._lib import check, lib
+def test_convlstm_large_vs_fp64(W, state, ncells):
+    """ncells cells with their own inputs and weights in one launch: every cell against fp64, and with more than one
+    cell every cell with the bits of its own one-cell launch."""
     B, H = 2, 37
     gen = torch.Generator(device=DEV).manual_seed(1000 + W + int(state))
-    x = torch.randn((B, 3, H, W), generator=gen, device=DEV) * 3
-    w = torch.randn((12, 6, 3, 3), generator=gen, device=DEV) * 2
-    b = torch.randn((12,), generator=gen, device=DEV)
-    cp = (torch.rand((B, 3, H, W), generator=gen, device=DEV) * 100 - 50) if state else None
-    hp = (torch.rand((B, 3, H, W), generator=gen, device=DEV) * 2 - 1) if state else None
-    h = torch.full((B, 3, H, W), NAN, device=DEV)
-    c = torch.full((B, 3, H, W), NAN, device=DEV)
-    P = lambda t: None if t is None else t.data_ptr()
-    check(lib().bin_convlstm_fwd(x.data_ptr(), P(cp), P(hp), w.data_ptr(), b.data_ptr(), h.data_ptr(), c.data_ptr(),
-                                 B, H, W, torch.cuda.current_stream().cuda_stream))
-    torch.cuda.synchronize()
-    c0 = cp.double() if state else torch.zeros((B, 3, H, W), dtype=torch.float64, device=DEV)
-    h0 = hp.double() if state else torch.zeros_like(c0)
-    xh = torch.cat((x.double(), h0), 1)
-    gi, gj, gf, go = F.conv2d(xh, w.double(), b.double(), padding=1).chunk(4, 1)
-    Gi, Gj, Gf, Go = F.conv2d(xh.abs(), w.double().abs(), b.double().abs(), padding=1).chunk(4, 1)
-    si, tj, sf, so = torch.sigmoid(gi), torch.tanh(gj), torch.sigmoid(gf + 1.0), torch.sigmoid(go)
-    c_ref = c0 * sf + si * tj
-    h_ref = torch.tanh(c_ref) * so
-    e_i, e_f, e_o = (0.25 * K_LSTM * U * G_ + T_LSTM for G_ in (Gi, Gf + 1.0, Go))
-    e_j = K_LSTM * U * Gj + T_LSTM
-    e_c = c0.abs() * e_f + tj.abs() * e_i + si.abs() * e_j + 3 * U * (c0 * sf).abs() + 3 * U * (si * tj).abs()
-    e_h = so.abs() * (e_c + T_LSTM) + torch.tanh(c_ref).abs() * e_o + U * h_ref.abs()
-    assert ((h.double() - h_ref).abs() / e_h).max().item() <= 1.0
-    assert ((c.double() - c_ref).abs() / e_c).max().item() <= 1.0
+    cells = []
+    for _ in range(ncells):
+        x = torch.randn((B, 3, H, W), generator=gen, device=DEV) * 3
+        w = torch.randn((12, 6, 3, 3), generator=gen, device=DEV) * 2
+        b = torch.randn((12,), generator=gen, device=DEV)
+        cp = (torch.rand((B, 3, H, W), generator=gen, device=DEV) * 100 - 50) if state else None
+        hp = (torch.rand((B, 3, H, W), generator=gen, device=DEV) * 2 - 1) if state else None
+        cells.append((x, w, b, cp, hp))
+    hs, cs = _convlstm_launch(cells, B, H, W)
+    for k, ((x, w, b, cp, hp), h, c) in enumerate(zip(cells, hs, cs)):
+        c0 = cp.double() if state else torch.zeros((B, 3, H, W), dtype=torch.float64, device=DEV)
+        h0 = hp.double() if state else torch.zeros_like(c0)
+        xh = torch.cat((x.double(), h0), 1)
+        gi, gj, gf, go = F.conv2d(xh, w.double(), b.double(), padding=1).chunk(4, 1)
+        Gi, Gj, Gf, Go = F.conv2d(xh.abs(), w.double().abs(), b.double().abs(), padding=1).chunk(4, 1)
+        si, tj, sf, so = torch.sigmoid(gi), torch.tanh(gj), torch.sigmoid(gf + 1.0), torch.sigmoid(go)
+        c_ref = c0 * sf + si * tj
+        h_ref = torch.tanh(c_ref) * so
+        e_i, e_f, e_o = (0.25 * K_LSTM * U * G_ + T_LSTM for G_ in (Gi, Gf + 1.0, Go))
+        e_j = K_LSTM * U * Gj + T_LSTM
+        e_c = c0.abs() * e_f + tj.abs() * e_i + si.abs() * e_j + 3 * U * (c0 * sf).abs() + 3 * U * (si * tj).abs()
+        e_h = so.abs() * (e_c + T_LSTM) + torch.tanh(c_ref).abs() * e_o + U * h_ref.abs()
+        assert ((h.double() - h_ref).abs() / e_h).max().item() <= 1.0, k
+        assert ((c.double() - c_ref).abs() / e_c).max().item() <= 1.0, k
+        if ncells > 1:
+            (h1,), (c1,) = _convlstm_launch([cells[k]], B, H, W)
+            assert torch.equal(_bits(h), _bits(h1)) and torch.equal(_bits(c), _bits(c1)), k

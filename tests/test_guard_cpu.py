@@ -228,7 +228,7 @@ def test_new_symbols_are_declared_bound_and_leave_the_abi_version():
     hdr = open(os.path.join(ROOT, "include", "bin_b200.h")).read()
     for name in ("bin_grad_audit_scratch_bytes", "bin_grad_audit", "bin_adam_step_guarded"):
         assert re.search(rf"\b{name}\s*\(", hdr) and name in _lib.exported_symbols()
-    assert _lib.ABI_VERSION == 5
+    assert _lib.ABI_VERSION == 6
 
 
 def test_entry_points_reject_bad_arguments_before_any_launch():

@@ -81,8 +81,29 @@ def test_workspace_queries_are_pure():
     from bin_b200 import _lib
     L = _lib.lib()
     assert L.bin_backbone_packed_bytes(2) > 5_000_000 and L.bin_backbone_packed_bytes(4) == 0
-    a = L.bin_window_workspace_bytes(1, 64, 64)
-    assert 0 < a < L.bin_window_workspace_bytes(1, 128, 128)
+    a = L.bin_backbone_workspace_bytes(2, 1, 64, 64)
+    assert 0 < a < L.bin_backbone_workspace_bytes(2, 1, 128, 128)
+
+
+def test_convlstm_cell_table_is_checked_before_any_launch():
+    """bin_convlstm_fwd refuses a bad cell table with BIN_ERR_ARG before it launches (the pointers are fake and never
+    dereferenced)."""
+    from bin_b200 import _lib
+    L = _lib.lib()
+    p = 1 << 20
+
+    def call(cells, n=None):
+        tab = (_lib.LstmCell * len(cells))(*[_lib.LstmCell(*c) for c in cells])
+        rc = L.bin_convlstm_fwd(tab if cells else None, len(cells) if n is None else n, 1, 8, 8, None)
+        return rc, L.bin_last_error().decode()
+
+    plain, stateful = (p, None, None, p, p, p, None), (p, p, p, p, p, p, p)
+    assert call([]) == (1, "convlstm: null cell table")
+    assert call([plain], 0) == (1, "convlstm: 1..3 cells per launch")
+    assert call([plain] * 4) == (1, "convlstm: 1..3 cells per launch")
+    assert call([plain, (p, None, None, p, p, None, None)]) == (1, "convlstm: null argument")
+    assert call([(p, p, None, p, p, p, None)]) == (1, "convlstm: give both c_prev and h_prev or neither")
+    assert call([stateful, plain]) == (1, "convlstm: cells of one launch must all have or all lack a state")
 
 
 def test_wgrad_rejects_bad_segments_before_any_launch():
@@ -281,7 +302,7 @@ def test_ctypes_structs_match_the_header_layout(tmp_path):
     probes = {"bin_act_t": (_lib.Act, ["ptr", "B", "planes", "H", "W"]),
               "bin_frames_t": (_lib.Frames, ["frame", "out", "ncalls", "nframes", "Bc"]),
               "bin_conv_args_t": (_lib.ConvArgs, [f[0] for f in _lib.ConvArgs._fields_]),
-              "bin_net_t": (_lib.Net, ["blob", "lstm_w", "lstm_b"])}
+              "bin_lstm_cell_t": (_lib.LstmCell, ["x", "c_prev", "h_prev", "w", "b", "h_out", "c_out"])}
     lines = ['#include <stdio.h>', '#include <stddef.h>', '#include "bin_b200.h"', 'int main(void) {']
     for cname, (_, fields) in probes.items():
         lines.append(f'  printf("{cname} %zu\\n", sizeof({cname}));')

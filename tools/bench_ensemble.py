@@ -11,8 +11,9 @@ Per size (H x W, B = 1, fp16 mode, synthetic weights and frames):
                what utils/test_util.py:110-132 does; timed alternately with the ensemble in the same loop;
   kernels      bin_flipx4_expand over the 6 frames and bin_flipx4_mean over the 14 outputs, 50 back-to-back launches
                each on preallocated tensors; GB/s = bytes each must move / kernel time, against 3.35 TB/s;
-  memory       torch.cuda.max_memory_allocated() growth of one ensemble call with no cached workspace, beside
-               bin_window_workspace_bytes_p(4B, H, W) + the frame and output tensors it needs.
+  memory       torch.cuda.max_memory_allocated() growth of one ensemble call with no cached workspace, beside the
+               workspace of the window's largest stage at 4B (bin_backbone_workspace_bytes_p) + the frame, intermediate
+               and output tensors it needs.
 Needs a CUDA device; there is no CPU fallback."""
 import argparse
 import ctypes as C
@@ -93,9 +94,10 @@ def run_size(net, H, W, reps, warmup):
         torch.cuda.synchronize()
         peak = torch.cuda.max_memory_allocated() - base
         del outs
-        ws = _lib.lib().bin_window_workspace_bytes_p(4 * B, H, W, 0)
-        tensors = (6 * 4 + 14 * 4 + 14) * plane                 # expanded frames, 4B outputs, the 14 means
-        res["memory"] = {"peak_growth_bytes": peak, "window_workspace_4B_bytes": ws, "tensor_bytes": tensors,
+        # (frames per call, calls) of the window's four stages; 9 intermediate images (6 ConvLSTM h, 3 step-1 outputs)
+        ws = max(_lib.lib().bin_backbone_workspace_bytes_p(nf, n * 4 * B, H, W, 0) for nf, n in ((2, 5), (3, 6), (5, 4), (5, 2)))
+        tensors = (6 * 4 + 14 * 4 + 9 * 4 + 14) * plane        # expanded frames, 4B outputs and intermediates, the 14 means
+        res["memory"] = {"peak_growth_bytes": peak, "stage_workspace_4B_bytes": ws, "tensor_bytes": tensors,
                          "peak_over_expected": peak / (ws + tensors)}
 
         ens = lambda: net(*frames)                              # noqa: E731
@@ -161,7 +163,7 @@ def main():
         print(f"  expand {k['expand_ms'] * 1e3:.0f} us ({k['expand_GBps']:.0f} GB/s, {k['expand_share_of_hbm_peak']:.0%} of 3.35 TB/s)"
               f" | mean {k['mean_ms'] * 1e3:.0f} us ({k['mean_GBps']:.0f} GB/s, {k['mean_share_of_hbm_peak']:.0%}) | both "
               f"{k['share_of_ensemble']:.2%} of the ensemble")
-        print(f"  peak memory growth {m['peak_growth_bytes'] / 1e9:.2f} GB vs workspace {m['window_workspace_4B_bytes'] / 1e9:.2f}"
+        print(f"  peak memory growth {m['peak_growth_bytes'] / 1e9:.2f} GB vs stage workspace {m['stage_workspace_4B_bytes'] / 1e9:.2f}"
               f" GB + tensors {m['tensor_bytes'] / 1e9:.2f} GB (ratio {m['peak_over_expected']:.3f})")
     out["card_after"] = card()
     c = out["card_after"]
