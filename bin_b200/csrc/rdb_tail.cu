@@ -57,7 +57,6 @@ struct alignas(64) RdbTailParams {
   int b0, y0, ny;
   int tiles_x, tiles_y, ntiles;
   __half* out; int out_planes, out_plane0;
-  const __half* res; int res_planes, res_plane0;
   int reverse;                          // walk the tiles last-to-first (zigzag L2 reuse across launches)
 };
 
@@ -141,9 +140,14 @@ __global__ void __launch_bounds__(384, 1) rdb_tail_kernel(const __grid_constant_
   float* xs = xs0 + (2 * m + (wq >> 1)) * kXsFloats<32>;
   const int xs_bar = 3 + 2 * m + (wq >> 1);      // named barrier of the warp pair (1, 2: wg_sync)
   float acc_c[kRtN / 2], acc_l[kRtN / 2];        // fragment: [4 i + 2 h + e] = row 16 wq + lane/4 + 8 h, column 8 i + 2 k4 + e
+  // residual x of this thread's pixels (rows 16 wq + lane/4 + 8 h), channels 8 i + 2 k4, +1: the centre of x chunks
+  // 0..2, read from their ring slots while the LFF consumes them (the bytes the TMA copied from x, so x' is unchanged)
+  uint32_t res[2][kRtN / 8];
+  const uint32_t res_off = (uint32_t)(m * 64 + wq * 16 + (lane >> 2) + kTWH + 1) * 16 + 4 * k4;
   uint32_t s = 0, ph = 0;
   for (int tq = blockIdx.x; tq < p.ntiles; tq += gridDim.x) {
     int prev = -1;
+#pragma unroll
     for (int c = 0; c < kRtChunks; ++c) {
       mbar_wait(&ctrl->full[s], ph);
       if (tq == (int)blockIdx.x) mbar_wait(&ctrl->wfull[c], 0);
@@ -163,6 +167,14 @@ __global__ void __launch_bounds__(384, 1) rdb_tail_kernel(const __grid_constant_
       for (int jj = 0; jj < kKC / 16; ++jj)                          // LFF: centre row, +1 pixel, B = slab 3
         Wgmma<kRtN>::mma(acc_l, gmma_desc(a_base + (kTWH + 1) * 16 + jj * 2 * kRtAPlane, kRtAPlane, 128),
                          gmma_desc(b_base + 3 * kRtSlab + jj * 2 * kRtN * 16, kRtN * 16, 128), jj == 0 ? first : 1u);
+      if (c < kRtN / 32) {                                           // x chunk: keep this thread's residual values
+        const uint8_t* st = stage0 + (size_t)s * kRtABytes + res_off;
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int q = 0; q < kKPL; ++q)
+            res[h][kKPL * c + q] = *reinterpret_cast<const uint32_t*>(st + h * 8 * 16 + q * kRtAPlane);
+      }
       wgmma_commit();
       wgmma_wait<1>();
       if (prev >= 0 && lane == 0) mbar_arrive(&ctrl->empty[prev]);
@@ -174,24 +186,17 @@ __global__ void __launch_bounds__(384, 1) rdb_tail_kernel(const __grid_constant_
     acc_fence(acc_l);
     if (lane == 0) mbar_arrive(&ctrl->empty[prev]);
 
-    // ---------------------------------------------------------- residual x of this thread's pixels
-    // issued before the g3 epilogue so that their latency hides behind it and the g3 LFF wgmma
+    // ---------------------------------------------------------- this thread's pixels
     int txi, tyi, b;
     tile_of(tq, txi, tyi, b);
     bool valid[2];
     int y[2], x[2];
-    uint32_t res[2][kRtN / 8];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int L = m * 64 + wq * 16 + (lane >> 2) + 8 * h;
       y[h] = p.y0 + tyi * kRtTH + (L >> 5);
       x[h] = txi * kRtTW + (L & 31);
       valid[h] = (L & 31) < kRtTW && y[h] < p.y0 + p.ny && x[h] < p.W;
-#pragma unroll
-      for (int i = 0; i < kRtN / 8; ++i) {
-        const size_t roff = ((((size_t)b * p.res_planes + p.res_plane0 + i) * p.H + y[h]) * p.W + x[h]) * 8 + 2 * k4;
-        res[h][i] = valid[h] ? *reinterpret_cast<const uint32_t*>(p.res + roff) : 0u;
-      }
     }
 
     // ---------------------------------------------------------- g3 = ReLU(D0[p] + D1[p+1] + D2[p+2] + b) -> smem
@@ -272,7 +277,6 @@ int launch_rdb_tail(const bin_act_t& x, int x_plane0, const bin_act_t& g, int g_
   p.tiles_y = (p.ny + kRtTH - 1) / kRtTH;
   p.ntiles = nb * p.tiles_x * p.tiles_y;
   p.out = reinterpret_cast<__half*>(out.ptr); p.out_planes = out.planes; p.out_plane0 = out_plane0;
-  p.res = reinterpret_cast<const __half*>(x.ptr); p.res_planes = x.planes; p.res_plane0 = x_plane0;
   p.reverse = reverse ? 1 : 0;
   BIN_TRY(make_p8_tmap(&p.tmap0, x, kRtRows));                // every argument is checked before the first tensor map
   BIN_TRY(make_p8_tmap(&p.tmap1, g, kRtRows));
