@@ -10,7 +10,7 @@ LIB_PATH = os.path.join(HERE, "libbin_b200.so")
 
 BIN_MAX_CALLS = 6
 BIN_MAX_FRAMES = 5
-BIN_BACKBONE_NCONV = 66
+BIN_BACKBONE_NCONV = 66               # convs of the shipped (G0 = 96, D = 12) backbone, the most any arch has
 BIN_FLIPX4_MAX_TENSORS = 14
 BIN_TRAIN_MAX_BATCH = 16
 BIN_TRAIN_FRAMES = 17
@@ -18,6 +18,11 @@ BIN_PNG_MAX_BATCH = 16
 EPI_P8, EPI_PIXSHUF, EPI_FINAL = 0, 1, 2
 BIN_DETERMINISTIC = 1                 # flags bit of the *_ex entry points
 ABI_VERSION = 6
+
+
+def backbone_arch(nframes: int, g0: int = 0, d: int = 0) -> int:
+    """BIN_BACKBONE_ARCH: the `arch` argument of the backbone calls; g0 = 0 and d = 0 stand for the shipped 96 and 12."""
+    return nframes | (g0 << 8) | (d << 16)
 
 
 class Act(C.Structure):
@@ -75,6 +80,7 @@ _SIGS = {
     "bin_convlstm_bwd": (C.c_int, [C.c_void_p] * 13 + [C.c_int] * 3 + [C.c_void_p]),
     "bin_convlstm_bwd_scratch_bytes": (C.c_size_t, [C.c_int] * 3),
     "bin_convlstm_bwd_ex": (C.c_int, [C.c_void_p] * 13 + [C.c_int] * 4 + [C.c_void_p, C.c_size_t, C.c_void_p]),
+    "bin_backbone_nconv": (C.c_int, [C.c_int]),
     "bin_backbone_packed_bytes": (C.c_size_t, [C.c_int]),
     "bin_backbone_pack": (C.c_int, [C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_void_p, C.c_void_p]),
     "bin_backbone_workspace_bytes": (C.c_size_t, [C.c_int] * 4),

@@ -49,18 +49,17 @@ def _input_key(model, frames):
     return tuple((t.data_ptr(), t._version) for t in list(model._conv_params()) + list(frames))
 
 
-def grad_plan(needs_input_grad, ncalls: int, nframes: int):
+def grad_plan(needs_input_grad, ncalls: int, nframes: int, nconv: int = _lib.BIN_BACKBONE_NCONV):
     """What one BackboneStageFn backward computes, from its ctx.needs_input_grad = (model, ncalls, *frames, *params):
-    (need, frame_needed).  need is the 2 * BIN_BACKBONE_NCONV-byte host mask of bin_backbone_bwd_masked, 1 where a
-    parameter (weight then bias of conv 0..65, the order of _conv_params) wants its gradient; frame_needed[k][f] says
-    whether frame f of call k does (its dframes pointer is NULL when not)."""
+    (need, frame_needed).  need is the 2 * nconv-byte host mask of bin_backbone_bwd_masked (nconv = the backbone's
+    bin_backbone_nconv), 1 where a parameter (weight then bias of each conv, the order of _conv_params) wants its
+    gradient; frame_needed[k][f] says whether frame f of call k does (its dframes pointer is NULL when not)."""
     nf = ncalls * nframes
     flags = tuple(needs_input_grad)[2:]
-    if len(flags) != nf + 2 * _lib.BIN_BACKBONE_NCONV:
-        raise BinB200Error(f"grad_plan: expected {nf + 2 * _lib.BIN_BACKBONE_NCONV} inputs after (model, ncalls), "
-                           f"got {len(flags)}")
+    if len(flags) != nf + 2 * nconv:
+        raise BinB200Error(f"grad_plan: expected {nf + 2 * nconv} inputs after (model, ncalls), got {len(flags)}")
     frame_needed = [[bool(flags[k * nframes + f]) for f in range(nframes)] for k in range(ncalls)]
-    need = (C.c_ubyte * (2 * _lib.BIN_BACKBONE_NCONV))(*[1 if x else 0 for x in flags[nf:]])
+    need = (C.c_ubyte * (2 * nconv))(*[1 if x else 0 for x in flags[nf:]])
     return need, frame_needed
 
 
@@ -77,7 +76,7 @@ def _grad_frames(dframes, B: int) -> _lib.Frames:
 class BackboneStageFn(torch.autograd.Function):
     """ncalls same-weight backbone calls (RDN.py:210-334) in one launch, with backward.
 
-    Default: the forward keeps the stage's whole training workspace (all 12 RDBs' growth maps) until the backward.
+    Default: the forward keeps the stage's whole training workspace (all its RDBs' growth maps) until the backward.
     With set_activation_checkpointing(net, "recompute") it keeps only its input frames: the forward is the inference
     forward into the shared per-stream workspace, and the backward runs that forward again and rebuilds each RDB's
     growth maps just before that RDB's backward.  Every kernel sees the same operands in both (DESIGN.md §4e).
@@ -88,7 +87,7 @@ class BackboneStageFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, model, ncalls: int, *args):
-        n = model.NFRAMES
+        n, arch = model.NFRAMES, model.arch
         frames = [a.detach().contiguous() for a in args[: ncalls * n]]
         calls = [frames[k * n:(k + 1) * n] for k in range(ncalls)]
         B, _, H, W = frames[0].shape
@@ -107,9 +106,9 @@ class BackboneStageFn(torch.autograd.Function):
                 save = None
             else:
                 fr = ops.make_frames(calls, outs)
-                nbytes = lib().bin_backbone_train_workspace_bytes(n, B * ncalls, H, W)
+                nbytes = lib().bin_backbone_train_workspace_bytes(arch, B * ncalls, H, W)
                 save = torch.empty(nbytes, dtype=torch.uint8, device=dev)          # owned by this node until backward
-                check(lib().bin_backbone_fwd_train(n, model.packed_blob().data_ptr(), C.byref(fr), H, W, save.data_ptr(),
+                check(lib().bin_backbone_fwd_train(arch, model.packed_blob().data_ptr(), C.byref(fr), H, W, save.data_ptr(),
                                                    save.numel(), _stream()))
         ctx.model, ctx.ncalls, ctx.save, ctx.shape, ctx.dev = model, ncalls, save, (B, H, W), dev
         ctx.recompute_key = _input_key(model, frames) if recompute else None
@@ -129,7 +128,7 @@ class BackboneStageFn(torch.autograd.Function):
         elif ctx.save is None:
             raise BinB200Error("bin_b200: backward through a backbone stage twice (retain_graph / double backward) is not "
                                "supported: the saved activations are released after the first backward")
-        n = model.NFRAMES
+        n, arch = model.NFRAMES, model.arch
         dev = ctx.dev
         flags = deterministic_flags()
         with torch.cuda.device(dev):
@@ -139,25 +138,25 @@ class BackboneStageFn(torch.autograd.Function):
             check(lib().bin_grad_scale(gp, ncalls, gouts[0].numel(), loss_scale_target(), sbuf.data_ptr(),
                                        sbuf.data_ptr() + 4, _stream()))
             scale = sbuf[:1]
-            need, frame_needed = grad_plan(ctx.needs_input_grad, ncalls, n)
+            need, frame_needed = grad_plan(ctx.needs_input_grad, ncalls, n, model.nconv)
             dframes = [[torch.empty((B, 3, H, W), device=dev) if want else None for want in call] for call in frame_needed]
             dout = ops.make_frames([[g] * n for g in gouts], gouts)             # only .out / ncalls / Bc are read
             dfr = _grad_frames(dframes, B)
-            gparams = torch.zeros(lib().bin_backbone_grad_param_floats(n), device=dev) if any(need) else None
+            gparams = torch.zeros(lib().bin_backbone_grad_param_floats(arch), device=dev) if any(need) else None
             gp_ptr = None if gparams is None else gparams.data_ptr()
-            gws = torch.empty(lib().bin_backbone_grad_workspace_bytes(n, B * ncalls, H, W), dtype=torch.uint8, device=dev)
+            gws = torch.empty(lib().bin_backbone_grad_workspace_bytes(arch, B * ncalls, H, W), dtype=torch.uint8, device=dev)
             if recompute:
                 frames = ctx.frames_keepalive
                 calls = [frames[k * n:(k + 1) * n] for k in range(ncalls)]
                 scratch = [torch.empty_like(frames[0]) for _ in range(ncalls)]   # the forward's outputs stay untouched
                 ws = _launch_stage(model, calls, scratch, prec=0)                  # fp16, as in the forward
-                check(lib().bin_backbone_bwd_recompute_masked(n, model.packed_blob().data_ptr(),
+                check(lib().bin_backbone_bwd_recompute_masked(arch, model.packed_blob().data_ptr(),
                                                               model._cached_pack("t").data_ptr(), C.byref(dout),
                                                               C.byref(dfr), H, W, ws.data_ptr(), ws.numel(),
                                                               gws.data_ptr(), gws.numel(), gp_ptr, scale.data_ptr(),
                                                               flags, need, _stream()))
             else:
-                check(lib().bin_backbone_bwd_masked(n, model._cached_pack("t").data_ptr(), C.byref(dout), C.byref(dfr), H, W,
+                check(lib().bin_backbone_bwd_masked(arch, model._cached_pack("t").data_ptr(), C.byref(dout), C.byref(dfr), H, W,
                                                     ctx.save.data_ptr(), gws.data_ptr(), gws.numel(), gp_ptr,
                                                     scale.data_ptr(), flags, need, _stream()))
         ctx.save = None

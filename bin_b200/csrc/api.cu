@@ -91,7 +91,7 @@ size_t png_max_bytes(int h, int w);
 size_t png_workspace_bytes(int n, int h, int w);
 int launch_png_encode_u8(const uint8_t* const* imgs_host, int n, int h, int w, uint8_t* out, size_t out_stride,
                          int64_t* sizes, void* workspace, size_t workspace_bytes, cudaStream_t s);
-int launch_rdb_tail(const bin_act_t& x, int x_plane0, const bin_act_t& g, int g_plane0, const void* w_conv,
+int launch_rdb_tail(int g0, const bin_act_t& x, int x_plane0, const bin_act_t& g, int g_plane0, const void* w_conv,
                     const float* b_conv, const void* w_lff, const float* b_lff, const bin_act_t& out, int out_plane0,
                     int b_begin, int b_count, int y_begin, int y_count, cudaStream_t s, bool reverse = false);
 int launch_tensor2img_u8(const float* x, int Hs, int Ws, int top, int left, int h, int w, uint8_t* out, cudaStream_t s);
@@ -104,6 +104,35 @@ int launch_convlstm_bwd(const float* x, const float* c_prev, const float* h_prev
 
 static inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
+// ------------------------------------------------------------------ backbone configuration
+// A backbone is 2, 3 or 5 frames wide, G0 = 64 or 96 channels, and D = 1..12 residual dense blocks of C = 4 growth
+// convs with G = 32 channels each (RDN.py:167-334).  The arch value of the C ABI carries all three
+// (BIN_BACKBONE_ARCH); its g0 and d fields are 0 for the shipped 96 and 12, so the shipped arch equals nframes.
+constexpr int kCgrow = 4, kG = 32;
+
+struct Arch {
+  int nframes, g0, d;
+  int nconv() const { return 5 * d + 6; }      // SFENet1, SFENet2, D x (4 conv + LFF), GFF.0, GFF.1, UPNet.0, UPNet.2
+  int planes() const { return g0 / 8; }        // P8 planes of one G0-channel feature map
+};
+
+static bool valid_nframes(int n) { return n == 2 || n == 3 || n == 5; }
+
+static bool decode_arch(int arch, Arch& a) {
+  if (arch < 0 || (arch >> 24) != 0) return false;
+  const int g0 = (arch >> 8) & 0xff, d = (arch >> 16) & 0xff;
+  a.nframes = arch & 0xff;
+  a.g0 = g0 ? g0 : 96;
+  a.d = d ? d : 12;
+  return valid_nframes(a.nframes) && (a.g0 == 64 || a.g0 == 96) && a.d >= 1 && a.d <= 12;
+}
+// decode_arch for an entry point: BIN_ERR_ARG, with `who` in the message, for an arch it rejects
+static int arch_or_fail(int arch, const char* who, Arch& a) {
+  if (decode_arch(arch, a)) return BIN_OK;
+  if (!valid_nframes(arch & 0xff)) return fail(BIN_ERR_ARG, std::string(who) + ": nframes must be 2, 3 or 5");
+  return fail(BIN_ERR_ARG, std::string(who) + ": G0 must be 64 or 96 and D 1..12 (BIN_BACKBONE_ARCH)");
+}
+
 // ------------------------------------------------------------------ backbone conv table
 // Order = nn.Module registration order of the reference backbones (RDN.py:187-208): SFENet1,
 // SFENet2, RDBs.{i}.convs.{0..3}, RDBs.{i}.LFF, GFF.0, GFF.1, UPNet.0, UPNet.2.
@@ -111,14 +140,13 @@ struct ConvSpec {
   int cin, cout, ks, cin_pad, cout_pad;
   size_t w_off, b_off;
 };
-constexpr int kG0 = 96, kD = 12, kCgrow = 4, kG = 32;
 
 struct BackboneLayout {
-  ConvSpec conv[BIN_BACKBONE_NCONV];
+  ConvSpec conv[BIN_BACKBONE_NCONV];   // the first a.nconv() entries are used
   size_t bytes;
 };
 
-static BackboneLayout backbone_layout(int nframes, int x3 = 0) {
+static BackboneLayout backbone_layout(const Arch& A, int x3 = 0) {
   BackboneLayout L;
   int k = 0;
   auto add = [&](int cin, int cout, int ks, int cout_pad) {
@@ -129,18 +157,19 @@ static BackboneLayout backbone_layout(int nframes, int x3 = 0) {
     c.w_off = c.b_off = 0;
     L.conv[k++] = c;
   };
-  add(12 * nframes, kG0, 5, 96);
-  add(kG0, kG0, 3, 96);
-  for (int i = 0; i < kD; ++i) {
-    for (int c = 0; c < kCgrow; ++c) add(kG0 + c * kG, kG, 3, 32);
-    add(kG0 + kCgrow * kG, kG0, 1, 96);
+  const int g0 = A.g0;
+  add(12 * A.nframes, g0, 5, g0);
+  add(g0, g0, 3, g0);
+  for (int i = 0; i < A.d; ++i) {
+    for (int c = 0; c < kCgrow; ++c) add(g0 + c * kG, kG, 3, 32);
+    add(g0 + kCgrow * kG, g0, 1, g0);
   }
-  add(kD * kG0, kG0, 1, 96);
-  add(kG0, kG0, 3, 96);
-  add(kG0, 256, 3, 256);
+  add(A.d * g0, g0, 1, g0);
+  add(g0, g0, 3, g0);
+  add(g0, 256, 3, 256);
   add(64, 3, 3, 16);
   size_t off = 0;
-  for (int i = 0; i < BIN_BACKBONE_NCONV; ++i) {
+  for (int i = 0; i < A.nconv(); ++i) {
     ConvSpec& c = L.conv[i];
     c.w_off = off;
     off = align_up(off + (size_t)c.cout_pad * c.cin_pad * c.ks * c.ks * sizeof(__half) * (x3 ? 3 : 1), 256);
@@ -151,16 +180,14 @@ static BackboneLayout backbone_layout(int nframes, int x3 = 0) {
   return L;
 }
 
-static bool valid_nframes(int n) { return n == 2 || n == 3 || n == 5; }
-
 // ------------------------------------------------------------------ backbone workspace
 struct BackboneWs {
   bin_act_t x0, f1, f2, cat, g, t1, t2, u;
   size_t bytes;
 };
-static BackboneWs backbone_ws(int nframes, int Btot, int H, int W, void* base, bool train = false, int x3 = 0) {
+static BackboneWs backbone_ws(const Arch& A, int Btot, int H, int W, void* base, bool train = false, int x3 = 0) {
   BackboneWs w;
-  const int h = H / 2, wd = W / 2;
+  const int h = H / 2, wd = W / 2, P = A.planes();
   size_t off = 0;
   auto carve = [&](int planes, int hh, int ww) {
     bin_act_t t;
@@ -169,13 +196,13 @@ static BackboneWs backbone_ws(int nframes, int Btot, int H, int W, void* base, b
     off = align_up(off + (size_t)Btot * t.planes * hh * ww * 16, 256);
     return t;
   };
-  w.x0 = carve((int)align_up(12 * nframes, kKC) / 8, h, wd);
-  w.f1 = carve(12, h, wd);
-  w.f2 = carve(12, h, wd);
-  w.cat = carve(12 * kD, h, wd);
-  w.g = carve(train ? 16 * kD : 16, h, wd);   // training keeps the growth maps of all 12 RDBs for the backward
-  w.t1 = carve(12, h, wd);
-  w.t2 = carve(12, h, wd);
+  w.x0 = carve((int)align_up(12 * A.nframes, kKC) / 8, h, wd);
+  w.f1 = carve(P, h, wd);
+  w.f2 = carve(P, h, wd);
+  w.cat = carve(P * A.d, h, wd);
+  w.g = carve(train ? 16 * A.d : 16, h, wd);   // training keeps the growth maps of all D RDBs for the backward
+  w.t1 = carve(P, h, wd);
+  w.t2 = carve(P, h, wd);
   w.u = carve(8, H, W);
   w.bytes = off;
   return w;
@@ -264,13 +291,13 @@ static std::vector<Band> plan_bands(int Btot, int h, int w) {
 static bool fuse_lff_enabled() { return options().fuse_lff; }
 // The first `nconv` growth convs of RDB i over one band (RDN.py:141-147): conv3x3 + ReLU of cat(x, g planes so far)
 // into g planes [g_plane0 + 4c, +4).  The forward runs them in run_rdb; the recomputing backward runs all four again.
-static int run_growth(const void* blob, const BackboneLayout& L, int i, const bin_act_t& xin, int x_plane0,
+static int run_growth(const Arch& A, const void* blob, const BackboneLayout& L, int i, const bin_act_t& xin, int x_plane0,
                       const bin_act_t& g, int g_plane0, int nconv, const Band& bd, cudaStream_t s, int x3) {
   const int base = 2 + i * (kCgrow + 1);
   const int h = xin.H;
   for (int c = 0; c < nconv; ++c) {
     bin_conv_args_t a = conv_args(blob, L.conv[base + c], x3);
-    a.in0 = xin; a.in0_plane0 = x_plane0; a.in0_planes = 12;
+    a.in0 = xin; a.in0_plane0 = x_plane0; a.in0_planes = A.planes();
     a.in1 = g; a.in1_plane0 = g_plane0; a.in1_planes = 4 * c;
     a.relu = 1; a.epilogue = BIN_EPI_P8;
     a.out = g; a.out_plane0 = g_plane0 + 4 * c;
@@ -285,24 +312,24 @@ static int run_growth(const void* blob, const BackboneLayout& L, int i, const bi
   return BIN_OK;
 }
 
-static int run_rdb(const void* blob, const BackboneLayout& L, int i, const bin_act_t& xin, int x_plane0,
+static int run_rdb(const Arch& A, const void* blob, const BackboneLayout& L, int i, const bin_act_t& xin, int x_plane0,
                    const bin_act_t& g, const bin_act_t& out, int out_plane0, const std::vector<Band>& bands,
                    cudaStream_t s, int g_plane0 = 0, int x3 = 0, bool keep_growth = false) {
   const int base = 2 + i * (kCgrow + 1);
   const bool fuse = !x3 && !keep_growth && fuse_lff_enabled();
   for (const Band& bd : bands) {
-    BIN_TRY(run_growth(blob, L, i, xin, x_plane0, g, g_plane0, fuse ? kCgrow - 1 : kCgrow, bd, s, x3));
+    BIN_TRY(run_growth(A, blob, L, i, xin, x_plane0, g, g_plane0, fuse ? kCgrow - 1 : kCgrow, bd, s, x3));
     if (fuse) {
       const ConvSpec& c3 = L.conv[base + kCgrow - 1];
       const ConvSpec& lf = L.conv[base + kCgrow];
-      BIN_TRY(launch_rdb_tail(xin, x_plane0, g, g_plane0, (const uint8_t*)blob + c3.w_off,
+      BIN_TRY(launch_rdb_tail(A.g0, xin, x_plane0, g, g_plane0, (const uint8_t*)blob + c3.w_off,
                               (const float*)((const uint8_t*)blob + c3.b_off), (const uint8_t*)blob + lf.w_off,
                               (const float*)((const uint8_t*)blob + lf.b_off), out, out_plane0, bd.b0, bd.nb, bd.y0,
                               bd.y1 - bd.y0, s, options().zigzag));
       continue;
     }
     bin_conv_args_t a = conv_args(blob, L.conv[base + kCgrow], x3);
-    a.in0 = xin; a.in0_plane0 = x_plane0; a.in0_planes = 12;
+    a.in0 = xin; a.in0_plane0 = x_plane0; a.in0_planes = A.planes();
     a.in1 = g; a.in1_plane0 = g_plane0; a.in1_planes = 16;
     a.epilogue = BIN_EPI_P8;
     a.out = out; a.out_plane0 = out_plane0;
@@ -313,17 +340,20 @@ static int run_rdb(const void* blob, const BackboneLayout& L, int i, const bin_a
   return BIN_OK;
 }
 
-static int run_backbone(int nframes, const void* blob, const bin_frames_t& fr, int H, int W, void* workspace,
+static int run_backbone(int arch, const void* blob, const bin_frames_t& fr, int H, int W, void* workspace,
                         size_t workspace_bytes, cudaStream_t s, bool train = false, int x3 = 0) {
-  if (!valid_nframes(nframes) || fr.nframes != nframes) return fail(BIN_ERR_ARG, "backbone: nframes must be 2, 3 or 5");
+  Arch A;
+  BIN_TRY(arch_or_fail(arch, "backbone", A));
+  if (fr.nframes != A.nframes) return fail(BIN_ERR_ARG, "backbone: nframes must be 2, 3 or 5");
   if (fr.ncalls < 1 || fr.ncalls > BIN_MAX_CALLS || fr.Bc < 1) return fail(BIN_ERR_ARG, "backbone: bad call table");
   if ((H & 1) || (W & 1) || H < 2 || W < 2) return fail(BIN_ERR_ARG, "backbone: H and W must be even (RDN.py:123-128)");
   const int Btot = fr.ncalls * fr.Bc;
   if (train && x3) return fail(BIN_ERR_UNSUPPORTED, "backbone: training runs in the fp16 mode only");
-  const BackboneLayout L = backbone_layout(nframes, x3);
-  const BackboneWs ws = backbone_ws(nframes, Btot, H, W, workspace, train, x3);
+  const BackboneLayout L = backbone_layout(A, x3);
+  const BackboneWs ws = backbone_ws(A, Btot, H, W, workspace, train, x3);
   if (ws.bytes > workspace_bytes) return fail(BIN_ERR_WORKSPACE, "backbone: workspace too small");
   if ((reinterpret_cast<uintptr_t>(workspace) & 255) != 0) return fail(BIN_ERR_ARG, "backbone: workspace must be 256-byte aligned");
+  const int P = A.planes(), nc = A.nconv();
 
   BIN_TRY(launch_pack_frames(fr, H, W, ws.x0, s, x3));                           // RDN.py:211
   {
@@ -333,32 +363,32 @@ static int run_backbone(int nframes, const void* blob, const bin_frames_t& fr, i
   }
   {
     bin_conv_args_t a = conv_args(blob, L.conv[1], x3);                              // SFENet2 (RDN.py:213)
-    a.in0 = ws.f1; a.in0_planes = 12; a.epilogue = BIN_EPI_P8; a.out = ws.f2;
+    a.in0 = ws.f1; a.in0_planes = P; a.epilogue = BIN_EPI_P8; a.out = ws.f2;
     BIN_TRY(launch_conv(a, s));
   }
   const std::vector<Band> bands = plan_bands(Btot, H / 2, W / 2);
-  for (int i = 0; i < kD; ++i) {                                                 // RDN.py:215-217
+  for (int i = 0; i < A.d; ++i) {                                                // RDN.py:215-217
     const int gp0 = train ? 16 * i : 0;
-    if (i == 0) BIN_TRY(run_rdb(blob, L, i, ws.f2, 0, ws.g, ws.cat, 0, bands, s, gp0, x3, train));
-    else BIN_TRY(run_rdb(blob, L, i, ws.cat, 12 * (i - 1), ws.g, ws.cat, 12 * i, bands, s, gp0, x3, train));
+    if (i == 0) BIN_TRY(run_rdb(A, blob, L, i, ws.f2, 0, ws.g, ws.cat, 0, bands, s, gp0, x3, train));
+    else BIN_TRY(run_rdb(A, blob, L, i, ws.cat, P * (i - 1), ws.g, ws.cat, P * i, bands, s, gp0, x3, train));
   }
   {
-    bin_conv_args_t a = conv_args(blob, L.conv[62], x3);                             // GFF.0 on the 1152-ch concat (RDN.py:218)
-    a.in0 = ws.cat; a.in0_planes = 12 * kD; a.epilogue = BIN_EPI_P8; a.out = ws.t1;
+    bin_conv_args_t a = conv_args(blob, L.conv[nc - 4], x3);                         // GFF.0 on the D*G0-ch concat (RDN.py:218)
+    a.in0 = ws.cat; a.in0_planes = P * A.d; a.epilogue = BIN_EPI_P8; a.out = ws.t1;
     BIN_TRY(launch_conv(a, s));
   }
   {
-    bin_conv_args_t a = conv_args(blob, L.conv[63], x3);                             // GFF.1, x += f__1 (RDN.py:219)
-    a.in0 = ws.t1; a.in0_planes = 12; a.epilogue = BIN_EPI_P8; a.out = ws.t2; a.res = ws.f1;
+    bin_conv_args_t a = conv_args(blob, L.conv[nc - 3], x3);                         // GFF.1, x += f__1 (RDN.py:219)
+    a.in0 = ws.t1; a.in0_planes = P; a.epilogue = BIN_EPI_P8; a.out = ws.t2; a.res = ws.f1;
     BIN_TRY(launch_conv(a, s));
   }
   {
-    bin_conv_args_t a = conv_args(blob, L.conv[64], x3);                             // UPNet.0 + PixelShuffle (RDN.py:205-206)
-    a.in0 = ws.t2; a.in0_planes = 12; a.epilogue = BIN_EPI_PIXSHUF; a.out = ws.u;
+    bin_conv_args_t a = conv_args(blob, L.conv[nc - 2], x3);                         // UPNet.0 + PixelShuffle (RDN.py:205-206)
+    a.in0 = ws.t2; a.in0_planes = P; a.epilogue = BIN_EPI_PIXSHUF; a.out = ws.u;
     BIN_TRY(launch_conv(a, s));
   }
   {
-    bin_conv_args_t a = conv_args(blob, L.conv[65], x3);                             // UPNet.2 + mean(frames) (RDN.py:207,221)
+    bin_conv_args_t a = conv_args(blob, L.conv[nc - 1], x3);                         // UPNet.2 + mean(frames) (RDN.py:207,221)
     a.in0 = ws.u; a.in0_planes = 8; a.epilogue = BIN_EPI_FINAL; a.fr = fr;
     BIN_TRY(launch_conv(a, s));
   }
@@ -368,7 +398,7 @@ static int run_backbone(int nframes, const void* blob, const bin_frames_t& fr, i
 // ------------------------------------------------------------------ backward of one backbone
 // Data gradients reuse conv_igemm_kernel: for a stride-1 / pad k/2 conv, dX = conv(dY, V) with
 // V[ci][co][ky][kx] = W[co][ci][k-1-ky][k-1-kx] (packed by launch_pack_weight_t, Cout' padded to a
-// multiple of 96 and clipped by store_planes).  Gradients are fp16 P8 tensors scaled by *scale (loss
+// multiple of 96 and clipped by store_planes; at G0 = 64 the G0-row parts run as 96-row launches that store 8 planes).  Gradients are fp16 P8 tensors scaled by *scale (loss
 // scaling, a device scalar) and un-scaled when they leave the backbone (frame grads, dW, db).
 int launch_pack_weight_t(const float* w, int cout, int cin, int ks, int row0, int nrows, int cout_pad_t, int cin_pad_t,
                          void* packed, cudaStream_t s);
@@ -400,8 +430,8 @@ struct BackboneLayoutT {
   TSpec g[BIN_BACKBONE_NCONV];      // growth part (RDB convs c>=1 and LFF); nrows = 0 if absent
   size_t zero_bias_off, bytes;
 };
-static BackboneLayoutT backbone_layout_t(int nframes) {
-  const BackboneLayout L = backbone_layout(nframes);
+static BackboneLayoutT backbone_layout_t(const Arch& A) {
+  const BackboneLayout L = backbone_layout(A);
   BackboneLayoutT T;
   size_t off = 0;
   auto mk = [&](int conv, int row0, int nrows) {
@@ -413,18 +443,18 @@ static BackboneLayoutT backbone_layout_t(int nframes) {
     if (nrows > 0) off = align_up(off + (size_t)t.cout_pad_t * t.cin_pad_t * t.ks * t.ks * sizeof(__half), 256);
     return t;
   };
-  for (int i = 0; i < BIN_BACKBONE_NCONV; ++i) {
+  for (int i = 0; i < A.nconv(); ++i) {
     const ConvSpec& c = L.conv[i];
-    const bool in_rdb = i >= 2 && i < 2 + kD * (kCgrow + 1);
+    const bool in_rdb = i >= 2 && i < 2 + A.d * (kCgrow + 1);
     if (in_rdb) {
-      T.x[i] = mk(i, 0, kG0);
-      T.g[i] = mk(i, kG0, c.cin - kG0);          // 0 rows for conv 0 of each RDB
+      T.x[i] = mk(i, 0, A.g0);
+      T.g[i] = mk(i, A.g0, c.cin - A.g0);        // 0 rows for conv 0 of each RDB
     } else {
       T.x[i] = mk(i, 0, c.cin);
       T.g[i] = mk(i, 0, 0);
     }
   }
-  T.zero_bias_off = off;
+  T.zero_bias_off = off;                     // zero bias of the widest data-gradient launch, GFF.0's D*G0 <= 1152 rows
   off = align_up(off + 1152 * sizeof(float), 256);
   T.bytes = off;
   return T;
@@ -442,9 +472,9 @@ static size_t bias_partial_bytes(int Btot, int H, int W) {
   const size_t a = bias_grad_partial_floats(Btot, H * W, 3), b = bias_grad_partial_floats(Btot, (H / 2) * (W / 2), 256);
   return (a > b ? a : b) * sizeof(float);
 }
-static GradWs grad_ws(int nframes, int Btot, int H, int W, void* base) {
+static GradWs grad_ws(const Arch& A, int Btot, int H, int W, void* base) {
   GradWs w;
-  const int h = H / 2, wd = W / 2;
+  const int h = H / 2, wd = W / 2, P = A.planes();
   size_t off = 0;
   auto carve = [&](int planes, int hh, int ww) {
     bin_act_t t;
@@ -456,12 +486,12 @@ static GradWs grad_ws(int nframes, int Btot, int H, int W, void* base) {
   w.dout16 = carve(4, H, W);
   w.du = carve(8, H, W);
   w.dup0 = carve(32, h, wd);
-  w.dt2 = carve(12, h, wd);
-  w.dt1 = carve(12, h, wd);
-  w.dcat = carve(12 * kD, h, wd);
-  w.df2 = carve(12, h, wd);
+  w.dt2 = carve(P, h, wd);
+  w.dt1 = carve(P, h, wd);
+  w.dcat = carve(P * A.d, h, wd);
+  w.df2 = carve(P, h, wd);
   w.dg = carve(16, h, wd);
-  w.dx0 = carve((int)align_up(12 * nframes, kKC) / 8, h, wd);
+  w.dx0 = carve((int)align_up(12 * A.nframes, kKC) / 8, h, wd);
   w.wg_partial = base ? (float*)((uint8_t*)base + off) : nullptr;
   const size_t wgb = wgrad_partial_bytes(), bb = bias_partial_bytes(Btot, H, W);
   w.wg_partial_floats = (wgb > bb ? wgb : bb) / sizeof(float);
@@ -471,11 +501,11 @@ static GradWs grad_ws(int nframes, int Btot, int H, int W, void* base) {
 }
 
 struct GradParamLayout { size_t w[BIN_BACKBONE_NCONV], b[BIN_BACKBONE_NCONV], floats; };
-static GradParamLayout grad_param_layout(int nframes) {
-  const BackboneLayout L = backbone_layout(nframes);
+static GradParamLayout grad_param_layout(const Arch& A) {
+  const BackboneLayout L = backbone_layout(A);
   GradParamLayout g;
   size_t off = 0;
-  for (int i = 0; i < BIN_BACKBONE_NCONV; ++i) {
+  for (int i = 0; i < A.nconv(); ++i) {
     g.w[i] = off; off += (size_t)L.conv[i].cout * L.conv[i].cin * L.conv[i].ks * L.conv[i].ks;
     g.b[i] = off; off += (size_t)L.conv[i].cout;
   }
@@ -484,30 +514,33 @@ static GradParamLayout grad_param_layout(int nframes) {
 }
 
 // act_ws holds the forward's activations.  recompute_blob == NULL: the saving layout of bin_backbone_fwd_train, with the
-// growth maps of all 12 RDBs (its size is the caller's; act_ws_bytes is not checked).  Otherwise: the inference layout
+// growth maps of all D RDBs (its size is the caller's; act_ws_bytes is not checked).  Otherwise: the inference layout
 // that bin_backbone_fwd left, checked against act_ws_bytes; before RDB i's backward its four growth convs are re-run
 // from cat[i-1] (f2 for RDB 0) with the forward weights in recompute_blob, into growth planes 0..15.  Same inputs, same
 // weights and the same launches as the saving forward, so the rebuilt maps have the same bits, and every launch of the
 // backward reads the same operands in both layouts.
 //
-// need (host, 2 * BIN_BACKBONE_NCONV bytes, weight then bias of each conv in grad_param_layout order; NULL = all) and the
+// need (host, 2 * A.nconv() bytes, weight then bias of each conv in grad_param_layout order; NULL = all) and the
 // NULL entries of dfr.frame say which gradients the caller reads.  Conv k's input depends on every conv with a lower
 // index, so the gradient with respect to it is needed iff a frame or some tensor of a lower conv needs one: U[k] below.
 // The backward walks the convs from the top; a weight or bias gradient nobody needs is not launched, a data gradient
 // runs only where U holds at the input it feeds, and the walk stops once U is false.  Whatever runs is the launch the full
 // backward makes, on the same operands and in the same order, so every gradient that is kept has the same bits.
-static int run_backbone_bwd(int nframes, const void* blob_t, const bin_frames_t& dout, const bin_frames_t& dfr, int H,
+static int run_backbone_bwd(int arch, const void* blob_t, const bin_frames_t& dout, const bin_frames_t& dfr, int H,
                             int W, const void* act_ws, size_t act_ws_bytes, const void* recompute_blob, void* gws_ptr,
                             size_t gws_bytes, float* gparams, const float* scale, cudaStream_t s, int flags,
                             const unsigned char* need) {
-  if (!valid_nframes(nframes) || dfr.nframes != nframes) return fail(BIN_ERR_ARG, "backbone_bwd: nframes must be 2, 3 or 5");
+  Arch A;
+  BIN_TRY(arch_or_fail(arch, "backbone_bwd", A));
+  if (dfr.nframes != A.nframes) return fail(BIN_ERR_ARG, "backbone_bwd: nframes must be 2, 3 or 5");
   if (flags & ~BIN_DETERMINISTIC) return fail(BIN_ERR_ARG, "backbone_bwd: unknown flags");
   const bool det = flags & BIN_DETERMINISTIC;
   if (dout.ncalls != dfr.ncalls || dout.Bc != dfr.Bc || dout.ncalls < 1 || dout.ncalls > BIN_MAX_CALLS)
     return fail(BIN_ERR_ARG, "backbone_bwd: bad call tables");
+  const int nc = A.nconv(), P = A.planes(), nframes = A.nframes;
   bool need_w[BIN_BACKBONE_NCONV], need_b[BIN_BACKBONE_NCONV], U[BIN_BACKBONE_NCONV + 1];
   bool any_param = false;
-  for (int i = 0; i < BIN_BACKBONE_NCONV; ++i) {
+  for (int i = 0; i < nc; ++i) {
     need_w[i] = !need || need[2 * i];
     need_b[i] = !need || need[2 * i + 1];
     any_param = any_param || need_w[i] || need_b[i];
@@ -516,23 +549,23 @@ static int run_backbone_bwd(int nframes, const void* blob_t, const bin_frames_t&
   U[0] = false;                                                // U[0]: some frame of some call wants its gradient
   for (int k = 0; k < dfr.ncalls; ++k)
     for (int f = 0; f < nframes; ++f) U[0] = U[0] || dfr.frame[k][f] != nullptr;
-  for (int i = 0; i < BIN_BACKBONE_NCONV; ++i) U[i + 1] = U[i] || need_w[i] || need_b[i];
+  for (int i = 0; i < nc; ++i) U[i + 1] = U[i] || need_w[i] || need_b[i];
   const int Btot = dout.ncalls * dout.Bc;
   const bool recompute = recompute_blob != nullptr;
-  const BackboneWs ws = backbone_ws(nframes, Btot, H, W, const_cast<void*>(act_ws), !recompute);
+  const BackboneWs ws = backbone_ws(A, Btot, H, W, const_cast<void*>(act_ws), !recompute);
   if (recompute && ws.bytes > act_ws_bytes) return fail(BIN_ERR_WORKSPACE, "backbone_bwd: forward workspace too small");
   if (recompute && (reinterpret_cast<uintptr_t>(act_ws) & 255) != 0)
     return fail(BIN_ERR_ARG, "backbone_bwd: forward workspace must be 256-byte aligned");
-  const BackboneLayout L = backbone_layout(nframes);
-  const BackboneLayoutT T = backbone_layout_t(nframes);
-  const GradParamLayout GP = grad_param_layout(nframes);
-  const GradWs gw = grad_ws(nframes, Btot, H, W, gws_ptr);
+  const BackboneLayout L = backbone_layout(A);
+  const BackboneLayoutT T = backbone_layout_t(A);
+  const GradParamLayout GP = grad_param_layout(A);
+  const GradWs gw = grad_ws(A, Btot, H, W, gws_ptr);
   if (gw.bytes > gws_bytes) return fail(BIN_ERR_WORKSPACE, "backbone_bwd: gradient workspace too small");
   // Deterministic bias partials of every conv must fit the slab region before the first launch (grad_ws sizes it from
   // bias_partial_bytes; this keeps that invariant explicit should a conv with more partials ever be added).
   if (det)
-    for (int i = 0; i < BIN_BACKBONE_NCONV; ++i) {
-      const int hw = i == BIN_BACKBONE_NCONV - 1 ? H * W : (H / 2) * (W / 2);   // UPNet.2 runs at full resolution
+    for (int i = 0; i < nc; ++i) {
+      const int hw = i == nc - 1 ? H * W : (H / 2) * (W / 2);   // UPNet.2 runs at full resolution
       if (bias_grad_partial_floats(Btot, hw, L.conv[i].cout) > gw.wg_partial_floats)
         return fail(BIN_ERR_WORKSPACE, "backbone_bwd: deterministic bias partials do not fit the gradient workspace");
     }
@@ -564,60 +597,61 @@ static int run_backbone_bwd(int nframes, const void* blob_t, const bin_frames_t&
   };
   const bin_act_t none = {nullptr, 0, 0, 0, 0};
 
-  if (!U[BIN_BACKBONE_NCONV]) return BIN_OK;                                     // nothing asked for
+  if (!U[nc]) return BIN_OK;                                                     // nothing asked for
+  const int up2 = nc - 1, up0 = nc - 2, gff1 = nc - 3, gff0 = nc - 4;
   BIN_TRY(launch_grad_out_to_p8(dout, H, W, gw.dout16, scale, s));
-  BIN_TRY(wgrad(65, ws.u, 0, 8, none, 0, 0, gw.dout16, 0));                          // UPNet.2
-  if (!U[65]) return BIN_OK;
-  BIN_TRY(dgrad(T.x[65], gw.dout16, 0, 4, gw.du, 0, 8, false));
+  BIN_TRY(wgrad(up2, ws.u, 0, 8, none, 0, 0, gw.dout16, 0));                         // UPNet.2
+  if (!U[up2]) return BIN_OK;
+  BIN_TRY(dgrad(T.x[up2], gw.dout16, 0, 4, gw.du, 0, 8, false));
   BIN_TRY(launch_pixel_unshuffle(gw.du, gw.dup0, s));                               // nn.PixelShuffle backward
-  BIN_TRY(wgrad(64, ws.t2, 0, 12, none, 0, 0, gw.dup0, 0));                          // UPNet.0
-  if (!U[64]) return BIN_OK;
-  BIN_TRY(dgrad(T.x[64], gw.dup0, 0, 32, gw.dt2, 0, 12, false));
-  BIN_TRY(wgrad(63, ws.t1, 0, 12, none, 0, 0, gw.dt2, 0));                           // GFF.1
-  if (!U[63]) return BIN_OK;
-  BIN_TRY(dgrad(T.x[63], gw.dt2, 0, 12, gw.dt1, 0, 12, false));                      // dt2 doubles as d f__1 (RDN.py:219)
-  BIN_TRY(wgrad(62, ws.cat, 0, 12 * kD, none, 0, 0, gw.dt1, 0));                     // GFF.0
-  if (!U[62]) return BIN_OK;
-  BIN_TRY(dgrad(T.x[62], gw.dt1, 0, 12, gw.dcat, 0, 12 * kD, false));
-  if (U[2]) BIN_CUDA_OK(cudaMemsetAsync(gw.df2.ptr, 0, (size_t)Btot * 12 * (H / 2) * (W / 2) * 16, s));
+  BIN_TRY(wgrad(up0, ws.t2, 0, P, none, 0, 0, gw.dup0, 0));                          // UPNet.0
+  if (!U[up0]) return BIN_OK;
+  BIN_TRY(dgrad(T.x[up0], gw.dup0, 0, 32, gw.dt2, 0, P, false));
+  BIN_TRY(wgrad(gff1, ws.t1, 0, P, none, 0, 0, gw.dt2, 0));                          // GFF.1
+  if (!U[gff1]) return BIN_OK;
+  BIN_TRY(dgrad(T.x[gff1], gw.dt2, 0, P, gw.dt1, 0, P, false));                      // dt2 doubles as d f__1 (RDN.py:219)
+  BIN_TRY(wgrad(gff0, ws.cat, 0, P * A.d, none, 0, 0, gw.dt1, 0));                   // GFF.0
+  if (!U[gff0]) return BIN_OK;
+  BIN_TRY(dgrad(T.x[gff0], gw.dt1, 0, P, gw.dcat, 0, P * A.d, false));
+  if (U[2]) BIN_CUDA_OK(cudaMemsetAsync(gw.df2.ptr, 0, (size_t)Btot * P * (H / 2) * (W / 2) * 16, s));
   const std::vector<Band> bands = recompute ? plan_bands(Btot, H / 2, W / 2) : std::vector<Band>();
   // Reaching RDB i means U holds at its output (base + 5).  Inside it, the growth-map gradients dg feed the growth convs
   // below the current one and the RDB input, so they are needed while U holds at the current conv; the parts that land
   // in the input gradient dxin (residual, x rows of every conv) are needed iff U holds at the RDB input.
-  for (int i = kD - 1; i >= 0; --i) {
+  for (int i = A.d - 1; i >= 0; --i) {
     const int base = 2 + i * (kCgrow + 1);
     const bin_act_t& xin = i == 0 ? ws.f2 : ws.cat;           // forward input of RDB i
-    const int xin_p = i == 0 ? 0 : 12 * (i - 1);
+    const int xin_p = i == 0 ? 0 : P * (i - 1);
     const bin_act_t& dxin = i == 0 ? gw.df2 : gw.dcat;        // its gradient (accumulated)
-    const int dxin_p = i == 0 ? 0 : 12 * (i - 1);
-    const int dxo_p = 12 * i;                                 // d x_{i+1}, complete at this point
+    const int dxin_p = i == 0 ? 0 : P * (i - 1);
+    const int dxo_p = P * i;                                  // d x_{i+1}, complete at this point
     const int gp0 = recompute ? 0 : 16 * i;                   // growth maps of RDB i
     const bool dx_in = U[base];
     // the growth maps are read by the LFF's wgrad and, below it, by the growth-map dgrads and ReLU masks; the LFF's
     // bias gradient alone reads only dcat
     if (need_w[base + kCgrow] || U[base + kCgrow])
-      for (const Band& bd : bands) BIN_TRY(run_growth(recompute_blob, L, i, xin, xin_p, ws.g, 0, kCgrow, bd, s, 0));
-    BIN_TRY(wgrad(base + kCgrow, xin, xin_p, 12, ws.g, gp0, 16, gw.dcat, dxo_p));                     // LFF
+      for (const Band& bd : bands) BIN_TRY(run_growth(A, recompute_blob, L, i, xin, xin_p, ws.g, 0, kCgrow, bd, s, 0));
+    BIN_TRY(wgrad(base + kCgrow, xin, xin_p, P, ws.g, gp0, 16, gw.dcat, dxo_p));                      // LFF
     if (!U[base + kCgrow]) return BIN_OK;
     if (dx_in) {
-      BIN_TRY(launch_p8_add(dxin, dxin_p, gw.dcat, dxo_p, 12, s));                                    // residual (RDN.py:165)
-      BIN_TRY(dgrad(T.x[base + kCgrow], gw.dcat, dxo_p, 12, dxin, dxin_p, 12, true));
+      BIN_TRY(launch_p8_add(dxin, dxin_p, gw.dcat, dxo_p, P, s));                                     // residual (RDN.py:165)
+      BIN_TRY(dgrad(T.x[base + kCgrow], gw.dcat, dxo_p, P, dxin, dxin_p, P, true));
     }
-    BIN_TRY(dgrad(T.g[base + kCgrow], gw.dcat, dxo_p, 12, gw.dg, 0, 16, false));
+    BIN_TRY(dgrad(T.g[base + kCgrow], gw.dcat, dxo_p, P, gw.dg, 0, 16, false));
     for (int c = kCgrow - 1; c >= 0; --c) {
       BIN_TRY(launch_relu_mask(gw.dg, 4 * c, ws.g, gp0 + 4 * c, 4, s));                               // RDN.py:142
-      BIN_TRY(wgrad(base + c, xin, xin_p, 12, ws.g, gp0, 4 * c, gw.dg, 4 * c));
+      BIN_TRY(wgrad(base + c, xin, xin_p, P, ws.g, gp0, 4 * c, gw.dg, 4 * c));
       if (!U[base + c]) return BIN_OK;
-      if (dx_in) BIN_TRY(dgrad(T.x[base + c], gw.dg, 4 * c, 4, dxin, dxin_p, 12, true));
+      if (dx_in) BIN_TRY(dgrad(T.x[base + c], gw.dg, 4 * c, 4, dxin, dxin_p, P, true));
       if (c > 0) BIN_TRY(dgrad(T.g[base + c], gw.dg, 4 * c, 4, gw.dg, 0, 4 * c, true));
     }
   }
-  BIN_TRY(wgrad(1, ws.f1, 0, 12, none, 0, 0, gw.df2, 0));                            // SFENet2
+  BIN_TRY(wgrad(1, ws.f1, 0, P, none, 0, 0, gw.df2, 0));                             // SFENet2
   if (!U[1]) return BIN_OK;
-  BIN_TRY(dgrad(T.x[1], gw.df2, 0, 12, gw.dt2, 0, 12, true));                        // d f__1 complete
+  BIN_TRY(dgrad(T.x[1], gw.df2, 0, P, gw.dt2, 0, P, true));                          // d f__1 complete
   BIN_TRY(wgrad(0, ws.x0, 0, ws.x0.planes, none, 0, 0, gw.dt2, 0));                  // SFENet1
   if (!U[0]) return BIN_OK;
-  BIN_TRY(dgrad(T.x[0], gw.dt2, 0, 12, gw.dx0, 0, gw.dx0.planes, false));
+  BIN_TRY(dgrad(T.x[0], gw.dt2, 0, P, gw.dx0, 0, gw.dx0.planes, false));
   return launch_unpack_frames_grad(gw.dx0, dout, dfr, H, W, scale, s);
 }
 
@@ -738,16 +772,26 @@ int bin_convlstm_bwd(const float* x, const float* c_prev, const float* h_prev, c
                              0, s);
 }
 
-size_t bin_backbone_packed_bytes(int nframes) { return valid_nframes(nframes) ? backbone_layout(nframes).bytes : 0; }
+int bin_backbone_nconv(int arch) {
+  Arch A;
+  return decode_arch(arch, A) ? A.nconv() : -1;
+}
 
-// all 66 weights + 66 biases of a backbone in ONE launch
-static int pack_backbone(int nframes, const float* const* w_host, const float* const* b_host, void* blob, int x3,
+size_t bin_backbone_packed_bytes(int arch) {
+  Arch A;
+  return decode_arch(arch, A) ? backbone_layout(A).bytes : 0;
+}
+
+// all weights + biases of a backbone in ONE launch
+static int pack_backbone(int arch, const float* const* w_host, const float* const* b_host, void* blob, int x3,
                          cudaStream_t s) {
+  Arch A;
+  BIN_TRY(arch_or_fail(arch, "backbone_pack", A));
   if (!w_host || !b_host || !blob) return fail(BIN_ERR_ARG, "backbone_pack: null argument");
-  const BackboneLayout L = backbone_layout(nframes, x3);
+  const BackboneLayout L = backbone_layout(A, x3);
   void* hb = pack_batch_new();
   int rc = BIN_OK;
-  for (int i = 0; i < BIN_BACKBONE_NCONV && rc == BIN_OK; ++i) {
+  for (int i = 0; i < A.nconv() && rc == BIN_OK; ++i) {
     const ConvSpec& c = L.conv[i];
     rc = pack_batch_add_weight(hb, w_host[i], c.cout, c.cin, c.ks, c.cout_pad, c.cin_pad, BIN_CONV_DEFAULT,
                                (uint8_t*)blob + c.w_off, x3);
@@ -757,31 +801,35 @@ static int pack_backbone(int nframes, const float* const* w_host, const float* c
   return rc != BIN_OK ? rc : rl;
 }
 
-int bin_backbone_pack(int nframes, const float* const* w_host, const float* const* b_host, void* blob,
+int bin_backbone_pack(int arch, const float* const* w_host, const float* const* b_host, void* blob,
                       bin_stream_t s) {
-  if (!valid_nframes(nframes)) return fail(BIN_ERR_ARG, "backbone_pack: nframes must be 2, 3 or 5");
-  return pack_backbone(nframes, w_host, b_host, blob, 0, (cudaStream_t)s);
+  return pack_backbone(arch, w_host, b_host, blob, 0, (cudaStream_t)s);
 }
 
-size_t bin_backbone_workspace_bytes(int nframes, int Btot, int H, int W) {
-  return valid_nframes(nframes) ? backbone_ws(nframes, Btot, H, W, nullptr).bytes : 0;
+size_t bin_backbone_workspace_bytes(int arch, int Btot, int H, int W) {
+  Arch A;
+  return decode_arch(arch, A) ? backbone_ws(A, Btot, H, W, nullptr).bytes : 0;
 }
 
-int bin_backbone_fwd(int nframes, const void* blob, const bin_frames_t* fr, int H, int W, void* workspace,
+int bin_backbone_fwd(int arch, const void* blob, const bin_frames_t* fr, int H, int W, void* workspace,
                      size_t workspace_bytes, bin_stream_t s) {
   if (!fr || !blob) return fail(BIN_ERR_ARG, "backbone_fwd: null argument");
-  return run_backbone(nframes, blob, *fr, H, W, workspace, workspace_bytes, (cudaStream_t)s);
+  return run_backbone(arch, blob, *fr, H, W, workspace, workspace_bytes, (cudaStream_t)s);
 }
 
-size_t bin_backbone_packed_t_bytes(int nframes) { return valid_nframes(nframes) ? backbone_layout_t(nframes).bytes : 0; }
+size_t bin_backbone_packed_t_bytes(int arch) {
+  Arch A;
+  return decode_arch(arch, A) ? backbone_layout_t(A).bytes : 0;
+}
 
-int bin_backbone_pack_t(int nframes, const float* const* w_host, void* blob_t, bin_stream_t s) {
-  if (!valid_nframes(nframes)) return fail(BIN_ERR_ARG, "backbone_pack_t: nframes must be 2, 3 or 5");
-  const BackboneLayout L = backbone_layout(nframes);
-  const BackboneLayoutT T = backbone_layout_t(nframes);
+int bin_backbone_pack_t(int arch, const float* const* w_host, void* blob_t, bin_stream_t s) {
+  Arch A;
+  BIN_TRY(arch_or_fail(arch, "backbone_pack_t", A));
+  const BackboneLayout L = backbone_layout(A);
+  const BackboneLayoutT T = backbone_layout_t(A);
   void* hb = pack_batch_new();
   int rc = BIN_OK;
-  for (int i = 0; i < BIN_BACKBONE_NCONV && rc == BIN_OK; ++i) {
+  for (int i = 0; i < A.nconv() && rc == BIN_OK; ++i) {
     const ConvSpec& c = L.conv[i];
     const TSpec* parts[2] = {&T.x[i], &T.g[i]};
     for (const TSpec* t : parts) {
@@ -797,57 +845,62 @@ int bin_backbone_pack_t(int nframes, const float* const* w_host, void* blob_t, b
   return BIN_OK;
 }
 
-size_t bin_backbone_train_workspace_bytes(int nframes, int Btot, int H, int W) {
-  return valid_nframes(nframes) ? backbone_ws(nframes, Btot, H, W, nullptr, true).bytes : 0;
+size_t bin_backbone_train_workspace_bytes(int arch, int Btot, int H, int W) {
+  Arch A;
+  return decode_arch(arch, A) ? backbone_ws(A, Btot, H, W, nullptr, true).bytes : 0;
 }
-int bin_backbone_fwd_train(int nframes, const void* blob, const bin_frames_t* fr, int H, int W, void* save_ws,
+int bin_backbone_fwd_train(int arch, const void* blob, const bin_frames_t* fr, int H, int W, void* save_ws,
                            size_t save_ws_bytes, bin_stream_t s) {
   if (!fr || !blob) return fail(BIN_ERR_ARG, "backbone_fwd_train: null argument");
-  return run_backbone(nframes, blob, *fr, H, W, save_ws, save_ws_bytes, (cudaStream_t)s, true);
+  return run_backbone(arch, blob, *fr, H, W, save_ws, save_ws_bytes, (cudaStream_t)s, true);
 }
-size_t bin_backbone_grad_workspace_bytes(int nframes, int Btot, int H, int W) {
-  return valid_nframes(nframes) ? grad_ws(nframes, Btot, H, W, nullptr).bytes : 0;
+size_t bin_backbone_grad_workspace_bytes(int arch, int Btot, int H, int W) {
+  Arch A;
+  return decode_arch(arch, A) ? grad_ws(A, Btot, H, W, nullptr).bytes : 0;
 }
-size_t bin_backbone_grad_param_floats(int nframes) { return valid_nframes(nframes) ? grad_param_layout(nframes).floats : 0; }
-int bin_backbone_bwd_masked(int nframes, const void* blob_t, const bin_frames_t* dout, const bin_frames_t* dframes, int H,
+size_t bin_backbone_grad_param_floats(int arch) {
+  Arch A;
+  return decode_arch(arch, A) ? grad_param_layout(A).floats : 0;
+}
+int bin_backbone_bwd_masked(int arch, const void* blob_t, const bin_frames_t* dout, const bin_frames_t* dframes, int H,
                             int W, const void* save_ws, void* grad_ws_ptr, size_t grad_ws_bytes, float* grad_params,
                             const float* scale_dev, int flags, const unsigned char* need_host, bin_stream_t s) {
   if (!blob_t || !dout || !dframes || !save_ws || !scale_dev) return fail(BIN_ERR_ARG, "backbone_bwd: null argument");
-  return run_backbone_bwd(nframes, blob_t, *dout, *dframes, H, W, save_ws, 0, nullptr, grad_ws_ptr, grad_ws_bytes,
+  return run_backbone_bwd(arch, blob_t, *dout, *dframes, H, W, save_ws, 0, nullptr, grad_ws_ptr, grad_ws_bytes,
                           grad_params, scale_dev, (cudaStream_t)s, flags, need_host);
 }
-int bin_backbone_bwd_ex(int nframes, const void* blob_t, const bin_frames_t* dout, const bin_frames_t* dframes, int H,
+int bin_backbone_bwd_ex(int arch, const void* blob_t, const bin_frames_t* dout, const bin_frames_t* dframes, int H,
                         int W, const void* save_ws, void* grad_ws_ptr, size_t grad_ws_bytes, float* grad_params,
                         const float* scale_dev, int flags, bin_stream_t s) {
-  return bin_backbone_bwd_masked(nframes, blob_t, dout, dframes, H, W, save_ws, grad_ws_ptr, grad_ws_bytes, grad_params,
+  return bin_backbone_bwd_masked(arch, blob_t, dout, dframes, H, W, save_ws, grad_ws_ptr, grad_ws_bytes, grad_params,
                                  scale_dev, flags, nullptr, s);
 }
-int bin_backbone_bwd(int nframes, const void* blob_t, const bin_frames_t* dout, const bin_frames_t* dframes, int H, int W,
+int bin_backbone_bwd(int arch, const void* blob_t, const bin_frames_t* dout, const bin_frames_t* dframes, int H, int W,
                      const void* save_ws, void* grad_ws_ptr, size_t grad_ws_bytes, float* grad_params,
                      const float* scale_dev, bin_stream_t s) {
-  return bin_backbone_bwd_ex(nframes, blob_t, dout, dframes, H, W, save_ws, grad_ws_ptr, grad_ws_bytes, grad_params,
+  return bin_backbone_bwd_ex(arch, blob_t, dout, dframes, H, W, save_ws, grad_ws_ptr, grad_ws_bytes, grad_params,
                              scale_dev, 0, s);
 }
-int bin_backbone_bwd_recompute_masked(int nframes, const void* blob, const void* blob_t, const bin_frames_t* dout,
+int bin_backbone_bwd_recompute_masked(int arch, const void* blob, const void* blob_t, const bin_frames_t* dout,
                                       const bin_frames_t* dframes, int H, int W, const void* fwd_ws, size_t fwd_ws_bytes,
                                       void* grad_ws_ptr, size_t grad_ws_bytes, float* grad_params, const float* scale_dev,
                                       int flags, const unsigned char* need_host, bin_stream_t s) {
   if (!blob || !blob_t || !dout || !dframes || !fwd_ws || !scale_dev) return fail(BIN_ERR_ARG, "backbone_bwd: null argument");
-  return run_backbone_bwd(nframes, blob_t, *dout, *dframes, H, W, fwd_ws, fwd_ws_bytes, blob, grad_ws_ptr, grad_ws_bytes,
+  return run_backbone_bwd(arch, blob_t, *dout, *dframes, H, W, fwd_ws, fwd_ws_bytes, blob, grad_ws_ptr, grad_ws_bytes,
                           grad_params, scale_dev, (cudaStream_t)s, flags, need_host);
 }
-int bin_backbone_bwd_recompute_ex(int nframes, const void* blob, const void* blob_t, const bin_frames_t* dout,
+int bin_backbone_bwd_recompute_ex(int arch, const void* blob, const void* blob_t, const bin_frames_t* dout,
                                   const bin_frames_t* dframes, int H, int W, const void* fwd_ws, size_t fwd_ws_bytes,
                                   void* grad_ws_ptr, size_t grad_ws_bytes, float* grad_params, const float* scale_dev,
                                   int flags, bin_stream_t s) {
-  return bin_backbone_bwd_recompute_masked(nframes, blob, blob_t, dout, dframes, H, W, fwd_ws, fwd_ws_bytes, grad_ws_ptr,
+  return bin_backbone_bwd_recompute_masked(arch, blob, blob_t, dout, dframes, H, W, fwd_ws, fwd_ws_bytes, grad_ws_ptr,
                                            grad_ws_bytes, grad_params, scale_dev, flags, nullptr, s);
 }
-int bin_backbone_bwd_recompute(int nframes, const void* blob, const void* blob_t, const bin_frames_t* dout,
+int bin_backbone_bwd_recompute(int arch, const void* blob, const void* blob_t, const bin_frames_t* dout,
                                const bin_frames_t* dframes, int H, int W, const void* fwd_ws, size_t fwd_ws_bytes,
                                void* grad_ws_ptr, size_t grad_ws_bytes, float* grad_params, const float* scale_dev,
                                bin_stream_t s) {
-  return bin_backbone_bwd_recompute_ex(nframes, blob, blob_t, dout, dframes, H, W, fwd_ws, fwd_ws_bytes, grad_ws_ptr,
+  return bin_backbone_bwd_recompute_ex(arch, blob, blob_t, dout, dframes, H, W, fwd_ws, fwd_ws_bytes, grad_ws_ptr,
                                        grad_ws_bytes, grad_params, scale_dev, 0, s);
 }
 
@@ -857,10 +910,11 @@ int bin_grad_scale(const float* const* gouts_host, int n, size_t numel, float ta
   return launch_grad_scale(gouts_host, n, numel, target, scale_dev, (unsigned*)tmp4_dev, (cudaStream_t)s);
 }
 
-int bin_rdb_fwd(const void* blob, int nframes, int index, const float* x, float* y, int B, int h, int w,
+int bin_rdb_fwd(const void* blob, int arch, int index, const float* x, float* y, int B, int h, int w,
                 void* workspace, size_t workspace_bytes, bin_stream_t s) {
-  if (!valid_nframes(nframes) || index < 0 || index >= kD) return fail(BIN_ERR_ARG, "rdb_fwd: bad nframes/index");
-  const BackboneLayout L = backbone_layout(nframes);
+  Arch A;
+  if (!decode_arch(arch, A) || index < 0 || index >= A.d) return fail(BIN_ERR_ARG, "rdb_fwd: bad nframes/index");
+  const BackboneLayout L = backbone_layout(A);
   size_t off = 0;
   auto carve = [&](int planes) {
     bin_act_t t;
@@ -868,34 +922,37 @@ int bin_rdb_fwd(const void* blob, int nframes, int index, const float* x, float*
     off = align_up(off + (size_t)B * planes * h * w * 16, 256);
     return t;
   };
-  bin_act_t xin = carve(12), g = carve(16), out = carve(12);
+  bin_act_t xin = carve(A.planes()), g = carve(16), out = carve(A.planes());
   if (off > workspace_bytes) return fail(BIN_ERR_WORKSPACE, "rdb_fwd: workspace too small");
-  BIN_TRY(launch_nchw_to_p8(x, kG0, xin, 0, (cudaStream_t)s));
-  BIN_TRY(run_rdb(blob, L, index, xin, 0, g, out, 0, plan_bands(B, h, w), (cudaStream_t)s));
-  return launch_p8_to_nchw(out, 0, kG0, y, (cudaStream_t)s);
+  BIN_TRY(launch_nchw_to_p8(x, A.g0, xin, 0, (cudaStream_t)s));
+  BIN_TRY(run_rdb(A, blob, L, index, xin, 0, g, out, 0, plan_bands(B, h, w), (cudaStream_t)s));
+  return launch_p8_to_nchw(out, 0, A.g0, y, (cudaStream_t)s);
 }
 
 /* precision-parameterised twins (BIN_PREC_*) */
-size_t bin_backbone_packed_bytes_p(int nframes, int prec) { return valid_nframes(nframes) ? backbone_layout(nframes, prec ? 1 : 0).bytes : 0; }
-int bin_backbone_pack_p(int nframes, const float* const* w_host, const float* const* b_host, void* blob, int prec,
+size_t bin_backbone_packed_bytes_p(int arch, int prec) {
+  Arch A;
+  return decode_arch(arch, A) ? backbone_layout(A, prec ? 1 : 0).bytes : 0;
+}
+int bin_backbone_pack_p(int arch, const float* const* w_host, const float* const* b_host, void* blob, int prec,
                         bin_stream_t s) {
-  if (!valid_nframes(nframes)) return fail(BIN_ERR_ARG, "backbone_pack: nframes must be 2, 3 or 5");
-  return pack_backbone(nframes, w_host, b_host, blob, prec ? 1 : 0, (cudaStream_t)s);
+  return pack_backbone(arch, w_host, b_host, blob, prec ? 1 : 0, (cudaStream_t)s);
 }
-size_t bin_backbone_workspace_bytes_p(int nframes, int Btot, int H, int W, int prec) {
-  return valid_nframes(nframes) ? backbone_ws(nframes, Btot, H, W, nullptr, false, prec ? 1 : 0).bytes : 0;
+size_t bin_backbone_workspace_bytes_p(int arch, int Btot, int H, int W, int prec) {
+  Arch A;
+  return decode_arch(arch, A) ? backbone_ws(A, Btot, H, W, nullptr, false, prec ? 1 : 0).bytes : 0;
 }
-int bin_backbone_fwd_p(int nframes, const void* blob, const bin_frames_t* fr, int H, int W, void* workspace,
+int bin_backbone_fwd_p(int arch, const void* blob, const bin_frames_t* fr, int H, int W, void* workspace,
                        size_t workspace_bytes, int prec, bin_stream_t s) {
   if (!fr || !blob) return fail(BIN_ERR_ARG, "backbone_fwd: null argument");
-  return run_backbone(nframes, blob, *fr, H, W, workspace, workspace_bytes, (cudaStream_t)s, false, prec ? 1 : 0);
+  return run_backbone(arch, blob, *fr, H, W, workspace, workspace_bytes, (cudaStream_t)s, false, prec ? 1 : 0);
 }
 
 int bin_rdb_tail_fwd(const bin_act_t* x, int x_plane0, const bin_act_t* g, int g_plane0, const void* w_conv,
                      const float* b_conv, const void* w_lff, const float* b_lff, const bin_act_t* out, int out_plane0,
                      int b_begin, int b_count, int y_begin, int y_count, bin_stream_t s) {
   if (!x || !g || !out) return fail(BIN_ERR_ARG, "rdb_tail_fwd: null argument");
-  return launch_rdb_tail(*x, x_plane0, *g, g_plane0, w_conv, b_conv, w_lff, b_lff, *out, out_plane0, b_begin, b_count,
+  return launch_rdb_tail(96, *x, x_plane0, *g, g_plane0, w_conv, b_conv, w_lff, b_lff, *out, out_plane0, b_begin, b_count,
                          y_begin, y_count, (cudaStream_t)s);
 }
 int bin_adam_step(const bin_adam_tensor_t* table_dev, const int* chunk_prefix_dev, int ntensors, int nchunks, float lr,

@@ -572,6 +572,10 @@ static int launch_conv_t(const bin_conv_args_t& a, cudaStream_t s, bool reverse)
     if (a.ksize == 3 && a.cout_pad % 96 == 0) return launch_inst<96, 3, BIN_EPI_P8, false, X3>(a, s, reverse);
     if (a.ksize == 5 && a.cout_pad == 96) return launch_inst<96, 5, BIN_EPI_P8, false, X3>(a, s, reverse);
     if (a.ksize == 1 && a.cout_pad % 96 == 0) return launch_inst<96, 1, BIN_EPI_P8, false, X3>(a, s, reverse);
+    // G0 = 64 backbones: SFENet1 (5x5), SFENet2 and GFF.1 (3x3), GFF.0 and the LFF (1x1)
+    if (a.ksize == 3 && a.cout_pad == 64) return launch_inst<64, 3, BIN_EPI_P8, false, X3>(a, s, reverse);
+    if (a.ksize == 5 && a.cout_pad == 64) return launch_inst<64, 5, BIN_EPI_P8, false, X3>(a, s, reverse);
+    if (a.ksize == 1 && a.cout_pad == 64) return launch_inst<64, 1, BIN_EPI_P8, false, X3>(a, s, reverse);
   } else if (a.epilogue == BIN_EPI_PIXSHUF) {
     if (a.ksize == 3 && a.cout_pad == 256) return launch_inst<128, 3, BIN_EPI_PIXSHUF, false, X3>(a, s, reverse);
   } else if (a.epilogue == BIN_EPI_FINAL) {

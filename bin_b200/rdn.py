@@ -107,14 +107,25 @@ class RDB_Conv(nn.Module):
         raise BinB200Error("RDB_Conv is a parameter holder; call the enclosing RDB / backbone (fused kernels)")
 
 
+G0_CHOICES = (64, 96)    # the widths the reference builds: 64 by default (RDN.py:171), 96 in bin_stage4_lstm (:418)
+D_MAX = 12               # the shipped depth; the library's tables, masks and workspaces are sized for it
+
+
+def _check_arch(G0, D, C, G) -> None:
+    if G0 not in G0_CHOICES or not (isinstance(D, int) and 1 <= D <= D_MAX) or C != 4 or G != 32:
+        raise BinB200Error(f"bin_b200 backbones support G0 in {G0_CHOICES}, 1 <= D <= {D_MAX}, C=4, G=32 (the "
+                           f"configurations of RDN.py); got G0={G0}, D={D}, C={C}, G={G}")
+
+
 class RDB(nn.Module):
     """Residual dense block, RDN.py:149-165.  Standalone forward (fp32 NCHW in/out) is the
     unit-test entry; inside a backbone the block runs through bin_backbone_fwd."""
 
     def __init__(self, growRate0, growRate, nConvLayers, kSize=3):
         super().__init__()
-        if (growRate0, growRate, nConvLayers, kSize) != (96, 32, 4, 3):
-            raise BinB200Error("bin_b200 RDB supports G0=96, G=32, C=4, k=3 (the shipped bin_stage4 configuration)")
+        if growRate0 not in G0_CHOICES or (growRate, nConvLayers, kSize) != (32, 4, 3):
+            raise BinB200Error(f"bin_b200 RDB supports G0 in {G0_CHOICES}, G=32, C=4, k=3 (the configurations of RDN.py)")
+        self.G0 = growRate0
         self.convs = nn.Sequential(*[RDB_Conv(growRate0 + c * growRate, growRate) for c in range(nConvLayers)])
         self.LFF = nn.Conv2d(growRate0 + nConvLayers * growRate, growRate0, 1, padding=0, stride=1)
 
@@ -122,18 +133,19 @@ class RDB(nn.Module):
         x = x.contiguous()
         B, Cc, h, w = x.shape
         dev = x.device
+        G0, P = self.G0, self.G0 // 8
         xin = ops.nchw_to_p8(x)
         g = ops.empty_p8(B, 16, h, w, dev)
-        out = ops.empty_p8(B, 12, h, w, dev)
+        out = ops.empty_p8(B, P, h, w, dev)
         for c in range(4):
             conv = self.convs[c].conv[0]
-            wp = ops.pack_conv_weight(conv.weight.detach(), 32, 96 + 32 * c)
-            ops.conv_fwd(xin, wp, ops.pad_bias(conv.bias.detach(), 32), 3, 32, in0_planes=12, in1=g, in1_planes=4 * c,
+            wp = ops.pack_conv_weight(conv.weight.detach(), 32, G0 + 32 * c)
+            ops.conv_fwd(xin, wp, ops.pad_bias(conv.bias.detach(), 32), 3, 32, in0_planes=P, in1=g, in1_planes=4 * c,
                          relu=True, out=g, out_plane0=4 * c)
-        wp = ops.pack_conv_weight(self.LFF.weight.detach(), 96, 224)
-        ops.conv_fwd(xin, wp, ops.pad_bias(self.LFF.bias.detach(), 96), 1, 96, in0_planes=12, in1=g, in1_planes=16,
+        wp = ops.pack_conv_weight(self.LFF.weight.detach(), G0, G0 + 128)
+        ops.conv_fwd(xin, wp, ops.pad_bias(self.LFF.bias.detach(), G0), 1, G0, in0_planes=P, in1=g, in1_planes=16,
                      out=out, res=xin)
-        return ops.p8_to_nchw(out, 96)
+        return ops.p8_to_nchw(out, G0)
 
 
 # --------------------------------------------------------------------------------------------
@@ -144,8 +156,7 @@ class _Backbone(nn.Module):
 
     def __init__(self, G0=64, D=6, C=4, G=32):
         super().__init__()
-        if (G0, D, C, G) != (96, 12, 4, 32):
-            raise BinB200Error("bin_b200 backbones support G0=96, D=12, C=4, G=32 (RDN.py:418) only")
+        _check_arch(G0, D, C, G)
         self.G0, self.D, self.C, self.G = G0, D, C, G
         k = 3
         self.SFENet1 = nn.Conv2d(12 * self.NFRAMES, G0, 5, padding=2, stride=1)
@@ -155,9 +166,22 @@ class _Backbone(nn.Module):
         self.UPNet = nn.Sequential(nn.Conv2d(G0, 256, k, padding=1, stride=1), nn.PixelShuffle(2),
                                    nn.Conv2d(64, 3, k, padding=1, stride=1))
 
+    @property
+    def arch(self) -> int:
+        """The `arch` argument of the library's backbone calls (BIN_BACKBONE_ARCH): the frame count alone for the shipped
+        G0 = 96, D = 12."""
+        if (self.G0, self.D) == (96, 12):
+            return self.NFRAMES
+        return _lib.backbone_arch(self.NFRAMES, self.G0, self.D)
+
+    @property
+    def nconv(self) -> int:
+        """Convs of this backbone, 5 D + 6 (66 for the shipped one)."""
+        return 5 * self.D + 6
+
     # -- packed weights (cached per parameter version / device) ---------------------------------
     def _conv_modules(self) -> List[nn.Conv2d]:
-        """The 66 convs in nn.Module registration order (= the order of bin_backbone_pack's pointer tables)."""
+        """The 5 D + 6 convs in nn.Module registration order (= the order of bin_backbone_pack's pointer tables)."""
         ms = [self.SFENet1, self.SFENet2]
         for blk in self.RDBs:
             ms += [rc.conv[0] for rc in blk.convs] + [blk.LFF]
@@ -171,8 +195,8 @@ class _Backbone(nn.Module):
         ps: List[torch.Tensor] = []
         for m in self._conv_modules():
             ps += [m.weight, m.bias]
-        if len(ps) != 2 * _lib.BIN_BACKBONE_NCONV:
-            raise BinB200Error("backbone does not hold the 66 convs of RDN.py:187-208")
+        if len(ps) != 2 * self.nconv:
+            raise BinB200Error(f"backbone does not hold the {self.nconv} convs of RDN.py:187-208")
         return ps
 
     def packed_blob(self, prec: int = 0) -> torch.Tensor:
@@ -196,9 +220,9 @@ class _Backbone(nn.Module):
         for p in ps:
             if p.dtype != torch.float32 or not p.is_contiguous():
                 raise BinB200Error("bin_b200: parameters must be contiguous fp32")
-        n, L = self.NFRAMES, lib()
-        wp = (C.c_void_p * _lib.BIN_BACKBONE_NCONV)(*[p.data_ptr() for p in ps[0::2]])
-        bp = (C.c_void_p * _lib.BIN_BACKBONE_NCONV)(*[p.data_ptr() for p in ps[1::2]])
+        n, L = self.arch, lib()
+        wp = (C.c_void_p * self.nconv)(*[p.data_ptr() for p in ps[0::2]])
+        bp = (C.c_void_p * self.nconv)(*[p.data_ptr() for p in ps[1::2]])
         with torch.cuda.device(dev):
             if kind == "t":
                 blob = torch.empty(L.bin_backbone_packed_t_bytes(n), dtype=torch.uint8, device=dev)
@@ -276,7 +300,7 @@ def _checkpointing_of(module) -> Optional[str]:
 def set_activation_checkpointing(net: nn.Module, mode: Optional[str]) -> nn.Module:
     """Choose what a grad-enabled forward keeps for the backward, for every module in `net.modules()` (so a DataParallel
     wrapper or a module holding the net works).  None (the default): each batched backbone stage keeps its training
-    workspace, growth maps of all 12 RDBs included, until its backward.  "recompute": each stage keeps only its input
+    workspace, growth maps of all its RDBs included, until its backward.  "recompute": each stage keeps only its input
     frames; its backward re-runs the inference forward and rebuilds each RDB's growth maps, so a step holds one stage's
     activations at a time instead of all of them, at the price of extra forward work.  Every kernel sees the same
     operands in both modes: outputs, frame gradients and conv weight gradients are bit-identical, and the values that
@@ -374,8 +398,8 @@ def _launch_stage(model: _Backbone, calls, outs, prec: int) -> torch.Tensor:
     into the shared per-(device, stream) workspace, which it returns: a recomputing backward reads what it left there."""
     B, _, H, W = calls[0][0].shape
     fr = ops.make_frames(calls, outs)
-    ws = _workspace(calls[0][0].device, lib().bin_backbone_workspace_bytes_p(model.NFRAMES, B * len(calls), H, W, prec))
-    check(lib().bin_backbone_fwd_p(model.NFRAMES, model.packed_blob(prec).data_ptr(), C.byref(fr), H, W, ws.data_ptr(),
+    ws = _workspace(calls[0][0].device, lib().bin_backbone_workspace_bytes_p(model.arch, B * len(calls), H, W, prec))
+    check(lib().bin_backbone_fwd_p(model.arch, model.packed_blob(prec).data_ptr(), C.byref(fr), H, W, ws.data_ptr(),
                                    ws.numel(), prec, ops._stream()))
     return ws
 
@@ -485,7 +509,7 @@ def _window_fwd(net, F, live, s1=None) -> tuple:
         # the shared workspace grows once, to the largest stage, before the first stage runs (also inside a graph capture)
         ncalls = [(pyr.model1_1, len(need))] + [(m, sum(1 for n in live if n[0] == st))
                                                  for st, m in ((2, pyr.model2_1), (3, pyr.model3_1), (4, pyr.model4_1))]
-        _workspace(F[0].device, max([lib().bin_backbone_workspace_bytes_p(m.NFRAMES, B * k, H, W, prec)
+        _workspace(F[0].device, max([lib().bin_backbone_workspace_bytes_p(m.arch, B * k, H, W, prec)
                                      for m, k in ncalls if k], default=0))
         stage = lambda model, calls: _batched(model, calls, prec)
         if need:

@@ -105,7 +105,7 @@ typedef struct {
   bin_act_t in1; int in1_plane0, in1_planes; /* in1_planes = 0 -> unused */
   const void* w_packed; const float* bias;   /* bias: fp32[cout_pad] */
   int ksize;     /* 1, 3 or 5; stride 1, zero padding ksize/2 (all convs of RDN.py) */
-  int cout_pad;  /* 16, 32, 256 or a multiple of 96 */
+  int cout_pad;  /* 16, 32, 64, 256 or a multiple of 96 */
   int relu;      /* RDN.py:142 */
   int epilogue;  /* BIN_EPI_* */
   int variant;   /* BIN_CONV_*; must match the variant the weights were packed with */
@@ -192,62 +192,72 @@ int bin_convlstm_bwd_ex(const float* x, const float* c_prev, const float* h_prev
                         bin_stream_t s);
 
 /* ---- one backbone (RDN_residual_interp_{2,2_1,4_1}_input.forward, RDN.py:210-334) ---------- */
-#define BIN_BACKBONE_NCONV 66 /* SFENet1, SFENet2, 12 x (4 conv + LFF), GFF.0, GFF.1, UPNet.0, UPNet.2 */
-size_t bin_backbone_packed_bytes(int nframes);
-/* w[i], b[i]: device fp32 parameters in nn.Module registration order (see bin_b200/rdn.py). */
-int bin_backbone_pack(int nframes, const float* const* w_host, const float* const* b_host, void* blob,
+/* Every backbone call takes an `arch`: the frame count (2, 3 or 5), the width G0 and the number D of residual dense
+ * blocks, as BIN_BACKBONE_ARCH(nframes, g0, d).  g0 is 64 or 96 and d is 1..12; g0 = 0
+ * and d = 0 stand for the shipped 96 and 12, so BIN_BACKBONE_ARCH(n, 0, 0) == n and a plain frame count keeps its
+ * meaning.  C = 4 growth convs of G = 32 channels per block, as every configuration of the reference.  G0 = 128 is not
+ * supported (the fused RDB tail's weights would not fit in shared memory), nor D > 12 (the tables below hold 66 convs).
+ * A size query returns 0 and an entry point fails with BIN_ERR_ARG, before any launch, on an arch outside this range. */
+#define BIN_BACKBONE_ARCH(nframes, g0, d) ((nframes) | ((g0) << 8) | ((d) << 16))
+#define BIN_BACKBONE_NCONV 66 /* convs of the shipped backbone: SFENet1, SFENet2, 12 x (4 conv + LFF), GFF.0, GFF.1,
+                                 UPNet.0, UPNet.2; the most any arch has */
+/* Convs of a backbone, 5 D + 6 in the order above; -1 for an arch the library rejects. */
+int bin_backbone_nconv(int arch);
+size_t bin_backbone_packed_bytes(int arch);
+/* w[i], b[i]: bin_backbone_nconv(arch) device fp32 parameters in nn.Module registration order (see bin_b200/rdn.py). */
+int bin_backbone_pack(int arch, const float* const* w_host, const float* const* b_host, void* blob,
                       bin_stream_t s);
-size_t bin_backbone_workspace_bytes(int nframes, int Btot, int H, int W);
-int bin_backbone_fwd(int nframes, const void* blob, const bin_frames_t* fr, int H, int W, void* workspace,
+size_t bin_backbone_workspace_bytes(int arch, int Btot, int H, int W);
+int bin_backbone_fwd(int arch, const void* blob, const bin_frames_t* fr, int H, int W, void* workspace,
                      size_t workspace_bytes, bin_stream_t s);
 /* ---- training: forward that keeps the activations + backward (bin_model.optimize_parameters,
  * bin_model.py:130-141 -> l_pix.backward()).  Gradients flow as loss-scaled fp16 P8 tensors:
  * *scale_dev (device float, a power of two chosen by the caller from max|dOut|) multiplies dOut on entry
  * and is divided out of every result (frame gradients, dW, db). */
-size_t bin_backbone_packed_t_bytes(int nframes);             /* data-gradient (transposed, tap-flipped) weights */
-int bin_backbone_pack_t(int nframes, const float* const* w_host, void* blob_t, bin_stream_t s);
-size_t bin_backbone_train_workspace_bytes(int nframes, int Btot, int H, int W);   /* saved activations */
-int bin_backbone_fwd_train(int nframes, const void* blob, const bin_frames_t* fr, int H, int W, void* save_ws,
+size_t bin_backbone_packed_t_bytes(int arch);             /* data-gradient (transposed, tap-flipped) weights */
+int bin_backbone_pack_t(int arch, const float* const* w_host, void* blob_t, bin_stream_t s);
+size_t bin_backbone_train_workspace_bytes(int arch, int Btot, int H, int W);   /* saved activations */
+int bin_backbone_fwd_train(int arch, const void* blob, const bin_frames_t* fr, int H, int W, void* save_ws,
                            size_t save_ws_bytes, bin_stream_t s);
-size_t bin_backbone_grad_workspace_bytes(int nframes, int Btot, int H, int W);
-size_t bin_backbone_grad_param_floats(int nframes);          /* fp32 [w0,b0,w1,b1,...] in nn.Module order */
+size_t bin_backbone_grad_workspace_bytes(int arch, int Btot, int H, int W);
+size_t bin_backbone_grad_param_floats(int arch);          /* fp32 [w0,b0,w1,b1,...] in nn.Module order */
 /* dout->out[k]: dL/d(output of call k), (Bc,3,H,W) fp32.  dframes->frame[k][f]: receives dL/d(frame f of call k)
  * (written, not accumulated; the caller sums frames that feed several calls).  grad_params is ACCUMULATED into. */
-int bin_backbone_bwd(int nframes, const void* blob_t, const bin_frames_t* dout, const bin_frames_t* dframes, int H, int W,
+int bin_backbone_bwd(int arch, const void* blob_t, const bin_frames_t* dout, const bin_frames_t* dframes, int H, int W,
                      const void* save_ws, void* grad_ws, size_t grad_ws_bytes, float* grad_params,
                      const float* scale_dev, bin_stream_t s);
 /* The same backward from the INFERENCE workspace (activation recomputation): fwd_ws (fwd_ws_bytes >=
  * bin_backbone_workspace_bytes) is what bin_backbone_fwd with `blob` just left for the same frames, which keeps every
- * activation the backward reads except the growth maps of the 12 RDBs.  Before each RDB's backward its four growth convs
+ * activation the backward reads except the growth maps of the D RDBs.  Before each RDB's backward its four growth convs
  * are re-run from its input with `blob`, into the workspace's one RDB of growth scratch.  Every launch then reads the
  * operands that bin_backbone_bwd reads after bin_backbone_fwd_train, so the frame and weight gradients have the same bits.
  * The bias gradients are summed with float atomics in both when flags = 0 (their last bits vary from run to run), and in
  * a fixed order with BIN_DETERMINISTIC (the same bits in both).  grad_ws, grad_params and scale_dev are as there.  A NULL
  * pointer, an undersized or unaligned fwd_ws fail (BIN_ERR_ARG / BIN_ERR_WORKSPACE) before any launch. */
-int bin_backbone_bwd_recompute(int nframes, const void* blob, const void* blob_t, const bin_frames_t* dout,
+int bin_backbone_bwd_recompute(int arch, const void* blob, const void* blob_t, const bin_frames_t* dout,
                                const bin_frames_t* dframes, int H, int W, const void* fwd_ws, size_t fwd_ws_bytes,
                                void* grad_ws, size_t grad_ws_bytes, float* grad_params, const float* scale_dev,
                                bin_stream_t s);
 /* The two backwards with flags (the calls above = flags 0).  BIN_DETERMINISTIC needs no extra memory: the bias-gradient
  * partials live in the wgrad region of grad_ws, which bin_backbone_grad_workspace_bytes sizes for both. */
-int bin_backbone_bwd_ex(int nframes, const void* blob_t, const bin_frames_t* dout, const bin_frames_t* dframes, int H,
+int bin_backbone_bwd_ex(int arch, const void* blob_t, const bin_frames_t* dout, const bin_frames_t* dframes, int H,
                         int W, const void* save_ws, void* grad_ws, size_t grad_ws_bytes, float* grad_params,
                         const float* scale_dev, int flags, bin_stream_t s);
-int bin_backbone_bwd_recompute_ex(int nframes, const void* blob, const void* blob_t, const bin_frames_t* dout,
+int bin_backbone_bwd_recompute_ex(int arch, const void* blob, const void* blob_t, const bin_frames_t* dout,
                                   const bin_frames_t* dframes, int H, int W, const void* fwd_ws, size_t fwd_ws_bytes,
                                   void* grad_ws, size_t grad_ws_bytes, float* grad_params, const float* scale_dev,
                                   int flags, bin_stream_t s);
 /* The two backwards for a partly frozen network (the _ex calls above = need_host NULL).  need_host: host array of
- * 2 * BIN_BACKBONE_NCONV bytes, nonzero where a gradient is wanted: weight then bias of conv 0..65, the order of
+ * 2 * bin_backbone_nconv(arch) bytes, nonzero where a gradient is wanted: weight then bias of each conv, the order of
  * grad_params; NULL = all.  A NULL dframes->frame[k][f] = no gradient for that frame.  Gradients not asked for are not
  * computed and their grad_params entries are left untouched; grad_params may be NULL when need_host asks for none.  The
  * data gradient of conv k's input is computed only if a frame or a tensor of a lower-index conv wants a gradient, and
  * the walk stops once none does.  Everything that is computed runs the launches of the full backward on the same
  * operands in the same order, so the gradients that are kept have its bits. */
-int bin_backbone_bwd_masked(int nframes, const void* blob_t, const bin_frames_t* dout, const bin_frames_t* dframes, int H,
+int bin_backbone_bwd_masked(int arch, const void* blob_t, const bin_frames_t* dout, const bin_frames_t* dframes, int H,
                             int W, const void* save_ws, void* grad_ws, size_t grad_ws_bytes, float* grad_params,
                             const float* scale_dev, int flags, const unsigned char* need_host, bin_stream_t s);
-int bin_backbone_bwd_recompute_masked(int nframes, const void* blob, const void* blob_t, const bin_frames_t* dout,
+int bin_backbone_bwd_recompute_masked(int arch, const void* blob, const void* blob_t, const bin_frames_t* dout,
                                       const bin_frames_t* dframes, int H, int W, const void* fwd_ws, size_t fwd_ws_bytes,
                                       void* grad_ws, size_t grad_ws_bytes, float* grad_params, const float* scale_dev,
                                       int flags, const unsigned char* need_host, bin_stream_t s);
@@ -257,17 +267,18 @@ int bin_backbone_bwd_recompute_masked(int nframes, const void* blob, const void*
 int bin_grad_scale(const float* const* gouts_host, int n, size_t numel, float target, float* scale_dev, void* tmp4_dev,
                    bin_stream_t s);
 
-/* Unit-test entry: one RDB (RDN.py:149-165) on fp32 NCHW (B,96,h,w), using RDB `index` of the blob. */
-int bin_rdb_fwd(const void* blob, int nframes, int index, const float* x, float* y, int B, int h, int w,
+/* Unit-test entry: one RDB (RDN.py:149-165) on fp32 NCHW (B,G0,h,w), using RDB `index` (< D) of a blob packed for
+ * `arch`; the block is G0 channels wide. */
+int bin_rdb_fwd(const void* blob, int arch, int index, const float* x, float* y, int B, int h, int w,
                 void* workspace, size_t workspace_bytes, bin_stream_t s);
 
 /* Precision-parameterised twins of the backbone calls (prec = BIN_PREC_F16 | BIN_PREC_F32X3).  In BIN_PREC_F32X3 the
  * packed blob is 3x and the workspace 2x as large; results match the fp32 reference to <=1e-5. */
-size_t bin_backbone_packed_bytes_p(int nframes, int prec);
-int bin_backbone_pack_p(int nframes, const float* const* w_host, const float* const* b_host, void* blob, int prec,
+size_t bin_backbone_packed_bytes_p(int arch, int prec);
+int bin_backbone_pack_p(int arch, const float* const* w_host, const float* const* b_host, void* blob, int prec,
                         bin_stream_t s);
-size_t bin_backbone_workspace_bytes_p(int nframes, int Btot, int H, int W, int prec);
-int bin_backbone_fwd_p(int nframes, const void* blob, const bin_frames_t* fr, int H, int W, void* workspace,
+size_t bin_backbone_workspace_bytes_p(int arch, int Btot, int H, int W, int prec);
+int bin_backbone_fwd_p(int arch, const void* blob, const bin_frames_t* fr, int H, int W, void* workspace,
                        size_t workspace_bytes, int prec, bin_stream_t s);
 
 /* ---- fused pixel loss (SURVEY 8f rank 3): bin_model.get_loss, bin_model.py:395-425 ---------------------- */
