@@ -1,8 +1,9 @@
 """The backbone configurations G0 in {64, 96}, 1 <= D <= 12 on the GPU: the conv instantiations the G0 = 64 backbones add,
-against fp64 per element; the G0 = 64 fused RDB tail against fp64 and bit for bit against its layer-by-layer path; every
-backbone class and the light window (net.model = RDN_residual_interp_5_input(lstm=True, GO=64, D=6)) against the
-reference's fixtures (oracle/make_golden_arch.py) and the oracle, with the shipped bars; the inference modes and the
-training stack on a light window."""
+and the G0 = 96 layers whose tensors change with D, against fp64 per element; the G0 = 64 fused RDB tail against fp64
+and bit for bit against its layer-by-layer path; every backbone class and the light window (net.model =
+RDN_residual_interp_5_input(lstm=True, GO=64, D=6)) against the reference's fixtures (oracle/make_golden_arch.py) and the
+oracle, with the shipped bars; the inference modes on a light window; per-tensor backbone gradients against fp64 at
+the depth edges of both widths, and the training stack on a light window."""
 import contextlib
 import math
 import os
@@ -70,27 +71,30 @@ def _phys(plane0, n, x3):
 
 
 # --------------------------------------------------------------------------------------------------------------------
-# part 1: the G0 = 64 conv instantiations <64,5>, <64,3>, <64,1> against fp64, both precisions
+# part 1: the G0 = 64 conv instantiations <64,5>, <64,3>, <64,1> against fp64, both precisions, and the G0 = 96 layers
+# whose tensors change with D
 # --------------------------------------------------------------------------------------------------------------------
-def _layer(kind, d=6, i=3, train=False):
-    """(k, cin, tensors {name: planes}, segs [(tensor, plane0, planes)], out (tensor, plane0), res) as the G0 = 64 backbone
-    launches the layer: SFENet1 on the packed frames, SFENet2, GFF.1 with f1, the LFF of RDB i (x = cat[8(i-1), +8) or f2,
-    g at 16 i when training, output cat[8 i]), GFF.0 on the D x 64-channel concat."""
+def _layer(kind, g0=64, d=6, i=3, train=False):
+    """(k, cin, tensors {name: planes}, segs [(tensor, plane0, planes)], out (tensor, plane0), res) as a backbone of
+    width g0 (P = g0 / 8 planes per feature map) launches the layer: SFENet1 on the packed frames, SFENet2, GFF.1 with
+    f1, the LFF of RDB i (x = cat[P(i-1), +P) or f2, g at 16 i when training, output cat[P i]), GFF.0 on the D x
+    g0-channel concat."""
+    P = g0 // 8
     if kind.startswith("sfe1"):
         cin = int(kind[4:])
         xp = (cin + 31) // 32 * 4
-        return 5, cin, dict(x0=xp, f1=8), [("x0", 0, xp)], ("f1", 0), None
+        return 5, cin, dict(x0=xp, f1=P), [("x0", 0, xp)], ("f1", 0), None
     if kind == "sfe2":
-        return 3, 64, dict(f1=16, f2=8), [("f1", 4, 8)], ("f2", 0), None
+        return 3, g0, dict(f1=2 * P, f2=P), [("f1", 4, P)], ("f2", 0), None
     if kind == "gff1":
-        return 3, 64, dict(t1=8, t2=8, f1=8), [("t1", 0, 8)], ("t2", 0), ("f1", 0)
+        return 3, g0, dict(t1=P, t2=P, f1=P), [("t1", 0, P)], ("t2", 0), ("f1", 0)
     if kind == "lff":
-        g0 = 16 * i if train else 0
-        x = ("cat", 8 * (i - 1), 8) if i else ("f2", 0, 8)
-        tensors = dict(g=16 * d if train else 16, cat=8 * d, f2=8)
-        return 1, 192, tensors, [x, ("g", g0, 16)], ("cat", 8 * i), x[:2]
+        gp0 = 16 * i if train else 0
+        x = ("cat", P * (i - 1), P) if i else ("f2", 0, P)
+        tensors = dict(g=16 * d if train else 16, cat=P * d, f2=P)
+        return 1, g0 + 128, tensors, [x, ("g", gp0, 16)], ("cat", P * i), x[:2]
     if kind == "gff0":
-        return 1, 64 * d, dict(cat=8 * d, t1=8), [("cat", 0, 8 * d)], ("t1", 0), None
+        return 1, g0 * d, dict(cat=P * d, t1=P), [("cat", 0, P * d)], ("t1", 0), None
     raise ValueError(kind)
 
 
@@ -112,21 +116,35 @@ CONV_CASES = {  # name: (layer kind, layer options, B, H, W, sub, magnitude)
     "gff0_d6": ("gff0", dict(d=6), 2, 7, 1, None, 1.0),
     "gff0_d12_many": ("gff0", dict(d=12), *MANY, None, 1.0),
 }
+# G0 = 96 (the <96,k> kernels): GFF.0 reads D x 12 planes, and the LFF of the last RDB writes the last 12 planes of cat
+CONV_CASES_G96 = {
+    "g96_gff0_d1": ("gff0", dict(g0=96, d=1), 2, 9, 33, None, 1.0),
+    "g96_gff0_d3": ("gff0", dict(g0=96, d=3), 3, 11, 47, (1, 2, 3, 7), 1.0),
+    "g96_gff0_d5": ("gff0", dict(g0=96, d=5), 1, 16, 61, None, 2.0 ** 5),
+    "g96_lff_last_d1": ("lff", dict(g0=96, d=1, i=0), 2, 9, 31, None, 1.0),
+    "g96_lff_last_d5_train": ("lff", dict(g0=96, d=5, i=4, train=True), 2, 15, 34, None, 1.0),
+}
 
 
 @pytest.mark.parametrize("x3", [False, True])
-@pytest.mark.parametrize("case", sorted(CONV_CASES))
+@pytest.mark.parametrize("case", sorted(CONV_CASES) + sorted(CONV_CASES_G96))
 def test_g64_conv_vs_fp64(case, x3):
     """NaN in every plane the call must not read, the sentinel in every element it must not write; per-element bars of
     test_gpu_forward_fuzz.py (fp16: ulp16(ref) + 32 u A; x3: the split-operand bar)."""
     from bin_b200 import ops
-    kind, opts, B, H, W, sub, mag = CONV_CASES[case]
+    if case in CONV_CASES:
+        kind, opts, B, H, W, sub, mag = CONV_CASES[case]
+        seed = 2 * sorted(CONV_CASES).index(case) + int(x3)
+    else:
+        kind, opts, B, H, W, sub, mag = CONV_CASES_G96[case]
+        seed = 1000 + 2 * sorted(CONV_CASES_G96).index(case) + int(x3)
+    g0 = opts.get("g0", 64)
     k, cin, tensors, segs, (on, op0), res = _layer(kind, **opts)
-    g = torch.Generator(device=DEV).manual_seed(2 * sorted(CONV_CASES).index(case) + int(x3))
+    g = torch.Generator(device=DEV).manual_seed(seed)
     rn = lambda *shape: torch.randn(shape, generator=g, device=DEV, dtype=torch.float64)
     opnd = (lambda t: t.float().double()) if x3 else (lambda t: t.half().double())
     vals = {n: torch.full((B, 8 * p, H, W), NAN, dtype=torch.float64, device=DEV) for n, p in tensors.items()}
-    for name, p0, np_ in list(segs) + ([(res[0], res[1], 8)] if res else []):
+    for name, p0, np_ in list(segs) + ([(res[0], res[1], g0 // 8)] if res else []):
         blk = vals[name][:, 8 * p0:8 * (p0 + np_)]
         fill = torch.isnan(blk)
         blk[fill] = opnd(rn(*blk.shape) * mag)[fill]
@@ -136,18 +154,18 @@ def test_g64_conv_vs_fp64(case, x3):
         vals[segs[0][0]][:, cin:] = 0
     if res is not None and res[0] == on:
         assert res[1] != op0
-    vals[on][:, 8 * op0:8 * op0 + 64] = SENTINEL
+    vals[on][:, 8 * op0:8 * op0 + g0] = SENTINEL
     dev_t = {n: _to_device(v, x3) for n, v in vals.items()}
     before = {n: t.clone() for n, t in dev_t.items()}
-    w32 = (rn(64, X.shape[1], k, k) / math.sqrt(cin * k * k)).float()
+    w32 = (rn(g0, X.shape[1], k, k) / math.sqrt(cin * k * k)).float()
     w32[:, cin:] = 0
-    b32 = (rn(64) * 0.1 * mag).float()
+    b32 = (rn(g0) * 0.1 * mag).float()
     kw = dict(in0_plane0=segs[0][1], in0_planes=segs[0][2], sub=sub, x3=x3, out=dev_t[on], out_plane0=op0)
     if len(segs) > 1:
         kw.update(in1=dev_t[segs[1][0]], in1_plane0=segs[1][1], in1_planes=segs[1][2])
     if res:
         kw.update(res=dev_t[res[0]], res_plane0=res[1])
-    ops.conv_fwd(dev_t[segs[0][0]], ops.pack_conv_weight(w32, 64, X.shape[1], prec=int(x3)), ops.pad_bias(b32, 64), k, 64,
+    ops.conv_fwd(dev_t[segs[0][0]], ops.pack_conv_weight(w32, g0, X.shape[1], prec=int(x3)), ops.pad_bias(b32, g0), k, g0,
                  **kw)
     torch.cuda.synchronize()
     w64, b64 = opnd(w32), b32.double()
@@ -155,7 +173,7 @@ def test_g64_conv_vs_fp64(case, x3):
     A = F.conv2d(X.abs(), w64.abs(), b64.abs(), padding=k // 2)
     rabs = 0.0
     if res:
-        r = vals[res[0]][:, 8 * res[1]:8 * res[1] + 64]
+        r = vals[res[0]][:, 8 * res[1]:8 * res[1] + g0]
         ref, rabs = ref + r, r.abs()
     if x3:
         W1 = w64.abs().sum((1, 2, 3)).view(1, -1, 1, 1)
@@ -163,18 +181,18 @@ def test_g64_conv_vs_fp64(case, x3):
         bar = C_X3 * U * (A + rabs) + 2.0 ** -22 * (3 * A + ref.abs() + 2 * rabs) + 2.0 ** -25 * (W1 + 2) + 2.0 ** -33 * X1
     else:
         bar = ulp16(ref) + C_F16 * U * A
-    got = _from_device(dev_t[on], op0, 8, x3)
+    got = _from_device(dev_t[on], op0, g0 // 8, x3)
     b0, nb, y0, ny = sub if sub else (0, B, 0, H)
     sl = (slice(b0, b0 + nb), slice(None), slice(y0, y0 + ny))
     assert torch.isfinite(got[sl]).all(), case
     ratio = ((got - ref)[sl].abs() / bar[sl]).max().item()
-    print(f"[g64 conv] {case} {'x3' if x3 else 'f16'}: worst err/bar {ratio:.3f}")
+    print(f"[conv G0={g0}] {case} {'x3' if x3 else 'f16'}: worst err/bar {ratio:.3f}")
     assert ratio <= 1.0, (case, x3, ratio)
     for name, t in dev_t.items():
         keep = torch.ones(t.shape, dtype=torch.bool, device=DEV)
         if name == on:
             pm = torch.zeros(t.shape[1], dtype=torch.bool, device=DEV)
-            pm[torch.tensor(_phys(op0, 8, x3), device=DEV)] = True
+            pm[torch.tensor(_phys(op0, g0 // 8, x3), device=DEV)] = True
             m = torch.zeros(t.shape, dtype=torch.bool, device=DEV)
             m[sl[0], :, sl[2]] = True
             keep &= ~(m & pm.view(1, -1, 1, 1, 1))
@@ -463,12 +481,52 @@ def _oracle_grads(pool, calls_idx, cots, sd, emulate):
     return [o.detach() for o in outs], list(grads[:len(fr)]), dict(zip(names, grads[len(fr):]))
 
 
-@pytest.mark.parametrize("n,ncalls,Bc,H,W", [(2, 1, 2, 44, 68), (3, 3, 1, 30, 50), (5, 1, 1, 30, 50)])
-def test_light_backbone_backward_without_relu_flips(n, ncalls, Bc, H, W):
-    """The per-tensor gradient check of test_gpu_backward_fuzz.py at G0 = 64, D = 6, with its bars: each gradient within
-    2x (4x for the bias of growth convs 0-2) the error an fp16-storage oracle makes, plus 1e-3 of the tensor's max."""
+def _backbone_grads(model, pool, calls_idx, cots, mode=None, frozen=(), frame_grad=True):
+    """One forward and backward of `model` on the calls, with activation checkpointing `mode`, the parameters whose names
+    start with one of `frozen` at requires_grad False and the frames at requires_grad `frame_grad`: every parameter's
+    and frame's gradient (None where none was asked for)."""
     from bin_b200 import autograd, rdn
-    g0, d, seed = 64, 6, 300 + n
+    rdn.set_activation_checkpointing(model, mode)
+    try:
+        model.zero_grad(set_to_none=True)
+        for k, p in model.named_parameters():
+            p.requires_grad_(not k.startswith(frozen))
+        frg = [p.cuda().requires_grad_(frame_grad) for p in pool]
+        outs = autograd.backbone_stage(model, [[frg[j] for j in idx] for idx in calls_idx])
+        sum((o * c.cuda()).sum() for o, c in zip(outs, cots)).backward()
+        grads = {k: None if p.grad is None else p.grad.clone() for k, p in model.named_parameters()}
+        grads.update({f"frame{j}": f.grad for j, f in enumerate(frg)})
+        return grads
+    finally:
+        rdn.set_activation_checkpointing(model, None)
+        for p in model.parameters():
+            p.requires_grad_(True)
+
+
+# (g0, d, n, ncalls, Bc, H, W, seed): G0 = 64, D = 6 keeps the ids and seeds it had as the only configuration; the depth
+# edges D = 1 (RDB 0 is the first and the last RDB, d cat one G0 block), odd D (GFF.0's rows and channels end in
+# partial blocks at G0 = 64) and D = 12 at G0 = 64 (d cat 96 planes, growth maps 192), the three backbone classes in turn
+BWD_CASES = [
+    pytest.param(64, 6, 2, 1, 2, 44, 68, 302, id="2-1-2-44-68"),
+    pytest.param(64, 6, 3, 3, 1, 30, 50, 303, id="3-3-1-30-50"),
+    pytest.param(64, 6, 5, 1, 1, 30, 50, 305, id="5-1-1-30-50"),
+    pytest.param(64, 1, 2, 1, 2, 30, 50, 401, id="g64-d1-n2"),
+    pytest.param(64, 5, 3, 1, 1, 30, 50, 402, id="g64-d5-n3"),
+    pytest.param(64, 12, 5, 1, 1, 30, 50, 403, id="g64-d12-n5"),
+    pytest.param(96, 1, 3, 3, 1, 30, 50, 404, id="g96-d1-n3-ncalls3"),
+    pytest.param(96, 5, 5, 1, 2, 30, 50, 405, id="g96-d5-n5"),
+    pytest.param(96, 6, 2, 1, 1, 44, 68, 406, id="g96-d6-n2"),
+]
+
+
+@pytest.mark.parametrize("g0,d,n,ncalls,Bc,H,W,seed", BWD_CASES)
+def test_light_backbone_backward_without_relu_flips(g0, d, n, ncalls, Bc, H, W, seed):
+    """The per-tensor gradient check of test_gpu_backward_fuzz.py at width g0 and depth d, with its bars: the forward
+    within TOL_FP16; each gradient within 2x (4x for the bias of growth convs 0-2) the error an fp16-storage oracle
+    makes, plus 1e-3 of the tensor's max; the "off" growth channels' weights and biases exactly 0.  Then, in
+    deterministic mode, bit for bit: a second backward, the recomputing backward, and backwards with SFENet1 and RDB 0
+    frozen (the need mask cuts both ends of the walk), with and without frame gradients."""
+    from bin_b200 import autograd, rdn
     tf32 = (torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32)
     torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = False
     try:
@@ -486,21 +544,47 @@ def test_light_backbone_backward_without_relu_flips(n, ncalls, Bc, H, W):
     model = model.cuda()
     frg = [p.cuda().requires_grad_(True) for p in pool]
     outs = autograd.backbone_stage(model, [[frg[j] for j in idx] for idx in calls_idx])
-    assert max((o.detach().double() - r).abs().max().item() for o, r in zip(outs, ref_outs)) <= TOL_FP16
+    fwd = max((o.detach().double() - r).abs().max().item() for o, r in zip(outs, ref_outs))
+    assert fwd <= TOL_FP16, fwd
     sum((o * c.cuda()).sum() for o, c in zip(outs, cots)).backward()
     params = dict(model.named_parameters())
     pairs = [(f"frame{j}", frg[j].grad, gfr[j], gfr_emu[j]) for j in range(len(pool))]
     pairs += [(k, params[k].grad, gp[k], gp_emu[k]) for k in gp]
     assert len(pairs) == len(pool) + 2 * (5 * d + 6)
-    bad = []
+    bad, worst = [], 0.0
     for key, got, ref, emu in pairs:
         assert got is not None, key
         mx = ref.abs().max().item()
         e, e_emu = (got.double() - ref).abs().max().item(), (emu - ref).abs().max().item()
         k_emu = 4.0 if key.endswith("bias") and ".convs." in key and ".convs.3." not in key else 2.0
+        worst = max(worst, e / (k_emu * e_emu + 1e-3 * mx))
         if not e <= k_emu * e_emu + 1e-3 * mx:
             bad.append((key, e / mx, e_emu / mx))
+    print(f"[light bwd G0={g0} D={d} n={n} ncalls={ncalls} Bc={Bc} {H}x{W}] forward {fwd:.1e}, worst gradient err/bar "
+          f"{worst:.3f} over {len(pairs)} tensors")
     assert not bad, bad
+    # the "off" channels' ReLU gradient is 0 everywhere: their growth weights and biases get exactly 0
+    for i in range(d):
+        for c in range(O.C):
+            pre = f"RDBs.{i}.convs.{c}.conv.0."
+            off = (sd[pre + "bias"] < 0).cuda()
+            assert params[pre + "weight"].grad[off].abs().max().item() == 0.0, pre
+            assert params[pre + "bias"].grad[off].abs().max().item() == 0.0, pre
+
+    frozen = ("SFENet1.", "RDBs.0.")
+    with _deterministic():
+        run = lambda **kw: _backbone_grads(model, pool, calls_idx, cots, **kw)
+        base = run()
+        runs = {"second backward": run(), "recompute": run(mode="recompute"), "frozen": run(frozen=frozen),
+                "frozen, no frame gradients": run(frozen=frozen, frame_grad=False)}
+    assert all(g is not None for g in base.values())
+    for what, grads in runs.items():
+        assert list(grads) == list(base), what
+        for k, g in grads.items():
+            if what.startswith("frozen") and (k.startswith(frozen) or k.startswith("frame") and "no frame" in what):
+                assert g is None, (what, k)
+            else:
+                assert g is not None and torch.equal(_bits(g), _bits(base[k])), (what, k)
 
 
 def _train_step(net, frames, gts):

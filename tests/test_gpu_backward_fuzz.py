@@ -1,10 +1,12 @@
 """Backward kernels against fp64, held tighter than the whole-network tests can hold them.
 
 Part 1 fuzzes bin_conv_wgrad and the data-gradient convs (bin_conv_fwd over dY with bin_pack_conv_weight_t weights) at
-every configuration the backbone backward launches, with the plane offsets it uses: segments at non-zero planes,
-transposed packs with row0 != 0, accumulating and in-place dgrad, Cout' clipped by store_planes, loss scales 2^-4..2^12,
-tile remainders, batch 3 and more tiles than SMs.  Every plane of every input tensor outside the ranges a call is given
-holds NaN, so a read of a wrong plane shows up as NaN rather than a small error.
+every configuration the backbone backward launches, at every backbone width G0 in {64, 96} and depth D in 1..12, with
+the plane offsets it uses (the launch table is backward_layers.py, which test_backward_layers_cpu.py holds to the
+library's conv list): segments at non-zero planes, transposed packs with row0 != 0, accumulating and in-place dgrad,
+Cout' clipped by store_planes, loss scales 2^-4..2^12, tile remainders, batch 3 and more tiles than SMs.  Every plane of
+every input tensor outside the ranges a call is given holds NaN, so a read of a wrong plane shows up as NaN rather than
+a small error.
 
 Part 2 runs whole backbones (all four, 1 or 3 calls per launch, batch 1 or 2) on weights whose RDB growth convs keep
 every ReLU input at least DELTA away from 0, so fp16 storage cannot flip a ReLU and the gradients can be held to the
@@ -17,6 +19,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from backward_layers import spec as _spec
 from oracle import bin_oracle as O
 
 pytestmark = pytest.mark.gpu
@@ -26,44 +29,6 @@ NAN = float("nan")
 # --------------------------------------------------------------------------------------------------------------------
 # part 1: dgrad / wgrad fuzz
 # --------------------------------------------------------------------------------------------------------------------
-def _spec(kind, rnd, **force):
-    """One backward conv as run_backbone_bwd launches it.  x: input segments (tensor planes, plane0, planes); dy: (tensor
-    planes, plane0) of the dY range; dgrad: data-gradient launches, out = (tensor planes, plane0, store_planes) with
-    tensor planes None when the output lives in the dY tensor itself."""
-    pick = lambda key, choices: force[key] if key in force else rnd.choice(choices)
-    if kind == "sfe1":                      # SFENet1 5x5 (12 n) -> 96; x0 = the packed frames, 4 or 8 planes
-        cin = pick("cin", [24, 36, 60])
-        xp = (cin + 31) // 32 * 4
-        return dict(cin=cin, cout=96, k=5, x=[(xp, 0, xp)], dy=(12, 0), dgrad=[dict(row0=0, nrows=cin, out=(xp, 0, xp), acc=False)])
-    if kind == "sfe2":                      # SFENet2 (dgrad accumulates into d f1) / GFF.1 (dgrad overwrites)
-        acc = pick("acc", [False, True])
-        return dict(cin=96, cout=96, k=3, x=[(12, 0, 12)], dy=(12, 0), dgrad=[dict(row0=0, nrows=96, out=(12, 0, 12), acc=acc)])
-    if kind == "rdb":                       # conv c of RDB i: x-stacked wgrad, dY = planes [4c, 4c+4) of the growth grads
-        c, i = pick("c", range(4)), pick("i", range(12))
-        xin = (144, 12 * (i - 1), 12) if i else (12, 0, 12)
-        dg = [dict(row0=0, nrows=96, out=xin, acc=True)]
-        if c:                               # growth rows accumulate in place into planes [0, 4c) of the dY tensor
-            dg.append(dict(row0=96, nrows=32 * c, out=(None, 0, 4 * c), acc=True))
-        return dict(cin=96 + 32 * c, cout=32, k=3, x=[xin] + ([(192, 16 * i, 4 * c)] if c else []), dy=(16, 4 * c), dgrad=dg,
-                    tag=f"c={c} i={i}")
-    if kind == "lff":                       # LFF 1x1 224 -> 96 of RDB i: dY = d x_{i+1} at planes 12 i of d cat
-        i = pick("i", range(12))
-        xin = (144, 12 * (i - 1), 12) if i else (12, 0, 12)
-        dx = (None, 12 * (i - 1), 12) if i else (12, 0, 12)
-        return dict(cin=224, cout=96, k=1, x=[xin, (192, 16 * i, 16)], dy=(144, 12 * i),
-                    dgrad=[dict(row0=0, nrows=96, out=dx, acc=True), dict(row0=96, nrows=128, out=(16, 0, 16), acc=False)],
-                    tag=f"i={i}")
-    if kind == "gff0":                      # GFF.0 1x1 1152 -> 96: 9 channel tiles of 128 in the wgrad
-        return dict(cin=1152, cout=96, k=1, x=[(144, 0, 144)], dy=(12, 0), dgrad=[dict(row0=0, nrows=1152, out=(144, 0, 144), acc=False)])
-    if kind == "up0":                       # UPNet.0 3x3 96 -> 256: N = 256, one tap per wgrad launch
-        return dict(cin=96, cout=256, k=3, x=[(12, 0, 12)], dy=(32, 0), dgrad=[dict(row0=0, nrows=96, out=(12, 0, 12), acc=False)])
-    if kind == "up2":                       # UPNet.2 3x3 64 -> 3: N = 16, dY channels 3..31 zero
-        return dict(cin=64, cout=3, k=3, x=[(8, 0, 8)], dy=(4, 0), dgrad=[dict(row0=0, nrows=64, out=(8, 0, 8), acc=False)])
-    if kind == "ring":                      # 5x5 with 128 < Cout <= 256: a one-stage wgrad ring
-        return dict(cin=36, cout=200, k=5, x=[(8, 0, 8)], dy=(28, 0), dgrad=[dict(row0=0, nrows=36, out=(8, 0, 8), acc=False)])
-    raise ValueError(kind)
-
-
 KINDS = ["sfe1", "sfe2", "rdb", "lff", "gff0", "rdb", "up0", "up2", "rdb", "lff", "ring", "rdb"]
 NRANDOM = 48
 FORCED = {  # name: (kind, forced choices, B, H, W)
@@ -82,6 +47,38 @@ FORCED = {  # name: (kind, forced choices, B, H, W)
     "sfe2_many_tiles": ("sfe2", dict(acc=True), 3, 72, 124),
     "rdb_many_tiles": ("rdb", dict(c=3, i=4), 3, 72, 124),
 }
+# Every backbone width and depth: each draw picks G0 in {64, 96} and D in 1..12 (and, for an RDB conv or LFF, a quarter
+# of the time the recompute layout of the growth maps).  At G0 = 64 the Cout = 64 wgrads run wgrad_kernel<64> (4 taps
+# per group) and the G0-row data gradients are 96-row launches clipped to 8 planes; GFF.0's D G0 rows and channels leave
+# remainders in the last 96-row block and the last 128-channel wgrad tile.
+ARCH_KINDS = ["sfe1", "sfe2", "rdb", "lff", "gff0", "rdb", "up0", "gff1", "rdb", "lff", "gff0", "rdb"]
+NARCH = 48
+FORCED_ARCH = {  # name: (kind, forced choices incl. g0 and d, B, H, W)
+    "g64_sfe1_n2_w1": ("sfe1", dict(g0=64, cin=24), 2, 13, 1),          # 5x5 at N = 64: tap groups 6 x 4 + 1
+    "g64_sfe1_n5_w1": ("sfe1", dict(g0=64, cin=60), 3, 15, 1),
+    "g64_sfe1_n3_w45": ("sfe1", dict(g0=64, cin=36), 2, 19, 45),        # at W = 1 the last group's tap (kx = 4) reads 0
+    "g64_sfe2_w33": ("sfe2", dict(g0=64, acc=True), 2, 23, 33),          # 3x3 at N = 64: tap groups 4 + 4 + 1
+    "g64_gff1_many_tiles": ("gff1", dict(g0=64), 3, 72, 124),
+    "g64_rdb_c0_i0": ("rdb", dict(g0=64, d=12, c=0, i=0), 2, 9, 21),      # 8 input planes, x = f2, d f2 ends the tensor
+    "g64_rdb_c1_i11": ("rdb", dict(g0=64, d=12, c=1, i=11), 1, 17, 30),  # 12 input planes, x = the last-but-one cat block
+    "g64_rdb_c2_i5_w2": ("rdb", dict(g0=64, d=12, c=2, i=5), 3, 7, 2),   # 16 input planes
+    "g64_rdb_c3_i11": ("rdb", dict(g0=64, d=12, c=3, i=11), 2, 11, 17),  # 20 input planes: a second 128-channel tile
+    "g64_rdb_c3_d1": ("rdb", dict(g0=64, d=1, c=3, i=0), 1, 8, 16),
+    "g64_rdb_many_tiles": ("rdb", dict(g0=64, d=12, c=3, i=4), 3, 72, 124),
+    "g64_lff_i0_d1": ("lff", dict(g0=64, d=1, i=0), 2, 9, 31),           # RDB 0 is also the last: d cat = 8 planes
+    "g64_lff_i11_d12": ("lff", dict(g0=64, d=12, i=11), 1, 15, 17),      # dY = the last 8 planes of d cat
+    "g64_gff0_d1": ("gff0", dict(g0=64, d=1), 2, 9, 33),                 # 64 rows, 8 planes: half a channel tile
+    "g64_gff0_d5": ("gff0", dict(g0=64, d=5), 2, 13, 40),                # 320 rows -> 384, last block stores 4 of 12
+    "g64_gff0_d12_many_tiles": ("gff0", dict(g0=64, d=12), 3, 80, 200),
+    "g96_gff0_d1": ("gff0", dict(g0=96, d=1), 1, 9, 47),                 # 12 planes: the tile's last box is skipped
+    "g96_gff0_d2": ("gff0", dict(g0=96, d=2), 2, 10, 19),                # 24 planes: tiles of 16 + 8
+    "g96_gff0_d3": ("gff0", dict(g0=96, d=3), 3, 5, 33),                 # 36 planes: 16 + 16 + 4
+    "g64_up0_w15": ("up0", dict(g0=64), 2, 7, 15),                       # 64 channels: 2 of 4 TMA boxes skipped, N = 256
+    "g64_rdb_recompute": ("rdb", dict(g0=64, d=12, c=3, i=7, recompute=True), 2, 12, 40),
+    "g96_rdb_recompute": ("rdb", dict(g0=96, d=6, c=2, i=3, recompute=True), 1, 16, 35),
+    "g64_lff_recompute": ("lff", dict(g0=64, d=6, i=5, recompute=True), 2, 10, 26),
+    "g96_lff_recompute": ("lff", dict(g0=96, d=5, i=0, recompute=True), 3, 6, 18),
+}
 
 
 def _case(case):
@@ -90,11 +87,23 @@ def _case(case):
         spec = _spec(KINDS[case % len(KINDS)], rnd)
         B, H, W = rnd.choice([1, 2, 3]), rnd.randint(1, 70), rnd.randint(1, 100)
         seed = case
-    else:
+    elif case in FORCED:
         kind, force, B, H, W = FORCED[case]
         rnd = random.Random(case)
         spec = _spec(kind, rnd, **force)
         seed = 1000 + sorted(FORCED).index(case)
+    elif case in FORCED_ARCH:
+        kind, force, B, H, W = FORCED_ARCH[case]
+        rnd = random.Random(case)
+        spec = _spec(kind, rnd, **force)
+        seed = 3000 + sorted(FORCED_ARCH).index(case)
+    else:                                   # "arch<k>"
+        k = int(case[4:])
+        rnd = random.Random(2000 + k)
+        g0, d, recompute = rnd.choice([64, 96]), rnd.randint(1, 12), rnd.random() < 0.25
+        spec = _spec(ARCH_KINDS[k % len(ARCH_KINDS)], rnd, g0, d, recompute=recompute)
+        B, H, W = rnd.choice([1, 2, 3]), rnd.randint(1, 70), rnd.randint(1, 100)
+        seed = 2000 + k
     spec["scale"] = 2.0 ** rnd.randint(-4, 12)
     return spec, B, H, W, seed
 
@@ -131,7 +140,7 @@ def _tiles_over_sms(B, H, W, k):
     return B * -(-H // 8) * -(-W // 16) > sms, B * -(-H // 8) * -(-W // conv_tw) > sms
 
 
-@pytest.mark.parametrize("case", list(range(NRANDOM)) + sorted(FORCED))
+@pytest.mark.parametrize("case", list(range(NRANDOM)) + sorted(FORCED) + [f"arch{k}" for k in range(NARCH)] + sorted(FORCED_ARCH))
 def test_backward_conv_fuzz(case):
     from bin_b200 import ops
     from bin_b200._lib import Act, check, lib
@@ -176,6 +185,7 @@ def test_backward_conv_fuzz(case):
         runs.append(dw)
     torch.cuda.synchronize()
     err = ((runs[0].double() - dw0.double()).cpu() - gw_ref).abs().max().item()
+    ratios = {"wgrad": err / (1e-4 * ref_max)}
     assert err <= 1e-4 * ref_max, ("wgrad", where, err, ref_max)
     assert _same_bits(runs[0], runs[1]), ("wgrad is not bit-reproducible", where)       # fixed-order slab reduction
     for t, t0 in zip(inputs, before):
@@ -209,12 +219,15 @@ def test_backward_conv_fuzz(case):
             exp += _planes_nchw(prefill, 0, nstore)
         got = _planes_nchw(outt, out_plane0, nstore)
         err = (got - exp).abs().max().item()
+        ratios[f"dgrad rows {row0}+{nrows}"] = err / (2e-3 * exp.abs().max().item())
         assert err <= 2e-3 * exp.abs().max().item(), ("dgrad", row0, nrows, acc, where, err, exp.abs().max().item())
         keep = torch.ones(outt.shape[1], dtype=torch.bool)
         keep[out_plane0:out_plane0 + nstore] = False
         assert _same_bits(outt[:, keep], out0[:, keep]), ("dgrad wrote outside its planes", row0, nrows, where)
         if out_total is not None:
             assert _same_bits(dyt, before[-1]), ("dgrad wrote into dY", where)
+    print(f"[bwd fuzz] {case} {spec.get('tag', '')} {cin}->{cout} k={k} B={B} {H}x{W}: worst err/bar "
+          + ", ".join(f"{key} {r:.3f}" for key, r in ratios.items()))
 
 
 # --------------------------------------------------------------------------------------------------------------------
