@@ -495,14 +495,20 @@ def _window_live(wanted) -> frozenset:
     return frozenset(live)
 
 
-def _window_fwd(net, F, live, s1=None) -> tuple:
+def _window_fwd(net, F, live, s1=None, keys=range(5)) -> tuple:
     """Inference of the window's nodes `live` (a set from _window_live) on the six contiguous frames F -> the 14 outputs,
-    None where not computed.  s1: the stage-1 outputs a caller already holds (StreamingBIN's cache), None where it has
-    none; the live stage-1 pairs without one run as one batched stage.  Stages 2-4 follow _window_schedule, every stage
-    in the net's precision, and the live cells of each recurrent hand-off run as one ConvLSTM launch."""
+    None where not computed.  s1: the stage-1 outputs a caller already holds (the streaming cache), None where it has
+    none; the live stage-1 pairs without one run as one batched stage.  keys: a name for the frame pair of each of the
+    five stage-1 positions; positions whose pairs share a name run once and share the output (an edge window of
+    stream_video reads the pair of frames 0, 0 twice).  Stages 2-4 follow _window_schedule, every stage in the net's
+    precision, and the live cells of each recurrent hand-off run as one ConvLSTM launch."""
     pyr = net.model
     s1 = [None] * 5 if s1 is None else list(s1)
-    need = [a for a in range(5) if (1, a) in live and s1[a] is None]
+    at = {}                                             # pair name -> the positions it fills
+    for a in range(5):
+        if (1, a) in live and s1[a] is None:
+            at.setdefault(keys[a], []).append(a)
+    need = [pos[0] for pos in at.values()]
     B, _, H, W = F[0].shape
     prec = _prec_of(net)
     with torch.cuda.device(F[0].device):
@@ -513,8 +519,9 @@ def _window_fwd(net, F, live, s1=None) -> tuple:
                                      for m, k in ncalls if k], default=0))
         stage = lambda model, calls: _batched(model, calls, prec)
         if need:
-            for a, out in zip(need, stage(pyr.model1_1, [(F[a], F[a + 1]) for a in need])):
-                s1[a] = out
+            for pos, out in zip(at.values(), stage(pyr.model1_1, [(F[a], F[a + 1]) for a in need])):
+                for a in pos:
+                    s1[a] = out
         gates = [getattr(net, n).Gates for n in _LSTM_NAMES]
         lstm = lambda group: ops.convlstm_group([(x, gates[k].weight.detach(), gates[k].bias.detach()) for k, x in group])
         return _window_schedule(stage, lstm, pyr, F, s1, live)

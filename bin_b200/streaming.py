@@ -6,18 +6,21 @@ they are pure functions of two frames and the stage-1 weights -- so a stream nee
 instead of the 17 unique ones (20 in the reference).  Every frame is uploaded once (as uint8) instead of six times.
 Stages 2-4 are NOT reusable: window k's step 1 used LSTM history where window k+1's step 0 duplicates its first
 input (RDN.py:375-389), so they are recomputed; the outputs are bit-identical to calling the module per window.
+
+stream_video walks a whole video in test.py's order (test.py:249-258, 334), the clamped windows at both ends included;
+StreamingBIN returns only the windows of six distinct frames.
 """
 from __future__ import annotations
 
-import ctypes as C
 from collections import OrderedDict
-from typing import Dict, List, Optional, Sequence, Tuple
+from typing import Dict, Iterable, List, NamedTuple, Optional, Tuple
 
 import torch
 
 from . import ops
 from ._lib import BinB200Error, check, lib
-from .rdn import _OUT_NODE, _ensemble_of, _flipx4_mean_at, _outputs_of, _selected, _window_fwd, _window_live
+from .rdn import (_OUT_NODE, _ensemble_of, _flipx4_mean_at, _outputs_of, _prec_of, _selected, _window_fwd,
+                  _window_live)
 
 
 def test_py_padding(h: int, w: int) -> Tuple[int, int, int, int]:
@@ -75,7 +78,10 @@ class StreamingBIN:
 
     With an output selection on the net (rdn.set_outputs) a window runs only the backbone calls its wanted outputs depend
     on, and returns what the net would: for (13, 8, 12) the pair of the two oldest frames is never evaluated, so the
-    first window costs 13 calls and every later one 10."""
+    first window costs 13 calls and every later one 10.
+
+    It returns only the windows of six distinct frames; stream_video walks a whole video in test.py's order, the
+    clamped windows at both ends included."""
 
     def __init__(self, net):
         self.net = net
@@ -113,21 +119,187 @@ class StreamingBIN:
         return self._window()
 
     def _window(self):
-        net = self.net
         ids = [i for i, _ in self.frames]
-        F = [f for _, f in self.frames]
-        sel = self.key[1]
-        wanted = range(14) if sel is None else sel[0]
-        live = _window_live(wanted)
-        # stage 1 runs only the live frame pairs not seen before (1 per window in steady state, 5 for the first)
-        pairs = [(ids[a], ids[a + 1]) for a in range(5)]
-        s1 = [self.s1.get(p) for p in pairs]
-        fresh = sum(1 for a in range(5) if (1, a) in live and s1[a] is None)
-        o = _window_fwd(net, F, live, s1)
-        self.backbone_calls += fresh + sum(1 for n in live if n[0] in (2, 3, 4))
-        for i, n in enumerate(_OUT_NODE):
-            if n[0] == 1 and o[i] is not None:
-                self.s1[pairs[n[1]]] = o[i]
-        if self.key[0] is not None:
-            o = tuple(_flipx4_mean_at(o, wanted))
-        return o if sel is None else _selected(o, sel)
+        o, calls = _cached_window(self.net, [f for _, f in self.frames], [(ids[a], ids[a + 1]) for a in range(5)],
+                                  self.s1, *self.key[:2])
+        self.backbone_calls += calls
+        return o
+
+
+def _later_calls(live) -> int:
+    """Backbone calls of stages 2-4 among the window nodes `live`: every window runs them anew."""
+    return sum(1 for n in live if n[0] in (2, 3, 4))
+
+
+def _cached_window(net, F, pairs, cache, ensemble, sel):
+    """One window on the six frames F in the net's modes (ensemble: F are expanded; sel: the net's output selection)
+    -> (what the net returns for it, the backbone calls run).  pairs names the frame pair of each stage-1 position.
+    Stage 1 runs only the live pairs `cache` does not hold, each distinct pair once, and adds them to it."""
+    wanted = range(14) if sel is None else sel[0]
+    live = _window_live(wanted)
+    s1 = [cache.get(p) for p in pairs]
+    fresh = {pairs[a] for a in range(5) if (1, a) in live and s1[a] is None}
+    o = _window_fwd(net, F, live, s1, keys=pairs)
+    for i, n in enumerate(_OUT_NODE):
+        if n[0] == 1 and o[i] is not None:
+            cache[pairs[n[1]]] = o[i]
+    if ensemble is not None:
+        o = tuple(_flipx4_mean_at(o, wanted))
+    return (o if sel is None else _selected(o, sel)), len(fresh) + _later_calls(live)
+
+
+def test_py_window(i: int, n: int) -> Tuple[int, ...]:
+    """The positions of the six frames that window i of an n-frame video reads in test.py: the five of
+    first_5_blurry_list, then the last of second_5_blurry_list (test.py:257-258, 334), clamped to the video, so the
+    first two windows and the last two repeat an end frame.  test.py runs the windows i = 0 .. n-2 (test.py:249-255):
+    a video of fewer than two frames has none, and one of two frames has the single window (0, 0, 0, 1, 1, 1)."""
+    if not 0 <= i <= n - 2:
+        raise BinB200Error(f"test.py runs windows 0..{n - 2} of a {n}-frame video; there is no window {i}")
+    return max(i - 2, 0), max(i - 1, 0), min(i, n - 1), min(i + 1, n - 1), min(i + 2, n - 1), min(i + 3, n - 1)
+
+
+def test_py_names(frame_num: int) -> Dict[int, str]:
+    """The files test.py writes for the window whose blurry frame is named frame_num (test.py:287-299, 380-419), by
+    output index: the interpolated frame Ft_p[13] at frame_num + 8, the first deblurred frame Ft_p[8] at frame_num + 4
+    and the second deblurred frame Ft_p[12] at frame_num + 12.  test_py_writes says which of them a window writes."""
+    return {k: str(frame_num + d).zfill(5) + ".png" for k, d in ((13, 8), (8, 4), (12, 12))}
+
+
+def test_py_writes(i: int, n: int) -> Tuple[int, ...]:
+    """The outputs that window i of an n-frame video writes in test.py, in its order (test.py:380-419), into an output
+    directory that starts empty: Ft_p[13] always; Ft_p[12] while i < n - 2 (test.py:404); Ft_p[8] only in window 0.
+    test.py writes a file only if it is not there yet, and from window 1 on the first deblurred frame is the file the
+    window before wrote as its second: the blurry frames are named 8 apart, as test.py assumes when it names its
+    inputs (test.py:262-263)."""
+    test_py_window(i, n)
+    return (13,) + ((12,) if i < n - 2 else ()) + ((8,) if i == 0 else ())
+
+
+class WindowStep(NamedTuple):
+    """One window of VideoPlan: what stream_video runs and what it drops after it."""
+    i: int                                          # window index, 0 .. N-2
+    frames: Tuple[int, ...]                         # the six frame positions it reads (test_py_window)
+    fresh: Tuple[Tuple[int, int], ...]              # live stage-1 pairs (frame positions) no earlier window evaluated
+    evict_pairs: Tuple[Tuple[int, int], ...]        # stage-1 outputs no later window reads
+    evict_frames: Tuple[int, ...]                   # frames no later window reads
+    backbone_calls: int                             # len(fresh) + the live calls of stages 2-4
+
+
+class VideoPlan:
+    """stream_video's schedule, without tensors: call arrive() once per frame and end() when the video ends; each
+    returns the windows (WindowStep) due at that point, in order.  Window i is due once frame i+3 has arrived; the last
+    two windows read no frame i+3 and are due at the end.  live is the window's node set (rdn._window_live).
+
+    A stage-1 output is named by its pair of frame positions and evaluated once per video, the first time a window
+    reads it at a live position.  Later windows never read below the first pair (and first frame) of the next window,
+    so after window i everything below window i+1's is dropped: at most six frames and five pairs are held.  With all
+    14 outputs an N-frame video costs N+1 stage-1 calls, 12 per window for stages 2-4, 13N - 11 in all."""
+
+    def __init__(self, live):
+        self.live1 = [a for a in range(5) if (1, a) in live]
+        self.later = _later_calls(live)
+        self.arrived = 0
+        self.ended = False
+        self.done = 0                               # windows returned so far
+        self.pairs: set = set()                     # pairs evaluated and not dropped
+        self.low = 0                                # the lowest frame position not dropped
+
+    def arrive(self) -> List[WindowStep]:
+        self.arrived += 1
+        return self._due(self.arrived - 3)
+
+    def end(self) -> List[WindowStep]:
+        self.ended = True
+        return self._due(self.arrived - 1)
+
+    def _due(self, stop: int) -> List[WindowStep]:
+        steps, n = [], self.arrived
+        for i in range(self.done, stop):
+            pos = test_py_window(i, n)              # while the video runs, i <= n-4: no window so far is clamped at the end
+            pairs = [(pos[a], pos[a + 1]) for a in self.live1]
+            fresh = tuple(dict.fromkeys(p for p in pairs if p not in self.pairs))
+            self.pairs.update(fresh)
+            if self.ended and i == n - 2:
+                first, low = (n, n), n              # the last window: drop everything
+            else:
+                nxt = test_py_window(i + 1, n)
+                first, low = (nxt[0], nxt[1]), nxt[0]
+            gone = tuple(sorted(p for p in self.pairs if p < first))
+            self.pairs.difference_update(gone)
+            steps.append(WindowStep(i, pos, fresh, gone, tuple(range(self.low, low)), len(fresh) + self.later))
+            self.low = low
+        self.done = max(self.done, stop)
+        return steps
+
+
+class VideoStream:
+    """The iterator stream_video returns: (i, outputs) per window; backbone_calls counts the calls run so far."""
+
+    def __init__(self, net, frames: Iterable[torch.Tensor]):
+        self.net = net
+        self.backbone_calls = 0
+        self._it = self._windows(iter(frames))
+
+    def __iter__(self) -> "VideoStream":
+        return self
+
+    def __next__(self):
+        return next(self._it)
+
+    def _windows(self, frames):
+        held: Dict[int, torch.Tensor] = {}          # frame position -> (B,3,H,W), or (4B,3,H,W) expanded
+        cache: Dict[Tuple[int, int], torch.Tensor] = {}     # frame-position pair -> stage-1 output
+        plan = mode = shape = None
+        for frame in frames:
+            if not (isinstance(frame, torch.Tensor) and frame.is_cuda and frame.dtype == torch.float32
+                    and frame.dim() == 4 and frame.shape[1] == 3):
+                raise BinB200Error("stream_video expects (B,3,H,W) fp32 CUDA frames (see upload_frame_u8)")
+            if plan is None:
+                mode, shape = self._mode(), (frame.shape, frame.device)
+                plan = VideoPlan(_window_live(range(14) if mode[1] is None else mode[1][0]))
+            elif (frame.shape, frame.device) != shape:
+                raise BinB200Error(f"stream_video: frame {plan.arrived} is {tuple(frame.shape)} on {frame.device}; "
+                                   f"the video's first frame is {tuple(shape[0])} on {shape[1]}")
+            frame = frame.contiguous()
+            if mode[0] is not None:
+                with torch.no_grad(), torch.cuda.device(frame.device):
+                    frame = ops.flipx4_expand([frame])[0]
+            held[plan.arrived] = frame
+            del frame                               # held[] alone keeps it, until the plan drops it
+            for step in plan.arrive():
+                yield self._run(step, held, cache, mode)
+        for step in plan.end() if plan is not None else ():
+            yield self._run(step, held, cache, mode)
+
+    def _mode(self):
+        return _ensemble_of(self.net), _outputs_of(self.net), _prec_of(self.net)
+
+    @torch.no_grad()
+    def _run(self, step: WindowStep, held, cache, mode):
+        if self._mode() != mode:
+            raise BinB200Error("stream_video: the net's self-ensemble, output selection or precision changed during "
+                               "the video; start a new stream_video after changing them")
+        pairs = [(step.frames[a], step.frames[a + 1]) for a in range(5)]
+        o, calls = _cached_window(self.net, [held[p] for p in step.frames], pairs, cache, *mode[:2])
+        self.backbone_calls += calls
+        for p in step.evict_pairs:
+            cache.pop(p, None)
+        for p in step.evict_frames:
+            del held[p]
+        return step.i, o
+
+
+def stream_video(net, frames: Iterable[torch.Tensor]) -> VideoStream:
+    """Every window test.py runs over a video, in its order: for frames F[0..N-1] (an iterable of (B,3,H,W) fp32 CUDA
+    frames, e.g. from upload_frame_u8), yields (i, outputs) for i = 0 .. N-2, where outputs is exactly what
+    net(*[F[j] for j in test_py_window(i, N)]) returns, in the net's precision, output selection and self-ensemble
+    modes (read when the first frame arrives; changing one during the video raises).  N need not be known: window i is
+    yielded once frame i+3 has arrived, and the last two windows when the iterable ends.
+
+    A stage-1 output is kept while a later window can still read it and evaluated once per video, so with all 14
+    outputs a video costs 13N - 11 backbone calls where calling the net per window costs 17(N-1) (VideoPlan); the
+    iterator's backbone_calls counts them.  At most six frames (expanded once each under the ensemble) and the stage-1
+    outputs a later window reads are held.  Outputs at positions 0-3 and 10 are those stage-1 tensors, shared with other
+    windows (and, in the first and the last window, between two positions of one tuple): read them, do not write them.  Inference
+    only: like StreamingBIN.push, every window runs under torch.no_grad()."""
+    return VideoStream(net, frames)
