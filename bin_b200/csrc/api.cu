@@ -6,7 +6,6 @@
 #include <string.h>
 
 #include <string>
-#include <vector>
 
 #include "internal.h"
 
@@ -18,26 +17,12 @@ int fail(int code, const std::string& msg) {
   return code;
 }
 
-static Options read_options() {
-  Options o;
-  auto env = [](const char* k) { const char* e = getenv(k); return (e && *e) ? e : nullptr; };
-  const char* e;
-  o.debug = (e = env("BIN_B200_DEBUG")) ? atoi(e) : 0;
-  o.fuse_lff = !((e = env("BIN_B200_FUSE_LFF")) && *e == '0');
-  o.zigzag = (e = env("BIN_B200_ZIGZAG")) && *e == '1';
-  o.stage_mmas = (e = env("BIN_B200_STAGE_MMAS")) ? atoi(e) : 12;
-  if (o.stage_mmas < 1) o.stage_mmas = 12;
-  o.band_budget = (e = env("BIN_B200_BAND_BUDGET_KB")) ? (size_t)atoll(e) << 10 : (~(size_t)0 >> 1);
-  o.max_sms = (e = env("BIN_B200_MAX_SMS")) ? atoi(e) : 0;
-  if (o.max_sms < 0) o.max_sms = 0;
-  return o;
-}
-const Options& options() {
-  static const Options o = read_options();
-  return o;
-}
-
 int num_sms() {
+  static const int cap = [] {                   // read once per process, not on the launch path
+    const char* e = getenv("BIN_B200_MAX_SMS");
+    const int n = (e && *e) ? atoi(e) : 0;
+    return n > 0 ? n : 0;
+  }();
   static std::atomic<int> cache[64];
   int dev = 0;
   cudaGetDevice(&dev);
@@ -45,8 +30,7 @@ int num_sms() {
   if (v == 0) {
     cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
     if (v <= 0) v = 132;
-    const int cap = options().max_sms;          // lowers the grids the library picks, nothing on the device
-    if (cap > 0 && cap < v) v = cap;
+    if (cap > 0 && cap < v) v = cap;            // lowers the grids the library picks, nothing on the device
     cache[dev & 63].store(v, std::memory_order_relaxed);
   }
   return v;
@@ -93,7 +77,7 @@ int launch_png_encode_u8(const uint8_t* const* imgs_host, int n, int h, int w, u
                          int64_t* sizes, void* workspace, size_t workspace_bytes, cudaStream_t s);
 int launch_rdb_tail(int g0, const bin_act_t& x, int x_plane0, const bin_act_t& g, int g_plane0, const void* w_conv,
                     const float* b_conv, const void* w_lff, const float* b_lff, const bin_act_t& out, int out_plane0,
-                    int b_begin, int b_count, int y_begin, int y_count, cudaStream_t s, bool reverse = false);
+                    int b_begin, int b_count, int y_begin, int y_count, cudaStream_t s);
 int launch_tensor2img_u8(const float* x, int Hs, int Ws, int top, int left, int h, int w, uint8_t* out, cudaStream_t s);
 int launch_u8_to_frame(const uint8_t* img, int h, int w, int pl, int pr, int pt, int pb, float* out, cudaStream_t s);
 size_t convlstm_bwd_scratch_bytes(int B, int H, int W);
@@ -219,125 +203,45 @@ static bin_conv_args_t conv_args(const void* blob, const ConvSpec& c, int x3 = 0
   return a;
 }
 
-// ------------------------------------------------------------------ L2 band plan for the RDB section
-// An RDB run layer-by-layer over the whole (batched) image moves 2 240 B/position through HBM
-// (each conv re-reads the growing concat); measured, that makes the RDB convs HBM-bound at ~50 % of
-// the tensor peak.  Walking the RDB band by band -- all 5 layers for one band before the next --
-// keeps x (192 B/px) + growth scratch (256 B/px) + x' (192 B/px) of the band inside the 50 MB L2,
-// so only x in / x' out (384 B/position) touch HBM.  Bands overlap by the 3-row receptive field of
-// the chained 3x3 convs (rows are recomputed, values identical).  Boundaries sit at rows 8k-3 so
-// every layer of a band has the same number of 8-row tile rows, and k is chosen to minimise the
-// number of one-CTA-per-SM waves.
-struct Band { int b0, nb, y0, y1; };   // batch items [b0,b0+nb), LFF output rows [y0,y1)
-constexpr size_t kBandBytesPerPx = 640;
-static size_t band_budget() {            // BIN_B200_BAND_BUDGET_KB overrides (tests force many bands)
-  // Default = one band (off): every band is a further launch of every RDB conv (prologue and drain per
-  // launch), and at 720p a band that fits the 50 MB L2 is only a few dozen rows.
-  return options().band_budget;
-}
-
-static std::vector<Band> plan_bands(int Btot, int h, int w) {
-  std::vector<Band> out;
-  const size_t px_max = band_budget() / kBandBytesPerPx;
-  const size_t img = (size_t)h * w;
-  if (img <= px_max) {                       // small images: several batch items per band, full rows
-    const size_t per_sz = px_max / img;
-    int per = per_sz >= (size_t)Btot ? Btot : (int)per_sz;
-    if (per < 1) per = 1;
-    for (int b = 0; b < Btot; b += per) out.push_back({b, (b + per <= Btot) ? per : Btot - b, 0, h});
-    return out;
-  }
-  const int tx = (w + 29) / 30;
-  const int T = (h + 7) / 8;                 // boundaries allowed at rows 8k-3, k = 1..T-1
-  const int maxrows = (int)(px_max / w);
-  const int sms = num_sms();
-  auto waves = [&](int rows) { int t = ((rows + 7) / 8) * tx; return (t + sms - 1) / sms; };
-  // dp[k] = min waves to cover rows [0, 8k-3) with bands ending at k; last band ends at h.
-  const int INF = 1 << 30;
-  std::vector<int> dp(T + 1, INF), prev(T + 1, -1);
-  dp[0] = 0;
-  int best = INF, best_k = -1;
-  for (int k = 0; k < T; ++k) {
-    if (dp[k] == INF) continue;
-    const int start = k == 0 ? 0 : 8 * k - 3;
-    for (int k2 = k + 1; k2 < T; ++k2) {     // middle band [start, 8*k2-3)
-      const int end = 8 * k2 - 3;
-      if (end <= start || end >= h) continue;
-      if (end - start > maxrows) break;
-      const int lo = start - 3 < 0 ? 0 : start - 3, hi = end + 3 > h ? h : end + 3;
-      const int c = dp[k] + waves(hi - lo);
-      if (c < dp[k2] || (c == dp[k2] && prev[k2] < k)) { dp[k2] = c; prev[k2] = k; }
-    }
-    if (h - start <= maxrows) {               // close with the last band [start, h)
-      const int lo = start - 3 < 0 ? 0 : start - 3;
-      const int c = dp[k] + waves(h - lo);
-      if (c < best) { best = c; best_k = k; }
-    }
-  }
-  std::vector<int> cuts;
-  for (int k = best_k; k > 0; k = prev[k]) cuts.push_back(8 * k - 3);
-  std::vector<int> edges = {0};
-  for (auto it = cuts.rbegin(); it != cuts.rend(); ++it) edges.push_back(*it);
-  edges.push_back(h);
-  if (best_k < 0) edges = {0, h};
-  for (int b = 0; b < Btot; ++b)
-    for (size_t i = 0; i + 1 < edges.size(); ++i) out.push_back({b, 1, edges[i], edges[i + 1]});
-  return out;
-}
-
-// One RDB: 4 x (conv3x3+ReLU -> growth planes) + LFF 1x1 + residual (RDN.py:149-165).
-// The last conv and the LFF run as one kernel (rdb_tail.cu) in fp16 inference; training keeps them apart because the
-// backward needs the fourth growth map, and the split-fp16 mode has no fused variant.  BIN_B200_FUSE_LFF=0 disables it.
-static bool fuse_lff_enabled() { return options().fuse_lff; }
-// The first `nconv` growth convs of RDB i over one band (RDN.py:141-147): conv3x3 + ReLU of cat(x, g planes so far)
-// into g planes [g_plane0 + 4c, +4).  The forward runs them in run_rdb; the recomputing backward runs all four again.
+// The first `nconv` growth convs of RDB i (RDN.py:141-147): conv3x3 + ReLU of cat(x, g planes so far) into g planes
+// [g_plane0 + 4c, +4).  The forward runs them in run_rdb; the recomputing backward runs all four again.
 static int run_growth(const Arch& A, const void* blob, const BackboneLayout& L, int i, const bin_act_t& xin, int x_plane0,
-                      const bin_act_t& g, int g_plane0, int nconv, const Band& bd, cudaStream_t s, int x3) {
+                      const bin_act_t& g, int g_plane0, int nconv, cudaStream_t s, int x3) {
   const int base = 2 + i * (kCgrow + 1);
-  const int h = xin.H;
   for (int c = 0; c < nconv; ++c) {
     bin_conv_args_t a = conv_args(blob, L.conv[base + c], x3);
     a.in0 = xin; a.in0_plane0 = x_plane0; a.in0_planes = A.planes();
     a.in1 = g; a.in1_plane0 = g_plane0; a.in1_planes = 4 * c;
     a.relu = 1; a.epilogue = BIN_EPI_P8;
     a.out = g; a.out_plane0 = g_plane0 + 4 * c;
-    const int ext = kCgrow - 1 - c;             // rows still needed by the convs downstream in this band
-    const int lo = bd.y0 - ext < 0 ? 0 : bd.y0 - ext, hi = bd.y1 + ext > h ? h : bd.y1 + ext;
-    a.b_begin = bd.b0; a.b_count = bd.nb; a.y_begin = lo; a.y_count = hi - lo;
-    // zigzag: conv0 forward, conv1 backward, conv2 forward, tail backward -- every launch starts on the tiles its
-    // predecessor touched last, which are the ones still in the 50 MB L2 (the tail ends at tile 0, where the next
-    // RDB's conv0 starts)
-    BIN_TRY(launch_conv(a, s, options().zigzag && (c & 1)));
+    BIN_TRY(launch_conv(a, s));
   }
   return BIN_OK;
 }
 
+// One RDB: 4 x (conv3x3+ReLU -> growth planes) + LFF 1x1 + residual (RDN.py:149-165).
+// The last conv and the LFF run as one kernel (rdb_tail.cu) in fp16 inference; training keeps them apart because the
+// backward needs the fourth growth map, and the split-fp16 mode has no fused variant.
 static int run_rdb(const Arch& A, const void* blob, const BackboneLayout& L, int i, const bin_act_t& xin, int x_plane0,
-                   const bin_act_t& g, const bin_act_t& out, int out_plane0, const std::vector<Band>& bands,
-                   cudaStream_t s, int g_plane0 = 0, int x3 = 0, bool keep_growth = false) {
+                   const bin_act_t& g, const bin_act_t& out, int out_plane0, cudaStream_t s, int g_plane0 = 0, int x3 = 0,
+                   bool keep_growth = false) {
   const int base = 2 + i * (kCgrow + 1);
-  const bool fuse = !x3 && !keep_growth && fuse_lff_enabled();
-  for (const Band& bd : bands) {
-    BIN_TRY(run_growth(A, blob, L, i, xin, x_plane0, g, g_plane0, fuse ? kCgrow - 1 : kCgrow, bd, s, x3));
-    if (fuse) {
-      const ConvSpec& c3 = L.conv[base + kCgrow - 1];
-      const ConvSpec& lf = L.conv[base + kCgrow];
-      BIN_TRY(launch_rdb_tail(A.g0, xin, x_plane0, g, g_plane0, (const uint8_t*)blob + c3.w_off,
-                              (const float*)((const uint8_t*)blob + c3.b_off), (const uint8_t*)blob + lf.w_off,
-                              (const float*)((const uint8_t*)blob + lf.b_off), out, out_plane0, bd.b0, bd.nb, bd.y0,
-                              bd.y1 - bd.y0, s, options().zigzag));
-      continue;
-    }
-    bin_conv_args_t a = conv_args(blob, L.conv[base + kCgrow], x3);
-    a.in0 = xin; a.in0_plane0 = x_plane0; a.in0_planes = A.planes();
-    a.in1 = g; a.in1_plane0 = g_plane0; a.in1_planes = 16;
-    a.epilogue = BIN_EPI_P8;
-    a.out = out; a.out_plane0 = out_plane0;
-    a.res = xin; a.res_plane0 = x_plane0;
-    a.b_begin = bd.b0; a.b_count = bd.nb; a.y_begin = bd.y0; a.y_count = bd.y1 - bd.y0;
-    BIN_TRY(launch_conv(a, s));
+  const bool fuse = !x3 && !keep_growth;
+  BIN_TRY(run_growth(A, blob, L, i, xin, x_plane0, g, g_plane0, fuse ? kCgrow - 1 : kCgrow, s, x3));
+  if (fuse) {
+    const ConvSpec& c3 = L.conv[base + kCgrow - 1];
+    const ConvSpec& lf = L.conv[base + kCgrow];
+    return launch_rdb_tail(A.g0, xin, x_plane0, g, g_plane0, (const uint8_t*)blob + c3.w_off,
+                           (const float*)((const uint8_t*)blob + c3.b_off), (const uint8_t*)blob + lf.w_off,
+                           (const float*)((const uint8_t*)blob + lf.b_off), out, out_plane0, 0, 0, 0, 0, s);
   }
-  return BIN_OK;
+  bin_conv_args_t a = conv_args(blob, L.conv[base + kCgrow], x3);
+  a.in0 = xin; a.in0_plane0 = x_plane0; a.in0_planes = A.planes();
+  a.in1 = g; a.in1_plane0 = g_plane0; a.in1_planes = 16;
+  a.epilogue = BIN_EPI_P8;
+  a.out = out; a.out_plane0 = out_plane0;
+  a.res = xin; a.res_plane0 = x_plane0;
+  return launch_conv(a, s);
 }
 
 static int run_backbone(int arch, const void* blob, const bin_frames_t& fr, int H, int W, void* workspace,
@@ -366,11 +270,10 @@ static int run_backbone(int arch, const void* blob, const bin_frames_t& fr, int 
     a.in0 = ws.f1; a.in0_planes = P; a.epilogue = BIN_EPI_P8; a.out = ws.f2;
     BIN_TRY(launch_conv(a, s));
   }
-  const std::vector<Band> bands = plan_bands(Btot, H / 2, W / 2);
   for (int i = 0; i < A.d; ++i) {                                                // RDN.py:215-217
     const int gp0 = train ? 16 * i : 0;
-    if (i == 0) BIN_TRY(run_rdb(A, blob, L, i, ws.f2, 0, ws.g, ws.cat, 0, bands, s, gp0, x3, train));
-    else BIN_TRY(run_rdb(A, blob, L, i, ws.cat, P * (i - 1), ws.g, ws.cat, P * i, bands, s, gp0, x3, train));
+    if (i == 0) BIN_TRY(run_rdb(A, blob, L, i, ws.f2, 0, ws.g, ws.cat, 0, s, gp0, x3, train));
+    else BIN_TRY(run_rdb(A, blob, L, i, ws.cat, P * (i - 1), ws.g, ws.cat, P * i, s, gp0, x3, train));
   }
   {
     bin_conv_args_t a = conv_args(blob, L.conv[nc - 4], x3);                         // GFF.0 on the D*G0-ch concat (RDN.py:218)
@@ -614,7 +517,6 @@ static int run_backbone_bwd(int arch, const void* blob_t, const bin_frames_t& do
   if (!U[gff0]) return BIN_OK;
   BIN_TRY(dgrad(T.x[gff0], gw.dt1, 0, P, gw.dcat, 0, P * A.d, false));
   if (U[2]) BIN_CUDA_OK(cudaMemsetAsync(gw.df2.ptr, 0, (size_t)Btot * P * (H / 2) * (W / 2) * 16, s));
-  const std::vector<Band> bands = recompute ? plan_bands(Btot, H / 2, W / 2) : std::vector<Band>();
   // Reaching RDB i means U holds at its output (base + 5).  Inside it, the growth-map gradients dg feed the growth convs
   // below the current one and the RDB input, so they are needed while U holds at the current conv; the parts that land
   // in the input gradient dxin (residual, x rows of every conv) are needed iff U holds at the RDB input.
@@ -627,10 +529,10 @@ static int run_backbone_bwd(int arch, const void* blob_t, const bin_frames_t& do
     const int dxo_p = P * i;                                  // d x_{i+1}, complete at this point
     const int gp0 = recompute ? 0 : 16 * i;                   // growth maps of RDB i
     const bool dx_in = U[base];
-    // the growth maps are read by the LFF's wgrad and, below it, by the growth-map dgrads and ReLU masks; the LFF's
-    // bias gradient alone reads only dcat
-    if (need_w[base + kCgrow] || U[base + kCgrow])
-      for (const Band& bd : bands) BIN_TRY(run_growth(A, recompute_blob, L, i, xin, xin_p, ws.g, 0, kCgrow, bd, s, 0));
+    // recomputing: rebuild the growth maps, which the LFF's wgrad and, below it, the growth-map dgrads and ReLU masks
+    // read; the LFF's bias gradient alone reads only dcat.  The saving layout already holds them, in planes 16 i.
+    if (recompute && (need_w[base + kCgrow] || U[base + kCgrow]))
+      BIN_TRY(run_growth(A, recompute_blob, L, i, xin, xin_p, ws.g, 0, kCgrow, s, 0));
     BIN_TRY(wgrad(base + kCgrow, xin, xin_p, P, ws.g, gp0, 16, gw.dcat, dxo_p));                      // LFF
     if (!U[base + kCgrow]) return BIN_OK;
     if (dx_in) {
@@ -925,7 +827,7 @@ int bin_rdb_fwd(const void* blob, int arch, int index, const float* x, float* y,
   bin_act_t xin = carve(A.planes()), g = carve(16), out = carve(A.planes());
   if (off > workspace_bytes) return fail(BIN_ERR_WORKSPACE, "rdb_fwd: workspace too small");
   BIN_TRY(launch_nchw_to_p8(x, A.g0, xin, 0, (cudaStream_t)s));
-  BIN_TRY(run_rdb(A, blob, L, index, xin, 0, g, out, 0, plan_bands(B, h, w), (cudaStream_t)s));
+  BIN_TRY(run_rdb(A, blob, L, index, xin, 0, g, out, 0, (cudaStream_t)s));
   return launch_p8_to_nchw(out, 0, A.g0, y, (cudaStream_t)s);
 }
 

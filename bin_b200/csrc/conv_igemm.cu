@@ -109,7 +109,6 @@ __global__ void __launch_bounds__(kThreads, 1) conv_igemm_kernel(const __grid_co
   using C = ConvCfg<NT, KS, SX>;
   static_assert(EPI != BIN_EPI_PIXSHUF || NT == 128, "the PixelShuffle staging buffer holds 4 output planes");
   constexpr int NA = C::NMMA / 2;                              // accumulator registers per thread and 64-row block
-  auto tile_at = [&](int tq) { return p.reverse ? p.ntiles - 1 - tq : tq; };
   extern __shared__ __align__(1024) uint8_t smem[];
   Ctrl* ctrl = reinterpret_cast<Ctrl*>(smem);
   float* sbias = reinterpret_cast<float*>(smem + 1024);
@@ -155,11 +154,11 @@ __global__ void __launch_bounds__(kThreads, 1) conv_igemm_kernel(const __grid_co
     }
     uint32_t s = 0, ph = 0;
     for (int tq = blockIdx.x; tq < p.ntiles; tq += gridDim.x) {
-      int t = tile_at(tq);
-      const int nh = t % p.nh; t /= p.nh;
-      const int txi = t % p.tiles_x; t /= p.tiles_x;
-      const int tyi = t % p.tiles_y;
-      const int b = p.b0 + t / p.tiles_y;
+      const int t1 = p.div_nh.div(tq), t2 = p.div_tx.div(t1), t3 = p.div_ty.div(t2);
+      const int nh = tq - t1 * p.nh;
+      const int txi = t1 - t2 * p.tiles_x;
+      const int tyi = t2 - t3 * p.tiles_y;
+      const int b = p.b0 + t3;
       const int x0 = txi * C::TW - C::PAD, y0 = p.y0 + tyi * kTH - C::PAD;
       int unit = 0;
       for (int j = 0; j < spt; ++j) {
@@ -200,11 +199,11 @@ __global__ void __launch_bounds__(kThreads, 1) conv_igemm_kernel(const __grid_co
   uint32_t s = 0, ph = 0;
   // tile tq -> (cout block nh, tile column txi, tile row tyi, image b)
   auto tile_coords = [&](int tq, int& nh, int& txi, int& tyi, int& b) {
-    int t = tile_at(tq);
-    nh = t % p.nh; t /= p.nh;
-    txi = t % p.tiles_x; t /= p.tiles_x;
-    tyi = t % p.tiles_y;
-    b = p.b0 + t / p.tiles_y;
+    const int t1 = p.div_nh.div(tq), t2 = p.div_tx.div(t1), t3 = p.div_ty.div(t2);
+    nh = tq - t1 * p.nh;
+    txi = t1 - t2 * p.tiles_x;
+    tyi = t2 - t3 * p.tiles_y;
+    b = p.b0 + t3;
   };
   // fragment of a 64-row block: acc[mb][4 i + 2 h + e] = row 16 wq + lane/4 + 8 h, column 8 i + 2 k4 + e
   auto pixel = [&](int txi, int tyi, int mb, int h, int& y, int& x) {
@@ -444,7 +443,7 @@ int make_p8_tmap_box(CUtensorMap* m, const bin_act_t& t, int box_px, int box_row
 // Every argument check of a conv launch runs before the first tensor map is encoded (launch_conv_t, then the
 // shared-memory fit here), so a rejected call has touched neither the driver nor the device.
 template <int NT, int KS, int EPI, bool SX, bool X3>
-static int launch_inst(const bin_conv_args_t& a, cudaStream_t s, bool reverse) {
+static int launch_inst(const bin_conv_args_t& a, cudaStream_t s) {
   using C = ConvCfg<NT, KS, SX>;
   ConvParams p;
   memset(&p, 0, sizeof(p));
@@ -462,6 +461,7 @@ static int launch_inst(const bin_conv_args_t& a, cudaStream_t s, bool reverse) {
   p.tiles_y = (p.ny + kTH - 1) / kTH;
   p.nh = a.cout_pad / NT;
   p.ntiles = nb * p.tiles_x * p.tiles_y * p.nh;
+  p.div_nh = fast_div(p.nh); p.div_tx = fast_div(p.tiles_x); p.div_ty = fast_div(p.tiles_y);
   p.relu = a.relu;
   const int nchunks = p.nch0 + p.nch1;
   const int xbytes = C::XS_BYTES + (EPI == BIN_EPI_PIXSHUF ? 8 * kPsWarpBytes<X3> : 0);   // + the consumer warps' staging
@@ -471,10 +471,9 @@ static int launch_inst(const bin_conv_args_t& a, cudaStream_t s, bool reverse) {
   const int res_bytes = p.resident ? nchunks * C::W_CHUNK : 0;
   const int unit_bytes = C::A_BYTES + (p.resident ? 0 : C::W_STAGE);
   const int nunits = nchunks * C::NSUB;
-  // units per pipeline stage: an mbarrier round trip costs a few hundred cycles, so a stage should
-  // carry >= ~12 wgmma instructions per warpgroup; one 1x1 unit is only 4.
+  // units per pipeline stage: enough for kStageMmas wgmma instructions per warpgroup
   const int mma_per_unit = kMT * C::TAPS_S * (kKC / 16);
-  int cps = (options().stage_mmas + mma_per_unit - 1) / mma_per_unit;
+  int cps = (kStageMmas + mma_per_unit - 1) / mma_per_unit;
   if (cps > nunits) cps = nunits;
   const int avail = kSmemMax - kCtrlBytes - res_bytes - xbytes - 256;
   while (cps > 1 && avail / (cps * unit_bytes) < 2) --cps;
@@ -488,7 +487,6 @@ static int launch_inst(const bin_conv_args_t& a, cudaStream_t s, bool reverse) {
   p.store_planes = a.store_planes > 0 ? a.store_planes : a.cout_pad / 8;
   p.res = reinterpret_cast<const __half*>(a.res.ptr); p.res_planes = a.res.planes; p.res_plane0 = a.res_plane0;
   p.fr = a.fr;
-  p.reverse = (reverse && EPI == BIN_EPI_P8) ? 1 : 0;
   BIN_TRY(make_p8_tmap(&p.tmap0, a.in0, C::ROWS));
   if (a.in1_planes > 0) BIN_TRY(make_p8_tmap(&p.tmap1, a.in1, C::ROWS));
   auto kern = conv_igemm_kernel<NT, KS, EPI, SX, X3>;
@@ -498,21 +496,11 @@ static int launch_inst(const bin_conv_args_t& a, cudaStream_t s, bool reverse) {
   if (grid < 1) return BIN_OK;
   kern<<<grid, kThreads, smem_bytes, s>>>(p);
   BIN_CUDA_OK(cudaGetLastError());
-  if (options().debug & 16) {              // debugging aid: synchronise and name the failing launch
-    cudaError_t e = cudaStreamSynchronize(s);
-    if (e != cudaSuccess)
-      return fail(BIN_ERR_CUDA, std::string("conv launch failed: ") + cudaGetErrorString(e) + " NT=" + std::to_string(NT) +
-                  " KS=" + std::to_string(KS) + " EPI=" + std::to_string(EPI) + " SX=" + std::to_string((int)SX) +
-                  " nch=" + std::to_string(p.nch0) + "+" + std::to_string(p.nch1) + " B/H/W=" + std::to_string(B) + "/" +
-                  std::to_string(H) + "/" + std::to_string(W) + " b0=" + std::to_string(p.b0) + " y0=" + std::to_string(p.y0) +
-                  " ny=" + std::to_string(p.ny) + " ntiles=" + std::to_string(p.ntiles) + " S=" + std::to_string(S) +
-                  " cps=" + std::to_string(cps) + " resident=" + std::to_string(p.resident));
-  }
   return BIN_OK;
 }
 
 template <bool X3>
-static int launch_conv_t(const bin_conv_args_t& a, cudaStream_t s, bool reverse) {
+static int launch_conv_t(const bin_conv_args_t& a, cudaStream_t s) {
   constexpr int f = X3 ? 2 : 1;      // X3 tensors hold hi+lo: twice the planes of their logical channel count
   // one past the last PHYSICAL plane that logical planes [plane0, plane0 + n) occupy (X3: the lo plane of the last one)
   auto plane_end = [](int plane0, int n) { return X3 ? 2 * ((plane0 + n - 1) & ~3) + ((plane0 + n - 1) & 3) + 5 : plane0 + n; };
@@ -567,26 +555,26 @@ static int launch_conv_t(const bin_conv_args_t& a, cudaStream_t s, bool reverse)
     }
   // ---- the instantiation
   if (a.epilogue == BIN_EPI_P8) {
-    if (sx) return launch_inst<32, 3, BIN_EPI_P8, true, X3>(a, s, reverse);
-    if (a.ksize == 3 && a.cout_pad == 32 && a.variant == BIN_CONV_PLAIN && !X3) return launch_inst<32, 3, BIN_EPI_P8, false, false>(a, s, reverse);
-    if (a.ksize == 3 && a.cout_pad % 96 == 0) return launch_inst<96, 3, BIN_EPI_P8, false, X3>(a, s, reverse);
-    if (a.ksize == 5 && a.cout_pad == 96) return launch_inst<96, 5, BIN_EPI_P8, false, X3>(a, s, reverse);
-    if (a.ksize == 1 && a.cout_pad % 96 == 0) return launch_inst<96, 1, BIN_EPI_P8, false, X3>(a, s, reverse);
+    if (sx) return launch_inst<32, 3, BIN_EPI_P8, true, X3>(a, s);
+    if (a.ksize == 3 && a.cout_pad == 32 && a.variant == BIN_CONV_PLAIN && !X3) return launch_inst<32, 3, BIN_EPI_P8, false, false>(a, s);
+    if (a.ksize == 3 && a.cout_pad % 96 == 0) return launch_inst<96, 3, BIN_EPI_P8, false, X3>(a, s);
+    if (a.ksize == 5 && a.cout_pad == 96) return launch_inst<96, 5, BIN_EPI_P8, false, X3>(a, s);
+    if (a.ksize == 1 && a.cout_pad % 96 == 0) return launch_inst<96, 1, BIN_EPI_P8, false, X3>(a, s);
     // G0 = 64 backbones: SFENet1 (5x5), SFENet2 and GFF.1 (3x3), GFF.0 and the LFF (1x1)
-    if (a.ksize == 3 && a.cout_pad == 64) return launch_inst<64, 3, BIN_EPI_P8, false, X3>(a, s, reverse);
-    if (a.ksize == 5 && a.cout_pad == 64) return launch_inst<64, 5, BIN_EPI_P8, false, X3>(a, s, reverse);
-    if (a.ksize == 1 && a.cout_pad == 64) return launch_inst<64, 1, BIN_EPI_P8, false, X3>(a, s, reverse);
+    if (a.ksize == 3 && a.cout_pad == 64) return launch_inst<64, 3, BIN_EPI_P8, false, X3>(a, s);
+    if (a.ksize == 5 && a.cout_pad == 64) return launch_inst<64, 5, BIN_EPI_P8, false, X3>(a, s);
+    if (a.ksize == 1 && a.cout_pad == 64) return launch_inst<64, 1, BIN_EPI_P8, false, X3>(a, s);
   } else if (a.epilogue == BIN_EPI_PIXSHUF) {
-    if (a.ksize == 3 && a.cout_pad == 256) return launch_inst<128, 3, BIN_EPI_PIXSHUF, false, X3>(a, s, reverse);
+    if (a.ksize == 3 && a.cout_pad == 256) return launch_inst<128, 3, BIN_EPI_PIXSHUF, false, X3>(a, s);
   } else if (a.epilogue == BIN_EPI_FINAL) {
-    if (a.ksize == 3 && a.cout_pad == 16 && a.variant == BIN_CONV_DEFAULT) return launch_inst<16, 3, BIN_EPI_FINAL, true, X3>(a, s, reverse);
-    if (a.ksize == 3 && a.cout_pad == 16 && a.variant == BIN_CONV_PLAIN && !X3) return launch_inst<16, 3, BIN_EPI_FINAL, false, false>(a, s, reverse);
+    if (a.ksize == 3 && a.cout_pad == 16 && a.variant == BIN_CONV_DEFAULT) return launch_inst<16, 3, BIN_EPI_FINAL, true, X3>(a, s);
+    if (a.ksize == 3 && a.cout_pad == 16 && a.variant == BIN_CONV_PLAIN && !X3) return launch_inst<16, 3, BIN_EPI_FINAL, false, false>(a, s);
   }
   return fail(BIN_ERR_UNSUPPORTED, "conv: no kernel instantiation for this conv (ksize/cout_pad/epilogue/precision)");
 }
 
-int launch_conv(const bin_conv_args_t& a, cudaStream_t s, bool reverse) {
-  return a.x3 ? launch_conv_t<true>(a, s, reverse) : launch_conv_t<false>(a, s, reverse);
+int launch_conv(const bin_conv_args_t& a, cudaStream_t s) {
+  return a.x3 ? launch_conv_t<true>(a, s) : launch_conv_t<false>(a, s);
 }
 
 }  // namespace binb

@@ -40,18 +40,10 @@ inline int ensure_dynamic_smem(Kernel kern, int bytes, std::atomic<unsigned long
   return BIN_OK;
 }
 
-// ------------------------------------------------------------------ process options
-// Environment knobs of the library (documented in DESIGN.md), read once per process (no getenv on the launch path).
-struct Options {
-  int debug;                 // BIN_B200_DEBUG   bit 4: synchronise after each conv launch
-  bool fuse_lff;             // BIN_B200_FUSE_LFF=0 runs conv3 and LFF as two launches instead of rdb_tail_kernel
-  bool zigzag;               // BIN_B200_ZIGZAG: consecutive RDB launches walk the tiles in opposite directions (L2 reuse)
-  int stage_mmas;            // BIN_B200_STAGE_MMAS: target wgmma instructions per pipeline stage of the conv kernel (default 12)
-  size_t band_budget;        // BIN_B200_BAND_BUDGET_KB (L2 band walker; default: one band)
-  int max_sms;               // BIN_B200_MAX_SMS=n: num_sms() reports at most n (grid sizes only; 0 = no cap)
-};
-const Options& options();
-int num_sms();               // SM count of the current device (cached per device), capped by BIN_B200_MAX_SMS
+// ------------------------------------------------------------------ SM count
+// SM count of the current device (cached per device).  BIN_B200_MAX_SMS=n, read once per process, caps it at n (grid
+// sizes only; 0 or unset = no cap), so one card can stand in for one with fewer SMs.
+int num_sms();
 // Grid of the weight-gradient kernel in deterministic mode (BIN_DETERMINISTIC): a constant, so dW does not depend on
 // the SM count.  132 = the SMs of an H100 SXM, where it equals the default grid.
 constexpr int kDetCtas = 132;
@@ -60,12 +52,30 @@ constexpr int kDetCtas = 132;
 constexpr int kTWH = 32;   // smem row pitch of an activation tile, in pixels (= 4 core-matrix row groups)
 constexpr int kTH = 8;     // output rows per CTA tile
 constexpr int kMT = 2;     // 128-row accumulators per CTA tile (kTH*kTWH/128), one per consumer warpgroup
+// target wgmma instructions per warpgroup and pipeline stage: an mbarrier round trip costs a few hundred cycles, so a
+// stage should carry >= ~12 of them; one 1x1 unit is only 4
+constexpr int kStageMmas = 12;
 constexpr int kKC = 32;    // input channels per pipeline stage
 constexpr int kKPL = 4;    // P8 planes per stage
 constexpr int kCtrlBytes = 2048;
 constexpr int kSmemMax = 227 * 1024;
 constexpr int kMaxStages = 8;
 constexpr int kMaxResidentChunks = 8;
+
+// n / d for 0 <= n < 2^31 without a division instruction: q = (umulhi(n, mul) + n) >> shift, with the round-up magic of
+// Granlund and Montgomery computed on the host (fast_div).  The conv kernel's tile coordinates then stay on the uniform
+// datapath instead of taking vector registers in the epilogue.
+struct FastDiv {
+  unsigned mul; int shift;
+#ifdef __CUDACC__
+  __device__ __forceinline__ int div(int n) const { return (int)((__umulhi((unsigned)n, mul) + (unsigned)n) >> shift); }
+#endif
+};
+inline FastDiv fast_div(int d) {   // d >= 1
+  int l = 0;
+  while ((1u << l) < (unsigned)d) ++l;
+  return {(unsigned)((((1ull << 32) * ((1ull << l) - (unsigned)d)) / (unsigned)d) + 1), l};
+}
 
 struct alignas(64) ConvParams {
   CUtensorMap tmap0, tmap1;
@@ -76,13 +86,14 @@ struct alignas(64) ConvParams {
   int H, W, Btot;                      // conv resolution
   int b0, y0, ny;                      // batch / row sub-range processed by this launch
   int tiles_x, tiles_y, ntiles, nh;    // nh = cout_pad / NT
-  int relu, resident, nstages, cps, reverse;
+  FastDiv div_nh, div_tx, div_ty;
+  int relu, resident, nstages, cps;
   __half* out; int out_planes, out_plane0, store_planes;
   const __half* res; int res_planes, res_plane0;
   bin_frames_t fr;
 };
 
-int launch_conv(const bin_conv_args_t& a, cudaStream_t s, bool reverse = false);   // reverse: walk the tiles last-to-first
+int launch_conv(const bin_conv_args_t& a, cudaStream_t s);
 
 // up to 3 independent ConvLSTM cells in one launch (aux_kernels.cu)
 struct LstmCells {

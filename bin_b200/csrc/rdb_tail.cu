@@ -69,7 +69,6 @@ struct alignas(64) RdbTailParams {
   int b0, y0, ny;
   int tiles_x, tiles_y, ntiles;
   __half* out; int out_planes, out_plane0;
-  int reverse;                          // walk the tiles last-to-first (zigzag L2 reuse across launches)
 };
 
 template <int G0>
@@ -105,7 +104,7 @@ __global__ void __launch_bounds__(384, 1) rdb_tail_kernel(const __grid_constant_
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);
   const int lane = threadIdx.x & 31;
   auto tile_of = [&](int tq, int& txi, int& tyi, int& b) {
-    int t = p.reverse ? p.ntiles - 1 - tq : tq;
+    int t = tq;
     txi = t % p.tiles_x; t /= p.tiles_x;
     tyi = t % p.tiles_y;
     b = p.b0 + t / p.tiles_y;
@@ -284,7 +283,7 @@ static int launch_rdb_tail_g(RdbTailParams& p, const bin_act_t& x, const bin_act
 
 int launch_rdb_tail(int g0, const bin_act_t& x, int x_plane0, const bin_act_t& g, int g_plane0, const void* w_conv,
                     const float* b_conv, const void* w_lff, const float* b_lff, const bin_act_t& out, int out_plane0,
-                    int b_begin, int b_count, int y_begin, int y_count, cudaStream_t s, bool reverse) {
+                    int b_begin, int b_count, int y_begin, int y_count, cudaStream_t s) {
   if (g0 != 64 && g0 != 96) return fail(BIN_ERR_ARG, "rdb_tail: G0 must be 64 or 96");
   const int H = x.H, W = x.W, B = x.B, P = g0 / 8;
   if (g.H != H || g.W != W || g.B != B || out.H != H || out.W != W || out.B != B)
@@ -308,7 +307,6 @@ int launch_rdb_tail(int g0, const bin_act_t& x, int x_plane0, const bin_act_t& g
   p.tiles_y = (p.ny + kRtTH - 1) / kRtTH;
   p.ntiles = nb * p.tiles_x * p.tiles_y;
   p.out = reinterpret_cast<__half*>(out.ptr); p.out_planes = out.planes; p.out_plane0 = out_plane0;
-  p.reverse = reverse ? 1 : 0;
   return g0 == 96 ? launch_rdb_tail_g<96>(p, x, g, s) : launch_rdb_tail_g<64>(p, x, g, s);
 }
 

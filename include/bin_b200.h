@@ -110,8 +110,7 @@ typedef struct {
   int epilogue;  /* BIN_EPI_* */
   int variant;   /* BIN_CONV_*; must match the variant the weights were packed with */
   /* optional sub-range of the output: batch items [b_begin, b_begin+b_count) and rows
-   * [y_begin, y_begin+y_count); counts of 0 mean "to the end".  Used to walk an RDB band by band
-   * so that its intermediate tensors stay L2-resident. */
+   * [y_begin, y_begin+y_count); counts of 0 mean "to the end". */
   int b_begin, b_count, y_begin, y_count;
   /* BIN_EPI_P8 only: number of output planes actually stored (0 = cout_pad/8); lets a conv whose Cout was
    * zero-padded up to a multiple of 96 (the data-gradient launches) write a narrower tensor. */

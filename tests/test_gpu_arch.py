@@ -7,8 +7,6 @@ the depth edges of both widths, and the training stack on a light window."""
 import contextlib
 import math
 import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -19,7 +17,6 @@ from oracle import arch_oracle as A
 from oracle import bin_oracle as O
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 DEV = "cuda"
 NAN = float("nan")
 SENTINEL = -1234.0
@@ -394,28 +391,6 @@ def test_light_flipx4_matches_the_oracle_ensemble(light):
     finally:
         rdn.set_self_ensemble(light, None)
     assert max((g.cpu() - r).abs().max().item() for g, r in zip(got, ref)) <= TOL_FP16
-
-
-def test_light_window_options_keep_the_bits(light, tmp_path):
-    """BIN_B200_FUSE_LFF=0 (conv3 and LFF as two launches) and a small band budget (the RDB band walker) give the default
-    window's bits.  The library reads its options once per process, so each runs in a child process."""
-    fr = [f.cuda() for f in O.synth_frames(6, 1, 112, 128, seed=21, smooth=True)]
-    with torch.no_grad():
-        ref = torch.stack(light(*fr)).cpu()
-    code = (
-        "import sys, torch; sys.path.insert(0, %r)\n"
-        "from oracle import arch_oracle as A, bin_oracle as O\n"
-        "from bin_b200 import rdn\n"
-        "net = rdn.bin_stage4_lstm(); net.model = rdn.RDN_residual_interp_5_input(lstm=True, GO=64, D=6)\n"
-        "net.load_state_dict(A.synth_state_dict(0, 64, 6), strict=True); net = net.cuda().eval()\n"
-        "fr = [f.cuda() for f in O.synth_frames(6, 1, 112, 128, seed=21, smooth=True)]\n"
-        "with torch.no_grad(): torch.save(torch.stack(net(*fr)).cpu(), sys.argv[1])\n" % ROOT)
-    for k, env in enumerate([dict(BIN_B200_FUSE_LFF="0"), dict(BIN_B200_BAND_BUDGET_KB="700")]):
-        path = str(tmp_path / f"out{k}.pt")
-        r = subprocess.run([sys.executable, "-c", code, path], env=dict(os.environ, **env), capture_output=True, text=True,
-                           timeout=600)
-        assert r.returncode == 0, r.stderr[-2000:]
-        assert torch.equal(_bits(torch.load(path)), _bits(ref)), env
 
 
 # --------------------------------------------------------------------------------------------------------------------
