@@ -133,6 +133,8 @@ class BackboneStageFn(torch.autograd.Function):
         flags = deterministic_flags()
         with torch.cuda.device(dev):
             gouts = [torch.zeros((B, 3, H, W), device=dev) if g is None else g.contiguous().float() for g in gouts]
+            # bin_grad_scale reads float4s: a contiguous view at an offset (e.g. a slice of a flat buffer) gets a copy
+            gouts = [g if g.data_ptr() % 16 == 0 else g.clone() for g in gouts]
             sbuf = torch.empty(2, device=dev)                                    # [scale, scratch]; stays on the device
             gp = (C.c_void_p * ncalls)(*[g.data_ptr() for g in gouts])
             check(lib().bin_grad_scale(gp, ncalls, gouts[0].numel(), loss_scale_target(), sbuf.data_ptr(),

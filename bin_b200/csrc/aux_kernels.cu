@@ -362,9 +362,17 @@ __global__ void __launch_bounds__(256) grad_absmax_kernel(const __grid_constant_
   for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
   if ((threadIdx.x & 31) == 0 && m > 0.f) atomicMax(bits, __float_as_uint(m));     // non-negative floats order like their bit patterns
 }
+// The exponent comes from ilogbf, not from log2f(target / gmax): that quotient rounds to a power of two when gmax is a
+// few ulps above one, and the scale came out twice too large.  s = 2^(ilogb(target) - ilogb(gmax)) has s * gmax <= target
+// iff gmax's significand is at most target's; halving once otherwise gives s * gmax <= target < 2 s gmax.  Both
+// products are exact (s is a power of two, the results are normal).  An all-zero gradient is clamped to 1e-30 (a finite
+// scale); an infinite one gives scale 0, so every gradient of that backward is NaN and the optimizer's guard skips it.
 __global__ void grad_scale_finalize_kernel(const unsigned* __restrict__ bits, float target, float* __restrict__ scale) {
   const float gmax = fmaxf(__uint_as_float(*bits), 1e-30f);
-  *scale = exp2f(floorf(log2f(target / gmax)));
+  if (isinf(gmax)) { *scale = 0.f; return; }
+  float s = ldexpf(1.f, ilogbf(target) - ilogbf(gmax));
+  if (s * gmax > target) s *= 0.5f;
+  *scale = s;
 }
 
 __global__ void pack_bias_kernel(const float* __restrict__ b, int cout, int cout_pad, float* __restrict__ dst) {

@@ -261,8 +261,11 @@ int bin_backbone_bwd_recompute_masked(int arch, const void* blob, const void* bl
                                       void* grad_ws, size_t grad_ws_bytes, float* grad_params, const float* scale_dev,
                                       int flags, const unsigned char* need_host, bin_stream_t s);
 /* Loss scale for one backbone backward: *scale_dev = 2^floor(log2(target / max_k max|gouts[k]|)) (a power of two, so
- * scaling and un-scaling are exact), computed on the device -- no host synchronisation.  gouts_host: host array of n
- * (<= BIN_MAX_CALLS) device pointers to fp32 tensors of `numel` elements, 16-byte aligned; tmp4_dev: 4 bytes of scratch. */
+ * scaling and un-scaling are exact), computed on the device -- no host synchronisation.  The exponent is exact:
+ * scale * max <= target < 2 * scale * max.  NaN elements do not count towards the maximum; a maximum of 0 (all zeros)
+ * counts as 1e-30, which keeps the scale finite; an infinite maximum gives scale 0 (the backward's gradients are then
+ * NaN).  gouts_host: host array of n (<= BIN_MAX_CALLS) device pointers to fp32 tensors of `numel` elements, 16-byte
+ * aligned; tmp4_dev: 4 bytes of scratch. */
 int bin_grad_scale(const float* const* gouts_host, int n, size_t numel, float target, float* scale_dev, void* tmp4_dev,
                    bin_stream_t s);
 
