@@ -212,7 +212,38 @@ __global__ void __launch_bounds__(kThreads, 1) conv_igemm_kernel(const __grid_co
     y = p.y0 + tyi * kTH + ty; x = txi * C::TW + tx;
     return (tx < C::TW) && (y < p.y0 + p.ny) && (x < p.W);
   };
+  // BIN_EPI_P8 residual: load_res reads accumulator row set (mb, h)'s residual words into r, r[i] = output channels
+  // 8 i + 2 k4, +1 of the tile's cout block (X3: hi, lo).  fp16 loads one row set ahead (RES_AHEAD): row set (0, 0)
+  // during the tile's last K stage, under its wgmmas, and row set k + 1 before the stores of row set k, so one memory
+  // round trip is in flight under each row's epilogue instead of four exposed after the MMAs.  X3 holds twice the words
+  // and has no registers to spare under the 168-register cap: it loads each row set just before its own stores.
+  constexpr bool RES = EPI == BIN_EPI_P8 && !SX;
+  constexpr bool RES_AHEAD = RES && !X3;
+  constexpr int NR = RES ? NT / 8 : 1;
+  // Offset of channel pair 2 k4 of pixel (y, x) in the first plane a tile of cout block nh touches; plane i of the
+  // block is x3_plane(i) (fp16: i) planes further on.  X3 plane offsets and each block's first plane are
+  // multiples of 4 (launch_conv_t checks the offsets), so x3_plane(plane0 + i) = x3_plane(plane0) + x3_plane(i) there.
+  // Computing the offset once per pixel instead of once per plane takes about a third of the epilogue's instructions.
+  static_assert(EPI != BIN_EPI_P8 || NT % 32 == 0, "a cout block starts at a multiple of 4 planes");
+  const size_t plane = (size_t)p.H * p.W * 8;                   // halves per P8 plane
+  auto plane_off = [&](int planes, int plane0, int nh, int b, int y, int x) {
+    const int lp = plane0 + (nh * NT) / 8;
+    return ((((size_t)b * planes + (X3 ? x3_plane(lp) : lp)) * p.H + y) * p.W + x) * 8 + 2 * k4;
+  };
+  auto load_res = [&](uint32_t (&r)[NR][X3 ? 2 : 1], int nh, int txi, int tyi, int b, int mb, int h) {
+    int y, x;
+    if (!pixel(txi, tyi, mb, h, y, x)) return;
+    const __half* src = p.res + plane_off(p.res_planes, p.res_plane0, nh, b, y, x);
+#pragma unroll
+    for (int i = 0; i < NR; ++i) {
+      if ((nh * NT) / 8 + i >= p.store_planes) continue;
+      const __half* q = src + (size_t)(X3 ? x3_plane(i) : i) * plane;
+      r[i][0] = *reinterpret_cast<const uint32_t*>(q);
+      if constexpr (X3) r[i][X3 ? 1 : 0] = *reinterpret_cast<const uint32_t*>(q + 4 * plane);
+    }
+  };
   for (int tq = blockIdx.x; tq < p.ntiles; tq += gridDim.x) {
+    uint32_t rcur[NR][X3 ? 2 : 1], rnxt[NR][X3 ? 2 : 1];      // this row set's residual words, the next one's
     // BIN_EPI_FINAL: the input frames this thread's outputs add are loaded here, so their latency hides behind the
     // main loop; the epilogue sums them.
     constexpr int NFR = EPI == BIN_EPI_FINAL ? BIN_MAX_FRAMES : 1;
@@ -246,6 +277,13 @@ __global__ void __launch_bounds__(kThreads, 1) conv_igemm_kernel(const __grid_co
       if (p.resident && tq == (int)blockIdx.x) {
         for (int u = 0; u < nu; ++u)
           if ((unit + u) % C::NSUB == 0) mbar_wait(&ctrl->wfull[(unit + u) / C::NSUB], 0);
+      }
+      if constexpr (RES_AHEAD) {
+        if (j == spt - 1 && p.res != nullptr) {
+          int nh, txi, tyi, b;
+          tile_coords(tq, nh, txi, tyi, b);
+          load_res(rcur, nh, txi, tyi, b, 0, 0);
+        }
       }
       const uint32_t st_base = smem_u32(stage0 + (size_t)s * stage_bytes);
       wgmma_fence();
@@ -296,22 +334,22 @@ __global__ void __launch_bounds__(kThreads, 1) conv_igemm_kernel(const __grid_co
         // value of output channel column 8 i + 2 k4 + e of this pixel (SX: xstack_sum has added the kx = 1, 2 groups)
         auto val = [&](int i, int e) { return acc[mb][4 * i + 2 * h + e] * kAcc; };
         if constexpr (EPI == BIN_EPI_P8) {
-          if (valid) {
-            // the row's residual values are all loaded before its first store: a store to p.out may alias p.res, so
-            // loads issued between the stores would each wait for a memory round trip of their own
-            constexpr int NR = SX ? 1 : NT / 8;
-            uint32_t rres[NR][X3 ? 2 : 1];
-            if (!SX && p.res != nullptr) {
-#pragma unroll
-              for (int i = 0; i < NR; ++i) {
-                const int rel = (nh * NT) / 8 + i;
-                if (rel >= p.store_planes) continue;
-                const int lp = p.res_plane0 + rel;
-                const size_t off = ((((size_t)b * p.res_planes + (X3 ? x3_plane(lp) : lp)) * p.H + y) * p.W + x) * 8 + 2 * k4;
-                rres[i][0] = *reinterpret_cast<const uint32_t*>(p.res + off);
-                if constexpr (X3) rres[i][X3 ? 1 : 0] = *reinterpret_cast<const uint32_t*>(p.res + off + (size_t)4 * p.H * p.W * 8);
+          // Residual loads come before the row's stores: a store to p.out may alias p.res, so the compiler keeps every
+          // load behind the stores that precede it in program order.  fp16 loads row set (mb, h) + 1 before the stores
+          // of row set (mb, h).  That order is exact even in place (out and res the same planes): row sets are disjoint
+          // pixels, each thread reads and writes only its own fragment's pixels, so the early loads read nothing that
+          // the stores between them and their use write.
+          if constexpr (RES) {
+            if (p.res != nullptr) {
+              if constexpr (RES_AHEAD) {
+                if (2 * mb + h < 3) load_res(rnxt, nh, txi, tyi, b, (2 * mb + h + 1) >> 1, (2 * mb + h + 1) & 1);
+              } else {
+                load_res(rcur, nh, txi, tyi, b, mb, h);
               }
             }
+          }
+          if (valid) {
+            __half* dst = p.out + plane_off(p.out_planes, p.out_plane0, nh, b, y, x);
 #pragma unroll
             for (int i = 0; i < NT / 8; ++i) {
               const int rel = (nh * NT) / 8 + i;                // channel plane relative to out_plane0
@@ -319,18 +357,26 @@ __global__ void __launch_bounds__(kThreads, 1) conv_igemm_kernel(const __grid_co
               const int n = nh * NT + 8 * i + 2 * k4;
               float f0 = val(i, 0) + bsrc[n], f1 = val(i, 1) + bsrc[n + 1];
               if (p.relu) { f0 = fmaxf(f0, 0.f); f1 = fmaxf(f1, 0.f); }
-              if (!SX && p.res != nullptr) {
-                const float2 g = unpack_h2(rres[SX ? 0 : i][0]);
+              if (RES && p.res != nullptr) {
+                const float2 g = unpack_h2(rcur[RES ? i : 0][0]);
                 f0 += g.x; f1 += g.y;
                 if constexpr (X3) {
-                  const float2 g2 = unpack_h2(rres[SX ? 0 : i][X3 ? 1 : 0]);
+                  const float2 g2 = unpack_h2(rcur[RES ? i : 0][X3 ? 1 : 0]);
                   f0 += g2.x; f1 += g2.y;
                 }
               }
-              const int op = p.out_plane0 + rel;
-              const size_t off = ((((size_t)b * p.out_planes + (X3 ? x3_plane(op) : op)) * p.H + y) * p.W + x) * 8 + 2 * k4;
-              store_pair<X3>(p.out + off, (size_t)4 * p.H * p.W * 8, f0, f1);
+              if constexpr (SX) {                                // the x-stacked kernels keep their own addressing
+                const int op = p.out_plane0 + rel;
+                const size_t off = ((((size_t)b * p.out_planes + (X3 ? x3_plane(op) : op)) * p.H + y) * p.W + x) * 8 + 2 * k4;
+                store_pair<X3>(p.out + off, (size_t)4 * p.H * p.W * 8, f0, f1);
+              } else {
+                store_pair<X3>(dst + (size_t)(X3 ? x3_plane(i) : i) * plane, 4 * plane, f0, f1);
+              }
             }
+          }
+          if constexpr (RES_AHEAD) {
+#pragma unroll
+            for (int i = 0; i < NR; ++i) rcur[i][0] = rnxt[i][0];
           }
         } else if constexpr (EPI == BIN_EPI_PIXSHUF) {
           // out[c, 2y+i, 2x+j] = conv[4c+2i+j, y, x]   (nn.PixelShuffle(2), RDN.py:206).  Column 8 (4 q + m) + 2 k4 + e
