@@ -13,6 +13,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from no_flip import check_no_relu_near_zero, no_flip_sd, oracle_grads
 from oracle import arch_oracle as A
 from oracle import bin_oracle as O
 
@@ -396,66 +397,6 @@ def test_light_flipx4_matches_the_oracle_ensemble(light):
 # --------------------------------------------------------------------------------------------------------------------
 # part 5: training
 # --------------------------------------------------------------------------------------------------------------------
-BETA = 0.05
-TARGET = 0.1 * BETA
-DELTA = 0.05 * BETA
-
-
-def _rdb_input(frames, sd):
-    return O.conv(O.conv(O.space_to_depth2(torch.cat(list(frames), 1)), sd, "SFENet1"), sd, "SFENet2")
-
-
-def _no_flip_sd(n, seed, g0, d, calls):
-    """The construction of test_gpu_backward_fuzz.py at width g0 and depth d: each RDB growth conv is rebuilt in fp64 on
-    these inputs so that every ReLU input is at least DELTA away from 0 (half the channels on, bias +BETA, the smallest
-    pre-activation at TARGET; the rest off, bias -BETA)."""
-    dev = calls[0][0].device
-    sd = {k: v.to(dev, torch.float64) for k, v in A.synth_backbone_sd(n, seed, g0, d).items()}
-    xs = [_rdb_input(c, sd) for c in calls]
-    for i in range(d):
-        feats = xs
-        for c in range(O.C):
-            name = f"RDBs.{i}.convs.{c}.conv.0"
-            w = sd[name + ".weight"]
-            w = w - w.mean((2, 3), keepdim=True)
-            u = torch.cat([F.conv2d(f, w, padding=1).transpose(0, 1).flatten(1) for f in feats], 1)
-            mu, sig, umin, umax = u.mean(1), u.std(1), u.min(1).values, u.max(1).values
-            sign = torch.where(mu - umin <= umax - mu, 1.0, -1.0).to(u)
-            tail = torch.minimum(mu - umin, umax - mu) / sig
-            on = torch.zeros(O.G, dtype=torch.bool, device=dev)
-            on[tail.argsort()[:O.G // 2]] = True
-            lowest = torch.where(sign > 0, umin, -umax)
-            alpha = torch.where(on, sign * (BETA - TARGET) / (-lowest), 0.5 * BETA / u.abs().max(1).values)
-            sd[name + ".weight"] = w * alpha.view(-1, 1, 1, 1)
-            sd[name + ".bias"] = torch.where(on, BETA, -BETA).to(u)
-            feats = [torch.cat((f, O.conv(f, sd, name).relu()), 1) for f in feats]
-        xs = [O.conv(f, sd, f"RDBs.{i}.LFF") + x for f, x in zip(feats, xs)]
-    margin = math.inf
-    feats_x = xs = [_rdb_input(c, sd) for c in calls]
-    for i in range(d):
-        feats = feats_x
-        for c in range(O.C):
-            name = f"RDBs.{i}.convs.{c}.conv.0"
-            on = sd[name + ".bias"] > 0
-            z = torch.cat([O.conv(f, sd, name).transpose(0, 1).flatten(1) for f in feats], 1)
-            margin = min(margin, z[on].min().item(), -z[~on].max().item())
-            feats = [torch.cat((f, O.conv(f, sd, name).relu()), 1) for f in feats]
-        feats_x = [O.conv(f, sd, f"RDBs.{i}.LFF") + x for f, x in zip(feats, feats_x)]
-    assert margin >= DELTA, margin
-    return {k: v.float().cpu() for k, v in sd.items()}
-
-
-def _oracle_grads(pool, calls_idx, cots, sd, emulate):
-    leaves = {k: v.to(DEV, torch.float64).requires_grad_(True) for k, v in sd.items()}
-    fr = [p.to(DEV, torch.float64).requires_grad_(True) for p in pool]
-    with O.emulate_fp16_storage(grads=True) if emulate else contextlib.nullcontext():
-        outs = [A.backbone([fr[j] for j in idx], leaves) for idx in calls_idx]
-    loss = sum((o * c.to(DEV, torch.float64)).sum() for o, c in zip(outs, cots))
-    names = list(leaves)
-    grads = torch.autograd.grad(loss, fr + [leaves[k] for k in names])
-    return [o.detach() for o in outs], list(grads[:len(fr)]), dict(zip(names, grads[len(fr):]))
-
-
 def _backbone_grads(model, pool, calls_idx, cots, mode=None, frozen=(), frame_grad=True):
     """One forward and backward of `model` on the calls, with activation checkpointing `mode`, the parameters whose names
     start with one of `frozen` at requires_grad False and the frames at requires_grad `frame_grad`: every parameter's
@@ -509,9 +450,10 @@ def test_light_backbone_backward_without_relu_flips(g0, d, n, ncalls, Bc, H, W, 
         calls_idx = [list(range(k, k + n - 1)) + [k + 1] for k in range(ncalls)]
         cots = [c - 0.5 for c in O.synth_frames(ncalls, Bc, H, W, seed=seed + 1)]
         pool64 = [p.to(DEV, torch.float64) for p in pool]
-        sd = _no_flip_sd(n, seed, g0, d, [[pool64[j] for j in idx] for idx in calls_idx])
-        ref_outs, gfr, gp = _oracle_grads(pool, calls_idx, cots, sd, emulate=False)
-        _, gfr_emu, gp_emu = _oracle_grads(pool, calls_idx, cots, sd, emulate=True)
+        sd = {k: v.cpu() for k, v in no_flip_sd(n, seed, [[pool64[j] for j in idx] for idx in calls_idx], g0, d).items()}
+        check_no_relu_near_zero([[pool64[j] for j in idx] for idx in calls_idx], sd, min_cv=None)
+        ref_outs, gfr, gp = oracle_grads(pool, calls_idx, cots, sd, emulate=False)
+        _, gfr_emu, gp_emu = oracle_grads(pool, calls_idx, cots, sd, emulate=True)
     finally:
         torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = tf32
     model = getattr(rdn, CLASSES[n])(G0=g0, D=d)

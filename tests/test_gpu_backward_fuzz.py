@@ -11,7 +11,6 @@ a small error.
 Part 2 runs whole backbones (all four, 1 or 3 calls per launch, batch 1 or 2) on weights whose RDB growth convs keep
 every ReLU input at least DELTA away from 0, so fp16 storage cannot flip a ReLU and the gradients can be held to the
 fp64 oracle per tensor, with no correlation fallback."""
-import contextlib
 import math
 import random
 
@@ -20,6 +19,7 @@ import torch
 import torch.nn.functional as F
 
 from backward_layers import spec as _spec
+from no_flip import BETA, check_no_relu_near_zero, no_flip_sd, oracle_grads
 from oracle import bin_oracle as O
 
 pytestmark = pytest.mark.gpu
@@ -235,78 +235,6 @@ def test_backward_conv_fuzz(case):
 # --------------------------------------------------------------------------------------------------------------------
 BACKBONES = [("model1_1", 2, 201), ("model2_1", 3, 202), ("model3_1", 5, 203), ("model4_1", 5, 204)]
 LAUNCHES = [(1, 1, 30, 50), (1, 2, 44, 68), (3, 1, 44, 68), (3, 2, 30, 50)]     # (ncalls, Bc, full-res H, W)
-BETA = 0.05              # |bias| of every growth conv channel
-TARGET = 0.1 * BETA      # the construction puts the smallest "on" pre-activation here
-DELTA = 0.05 * BETA      # margin asserted on every run: every ReLU input is >= DELTA or <= -DELTA
-MIN_CV = 0.2             # every "on" channel: spatial std >= 20 % of its mean
-
-
-def _rdb_input(frames, sd):
-    return O.conv(O.conv(O.space_to_depth2(torch.cat(list(frames), 1)), sd, "SFENet1"), sd, "SFENet2")
-
-
-def _no_flip_sd(n, seed, calls):
-    """O.synth_backbone_sd(n, seed) with the 48 RDB growth convs rebuilt, in fp64 on these inputs, so that no ReLU input
-    is near 0: each channel's 3x3 taps lose their mean (a locally constant input then gives ~0, which centres the
-    channel), half the channels ("on", the 16 whose pre-activations have the lightest tail, flipped to point down) get
-    bias +BETA and a scale that puts their smallest pre-activation at TARGET, the rest bias -BETA and a scale that keeps
-    them within [-1.5 BETA, -0.5 BETA]."""
-    dev = calls[0][0].device
-    sd = {k: v.to(dev, torch.float64) for k, v in O.synth_backbone_sd(n, seed).items()}
-    xs = [_rdb_input(c, sd) for c in calls]
-    for i in range(O.D):
-        feats = xs
-        for c in range(O.C):
-            name = f"RDBs.{i}.convs.{c}.conv.0"
-            w = sd[name + ".weight"]
-            w = w - w.mean((2, 3), keepdim=True)
-            u = torch.cat([F.conv2d(f, w, padding=1).transpose(0, 1).flatten(1) for f in feats], 1)
-            mu, sig, umin, umax = u.mean(1), u.std(1), u.min(1).values, u.max(1).values
-            sign = torch.where(mu - umin <= umax - mu, 1.0, -1.0).to(u)
-            tail = torch.minimum(mu - umin, umax - mu) / sig
-            on = torch.zeros(O.G, dtype=torch.bool, device=dev)
-            on[tail.argsort()[:O.G // 2]] = True
-            lowest = torch.where(sign > 0, umin, -umax)
-            alpha = torch.where(on, sign * (BETA - TARGET) / (-lowest), 0.5 * BETA / u.abs().max(1).values)
-            sd[name + ".weight"] = w * alpha.view(-1, 1, 1, 1)
-            sd[name + ".bias"] = torch.where(on, BETA, -BETA).to(u)
-            feats = [torch.cat((f, O.conv(f, sd, name).relu()), 1) for f in feats]
-        xs = [O.conv(f, sd, f"RDBs.{i}.LFF") + x for f, x in zip(feats, xs)]
-    return {k: v.float() for k, v in sd.items()}
-
-
-def _assert_no_relu_near_zero(calls, sd):
-    """The premise of part 2, on the weights as the backbone runs them (fp32 values, fp64 arithmetic): every growth-conv
-    pre-activation of every call is >= DELTA ("on" channels, bias > 0) or <= -DELTA, and every "on" channel varies
-    across pixels (std >= MIN_CV of its mean), so tap and pixel shifts in the backward stay visible."""
-    sd = {k: v.to(calls[0][0].device, torch.float64) for k, v in sd.items()}
-    feats_x = [_rdb_input([f.double() for f in c], sd) for c in calls]
-    worst_margin, worst_cv = math.inf, math.inf
-    for i in range(O.D):
-        feats = feats_x
-        for c in range(O.C):
-            name = f"RDBs.{i}.convs.{c}.conv.0"
-            on = sd[name + ".bias"] > 0
-            z = torch.cat([O.conv(f, sd, name).transpose(0, 1).flatten(1) for f in feats], 1)
-            margin = min(z[on].min().item(), -z[~on].max().item())
-            cv = (z[on].std(1) / z[on].mean(1)).min().item()
-            assert 12 <= int(on.sum()) <= 20 and margin >= DELTA and cv >= MIN_CV, (name, int(on.sum()), margin, cv)
-            worst_margin, worst_cv = min(worst_margin, margin), min(worst_cv, cv)
-            feats = [torch.cat((f, O.conv(f, sd, name).relu()), 1) for f in feats]
-        feats_x = [O.conv(f, sd, f"RDBs.{i}.LFF") + x for f, x in zip(feats, feats_x)]
-    return worst_margin, worst_cv
-
-
-def _oracle_grads(pool, calls_idx, cots, sd, emulate):
-    """fp64 autograd through O.backbone on the GPU (optionally with fp16-rounded storage of activations and gradients)."""
-    leaves = {k: v.to("cuda", torch.float64).requires_grad_(True) for k, v in sd.items()}
-    fr = [p.to("cuda", torch.float64).requires_grad_(True) for p in pool]
-    with O.emulate_fp16_storage(grads=True) if emulate else contextlib.nullcontext():
-        outs = [O.backbone([fr[j] for j in idx], leaves) for idx in calls_idx]
-    loss = sum((o * c.to("cuda", torch.float64)).sum() for o, c in zip(outs, cots))
-    names = list(leaves)
-    grads = torch.autograd.grad(loss, fr + [leaves[k] for k in names])
-    return [o.detach() for o in outs], list(grads[:len(fr)]), dict(zip(names, grads[len(fr):]))
 
 
 @pytest.mark.parametrize("ncalls,Bc,H,W", LAUNCHES)
@@ -323,10 +251,10 @@ def test_backbone_backward_without_relu_flips(name, n, seed, ncalls, Bc, H, W):
         calls_idx = [list(range(k, k + n - 1)) + [k + 1] for k in range(ncalls)]
         cots = [c - 0.5 for c in O.synth_frames(ncalls, Bc, H, W, seed=seed + 1)]
         pool64 = [p.to("cuda", torch.float64) for p in pool]
-        sd = {k: v.cpu() for k, v in _no_flip_sd(n, seed, [[pool64[j] for j in idx] for idx in calls_idx]).items()}
-        margin, cv = _assert_no_relu_near_zero([[pool64[j] for j in idx] for idx in calls_idx], sd)
-        ref_outs, gfr, gp = _oracle_grads(pool, calls_idx, cots, sd, emulate=False)
-        _, gfr_emu, gp_emu = _oracle_grads(pool, calls_idx, cots, sd, emulate=True)
+        sd = {k: v.cpu() for k, v in no_flip_sd(n, seed, [[pool64[j] for j in idx] for idx in calls_idx]).items()}
+        margin, cv = check_no_relu_near_zero([[pool64[j] for j in idx] for idx in calls_idx], sd)
+        ref_outs, gfr, gp = oracle_grads(pool, calls_idx, cots, sd, emulate=False)
+        _, gfr_emu, gp_emu = oracle_grads(pool, calls_idx, cots, sd, emulate=True)
     finally:
         torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = tf32
 
