@@ -15,6 +15,8 @@ BIN_FLIPX4_MAX_TENSORS = 14
 BIN_TRAIN_MAX_BATCH = 16
 BIN_TRAIN_FRAMES = 17
 BIN_PNG_MAX_BATCH = 16
+BIN_METRICS_MAX_BATCH = 16
+BIN_METRICS_BGR = 1
 EPI_P8, EPI_PIXSHUF, EPI_FINAL = 0, 1, 2
 BIN_DETERMINISTIC = 1                 # flags bit of the *_ex entry points
 ABI_VERSION = 6
@@ -133,6 +135,9 @@ _SIGS = {
     "bin_image_metrics_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int]),
     "bin_image_metrics_u8": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t,
                                        C.c_void_p]),
+    "bin_image_metrics_batch_workspace_bytes": (C.c_size_t, [C.c_int] * 3),
+    "bin_image_metrics_batch_u8": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)] + [C.c_int] * 5
+                                   + [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "bin_flipx4_expand": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)] + [C.c_int] * 4 + [C.c_void_p]),
     "bin_flipx4_mean": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)] + [C.c_int] * 4 + [C.c_void_p]),
     "bin_train_batch_u8": (C.c_int, [C.POINTER(TrainSample)] + [C.c_int] * 3 + [C.c_void_p, C.c_int, C.c_int, C.c_void_p]),

@@ -68,6 +68,9 @@ int launch_blur_average_u8(const uint8_t* frames, int T, size_t frame_bytes, int
 size_t metrics_workspace_bytes(int h, int w);
 int launch_image_metrics_u8(const uint8_t* a, const uint8_t* b, int h, int w, int c, double* out4, void* workspace,
                             size_t workspace_bytes, cudaStream_t s);
+size_t metrics_batch_workspace_bytes(int n, int h, int w);
+int launch_image_metrics_batch_u8(const uint8_t* const* a_host, const uint8_t* const* b_host, int n, int h, int w, int c,
+                                  int flags, double* out, void* workspace, size_t workspace_bytes, cudaStream_t s);
 int launch_flipx4(int expand, const float* const* src, float* const* dst, int n, int B, int H, int W, cudaStream_t s);
 int launch_train_batch_u8(const bin_train_sample_t* samples, int B, int h, int w, float* dst, int dst_B, int b0,
                           cudaStream_t s);
@@ -895,6 +898,11 @@ size_t bin_image_metrics_workspace_bytes(int h, int w) { return metrics_workspac
 int bin_image_metrics_u8(const uint8_t* a, const uint8_t* b, int h, int w, int c, double* out4, void* workspace,
                          size_t workspace_bytes, bin_stream_t s) {
   return launch_image_metrics_u8(a, b, h, w, c, out4, workspace, workspace_bytes, (cudaStream_t)s);
+}
+size_t bin_image_metrics_batch_workspace_bytes(int n, int h, int w) { return metrics_batch_workspace_bytes(n, h, w); }
+int bin_image_metrics_batch_u8(const uint8_t* const* a_host, const uint8_t* const* b_host, int n, int h, int w, int c,
+                               int flags, double* out, void* workspace, size_t workspace_bytes, bin_stream_t s) {
+  return launch_image_metrics_batch_u8(a_host, b_host, n, h, w, c, flags, out, workspace, workspace_bytes, (cudaStream_t)s);
 }
 int bin_flipx4_expand(const float* const* src_host, float* const* dst_host, int n, int B, int H, int W, bin_stream_t s) {
   return launch_flipx4(1, src_host, dst_host, n, B, H, W, (cudaStream_t)s);

@@ -5,7 +5,8 @@
 // metrics_tile_kernel: one CTA per kTile x kTile block of the image.  It stages the block plus a 5-pixel halo of both
 // images in shared memory, then per channel runs the horizontal passes of both windows (Gaussian in fp64, box in
 // int32: exact) into shared memory and the vertical passes over the valid outputs of the block.  Each CTA writes its
-// four partial sums to the workspace; metrics_reduce_kernel adds them in tile order.  The grid depends only on
+// four partial sums to the workspace; metrics_reduce_kernel adds them in tile order.  The batch kernels run n pairs of
+// one shape with the same per-tile code and the same tile-order sum, so each pair gets the single call's bits.  The grid depends only on
 // (h, w), every sum has a fixed order, so the result is bit-reproducible and independent of the SM count.
 #include <stdint.h>
 
@@ -48,8 +49,10 @@ __device__ __forceinline__ T block_sum(T v, T* red) {   // fixed tree: determini
   return t;   // valid in thread 0
 }
 
-__global__ void __launch_bounds__(kMetThreads) metrics_tile_kernel(const uint8_t* __restrict__ A, const uint8_t* __restrict__ B,
-                                                                   int h, int w, int c, MetricsPartial* __restrict__ part) {
+// One tile of one pair; bgr stages source channel 2-ch as channel ch (c = 3), so the per-thread channel loop sums in RGB
+// order over a BGR image.
+__device__ __forceinline__ void metrics_tile(const uint8_t* __restrict__ A, const uint8_t* __restrict__ B, int h, int w,
+                                             int c, bool bgr, MetricsPartial* __restrict__ part) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
   MetricsSmem& S = *reinterpret_cast<MetricsSmem*>(smem_raw);
   const int tid = threadIdx.x;
@@ -67,8 +70,9 @@ __global__ void __launch_bounds__(kMetThreads) metrics_tile_kernel(const uint8_t
       va = A[off];
       vb = B[off];
     }
-    S.a[ch][r][px] = va;
-    S.b[ch][r][px] = vb;
+    const int sc = bgr ? 2 - ch : ch;
+    S.a[sc][r][px] = va;
+    S.b[sc][r][px] = vb;
   }
   __syncthreads();
 
@@ -146,8 +150,25 @@ __global__ void __launch_bounds__(kMetThreads) metrics_tile_kernel(const uint8_t
   if (tid == 0) part[blockIdx.y * gridDim.x + blockIdx.x] = p;
 }
 
-__global__ void __launch_bounds__(kRedThreads) metrics_reduce_kernel(const MetricsPartial* __restrict__ part, int ntiles,
-                                                                     double n_gauss, double n_box, double* __restrict__ out4) {
+__global__ void __launch_bounds__(kMetThreads) metrics_tile_kernel(const uint8_t* __restrict__ A, const uint8_t* __restrict__ B,
+                                                                   int h, int w, int c, MetricsPartial* __restrict__ part) {
+  metrics_tile(A, B, h, w, c, false, part);
+}
+
+struct MetricsPairs {
+  const uint8_t* a[BIN_METRICS_MAX_BATCH];
+  const uint8_t* b[BIN_METRICS_MAX_BATCH];
+};
+
+// blockIdx.z = pair; pair z's tiles occupy part[z * ntiles, (z + 1) * ntiles) in the single-pair kernel's tile order.
+__global__ void __launch_bounds__(kMetThreads) metrics_tile_batch_kernel(const MetricsPairs pairs, int h, int w, int c, int bgr,
+                                                                         MetricsPartial* __restrict__ part) {
+  const int z = blockIdx.z;
+  metrics_tile(pairs.a[z], pairs.b[z], h, w, c, bgr != 0, part + (size_t)z * gridDim.x * gridDim.y);
+}
+
+__device__ __forceinline__ void metrics_reduce(const MetricsPartial* __restrict__ part, int ntiles, double n_gauss,
+                                               double n_box, double* __restrict__ out4) {
   unsigned long long a = 0, q = 0;
   double g = 0.0, bx = 0.0;
   for (int i = threadIdx.x; i < ntiles; i += kRedThreads) {
@@ -168,6 +189,18 @@ __global__ void __launch_bounds__(kRedThreads) metrics_reduce_kernel(const Metri
   }
 }
 
+__global__ void __launch_bounds__(kRedThreads) metrics_reduce_kernel(const MetricsPartial* __restrict__ part, int ntiles,
+                                                                     double n_gauss, double n_box, double* __restrict__ out4) {
+  metrics_reduce(part, ntiles, n_gauss, n_box, out4);
+}
+
+// One CTA per pair: the same tile-order sum as metrics_reduce_kernel over that pair's slice.
+__global__ void __launch_bounds__(kRedThreads) metrics_reduce_batch_kernel(const MetricsPartial* __restrict__ part, int ntiles,
+                                                                           double n_gauss, double n_box,
+                                                                           double* __restrict__ out) {
+  metrics_reduce(part + (size_t)blockIdx.x * ntiles, ntiles, n_gauss, n_box, out + 4 * blockIdx.x);
+}
+
 static inline int metrics_ntiles(int h, int w) { return ((h + kTile - 1) / kTile) * ((w + kTile - 1) / kTile); }
 
 size_t metrics_workspace_bytes(int h, int w) {
@@ -175,16 +208,22 @@ size_t metrics_workspace_bytes(int h, int w) {
   return (size_t)metrics_ntiles(h, w) * sizeof(MetricsPartial);
 }
 
+static int check_metrics_args(const char* fn, int h, int w, int c, const double* out, const void* workspace) {
+  if (!out || !workspace) return fail(BIN_ERR_ARG, std::string(fn) + ": null argument");
+  if (c != 1 && c != 3) return fail(BIN_ERR_ARG, std::string(fn) + ": c must be 1 or 3");
+  if (h < 7 || w < 7) return fail(BIN_ERR_ARG, std::string(fn) + ": h and w must be at least 7 (the 7x7 SSIM window)");
+  if (h > 65535 || w > 65535 || (long long)h * w * c >= (1ll << 31))
+    return fail(BIN_ERR_ARG, std::string(fn) + ": image too large (h, w <= 65535 and h*w*c < 2^31)");
+  if ((reinterpret_cast<uintptr_t>(workspace) & 7) || (reinterpret_cast<uintptr_t>(out) & 7))
+    return fail(BIN_ERR_ARG, std::string(fn) + ": workspace and the output must be 8-byte aligned");
+  return BIN_OK;
+}
+
 int launch_image_metrics_u8(const uint8_t* a, const uint8_t* b, int h, int w, int c, double* out4, void* workspace,
                             size_t workspace_bytes, cudaStream_t s) {
   // every check precedes the first CUDA call
-  if (!a || !b || !out4 || !workspace) return fail(BIN_ERR_ARG, "image_metrics: null argument");
-  if (c != 1 && c != 3) return fail(BIN_ERR_ARG, "image_metrics: c must be 1 or 3");
-  if (h < 7 || w < 7) return fail(BIN_ERR_ARG, "image_metrics: h and w must be at least 7 (the 7x7 SSIM window)");
-  if (h > 65535 || w > 65535 || (long long)h * w * c >= (1ll << 31))
-    return fail(BIN_ERR_ARG, "image_metrics: image too large (h, w <= 65535 and h*w*c < 2^31)");
-  if ((reinterpret_cast<uintptr_t>(workspace) & 7) || (reinterpret_cast<uintptr_t>(out4) & 7))
-    return fail(BIN_ERR_ARG, "image_metrics: workspace and out4 must be 8-byte aligned");
+  if (!a || !b) return fail(BIN_ERR_ARG, "image_metrics: null argument");
+  BIN_TRY(check_metrics_args("image_metrics", h, w, c, out4, workspace));
   if (workspace_bytes < metrics_workspace_bytes(h, w))
     return fail(BIN_ERR_ARG, "image_metrics: workspace too small (see bin_image_metrics_workspace_bytes)");
 
@@ -197,6 +236,41 @@ int launch_image_metrics_u8(const uint8_t* a, const uint8_t* b, int h, int w, in
   const double n_gauss = (h >= 11 && w >= 11) ? (double)c * (h - 10) * (w - 10) : 0.0;
   const double n_box = (double)c * (h - 6) * (w - 6);
   metrics_reduce_kernel<<<1, kRedThreads, 0, s>>>(part, metrics_ntiles(h, w), n_gauss, n_box, out4);
+  BIN_CUDA_OK(cudaGetLastError());
+  return BIN_OK;
+}
+
+size_t metrics_batch_workspace_bytes(int n, int h, int w) {
+  if (n < 1 || n > BIN_METRICS_MAX_BATCH) return 0;
+  return (size_t)n * metrics_workspace_bytes(h, w);
+}
+
+int launch_image_metrics_batch_u8(const uint8_t* const* a_host, const uint8_t* const* b_host, int n, int h, int w, int c,
+                                  int flags, double* out, void* workspace, size_t workspace_bytes, cudaStream_t s) {
+  // every check precedes the first CUDA call
+  if (!a_host || !b_host) return fail(BIN_ERR_ARG, "image_metrics_batch: null pointer table");
+  if (n < 1 || n > BIN_METRICS_MAX_BATCH) return fail(BIN_ERR_ARG, "image_metrics_batch: n must be 1..BIN_METRICS_MAX_BATCH");
+  if (flags & ~BIN_METRICS_BGR) return fail(BIN_ERR_ARG, "image_metrics_batch: unknown flag");
+  if ((flags & BIN_METRICS_BGR) && c != 3) return fail(BIN_ERR_ARG, "image_metrics_batch: BIN_METRICS_BGR needs c = 3");
+  BIN_TRY(check_metrics_args("image_metrics_batch", h, w, c, out, workspace));
+  if (workspace_bytes < metrics_batch_workspace_bytes(n, h, w))
+    return fail(BIN_ERR_ARG, "image_metrics_batch: workspace too small (see bin_image_metrics_batch_workspace_bytes)");
+  MetricsPairs pairs = {};
+  for (int i = 0; i < n; ++i) {
+    if (!a_host[i] || !b_host[i]) return fail(BIN_ERR_ARG, "image_metrics_batch: null image pointer");
+    pairs.a[i] = a_host[i];
+    pairs.b[i] = b_host[i];
+  }
+
+  static std::atomic<unsigned long long> smem_mask{0};
+  BIN_TRY(ensure_dynamic_smem(metrics_tile_batch_kernel, (int)sizeof(MetricsSmem), smem_mask));
+  MetricsPartial* part = static_cast<MetricsPartial*>(workspace);
+  const dim3 grid((w + kTile - 1) / kTile, (h + kTile - 1) / kTile, n);
+  metrics_tile_batch_kernel<<<grid, kMetThreads, sizeof(MetricsSmem), s>>>(pairs, h, w, c, flags & BIN_METRICS_BGR, part);
+  BIN_CUDA_OK(cudaGetLastError());
+  const double n_gauss = (h >= 11 && w >= 11) ? (double)c * (h - 10) * (w - 10) : 0.0;
+  const double n_box = (double)c * (h - 6) * (w - 6);
+  metrics_reduce_batch_kernel<<<n, kRedThreads, 0, s>>>(part, metrics_ntiles(h, w), n_gauss, n_box, out);
   BIN_CUDA_OK(cudaGetLastError());
   return BIN_OK;
 }

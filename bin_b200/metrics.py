@@ -3,7 +3,8 @@
 ``image_metrics`` runs one sm_90a kernel pair (bin_image_metrics_u8) over a uint8 pair and returns its mean |a-b|,
 MSE, Gaussian-11 SSIM (utils/util.py:211-231) and box-7 SSIM (skimage <= 0.17 compare_ssim defaults).  PSNR is
 computed on the host from the exact integer sum of squares with the reference's own expressions, so it equals the
-reference bit for bit.
+reference bit for bit.  ``image_metrics_batch`` scores up to 16 pairs per launch and leaves the sums on the device, so
+an evaluation loop reads them one window late instead of synchronising per call.
 
 Drop-ins with the reference's names, signatures and return conventions:
   * ``calculate_psnr`` / ``calculate_ssim``  -- utils/util.py:201-250 (test.py:39-40, use_default_ssim = 0);
@@ -13,6 +14,7 @@ Only uint8 images and the default options test.py uses are supported; anything e
 there is no CPU path."""
 from __future__ import annotations
 
+import ctypes as C
 import math
 import sys
 import types
@@ -20,7 +22,7 @@ import types
 import numpy as np
 import torch
 
-from ._lib import BinB200Error, check, lib
+from ._lib import BIN_METRICS_BGR, BIN_METRICS_MAX_BATCH, BinB200Error, check, lib
 
 _DIMS_MSG = "Input images must have the same dimensions."      # utils/util.py:240, skimage _assert_compatible
 
@@ -72,6 +74,52 @@ def image_metrics(a, b):
     w < 11), box-7 SSIM), all Python floats."""
     s_abs, s_sq, g, bx, n = _metric_sums(a, b, "image_metrics")
     return s_abs / n, s_sq / n, g, bx
+
+
+def image_metrics_batch(pairs, bgr: bool = False) -> torch.Tensor:
+    """pairs: (a, b) uint8 CUDA tensors, all (h, w) or all (h, w, c) of one shape on one device, c = 1 or 3, h, w >= 7;
+    pairs may share a tensor.  Enqueues bin_image_metrics_batch_u8 on the current stream, one tile and one reduce launch
+    per BIN_METRICS_MAX_BATCH pairs, and returns at once, with no host synchronisation: a float64 (n, 4) device tensor
+    whose row i is { sum |a-b|, sum (a-b)^2, Gaussian-11 SSIM, box-7 SSIM } of pair i, the bits image_metrics' sums
+    come from.  bgr=True (c = 3) scores each image as its channel-reversed view: a BGR image (cv2, tensor2img_u8) gets
+    exactly the values of its RGB array, which is what test.py scores (read_image_np, test.py:58-66)."""
+    pairs = [tuple(p) for p in pairs]
+    if not pairs or any(len(p) != 2 for p in pairs):
+        raise BinB200Error("image_metrics_batch: give one or more (a, b) pairs")
+    first = pairs[0][0]
+    for x in (t for p in pairs for t in p):
+        if not isinstance(x, torch.Tensor) or not x.is_cuda or x.dtype != torch.uint8:
+            raise BinB200Error("image_metrics_batch: uint8 CUDA tensors only")
+        if x.shape != first.shape:
+            raise ValueError(_DIMS_MSG)
+        if x.device != first.device:
+            raise BinB200Error(f"image_metrics_batch: images on different devices ({first.device}, {x.device})")
+    shape = tuple(first.shape)
+    if len(shape) == 2:
+        c = 1
+    elif len(shape) == 3 and shape[2] in (1, 3):
+        c = shape[2]
+    else:
+        raise BinB200Error(f"image_metrics_batch: images must be (h, w), (h, w, 1) or (h, w, 3), got {shape}")
+    if bgr and c != 3:
+        raise BinB200Error("image_metrics_batch: bgr=True needs (h, w, 3) images")
+    h, w = shape[0], shape[1]
+    L = lib()
+    flags = BIN_METRICS_BGR if bgr else 0
+    with torch.cuda.device(first.device):
+        imgs = [(a.contiguous(), b.contiguous()) for a, b in pairs]
+        out = torch.empty((len(pairs), 4), dtype=torch.float64, device=first.device)
+        stream = torch.cuda.current_stream()
+        for k in range(0, len(imgs), BIN_METRICS_MAX_BATCH):
+            group = imgs[k:k + BIN_METRICS_MAX_BATCH]
+            n = len(group)
+            ws = torch.empty(max(int(L.bin_image_metrics_batch_workspace_bytes(n, h, w)), 8), dtype=torch.uint8,
+                             device=first.device)
+            pa = (C.c_void_p * n)(*[a.data_ptr() for a, _ in group])
+            pb = (C.c_void_p * n)(*[b.data_ptr() for _, b in group])
+            check(L.bin_image_metrics_batch_u8(pa, pb, n, h, w, c, flags, out[k].data_ptr(), ws.data_ptr(), ws.numel(),
+                                               stream.cuda_stream))
+    return out
 
 
 # ----------------------------------------------------------------------------- utils/util.py:201-250

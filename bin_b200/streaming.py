@@ -186,41 +186,87 @@ class WindowStep(NamedTuple):
 
 
 class VideoPlan:
-    """stream_video's schedule, without tensors: call arrive() once per frame and end() when the video ends; each
-    returns the windows (WindowStep) due at that point, in order.  Window i is due once frame i+3 has arrived; the last
-    two windows read no frame i+3 and are due at the end.  live is the window's node set (rdn._window_live).
+    """stream_video's schedule, without tensors: call arrive() once per frame and end() when the frames end; each
+    returns the windows (WindowStep) due at that point, in order.  Window i is due once frame min(i+3, N-1) has arrived;
+    without n the last two windows read no frame i+3 and are due at the end.  live is the window's node set
+    (rdn._window_live).
 
-    A stage-1 output is named by its pair of frame positions and evaluated once per video, the first time a window
-    reads it at a live position.  Later windows never read below the first pair (and first frame) of the next window,
-    so after window i everything below window i+1's is dropped: at most six frames and five pairs are held.  With all
-    14 outputs an N-frame video costs N+1 stage-1 calls, 12 per window for stages 2-4, 13N - 11 in all."""
+    windows = range(a, b) plans only windows a .. b-1 of the video, from frames that start at position max(a-2, 0)
+    (next_pos names the position the next frame takes); n, the video's frame count, is needed only when window b-1 reads
+    a clamped end frame (b-1 >= n-3), and end() raises when it was needed and not given.  complete says that every
+    window of the range is out, so no more frames need to arrive.
 
-    def __init__(self, live):
+    A stage-1 output is named by its pair of frame positions and evaluated once, the first time a window of the plan
+    reads it at a live position (so the first window of a range evaluates all its live pairs).  Later windows never read
+    below the first pair (and first frame) of the next window, so after window i everything below window i+1's is
+    dropped: at most six frames and five pairs are held.  With all 14 outputs an N-frame video costs N+1 stage-1 calls,
+    12 per window for stages 2-4, 13N - 11 in all; a range of windows that reads no clamped frame b-a+4 stage-1 calls
+    and 12 (b-a) for stages 2-4."""
+
+    def __init__(self, live, windows: Optional[range] = None, n: Optional[int] = None):
+        if windows is not None and (not isinstance(windows, range) or windows.step != 1 or not 0 <= windows.start < windows.stop):
+            raise BinB200Error(f"windows must be a non-empty range(a, b) with 0 <= a < b; got {windows!r}")
+        if n is not None and windows is not None and windows.stop > n - 1:
+            raise BinB200Error(f"an {n}-frame video has windows 0..{n - 2}; {windows!r} is not among them")
         self.live1 = [a for a in range(5) if (1, a) in live]
         self.later = _later_calls(live)
+        self.n = n
+        self.first = 0 if windows is None else windows.start
+        self.stop = None if windows is None else windows.stop          # None: to the end of the video
+        if self.stop is None and n is not None:
+            self.stop = max(n - 1, 0)
+        self.start = max(self.first - 2, 0)         # position of the first frame
         self.arrived = 0
         self.ended = False
-        self.done = 0                               # windows returned so far
+        self.done = self.first                      # the next window to return
         self.pairs: set = set()                     # pairs evaluated and not dropped
-        self.low = 0                                # the lowest frame position not dropped
+        self.low = self.start                       # the lowest frame position not dropped
+
+    @property
+    def next_pos(self) -> int:
+        return self.start + self.arrived
+
+    @property
+    def complete(self) -> bool:
+        return self.stop is not None and self.done >= self.stop
 
     def arrive(self) -> List[WindowStep]:
+        if self.complete or (self.n is not None and self.next_pos >= self.n):
+            raise BinB200Error(f"VideoPlan: frame {self.next_pos} arrived after the plan's last window")
         self.arrived += 1
-        return self._due(self.arrived - 3)
+        stop = self.next_pos - 3
+        if self.n is not None and self.next_pos == self.n:
+            stop = self.stop                        # the last frame: the clamped windows are due
+        return self._due(stop if self.stop is None else min(stop, self.stop))
 
     def end(self) -> List[WindowStep]:
         self.ended = True
-        return self._due(self.arrived - 1)
+        n = self.next_pos
+        if self.stop is None:
+            return self._due(n - 1)
+        if self.complete:
+            return []
+        if self.n is not None:
+            raise BinB200Error(f"the frames ended at position {n - 1}; windows up to {self.stop - 1} of the "
+                               f"{self.n}-frame video need frames up to {min(self.stop + 2, self.n - 1)}")
+        raise BinB200Error(f"the frames ended at position {n - 1} before window {self.done} was due: windows "
+                           f"{self.done}..{self.stop - 1} read clamped end frames, so the video's length n is needed")
+
+    def _n(self) -> int:
+        """The frame count windows are clamped to: n, or while it is unknown the frames so far (no window due before
+        the end of an unknown-length video reads a clamped end frame)."""
+        return self.n if self.n is not None else self.next_pos
 
     def _due(self, stop: int) -> List[WindowStep]:
-        steps, n = [], self.arrived
+        steps, n = [], self._n()
+        last = self.stop - 1 if self.stop is not None else (n - 2 if self.ended else None)
         for i in range(self.done, stop):
-            pos = test_py_window(i, n)              # while the video runs, i <= n-4: no window so far is clamped at the end
+            pos = test_py_window(i, n)
             pairs = [(pos[a], pos[a + 1]) for a in self.live1]
             fresh = tuple(dict.fromkeys(p for p in pairs if p not in self.pairs))
             self.pairs.update(fresh)
-            if self.ended and i == n - 2:
-                first, low = (n, n), n              # the last window: drop everything
+            if i == last:
+                first, low = (n, n), self.next_pos  # the plan's last window: drop everything
             else:
                 nxt = test_py_window(i + 1, n)
                 first, low = (nxt[0], nxt[1]), nxt[0]
@@ -235,9 +281,11 @@ class VideoPlan:
 class VideoStream:
     """The iterator stream_video returns: (i, outputs) per window; backbone_calls counts the calls run so far."""
 
-    def __init__(self, net, frames: Iterable[torch.Tensor]):
+    def __init__(self, net, frames: Iterable[torch.Tensor], windows: Optional[range] = None, n: Optional[int] = None):
         self.net = net
         self.backbone_calls = 0
+        self._range = (windows, n)
+        VideoPlan(frozenset(), windows, n)          # reject a bad range now rather than at the first frame
         self._it = self._windows(iter(frames))
 
     def __iter__(self) -> "VideoStream":
@@ -256,7 +304,7 @@ class VideoStream:
                 raise BinB200Error("stream_video expects (B,3,H,W) fp32 CUDA frames (see upload_frame_u8)")
             if plan is None:
                 mode, shape = self._mode(), (frame.shape, frame.device)
-                plan = VideoPlan(_window_live(range(14) if mode[1] is None else mode[1][0]))
+                plan = VideoPlan(_window_live(range(14) if mode[1] is None else mode[1][0]), *self._range)
             elif (frame.shape, frame.device) != shape:
                 raise BinB200Error(f"stream_video: frame {plan.arrived} is {tuple(frame.shape)} on {frame.device}; "
                                    f"the video's first frame is {tuple(shape[0])} on {shape[1]}")
@@ -264,11 +312,15 @@ class VideoStream:
             if mode[0] is not None:
                 with torch.no_grad(), torch.cuda.device(frame.device):
                     frame = ops.flipx4_expand([frame])[0]
-            held[plan.arrived] = frame
+            held[plan.next_pos] = frame
             del frame                               # held[] alone keeps it, until the plan drops it
             for step in plan.arrive():
                 yield self._run(step, held, cache, mode)
-        for step in plan.end() if plan is not None else ():
+            if plan.complete:
+                return                              # the range is out: read no further frame
+        if plan is None:
+            plan = VideoPlan(frozenset(), *self._range)
+        for step in plan.end():
             yield self._run(step, held, cache, mode)
 
     def _mode(self):
@@ -289,7 +341,8 @@ class VideoStream:
         return step.i, o
 
 
-def stream_video(net, frames: Iterable[torch.Tensor]) -> VideoStream:
+def stream_video(net, frames: Iterable[torch.Tensor], windows: Optional[range] = None,
+                 n: Optional[int] = None) -> VideoStream:
     """Every window test.py runs over a video, in its order: for frames F[0..N-1] (an iterable of (B,3,H,W) fp32 CUDA
     frames, e.g. from upload_frame_u8), yields (i, outputs) for i = 0 .. N-2, where outputs is exactly what
     net(*[F[j] for j in test_py_window(i, N)]) returns, in the net's precision, output selection and self-ensemble
@@ -301,5 +354,11 @@ def stream_video(net, frames: Iterable[torch.Tensor]) -> VideoStream:
     iterator's backbone_calls counts them.  At most six frames (expanded once each under the ensemble) and the stage-1
     outputs a later window reads are held.  Outputs at positions 0-3 and 10 are those stage-1 tensors, shared with other
     windows (and, in the first and the last window, between two positions of one tuple): read them, do not write them.  Inference
-    only: like StreamingBIN.push, every window runs under torch.no_grad()."""
-    return VideoStream(net, frames)
+    only: like StreamingBIN.push, every window runs under torch.no_grad().
+
+    windows = range(a, b) runs only windows a .. b-1 (a piece of the video, e.g. one rank's share): `frames` then starts
+    at position max(a-2, 0), and no frame after position min(b+2, N-1) is read.  n = N is needed only when a window of
+    the range reads a clamped end frame (b-1 >= N-3); without it that raises when the frames end.  The first window of
+    a range evaluates all its live stage-1 pairs, so a range costs at most 4 stage-1 calls more than the same windows
+    inside a whole-video stream."""
+    return VideoStream(net, frames, windows, n)

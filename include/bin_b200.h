@@ -369,6 +369,18 @@ size_t bin_image_metrics_workspace_bytes(int h, int w);
  * is checked (BIN_ERR_ARG) before the first CUDA call. */
 int bin_image_metrics_u8(const uint8_t* a, const uint8_t* b, int h, int w, int c, double* out4,
                          void* workspace, size_t workspace_bytes, bin_stream_t s);
+/* Up to BIN_METRICS_MAX_BATCH pairs of one shape in one tile launch (tiles x pairs) and one reduce launch (one CTA per
+ * pair), with no host synchronisation.  a_host[i], b_host[i]: device pointers as for bin_image_metrics_u8; pairs may
+ * share an operand.  out (device fp64[4n]): out[4i..4i+3] = the four values bin_image_metrics_u8 writes for pair i, bit
+ * for bit; out[4n..] is not written.  flags: BIN_METRICS_BGR (c = 3 only) stages source channel 2-ch as channel ch, so a
+ * BGR image scores exactly what its RGB view scores (the SSIM sums run over the channels in order).  Workspace:
+ * bin_image_metrics_batch_workspace_bytes(n, h, w) (0 if n, h or w is out of range).  Every argument is checked
+ * (BIN_ERR_ARG) before the first CUDA call. */
+#define BIN_METRICS_MAX_BATCH 16
+#define BIN_METRICS_BGR 1
+size_t bin_image_metrics_batch_workspace_bytes(int n, int h, int w);
+int bin_image_metrics_batch_u8(const uint8_t* const* a_host, const uint8_t* const* b_host, int n, int h, int w, int c,
+                               int flags, double* out, void* workspace, size_t workspace_bytes, bin_stream_t s);
 
 /* ---- x4 flip self-ensemble: utils/test_util.py:110-132 flipx4_forward, for a whole 6-frame window ---------------- */
 /* Orientation o of an image x: 0 = x, 1 = flip W (torch.flip(x, (-1,))), 2 = flip H ((-2,)), 3 = flip H and W ((-2, -1)).
