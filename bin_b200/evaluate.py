@@ -441,9 +441,9 @@ def _flag(v: str) -> bool:
     raise argparse.ArgumentTypeError(f"not a truth value: {v!r}")
 
 
-def load_weights(net, path: str) -> None:
+def load_weights(net, path: str, strict: bool = True) -> None:
     """base_model.load_network (base_model.py:89-103): the checkpoint's keys without their 'InterpNet.' / 'module.'
-    prefix, loaded with strict=True."""
+    prefix, loaded with `strict` (path.strict_load of a train yml)."""
     sd = torch.load(path, map_location="cpu")
     clean = collections.OrderedDict()
     for k, v in sd.items():
@@ -451,7 +451,7 @@ def load_weights(net, path: str) -> None:
             if k.startswith(pre):
                 k = k[len(pre):]
         clean[k] = v
-    net.load_state_dict(clean, strict=True)
+    net.load_state_dict(clean, strict=strict)
 
 
 def main(argv=None) -> None:

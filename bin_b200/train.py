@@ -1,0 +1,585 @@
+"""Training BIN from the reference's option file (options/train/train_adobe_stage4.yml), on one GPU or one process per
+GPU under torchrun.  The reference never shipped its trainer; this is the loop its INTEGRATION recipe asks a user to
+write around bin_model, with every step of the hot path on the GPU:
+
+  * batches: trainset.DeviceBINDataset (BINDataset + create_dataloader, bit for bit), in create_dataloader's order:
+    sequential with one process, DistIterSampler under torchrun (restated here as `DistIterSampler`);
+  * step: bin_model.optimize_parameters (bin_model.py:130-141): zero_grad, the window on LQs[:, 0..5], loss.pixel_loss
+    of the 14 outputs against get_info's GT list with the cycle terms, x pixel_weight, backward, optim.Adam.step;
+  * the per-output losses are running sums on the device, read only at print_freq iterations, so an ordinary iteration
+    does not synchronise the host with the device;
+  * validation every val_freq iterations at batch 1: the 14 losses and their mean, PSNR and SSIM of each output
+    (utils/util.py calculate_psnr / calculate_ssim on tensor2img images), windows sharded over the ranks and the sums
+    all-reduced; ReduceLROnPlateau steps on the mean validation loss;
+  * checkpoints `<iter>_G.pth` (base_model.save_network) and `<iter>.state` (save_training_state), and resume from
+    them at the exact batch, crop and flip the saved run would have drawn next.
+
+Where it departs from the reference: validation crops come from a `random.Random(manual_seed)` made afresh at every
+validation, where the reference's validation would draw from the global `random` the training crops draw from.  Every
+validation then scores the same crops, and validating does not change the training batches.
+
+python -m bin_b200.train -opt <yml> [--checkpointing recompute] [--max_grad_norm X] [--skip_nonfinite]
+[--deterministic] [--from_sharp] [--arch G0,D]; under torchrun each rank trains on its own GPU."""
+from __future__ import annotations
+
+import argparse
+import logging
+import math
+import os
+import random
+import sys
+from dataclasses import dataclass, field
+from typing import Dict, Iterator, List, Optional, Sequence, Tuple
+
+import numpy as np
+import torch
+
+from . import rdn
+from ._lib import BinB200Error
+from .evaluate import load_weights
+from .loss import pixel_loss
+from .metrics import image_metrics_batch
+from .optim import Adam
+from .streaming import tensor2img_u8
+from .trainset import DeviceBINDataset, DeviceClip
+
+NOUT = 14
+# bin_model.get_info (nframes 6, bin_model.py:530-534): output k is scored against I_GT_OF[k]; feed_data maps I(2m+1) to
+# GTenh[:, m] and I(2m) to GTinp[:, m-1] (bin_model.py:164-174)
+I_GT_OF = (2, 4, 6, 8, 3, 5, 7, 4, 6, 5, 10, 9, 8, 7)
+IGNORED = ("gpu_ids", "datasets.train.n_workers", "datasets.val.n_workers")
+LOG_FORMAT = logging.Formatter('%(asctime)s.%(msecs)03d - %(levelname)s: %(message)s', datefmt='%y-%m-%d %H:%M:%S')
+
+
+# ----------------------------------------------------------------------------- options
+@dataclass
+class Options:
+    """The keys of a train yml this driver honours (options/train/train_adobe_stage4.yml)."""
+    name: str
+    train_root: str                      # datasets.train.dataroot_LQ
+    train_mode: str                      # datasets.train.name: <root>/<mode>, <mode>_blur, <mode>_list
+    batch_size: int                      # global: batch_size // world per rank
+    train_lq_size: Tuple[int, int, int]
+    use_shuffle: bool                    # read; create_dataloader passes shuffle=False whatever it says
+    val_root: Optional[str]              # None: no datasets.val, no validation
+    val_mode: Optional[str]
+    val_lq_size: Optional[Tuple[int, int, int]]
+    version: int
+    pretrain_model_G: Optional[str]
+    strict_load: bool
+    resume_state: Optional[str]
+    save_path: str
+    lr: float
+    beta1: float
+    beta2: float
+    weight_decay: float
+    pixel_criterion: str
+    pixel_weight: float
+    factor: float
+    patience: int
+    epochs: int
+    val_freq: int
+    manual_seed: int
+    print_freq: int
+    save_freq: int
+    ignored: List[str] = field(default_factory=list)
+
+    @property
+    def experiments_root(self) -> str:
+        return os.path.join(self.save_path, "experiments", self.name)      # options.parse
+
+    @property
+    def models_dir(self) -> str:
+        return os.path.join(self.experiments_root, "models")
+
+    @property
+    def state_dir(self) -> str:
+        return os.path.join(self.experiments_root, "training_state")
+
+
+def _get(opt: dict, key: str, default=KeyError):
+    node = opt
+    for part in key.split("."):
+        if not isinstance(node, dict) or part not in node:
+            if default is KeyError:
+                raise BinB200Error(f"train options: {key} is missing")
+            return default
+        node = node[part]
+    return node
+
+
+def _path(p) -> Optional[str]:
+    return None if p in (None, "") else os.path.expanduser(str(p))
+
+
+def parse_options(opt: dict) -> Options:
+    """The honoured keys of a parsed train yml.  Raises BinB200Error naming the key for what this driver does not do:
+    another model than bin_stage4, nframes other than 6, another lr_scheme than ReduceLROnPlateau, ft_tsa_only, an
+    unknown pixel_criterion."""
+    if _get(opt, "network_G.which_model_G") != "bin_stage4":
+        raise BinB200Error(f"network_G.which_model_G: {_get(opt, 'network_G.which_model_G')!r} is not trained here; "
+                           "only bin_stage4 is")
+    if int(_get(opt, "network_G.nframes")) != 6:
+        raise BinB200Error("network_G.nframes: only 6 (the 14-output bin_stage4 window) is trained here")
+    if _get(opt, "train.lr_scheme") != "ReduceLROnPlateau":
+        raise BinB200Error(f"train.lr_scheme: {_get(opt, 'train.lr_scheme')!r} is not supported; only "
+                           "ReduceLROnPlateau is")
+    if _get(opt, "train.ft_tsa_only", None):
+        raise BinB200Error("train.ft_tsa_only is not supported")
+    crit = _get(opt, "train.pixel_criterion")
+    if crit not in ("l1", "l2", "cb"):
+        raise BinB200Error(f"train.pixel_criterion: {crit!r} is not one of l1, l2, cb (bin_model.py:54-61)")
+    val = _get(opt, "datasets.val", None)
+    return Options(
+        name=str(_get(opt, "name")),
+        train_root=_path(_get(opt, "datasets.train.dataroot_LQ")),
+        train_mode=str(_get(opt, "datasets.train.name")),
+        batch_size=int(_get(opt, "datasets.train.batch_size")),
+        train_lq_size=tuple(int(v) for v in _get(opt, "datasets.train.LQ_size")),
+        use_shuffle=bool(_get(opt, "datasets.train.use_shuffle", False)),
+        val_root=_path(_get(opt, "datasets.val.dataroot_LQ")) if val else None,
+        val_mode=str(_get(opt, "datasets.val.name")) if val else None,
+        val_lq_size=tuple(int(v) for v in _get(opt, "datasets.val.LQ_size")) if val else None,
+        version=int(_get(opt, "network_G.version")),
+        pretrain_model_G=_path(_get(opt, "path.pretrain_model_G", None)),
+        strict_load=bool(_get(opt, "path.strict_load", True)),
+        resume_state=_path(_get(opt, "path.resume_state", None)),
+        save_path=_path(_get(opt, "path.save_path")),
+        lr=float(_get(opt, "train.lr_G")),
+        beta1=float(_get(opt, "train.beta1")),
+        beta2=float(_get(opt, "train.beta2")),
+        weight_decay=float(_get(opt, "train.weight_decay_G", 0) or 0),     # bin_model.py:65
+        pixel_criterion=crit,
+        pixel_weight=float(_get(opt, "train.pixel_weight")),
+        factor=float(_get(opt, "train.factor")),
+        patience=int(_get(opt, "train.patience")),
+        epochs=int(_get(opt, "train.epoch")),
+        val_freq=int(float(_get(opt, "train.val_freq"))),
+        manual_seed=int(_get(opt, "train.manual_seed")),
+        print_freq=int(float(_get(opt, "logger.print_freq"))),
+        save_freq=int(float(_get(opt, "logger.save_checkpoint_freq"))),
+        ignored=[k for k in IGNORED if _get(opt, k, None) is not None])
+
+
+def load_options(path: str) -> Options:
+    import yaml
+    with open(path) as fh:
+        return parse_options(yaml.safe_load(fh))
+
+
+# ----------------------------------------------------------------------------- order and schedule
+class DistIterSampler:
+    """data/data_sampler.py DistIterSampler over a dataset of n samples: each epoch, randperm(total_size) seeded by the
+    epoch, every index % n, then rank, rank + world, ... (total_size = world * ceil(n * ratio / world))."""
+
+    def __init__(self, n: int, world: int, rank: int, ratio: int = 100):
+        self.n, self.world, self.rank, self.epoch = n, world, rank, 0
+        self.num_samples = int(math.ceil(n * ratio / world))
+        self.total_size = self.num_samples * world
+
+    def set_epoch(self, epoch: int) -> None:
+        self.epoch = epoch
+
+    def __iter__(self) -> Iterator[int]:
+        g = torch.Generator()
+        g.manual_seed(self.epoch)
+        idx = [v % self.n for v in torch.randperm(self.total_size, generator=g).tolist()]
+        return iter(idx[self.rank:self.total_size:self.world])
+
+    def __len__(self) -> int:
+        return self.num_samples
+
+
+class SequentialSampler:
+    """create_dataloader with one process: shuffle=False, so each epoch walks the (once shuffled) dataset in order."""
+
+    def __init__(self, n: int):
+        self.n = n
+
+    def set_epoch(self, epoch: int) -> None:
+        pass
+
+    def __iter__(self) -> Iterator[int]:
+        return iter(range(self.n))
+
+    def __len__(self) -> int:
+        return self.n
+
+
+def make_sampler(n: int, world: int, rank: int, ratio: int = 100):
+    return SequentialSampler(n) if world == 1 else DistIterSampler(n, world, rank, ratio)
+
+
+def per_rank_batch(batch_size: int, world: int) -> int:
+    if batch_size % world:
+        raise BinB200Error(f"datasets.train.batch_size {batch_size} is not divisible by the {world} ranks "
+                           "(create_dataloader asserts it)")
+    return batch_size // world
+
+
+def events(step: int, print_freq: int, val_freq: int, save_freq: int) -> Tuple[str, ...]:
+    """What runs after iteration `step` (1-based): 'print', 'val', 'save', in that order."""
+    return tuple(k for k, f in (("print", print_freq), ("val", val_freq), ("save", save_freq)) if f > 0 and step % f == 0)
+
+
+def resume_position(state_epoch: int, state_iter: int, iters_per_epoch: int) -> Tuple[int, int]:
+    """-> (epoch, batches of it already run) after `state_iter` iterations of `iters_per_epoch` each, from epoch 0.
+    A state saved after the last batch of epoch e says epoch e and resumes at batch 0 of epoch e + 1."""
+    if iters_per_epoch < 1:
+        raise BinB200Error("resume: an epoch of this dataset has no full batch")
+    epoch, done = divmod(state_iter, iters_per_epoch)
+    if state_epoch != (epoch - 1 if done == 0 and state_iter > 0 else epoch):
+        raise BinB200Error(f"resume: iteration {state_iter} is in epoch {epoch} at {iters_per_epoch} iterations per "
+                           f"epoch, but the state says epoch {state_epoch}; the dataset or batch size differs from "
+                           "the saved run's")
+    return epoch, done
+
+
+def gt_list(batch: Dict) -> List[torch.Tensor]:
+    """get_info(mode=1)'s GT list of a DeviceBINDataset batch."""
+    return [batch["GTenh"][:, i // 2] if i % 2 else batch["GTinp"][:, i // 2 - 1] for i in I_GT_OF]
+
+
+# ----------------------------------------------------------------------------- logs
+def train_message(epoch: int, step: int, lr: float, avg: Sequence[float], guard: Optional[Tuple[int, float]]) -> str:
+    """avg: the 14 per-output losses and their mean (get_current_log('train')'s '0'..'13', 'Al'), averaged since the
+    last message; guard: (skipped steps, last grad norm) when the step is guarded."""
+    msg = "<epoch:{:3d}, iter:{:8,d}, lr:{:.3e}> ".format(epoch, step, lr)
+    msg += "".join("{:s}: {:.4e} ".format(k, v) for k, v in zip([str(i) for i in range(NOUT)] + ["Al"], avg))
+    if guard is not None:
+        skipped, norm = guard
+        msg += "skipped: {:d} grad_norm: {} ".format(skipped, "n/a" if norm is None else "{:.4e}".format(norm))
+    return msg.rstrip()
+
+
+def val_log(sums: Sequence[float]):
+    """get_current_log('val') from the reduced sums [14 losses, mean loss, 14 PSNR, 14 SSIM, window count]:
+    -> (avg_log_dict, avg_psnr_dict, mean PSNR, mean SSIM, mean loss)."""
+    sums = [float(v) for v in sums]
+    n = sums[-1]
+    loss, psnr, ssim = sums[:NOUT + 1], sums[NOUT + 1:2 * NOUT + 1], sums[2 * NOUT + 1:3 * NOUT + 1]
+    avg_log = {"Al" + str(i): loss[i] / n for i in range(NOUT)}
+    avg_log["Al"] = loss[NOUT] / n
+    avg_psnr = {"Ap" + str(i): psnr[i] / n for i in range(NOUT)}
+    psnr_mean = sum(psnr[i] / n for i in range(NOUT)) / NOUT
+    avg_psnr["Ap"] = psnr_mean
+    return avg_log, avg_psnr, psnr_mean, sum(ssim[i] / n for i in range(NOUT)) / NOUT, loss[NOUT] / n
+
+
+def val_message(epoch: int, step: int, log) -> str:
+    avg_log, avg_psnr, _, ssim_mean, _ = log
+    msg = "<epoch:{:3d}, iter:{:8,d}> # Validation # ".format(epoch, step)
+    msg += "".join("{:s}: {:.4e} ".format(k, v) for k, v in avg_log.items())
+    msg += "".join("{:s}: {:.4f} ".format(k, v) for k, v in avg_psnr.items())
+    return msg + "As: {:.4f}".format(ssim_mean)
+
+
+def window_scores(rows: np.ndarray, losses: np.ndarray, h: int, w: int) -> List[float]:
+    """One validation window's terms, as the reference's meters take them: rows (14, 4) float64 of image_metrics_batch
+    (sum |a-b|, sum (a-b)^2, Gaussian SSIM, box SSIM) of each output against its GT; losses (15,) float32 (14 + mean).
+    -> [14 losses, mean loss, 14 calculate_psnr, 14 calculate_ssim] as Python floats."""
+    n = h * w * 3
+    psnr = []
+    for r in rows:
+        mse = int(r[1]) / n                                 # utils/util.py:201-208, as metrics.calculate_psnr
+        psnr.append(float('inf') if mse == 0 else 20 * math.log10(255.0 / math.sqrt(mse)))
+    return [float(v) for v in losses] + psnr + [float(np.float64(r[2])) for r in rows]
+
+
+def reduce_sums(sums: torch.Tensor) -> torch.Tensor:
+    """All-reduce (sum) a float64 tensor over the ranks of the initialised process group, in place."""
+    if torch.distributed.is_available() and torch.distributed.is_initialized() and torch.distributed.get_world_size() > 1:
+        torch.distributed.all_reduce(sums)
+    return sums
+
+
+# ----------------------------------------------------------------------------- data
+def _from_sharp_tree(root: str, mode: str, device, lq_size, rng) -> DeviceBINDataset:
+    """Clips built by DeviceClip.from_sharp from <root>/<mode>/<folder> alone, folders in os.listdir order."""
+    import cv2
+    clips = []
+    for folder in os.listdir(os.path.join(root, mode)):
+        d = os.path.join(root, mode, folder)
+        names = sorted(os.listdir(d))
+        want = [str(k).zfill(5) + ".png" for k in range(1, len(names) + 1)]
+        if names != want:
+            raise BinB200Error(f"--from_sharp: the sharp frames of {d} must be named 00001.png, 00002.png, ...")
+        imgs = []
+        for nm in names:
+            img = cv2.imread(os.path.join(d, nm), cv2.IMREAD_UNCHANGED)
+            if img is None or img.dtype != np.uint8 or img.ndim != 3 or img.shape[2] < 3:
+                raise BinB200Error(f"--from_sharp: {os.path.join(d, nm)} is not an 8-bit colour image")
+            imgs.append(torch.from_numpy(np.ascontiguousarray(img[:, :, :3])))
+        clips.append(DeviceClip.from_sharp(folder, torch.stack(imgs).to(device)))
+    return DeviceBINDataset(clips, lq_size=lq_size, rng=rng)
+
+
+def build_dataset(root: str, mode: str, device, lq_size, rng, from_sharp: bool) -> DeviceBINDataset:
+    if from_sharp:
+        return _from_sharp_tree(root, mode, device, lq_size, rng)
+    return DeviceBINDataset.from_tree(root, mode=mode, device=device, lq_size=lq_size, rng=rng)
+
+
+# ----------------------------------------------------------------------------- the driver
+class Trainer:
+    """One rank's training run.  `run()` trains to the end of the yml's epochs (or `max_iters` iterations in all);
+    `net` is the unwrapped module, `opt` the optimizer, `scheduler` the ReduceLROnPlateau.
+
+    rank / world default to the initialised process group, else (0, 1); the device is cuda:<LOCAL_RANK> under a
+    process group, else the current device.  sync_debug: a torch.cuda.set_sync_debug_mode level under which every
+    iteration after the first (batch, step, running sums) runs, for checking that it never waits on the device."""
+
+    def __init__(self, opts: Options, *, checkpointing: Optional[str] = None, max_grad_norm: Optional[float] = None,
+                 skip_nonfinite: bool = False, deterministic: bool = False, from_sharp: bool = False,
+                 arch: Optional[Tuple[int, int]] = None, ratio: int = 100, sync_debug: Optional[str] = None,
+                 stdout: bool = True):
+        self.o = opts
+        dist = torch.distributed.is_available() and torch.distributed.is_initialized()
+        self.rank = torch.distributed.get_rank() if dist else 0
+        self.world = torch.distributed.get_world_size() if dist else 1
+        self.dev = torch.device("cuda", int(os.environ.get("LOCAL_RANK", "0")) if dist else torch.cuda.current_device())
+        self.sync_debug = sync_debug
+        self.log = logging.Logger(f"bin_b200.train.{id(self)}", logging.INFO)
+        if self.rank == 0:
+            os.makedirs(opts.models_dir, exist_ok=True)
+            os.makedirs(opts.state_dir, exist_ok=True)
+            for h in [logging.FileHandler(os.path.join(opts.experiments_root, f"train_{opts.name}.log"), mode="a")] + \
+                     ([logging.StreamHandler(sys.stdout)] if stdout else []):
+                h.setFormatter(LOG_FORMAT)
+                self.log.addHandler(h)
+        for k in opts.ignored:
+            self.log.info(f"{k} is ignored: one process per GPU under torchrun, batches are built on the GPU")
+        if deterministic:
+            torch.use_deterministic_algorithms(True)
+            torch.utils.deterministic.fill_uninitialized_memory = False     # every workspace byte read is written
+        self.B = per_rank_batch(opts.batch_size, self.world)
+
+        random.seed(opts.manual_seed)
+        torch.manual_seed(opts.manual_seed)
+        with torch.cuda.device(self.dev):
+            self.train_set = build_dataset(opts.train_root, opts.train_mode, self.dev, opts.train_lq_size, random,
+                                           from_sharp)
+            self.val_set = None
+            if opts.val_root is not None:
+                self.val_set = build_dataset(opts.val_root, opts.val_mode, self.dev, opts.val_lq_size,
+                                             random.Random(opts.manual_seed), from_sharp)
+        self.sampler = make_sampler(len(self.train_set), self.world, self.rank, ratio)
+        self.iters_per_epoch = len(self.sampler) // self.B
+        if self.iters_per_epoch < 1:
+            raise BinB200Error(f"{len(self.train_set)} training windows make no batch of {self.B} per rank")
+        self.log.info(f"Training {opts.name}: {len(self.train_set)} windows, batch {opts.batch_size} over {self.world} "
+                      f"rank(s), {self.iters_per_epoch} iterations per epoch, {opts.epochs} epochs")
+
+        net = rdn.bin_stage4_lstm()
+        if arch is not None:
+            net.model = rdn.RDN_residual_interp_5_input(lstm=True, GO=arch[0], D=arch[1])
+        if opts.pretrain_model_G and not opts.resume_state:
+            load_weights(net, opts.pretrain_model_G, strict=opts.strict_load)
+            self.log.info(f"Loading model for G [{opts.pretrain_model_G:s}] ...")
+        self.net = net.to(self.dev).train()
+        if checkpointing is not None:
+            rdn.set_activation_checkpointing(self.net, checkpointing)
+        params = []
+        for k, v in self.net.named_parameters():
+            if v.requires_grad:
+                params.append(v)
+            else:
+                self.log.warning(f"Params [{k:s}] will not optimize.")
+        self.opt = Adam(params, lr=opts.lr, weight_decay=opts.weight_decay, betas=(opts.beta1, opts.beta2),
+                        max_grad_norm=max_grad_norm, skip_nonfinite=skip_nonfinite)
+        self.guarded = max_grad_norm is not None or skip_nonfinite
+        self.scheduler = torch.optim.lr_scheduler.ReduceLROnPlateau(self.opt, "min", factor=opts.factor,
+                                                                    patience=opts.patience)
+        self.model = self.net
+        if self.world > 1:
+            from torch.nn.parallel import DistributedDataParallel
+            self.model = DistributedDataParallel(self.net, device_ids=[self.dev.index])   # bin_model.py:39-41
+
+        self.step = 0
+        if opts.resume_state:
+            self._resume(opts.resume_state)
+        with torch.cuda.device(self.dev):
+            self.loss_sums = torch.zeros(NOUT + 1, dtype=torch.float32, device=self.dev)
+        self.loss_count = 0
+
+    # ------------------------------------------------------------------ checkpoints
+    def _resume(self, path: str) -> None:
+        state = torch.load(path, map_location=self.dev)
+        weights = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(path))), "models",
+                               "{}_G.pth".format(state["iter"]))
+        load_weights(self.net, weights, strict=True)
+        if len(state["optimizers"]) != 1 or len(state["schedulers"]) != 1:
+            raise BinB200Error(f"resume: {path} holds {len(state['optimizers'])} optimizers and "
+                               f"{len(state['schedulers'])} schedulers; this driver has one of each")
+        self.opt.load_state_dict(state["optimizers"][0])
+        self.scheduler.load_state_dict(state["schedulers"][0])
+        resume_position(int(state["epoch"]), int(state["iter"]), self.iters_per_epoch)
+        self.step = int(state["iter"])
+        # the crops and flips of the samples the saved run drew (every iteration draws for B samples)
+        self.train_set.skip_draws(self.step * self.B)
+        self.log.info(f"Resuming training from epoch: {self.epoch}, iter: {self.step} ({weights}).")
+
+    def save(self) -> None:
+        """base_model.save_network and save_training_state at the current iteration (rank 0 writes)."""
+        opt_sd, sch_sd = self.opt.state_dict(), self.scheduler.state_dict()
+        if self.rank != 0:
+            return
+        sd = self.net.state_dict()
+        for k, v in sd.items():
+            sd[k] = v.cpu()
+        torch.save(sd, os.path.join(self.o.models_dir, "{}_G.pth".format(self.step)))
+        torch.save({"epoch": self.epoch, "iter": self.step, "schedulers": [sch_sd], "optimizers": [opt_sd]},
+                   os.path.join(self.o.state_dir, "{}.state".format(self.step)))
+        self.log.info("Saving models and training states.")
+
+    # ------------------------------------------------------------------ one iteration
+    def train_step(self, batch: Dict) -> Tuple[torch.Tensor, List[torch.Tensor]]:
+        """bin_model.optimize_parameters on one batch: -> (loss, the 14 per-output losses), on the device."""
+        self.opt.zero_grad(set_to_none=True)
+        outs = self.model(*[batch["LQs"][:, k] for k in range(6)])
+        loss, losses = pixel_loss(outs, gt_list(batch), self.o.pixel_criterion, nframes=6, version=self.o.version)
+        (self.o.pixel_weight * loss).backward()
+        self.opt.step()
+        return loss, losses
+
+    def _batches(self) -> Iterator[Dict]:
+        """The batches of the epoch the next iteration is in, from the next one on."""
+        epoch, done = divmod(self.step, self.iters_per_epoch)
+        self.sampler.set_epoch(epoch)
+        it = iter(self.sampler)
+        for _ in range(done * self.B):
+            next(it)
+        return self.train_set.batches(it, self.B)
+
+    def run(self, max_iters: Optional[int] = None) -> None:
+        """Train to the end of the last epoch, or until `max_iters` iterations in all have run."""
+        o = self.o
+        end = o.epochs * self.iters_per_epoch
+        if max_iters is not None:
+            end = min(end, max_iters)
+        saved, first = None, True
+        with torch.cuda.device(self.dev):
+            while self.step < end:
+                batches = self._batches()
+                for _ in range(min(end, (self.step // self.iters_per_epoch + 1) * self.iters_per_epoch) - self.step):
+                    mode = torch.cuda.get_sync_debug_mode()
+                    if self.sync_debug is not None and not first:
+                        torch.cuda.set_sync_debug_mode(self.sync_debug)
+                    try:
+                        loss, losses = self.train_step(next(batches))
+                        self.loss_sums += torch.stack(list(losses) + [loss.detach()])
+                    finally:
+                        torch.cuda.set_sync_debug_mode(mode)
+                    first = False
+                    self.step += 1
+                    self.loss_count += 1
+                    ev = events(self.step, o.print_freq, o.val_freq, o.save_freq)
+                    if "print" in ev:
+                        self._print()
+                    if "val" in ev and self.val_set is not None:
+                        log = self.validate()
+                        self.scheduler.step(log[4])
+                        self.log.info(val_message(self.epoch, self.step, log))
+                    if "save" in ev:
+                        self.save()
+                        saved = self.step
+            if saved != self.step:
+                self.save()
+            torch.cuda.synchronize(self.dev)
+        self.log.info("End of training.")
+
+    @property
+    def epoch(self) -> int:
+        """The epoch of the last iteration run (0 before the first)."""
+        return max(self.step - 1, 0) // self.iters_per_epoch
+
+    def _print(self) -> None:
+        avg = [v / self.loss_count for v in self.loss_sums.tolist()]
+        guard = None
+        if self.guarded:
+            self.opt.resolve()
+            guard = (self.opt.skipped_steps, self.opt.last_grad_norm)
+        self.log.info(train_message(self.epoch, self.step, self.opt.param_groups[0]["lr"], avg, guard))
+        self.loss_sums.zero_()
+        self.loss_count = 0
+
+    # ------------------------------------------------------------------ validation
+    @torch.no_grad()
+    def validate(self) -> tuple:
+        """The val split at batch 1, this rank's share of its windows (i = rank, rank + world, ...), the crops drawn
+        from a fresh random.Random(manual_seed) for every window in order.  -> get_current_log('val') of the sums over
+        all ranks (val_log)."""
+        vs = self.val_set
+        vs.rng = random.Random(self.o.manual_seed)
+        rows, losses = [], []
+        for i in range(len(vs)):
+            if i % self.world != self.rank:
+                vs.skip_draws(1)
+                continue
+            b = vs.batch([i])
+            outs = self.net(*[b["LQs"][:, k] for k in range(6)])
+            loss, lst = pixel_loss(outs, gt_list(b), self.o.pixel_criterion, nframes=6, version=self.o.version)
+            pairs = [(tensor2img_u8(outs[k][0]), tensor2img_u8(g[0])) for k, g in enumerate(gt_list(b))]
+            rows.append(image_metrics_batch(pairs))
+            losses.append(torch.stack(lst + [loss]))
+        sums = [0] * (3 * NOUT + 1)                          # AverageMeter: sum += val, in window order
+        if rows:
+            h, w = vs.h, vs.w
+            for r, l in zip(torch.stack(rows).cpu().numpy(), torch.stack(losses).cpu().numpy()):
+                for k, v in enumerate(window_scores(r, l, h, w)):
+                    sums[k] += v
+        t = torch.tensor(sums + [len(rows)], dtype=torch.float64, device=self.dev)
+        self.val_sums = reduce_sums(t).tolist()
+        return val_log(self.val_sums)
+
+    def close(self) -> None:
+        for h in list(self.log.handlers):
+            h.close()
+            self.log.removeHandler(h)
+
+
+# ----------------------------------------------------------------------------- command line
+def _arch(v: str) -> Tuple[int, int]:
+    try:
+        g0, d = (int(x) for x in v.split(","))
+    except ValueError:
+        raise argparse.ArgumentTypeError(f"--arch takes G0,D (e.g. 64,6), got {v!r}") from None
+    return g0, d
+
+
+def main(argv=None) -> None:
+    ap = argparse.ArgumentParser(description="Train bin_stage4 from a train yml of the reference (one process per GPU "
+                                             "under torchrun)")
+    ap.add_argument("-opt", required=True, help="e.g. options/train/train_adobe_stage4.yml")
+    ap.add_argument("--checkpointing", choices=("recompute",), default=None,
+                    help="rebuild each backbone stage's activations in its backward")
+    ap.add_argument("--max_grad_norm", type=float, default=None, help="clip the gradients by their global norm")
+    ap.add_argument("--skip_nonfinite", action="store_true", help="skip a step with an inf or NaN gradient")
+    ap.add_argument("--deterministic", action="store_true", help="torch.use_deterministic_algorithms(True)")
+    ap.add_argument("--from_sharp", action="store_true",
+                    help="synthesise the blurry frames from <root>/<mode>/<folder> (DeviceClip.from_sharp)")
+    ap.add_argument("--arch", type=_arch, default=None, help="backbone G0,D of a light window, e.g. 64,6")
+    ap.add_argument("--ratio", type=int, default=100, help="DistIterSampler's epoch enlargement under torchrun")
+    args = ap.parse_args(argv)
+    opts = load_options(args.opt)
+
+    distributed = int(os.environ.get("WORLD_SIZE", "1")) > 1
+    local = int(os.environ.get("LOCAL_RANK", "0"))
+    torch.cuda.set_device(local)
+    if distributed:
+        torch.distributed.init_process_group("nccl", device_id=torch.device("cuda", local))
+    try:
+        t = Trainer(opts, checkpointing=args.checkpointing, max_grad_norm=args.max_grad_norm,
+                    skip_nonfinite=args.skip_nonfinite, deterministic=args.deterministic, from_sharp=args.from_sharp,
+                    arch=args.arch, ratio=args.ratio)
+        try:
+            t.run()
+        finally:
+            t.close()
+    finally:
+        if distributed:
+            torch.distributed.destroy_process_group()
+
+
+if __name__ == "__main__":
+    main()

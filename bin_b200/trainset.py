@@ -121,6 +121,12 @@ class DeviceBINDataset:
         flip = self.rng.randint(0, 1)
         return (clip.frames(j, order), top, left, flip), key
 
+    def skip_draws(self, count: int) -> None:
+        """Make the draws of `count` samples on `rng` without building them: what `count` samples of `batch` would
+        have drawn (a resumed run's crops and flips, or the samples another rank builds)."""
+        for _ in range(count):
+            self._draw(0)
+
     def batch(self, indices: Sequence[int]) -> Dict:
         """default_collate of [ds[i] for i in indices], with the draws made in that order: 'LQs' (B,6,3,h,w), 'GTenh'
         (B,6,3,h,w), 'GTinp' (B,5,3,h,w) fp32 views of one (17,B,3,h,w) buffer, so `LQs[:, k]` is a contiguous
