@@ -36,59 +36,6 @@ int num_sms() {
   return v;
 }
 
-int launch_nchw_to_p8(const float* x, int C, const bin_act_t& dst, int plane0, cudaStream_t s);
-int launch_p8_to_nchw(const bin_act_t& src, int plane0, int C, float* y, cudaStream_t s);
-int launch_pack_frames(const bin_frames_t& fr, int H, int W, const bin_act_t& dst, cudaStream_t s, int x3 = 0);
-int launch_pack_weight(const float* w, int cout, int cin, int ks, int cout_pad, int cin_pad, int variant,
-                       void* packed, cudaStream_t s, int x3 = 0);
-int launch_pack_bias(const float* b, int cout, int cout_pad, float* dst, cudaStream_t s);
-int launch_grad_scale(const float* const* gouts, int n, size_t numel, float target, float* scale_dev, unsigned* tmp_dev,
-                      cudaStream_t s);
-// batched packing: all tensors of one blob in one launch (aux_kernels.cu)
-void* pack_batch_new();
-int pack_batch_add_weight(void* hb, const float* w, int cout, int cin, int ks, int cout_pad, int cin_pad, int variant,
-                          void* packed, int x3);
-int pack_batch_add_weight_t(void* hb, const float* w, int cout, int cin, int ks, int row0, int nrows, int cout_pad_t,
-                            int cin_pad_t, void* packed);
-int pack_batch_add_bias(void* hb, const float* b, int cout, int cout_pad, float* dst);
-int pack_batch_launch(void* hb, cudaStream_t s);   // launches and frees the batch
-size_t pixel_loss_scratch_bytes(int npairs, size_t n);
-int launch_pixel_loss_fwd(const float* const* a, const float* const* b, int npairs, size_t n, int kind, float eps,
-                          float* pair_loss, cudaStream_t s, int flags, void* scratch, size_t scratch_bytes);
-int launch_pixel_loss_bwd(const float* const* a, const float* const* b, float* const* da, float* const* db, int npairs,
-                          size_t n, int kind, float eps, const float* upstream, cudaStream_t s);
-int launch_adam_step(const bin_adam_tensor_t* table, const int* chunk_prefix, int ntensors, int nchunks, float lr,
-                     float beta1, float beta2, float eps, float weight_decay, float bias_correction1,
-                     float bias_correction2, float grad_scale, const bin_grad_audit_t* audit, cudaStream_t s);   // audit: NULL = unguarded
-size_t grad_audit_scratch_bytes(int nchunks);
-int launch_grad_audit(const bin_adam_tensor_t* table, const int* chunk_prefix, int ntensors, int nchunks, float grad_scale,
-                      float max_norm, void* scratch, bin_grad_audit_t* audit, cudaStream_t s);
-int launch_blur_average_u8(const uint8_t* frames, int T, size_t frame_bytes, int window_size, int first_mid, int stride,
-                           int nwin, uint8_t* out, cudaStream_t s);
-size_t metrics_workspace_bytes(int h, int w);
-int launch_image_metrics_u8(const uint8_t* a, const uint8_t* b, int h, int w, int c, double* out4, void* workspace,
-                            size_t workspace_bytes, cudaStream_t s);
-size_t metrics_batch_workspace_bytes(int n, int h, int w);
-int launch_image_metrics_batch_u8(const uint8_t* const* a_host, const uint8_t* const* b_host, int n, int h, int w, int c,
-                                  int flags, double* out, void* workspace, size_t workspace_bytes, cudaStream_t s);
-int launch_flipx4(int expand, const float* const* src, float* const* dst, int n, int B, int H, int W, cudaStream_t s);
-int launch_train_batch_u8(const bin_train_sample_t* samples, int B, int h, int w, float* dst, int dst_B, int b0,
-                          cudaStream_t s);
-size_t png_max_bytes(int h, int w);
-size_t png_workspace_bytes(int n, int h, int w);
-int launch_png_encode_u8(const uint8_t* const* imgs_host, int n, int h, int w, uint8_t* out, size_t out_stride,
-                         int64_t* sizes, void* workspace, size_t workspace_bytes, cudaStream_t s);
-int launch_rdb_tail(int g0, const bin_act_t& x, int x_plane0, const bin_act_t& g, int g_plane0, const void* w_conv,
-                    const float* b_conv, const void* w_lff, const float* b_lff, const bin_act_t& out, int out_plane0,
-                    int b_begin, int b_count, int y_begin, int y_count, cudaStream_t s);
-int launch_tensor2img_u8(const float* x, int Hs, int Ws, int top, int left, int h, int w, uint8_t* out, cudaStream_t s);
-int launch_u8_to_frame(const uint8_t* img, int h, int w, int pl, int pr, int pt, int pb, float* out, cudaStream_t s);
-size_t convlstm_bwd_scratch_bytes(int B, int H, int W);
-int launch_convlstm_bwd(const float* x, const float* c_prev, const float* h_prev, const float* w, const float* b,
-                        const float* dh, const float* dc, float* dgates_ws, float* dx, float* dc_prev, float* dh_prev,
-                        float* dw, float* db, int B, int H, int W, cudaStream_t s, int flags, void* scratch,
-                        size_t scratch_bytes);
-
 static inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
 // ------------------------------------------------------------------ backbone configuration
@@ -167,7 +114,22 @@ static BackboneLayout backbone_layout(const Arch& A, int x3 = 0) {
   return L;
 }
 
-// ------------------------------------------------------------------ backbone workspace
+// ------------------------------------------------------------------ workspaces
+// Lays P8 tensors of B items out one after another from `base`, each at a 256-byte boundary; `off` is the bytes used so
+// far.  A NULL base only sizes the layout.  Each tensor gets plane_mult times the planes asked for.
+struct P8Carver {
+  void* base;
+  int B, plane_mult;
+  size_t off;
+  bin_act_t operator()(int planes, int h, int w) {
+    bin_act_t t;
+    t.ptr = base ? (void*)((uint8_t*)base + off) : nullptr;
+    t.B = B; t.planes = planes * plane_mult; t.H = h; t.W = w;
+    off = align_up(off + (size_t)B * t.planes * h * w * 16, 256);
+    return t;
+  }
+};
+
 struct BackboneWs {
   bin_act_t x0, f1, f2, cat, g, t1, t2, u;
   size_t bytes;
@@ -175,14 +137,7 @@ struct BackboneWs {
 static BackboneWs backbone_ws(const Arch& A, int Btot, int H, int W, void* base, bool train = false, int x3 = 0) {
   BackboneWs w;
   const int h = H / 2, wd = W / 2, P = A.planes();
-  size_t off = 0;
-  auto carve = [&](int planes, int hh, int ww) {
-    bin_act_t t;
-    t.ptr = base ? (void*)((uint8_t*)base + off) : nullptr;
-    t.B = Btot; t.planes = planes * (x3 ? 2 : 1); t.H = hh; t.W = ww;      // x3: hi + lo plane groups
-    off = align_up(off + (size_t)Btot * t.planes * hh * ww * 16, 256);
-    return t;
-  };
+  P8Carver carve{base, Btot, x3 ? 2 : 1, 0};      // x3: hi + lo plane groups
   w.x0 = carve((int)align_up(12 * A.nframes, kKC) / 8, h, wd);
   w.f1 = carve(P, h, wd);
   w.f2 = carve(P, h, wd);
@@ -191,7 +146,7 @@ static BackboneWs backbone_ws(const Arch& A, int Btot, int H, int W, void* base,
   w.t1 = carve(P, h, wd);
   w.t2 = carve(P, h, wd);
   w.u = carve(8, H, W);
-  w.bytes = off;
+  w.bytes = carve.off;
   return w;
 }
 
@@ -303,24 +258,10 @@ static int run_backbone(int arch, const void* blob, const bin_frames_t& fr, int 
 
 // ------------------------------------------------------------------ backward of one backbone
 // Data gradients reuse conv_igemm_kernel: for a stride-1 / pad k/2 conv, dX = conv(dY, V) with
-// V[ci][co][ky][kx] = W[co][ci][k-1-ky][k-1-kx] (packed by launch_pack_weight_t, Cout' padded to a
+// V[ci][co][ky][kx] = W[co][ci][k-1-ky][k-1-kx] (packed by pack_batch_add_weight_t, Cout' padded to a
 // multiple of 96 and clipped by store_planes; at G0 = 64 the G0-row parts run as 96-row launches that store 8 planes).  Gradients are fp16 P8 tensors scaled by *scale (loss
 // scaling, a device scalar) and un-scaled when they leave the backbone (frame grads, dW, db).
-int launch_pack_weight_t(const float* w, int cout, int cin, int ks, int row0, int nrows, int cout_pad_t, int cin_pad_t,
-                         void* packed, cudaStream_t s);
-int launch_p8_add(const bin_act_t& dst, int dplane0, const bin_act_t& src, int splane0, int nplanes, cudaStream_t s);
-int launch_relu_mask(const bin_act_t& dg, int dplane0, const bin_act_t& g, int gplane0, int nplanes, cudaStream_t s);
-int launch_pixel_unshuffle(const bin_act_t& du, const bin_act_t& dst, cudaStream_t s);
-int launch_unpack_frames_grad(const bin_act_t& dx0, const bin_frames_t& dout, const bin_frames_t& dfr, int H, int W,
-                              const float* scale, cudaStream_t s);
-int launch_grad_out_to_p8(const bin_frames_t& dout, int H, int W, const bin_act_t& dst, const float* scale, cudaStream_t s);
-// partial == NULL: atomic per-block sums; otherwise the deterministic two-launch reduction through `partial`
-size_t bias_grad_partial_floats(int B, int hw, int C);
-int launch_bias_grad(const bin_act_t& dy, int plane0, int C, const float* scale, float* db, cudaStream_t s,
-                     float* partial = nullptr, size_t partial_floats = 0);
-int launch_wgrad(const bin_act_t& x0, int x0_plane0, int x0_planes, const bin_act_t& x1, int x1_plane0, int x1_planes,
-                 const bin_act_t& dy, int dy_plane0, int cout, int cin, int ks, const float* scale, float* dw,
-                 float* partial_ws, cudaStream_t s, bool det = false);
+
 // per-CTA accumulator slabs: grid = #SMs by default, kDetCtas in deterministic mode
 static size_t wgrad_partial_bytes() {
   const int ctas = num_sms() > kDetCtas ? num_sms() : kDetCtas;
@@ -381,14 +322,7 @@ static size_t bias_partial_bytes(int Btot, int H, int W) {
 static GradWs grad_ws(const Arch& A, int Btot, int H, int W, void* base) {
   GradWs w;
   const int h = H / 2, wd = W / 2, P = A.planes();
-  size_t off = 0;
-  auto carve = [&](int planes, int hh, int ww) {
-    bin_act_t t;
-    t.ptr = base ? (void*)((uint8_t*)base + off) : nullptr;
-    t.B = Btot; t.planes = planes; t.H = hh; t.W = ww;
-    off = align_up(off + (size_t)Btot * planes * hh * ww * 16, 256);
-    return t;
-  };
+  P8Carver carve{base, Btot, 1, 0};
   w.dout16 = carve(4, H, W);
   w.du = carve(8, H, W);
   w.dup0 = carve(32, h, wd);
@@ -398,11 +332,10 @@ static GradWs grad_ws(const Arch& A, int Btot, int H, int W, void* base) {
   w.df2 = carve(P, h, wd);
   w.dg = carve(16, h, wd);
   w.dx0 = carve((int)align_up(12 * A.nframes, kKC) / 8, h, wd);
-  w.wg_partial = base ? (float*)((uint8_t*)base + off) : nullptr;
+  w.wg_partial = base ? (float*)((uint8_t*)base + carve.off) : nullptr;
   const size_t wgb = wgrad_partial_bytes(), bb = bias_partial_bytes(Btot, H, W);
   w.wg_partial_floats = (wgb > bb ? wgb : bb) / sizeof(float);
-  off = align_up(off + w.wg_partial_floats * sizeof(float), 256);
-  w.bytes = off;
+  w.bytes = align_up(carve.off + w.wg_partial_floats * sizeof(float), 256);
   return w;
 }
 
@@ -594,7 +527,7 @@ size_t bin_packed_weight_bytes(int cout_pad, int cin_pad, int ksize) {
 }
 int bin_pack_conv_weight(const float* w_oihw, int cout, int cin, int ksize, int cout_pad, int cin_pad, int variant,
                          void* packed, bin_stream_t s) {
-  return launch_pack_weight(w_oihw, cout, cin, ksize, cout_pad, cin_pad, variant, packed, (cudaStream_t)s);
+  return bin_pack_conv_weight_p(w_oihw, cout, cin, ksize, cout_pad, cin_pad, variant, BIN_PREC_F16, packed, s);
 }
 int bin_pack_frames_p(const bin_frames_t* fr, int H, int W, bin_act_t dst, int prec, bin_stream_t s) {
   if (!fr) return fail(BIN_ERR_ARG, "pack_frames: null frame table");
@@ -604,12 +537,15 @@ int bin_pack_frames_p(const bin_frames_t* fr, int H, int W, bin_act_t dst, int p
 int bin_pack_conv_weight_p(const float* w_oihw, int cout, int cin, int ksize, int cout_pad, int cin_pad, int variant,
                            int prec, void* packed, bin_stream_t s) {
   if (prec != BIN_PREC_F16 && prec != BIN_PREC_F32X3) return fail(BIN_ERR_ARG, "pack_conv_weight: unknown precision");
-  return launch_pack_weight(w_oihw, cout, cin, ksize, cout_pad, cin_pad, variant, packed, (cudaStream_t)s,
-                            prec == BIN_PREC_F32X3);
+  PackBatch b;
+  BIN_TRY(pack_batch_add_weight(b, w_oihw, cout, cin, ksize, cout_pad, cin_pad, variant, packed, prec == BIN_PREC_F32X3));
+  return pack_batch_launch(b, (cudaStream_t)s);
 }
 int bin_pack_conv_weight_t(const float* w_oihw, int cout, int cin, int ksize, int row0, int nrows, int cout_pad_t,
                            int cin_pad_t, void* packed, bin_stream_t s) {
-  return launch_pack_weight_t(w_oihw, cout, cin, ksize, row0, nrows, cout_pad_t, cin_pad_t, packed, (cudaStream_t)s);
+  PackBatch b;
+  BIN_TRY(pack_batch_add_weight_t(b, w_oihw, cout, cin, ksize, row0, nrows, cout_pad_t, cin_pad_t, packed));
+  return pack_batch_launch(b, (cudaStream_t)s);
 }
 size_t bin_conv_wgrad_workspace_bytes(void) { return wgrad_partial_bytes(); }
 int bin_conv_wgrad(bin_act_t x0, int x0_plane0, int x0_planes, bin_act_t x1, int x1_plane0, int x1_planes, bin_act_t dy,
@@ -694,16 +630,14 @@ static int pack_backbone(int arch, const float* const* w_host, const float* cons
   BIN_TRY(arch_or_fail(arch, "backbone_pack", A));
   if (!w_host || !b_host || !blob) return fail(BIN_ERR_ARG, "backbone_pack: null argument");
   const BackboneLayout L = backbone_layout(A, x3);
-  void* hb = pack_batch_new();
-  int rc = BIN_OK;
-  for (int i = 0; i < A.nconv() && rc == BIN_OK; ++i) {
+  PackBatch b;
+  for (int i = 0; i < A.nconv(); ++i) {
     const ConvSpec& c = L.conv[i];
-    rc = pack_batch_add_weight(hb, w_host[i], c.cout, c.cin, c.ks, c.cout_pad, c.cin_pad, BIN_CONV_DEFAULT,
-                               (uint8_t*)blob + c.w_off, x3);
-    if (rc == BIN_OK) rc = pack_batch_add_bias(hb, b_host[i], c.cout, c.cout_pad, (float*)((uint8_t*)blob + c.b_off));
+    BIN_TRY(pack_batch_add_weight(b, w_host[i], c.cout, c.cin, c.ks, c.cout_pad, c.cin_pad, BIN_CONV_DEFAULT,
+                                  (uint8_t*)blob + c.w_off, x3));
+    BIN_TRY(pack_batch_add_bias(b, b_host[i], c.cout, c.cout_pad, (float*)((uint8_t*)blob + c.b_off)));
   }
-  const int rl = pack_batch_launch(hb, s);      // always frees the batch
-  return rc != BIN_OK ? rc : rl;
+  return pack_batch_launch(b, s);
 }
 
 int bin_backbone_pack(int arch, const float* const* w_host, const float* const* b_host, void* blob,
@@ -732,20 +666,17 @@ int bin_backbone_pack_t(int arch, const float* const* w_host, void* blob_t, bin_
   BIN_TRY(arch_or_fail(arch, "backbone_pack_t", A));
   const BackboneLayout L = backbone_layout(A);
   const BackboneLayoutT T = backbone_layout_t(A);
-  void* hb = pack_batch_new();
-  int rc = BIN_OK;
-  for (int i = 0; i < A.nconv() && rc == BIN_OK; ++i) {
+  PackBatch b;
+  for (int i = 0; i < A.nconv(); ++i) {
     const ConvSpec& c = L.conv[i];
     const TSpec* parts[2] = {&T.x[i], &T.g[i]};
     for (const TSpec* t : parts) {
-      if (t->nrows <= 0 || rc != BIN_OK) continue;
-      rc = pack_batch_add_weight_t(hb, w_host[i], c.cout, c.cin, c.ks, t->row0, t->nrows, t->cout_pad_t, t->cin_pad_t,
-                                   (uint8_t*)blob_t + t->off);
+      if (t->nrows <= 0) continue;
+      BIN_TRY(pack_batch_add_weight_t(b, w_host[i], c.cout, c.cin, c.ks, t->row0, t->nrows, t->cout_pad_t, t->cin_pad_t,
+                                      (uint8_t*)blob_t + t->off));
     }
   }
-  const int rl = pack_batch_launch(hb, (cudaStream_t)s);
-  if (rc != BIN_OK) return rc;
-  BIN_TRY(rl);
+  BIN_TRY(pack_batch_launch(b, (cudaStream_t)s));
   BIN_CUDA_OK(cudaMemsetAsync((uint8_t*)blob_t + T.zero_bias_off, 0, 1152 * sizeof(float), (cudaStream_t)s));
   return BIN_OK;
 }
@@ -820,15 +751,9 @@ int bin_rdb_fwd(const void* blob, int arch, int index, const float* x, float* y,
   Arch A;
   if (!decode_arch(arch, A) || index < 0 || index >= A.d) return fail(BIN_ERR_ARG, "rdb_fwd: bad nframes/index");
   const BackboneLayout L = backbone_layout(A);
-  size_t off = 0;
-  auto carve = [&](int planes) {
-    bin_act_t t;
-    t.ptr = (uint8_t*)workspace + off; t.B = B; t.planes = planes; t.H = h; t.W = w;
-    off = align_up(off + (size_t)B * planes * h * w * 16, 256);
-    return t;
-  };
-  bin_act_t xin = carve(A.planes()), g = carve(16), out = carve(A.planes());
-  if (off > workspace_bytes) return fail(BIN_ERR_WORKSPACE, "rdb_fwd: workspace too small");
+  P8Carver carve{workspace, B, 1, 0};
+  bin_act_t xin = carve(A.planes(), h, w), g = carve(16, h, w), out = carve(A.planes(), h, w);
+  if (carve.off > workspace_bytes) return fail(BIN_ERR_WORKSPACE, "rdb_fwd: workspace too small");
   BIN_TRY(launch_nchw_to_p8(x, A.g0, xin, 0, (cudaStream_t)s));
   BIN_TRY(run_rdb(A, blob, L, index, xin, 0, g, out, 0, (cudaStream_t)s));
   return launch_p8_to_nchw(out, 0, A.g0, y, (cudaStream_t)s);
@@ -902,7 +827,8 @@ int bin_image_metrics_u8(const uint8_t* a, const uint8_t* b, int h, int w, int c
 size_t bin_image_metrics_batch_workspace_bytes(int n, int h, int w) { return metrics_batch_workspace_bytes(n, h, w); }
 int bin_image_metrics_batch_u8(const uint8_t* const* a_host, const uint8_t* const* b_host, int n, int h, int w, int c,
                                int flags, double* out, void* workspace, size_t workspace_bytes, bin_stream_t s) {
-  return launch_image_metrics_batch_u8(a_host, b_host, n, h, w, c, flags, out, workspace, workspace_bytes, (cudaStream_t)s);
+  return launch_image_metrics_batch_u8("image_metrics_batch", a_host, b_host, n, h, w, c, flags, out, workspace,
+                                       workspace_bytes, (cudaStream_t)s);
 }
 int bin_flipx4_expand(const float* const* src_host, float* const* dst_host, int n, int B, int H, int W, bin_stream_t s) {
   return launch_flipx4(1, src_host, dst_host, n, B, H, W, (cudaStream_t)s);

@@ -103,14 +103,6 @@ __global__ void __launch_bounds__(256) pack_frames_kernel(const __grid_constant_
 // (a conv with V over dY gives dX for stride-1 / pad k/2 convs), co' < nrows, ci' < cout.
 // x3 != 0 (BIN_PREC_F32X3): three slabs per logical chunk -- hi, hi, lo of (w * 2^8) -- matching the kernel's
 // x_hi*W_hi + x_lo*W_hi + x_hi*W_lo chunk order.
-struct PackJob {            // one conv's weight tensor (or bias vector) of a batched pack launch
-  const float* src; void* dst;
-  int cout, cin, ks, cout_pad, cin_pad, nt, stackx, transpose, row0, nrows, x3, is_bias;
-  int block0, nblocks;     // this job's blocks are [block0, block0 + nblocks) of the launch
-};
-constexpr int kPackMaxJobs = 136;      // 66 weights + 66 biases (forward blob) / 66 + 48 transposed slabs, + slack
-struct PackBatch { PackJob job[kPackMaxJobs]; int njobs; };   // ~10 KB of kernel parameters (limit 32 KB)
-
 __device__ __forceinline__ void pack_weight_range(const float* __restrict__ w, int cout, int cin, int ks, int cout_pad, int cin_pad,
                                                   int nt, int stackx, int transpose, int row0, int nrows, int x3,
                                                   __half* __restrict__ dst, size_t first, size_t stride) {
@@ -151,14 +143,9 @@ __device__ __forceinline__ void pack_weight_range(const float* __restrict__ w, i
     }
   }
 }
-__global__ void pack_weight_kernel(const float* __restrict__ w, int cout, int cin, int ks, int cout_pad, int cin_pad,
-                                   int nt, int stackx, int transpose, int row0, int nrows, int x3,
-                                   __half* __restrict__ dst) {
-  pack_weight_range(w, cout, cin, ks, cout_pad, cin_pad, nt, stackx, transpose, row0, nrows, x3, dst,
-                    blockIdx.x * (size_t)blockDim.x + threadIdx.x, (size_t)gridDim.x * blockDim.x);
-}
 // All conv weights + biases of one backbone in ONE launch (a training step re-packs 4 backbones x 2 layouts after every
-// optimizer step: 720 launches of the per-tensor kernel before).  Block -> job by binary search in the parameter table.
+// optimizer step: 720 launches of a per-tensor kernel).  The per-tensor entry points run one-job batches.  Block -> job
+// by binary search in the parameter table.
 __global__ void __launch_bounds__(256) pack_batch_kernel(const __grid_constant__ PackBatch P) {
   int lo = 0, hi = P.njobs - 1;
   while (lo < hi) {
@@ -373,11 +360,6 @@ __global__ void grad_scale_finalize_kernel(const unsigned* __restrict__ bits, fl
   float s = ldexpf(1.f, ilogbf(target) - ilogbf(gmax));
   if (s * gmax > target) s *= 0.5f;
   *scale = s;
-}
-
-__global__ void pack_bias_kernel(const float* __restrict__ b, int cout, int cout_pad, float* __restrict__ dst) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < cout_pad) dst[i] = i < cout ? b[i] : 0.f;
 }
 
 // ------------------------------------------------------------------ K5: ConvLSTMCell (RDN.py:50-95)
@@ -1122,47 +1104,21 @@ int launch_pack_frames(const bin_frames_t& fr, int H, int W, const bin_act_t& ds
   BIN_CUDA_OK(cudaGetLastError());
   return BIN_OK;
 }
-int launch_pack_weight(const float* w, int cout, int cin, int ks, int cout_pad, int cin_pad, int variant,
-                       void* packed, cudaStream_t s, int x3) {
-  if (cin_pad % kKC || cout_pad % 16 || cout > cout_pad || cin > cin_pad)
-    return fail(BIN_ERR_ARG, "pack_conv_weight: cin_pad must be a multiple of 32, cout_pad of 16");
-  const int nt = conv_nt(cout_pad);
-  if (cout_pad % nt) return fail(BIN_ERR_ARG, "pack_conv_weight: cout_pad must be <=128, or a multiple of 96 or 128");
-  const size_t total = (size_t)cout_pad * cin_pad * ks * ks * (x3 ? 3 : 1);
-  const int stackx = (ks == 3 && (cout_pad == 32 || cout_pad == 16) && variant == BIN_CONV_DEFAULT) ? 1 : 0;
-  pack_weight_kernel<<<grid_for(total, 256), 256, 0, s>>>(w, cout, cin, ks, cout_pad, cin_pad, nt, stackx, 0, 0, 0, x3,
-                                                          (__half*)packed);
-  BIN_CUDA_OK(cudaGetLastError());
-  return BIN_OK;
+// ---- weight packing
+static int pack_batch_blocks(const PackBatch& b) {
+  return b.njobs ? b.job[b.njobs - 1].block0 + b.job[b.njobs - 1].nblocks : 0;
 }
-// data-gradient weights of a conv (cout,cin,ks): output rows [row0,row0+nrows) of the cin axis, padded to
-// cout_pad_t (multiple of 96); K = cout padded to cin_pad_t (multiple of 32).
-int launch_pack_weight_t(const float* w, int cout, int cin, int ks, int row0, int nrows, int cout_pad_t, int cin_pad_t,
-                         void* packed, cudaStream_t s) {
-  if (cin_pad_t % kKC || cout_pad_t % 96 || nrows > cout_pad_t || cout > cin_pad_t || row0 + nrows > cin)
-    return fail(BIN_ERR_ARG, "pack_conv_weight_t: bad padding / row range");
-  const size_t total = (size_t)cout_pad_t * cin_pad_t * ks * ks;
-  pack_weight_kernel<<<grid_for(total, 256), 256, 0, s>>>(w, cout, cin, ks, cout_pad_t, cin_pad_t, 96, 0, 1, row0, nrows, 0,
-                                                          (__half*)packed);
-  BIN_CUDA_OK(cudaGetLastError());
-  return BIN_OK;
-}
-// ---- batched packing (one launch per backbone blob)
-struct PackBatchHost { PackBatch b; int nblocks; };
-void* pack_batch_new() { PackBatchHost* h = new PackBatchHost; h->b.njobs = 0; h->nblocks = 0; return h; }
-static int pack_batch_add(void* hb, const PackJob& job, size_t total) {
-  PackBatchHost* h = static_cast<PackBatchHost*>(hb);
-  if (h->b.njobs >= kPackMaxJobs) return fail(BIN_ERR_UNSUPPORTED, "pack batch: too many tensors");
+static int pack_batch_add(PackBatch& b, const PackJob& job, size_t total) {
+  if (b.njobs >= kPackMaxJobs) return fail(BIN_ERR_UNSUPPORTED, "pack batch: too many tensors");
   PackJob j = job;
   size_t nb = (total + 256 * 8 - 1) / (256 * 8);               // ~8 elements per thread
   if (nb < 1) nb = 1;
   if (nb > 64) nb = 64;
-  j.block0 = h->nblocks; j.nblocks = (int)nb;
-  h->nblocks += (int)nb;
-  h->b.job[h->b.njobs++] = j;
+  j.block0 = pack_batch_blocks(b); j.nblocks = (int)nb;
+  b.job[b.njobs++] = j;
   return BIN_OK;
 }
-int pack_batch_add_weight(void* hb, const float* w, int cout, int cin, int ks, int cout_pad, int cin_pad, int variant,
+int pack_batch_add_weight(PackBatch& b, const float* w, int cout, int cin, int ks, int cout_pad, int cin_pad, int variant,
                           void* packed, int x3) {
   if (cin_pad % kKC || cout_pad % 16 || cout > cout_pad || cin > cin_pad)
     return fail(BIN_ERR_ARG, "pack_conv_weight: cin_pad must be a multiple of 32, cout_pad of 16");
@@ -1173,9 +1129,9 @@ int pack_batch_add_weight(void* hb, const float* w, int cout, int cin, int ks, i
   j.src = w; j.dst = packed; j.cout = cout; j.cin = cin; j.ks = ks; j.cout_pad = cout_pad; j.cin_pad = cin_pad; j.nt = nt;
   j.stackx = (ks == 3 && (cout_pad == 32 || cout_pad == 16) && variant == BIN_CONV_DEFAULT) ? 1 : 0;
   j.x3 = x3;
-  return pack_batch_add(hb, j, (size_t)cout_pad * cin_pad * ks * ks * (x3 ? 3 : 1));
+  return pack_batch_add(b, j, (size_t)cout_pad * cin_pad * ks * ks * (x3 ? 3 : 1));
 }
-int pack_batch_add_weight_t(void* hb, const float* w, int cout, int cin, int ks, int row0, int nrows, int cout_pad_t,
+int pack_batch_add_weight_t(PackBatch& b, const float* w, int cout, int cin, int ks, int row0, int nrows, int cout_pad_t,
                             int cin_pad_t, void* packed) {
   if (cin_pad_t % kKC || cout_pad_t % 96 || nrows > cout_pad_t || cout > cin_pad_t || row0 + nrows > cin)
     return fail(BIN_ERR_ARG, "pack_conv_weight_t: bad padding / row range");
@@ -1183,28 +1139,19 @@ int pack_batch_add_weight_t(void* hb, const float* w, int cout, int cin, int ks,
   memset(&j, 0, sizeof(j));
   j.src = w; j.dst = packed; j.cout = cout; j.cin = cin; j.ks = ks; j.cout_pad = cout_pad_t; j.cin_pad = cin_pad_t; j.nt = 96;
   j.transpose = 1; j.row0 = row0; j.nrows = nrows;
-  return pack_batch_add(hb, j, (size_t)cout_pad_t * cin_pad_t * ks * ks);
+  return pack_batch_add(b, j, (size_t)cout_pad_t * cin_pad_t * ks * ks);
 }
-int pack_batch_add_bias(void* hb, const float* b, int cout, int cout_pad, float* dst) {
+int pack_batch_add_bias(PackBatch& b, const float* bias, int cout, int cout_pad, float* dst) {
   PackJob j;
   memset(&j, 0, sizeof(j));
-  j.src = b; j.dst = dst; j.cout = cout; j.cout_pad = cout_pad; j.is_bias = 1;
-  return pack_batch_add(hb, j, (size_t)cout_pad);
+  j.src = bias; j.dst = dst; j.cout = cout; j.cout_pad = cout_pad; j.is_bias = 1;
+  return pack_batch_add(b, j, (size_t)cout_pad);
 }
-int pack_batch_launch(void* hb, cudaStream_t s) {
-  PackBatchHost* h = static_cast<PackBatchHost*>(hb);
-  int rc = BIN_OK;
-  if (h->b.njobs > 0) {
-    pack_batch_kernel<<<h->nblocks, 256, 0, s>>>(h->b);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) rc = fail(BIN_ERR_CUDA, std::string("pack_batch_kernel: ") + cudaGetErrorString(e));
-  }
-  delete h;
-  return rc;
-}
-int launch_pack_bias(const float* b, int cout, int cout_pad, float* dst, cudaStream_t s) {
-  pack_bias_kernel<<<(cout_pad + 127) / 128, 128, 0, s>>>(b, cout, cout_pad, dst);
-  BIN_CUDA_OK(cudaGetLastError());
+int pack_batch_launch(const PackBatch& b, cudaStream_t s) {
+  if (b.njobs == 0) return BIN_OK;
+  pack_batch_kernel<<<pack_batch_blocks(b), 256, 0, s>>>(b);
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return fail(BIN_ERR_CUDA, std::string("pack_batch_kernel: ") + cudaGetErrorString(e));
   return BIN_OK;
 }
 int launch_convlstm_multi(const LstmCells& cells, int ncells, int B, int H, int W, cudaStream_t s) {
@@ -1417,15 +1364,6 @@ int launch_convlstm_bwd(const float* x, const float* c_prev, const float* h_prev
     BIN_CUDA_OK(cudaGetLastError());
   }
   return BIN_OK;
-}
-int launch_wgrad_impl(const bin_act_t& x0, int x0_plane0, int x0_planes, const bin_act_t& x1, int x1_plane0, int x1_planes,
-                      const bin_act_t& dy, int dy_plane0, int cout, int cin, int ks, const float* scale, float* dw,
-                      float* partial_ws, cudaStream_t s, bool det);
-int launch_wgrad(const bin_act_t& x0, int x0_plane0, int x0_planes, const bin_act_t& x1, int x1_plane0, int x1_planes,
-                 const bin_act_t& dy, int dy_plane0, int cout, int cin, int ks, const float* scale, float* dw,
-                 float* partial_ws, cudaStream_t s, bool det) {
-  return launch_wgrad_impl(x0, x0_plane0, x0_planes, x1, x1_plane0, x1_planes, dy, dy_plane0, cout, cin, ks, scale, dw,
-                           partial_ws, s, det);
 }
 // expand = 1: bin_flipx4_expand, 0: bin_flipx4_mean.  Every check runs before the first CUDA call.
 int launch_flipx4(int expand, const float* const* src, float* const* dst, int n, int B, int H, int W, cudaStream_t s) {

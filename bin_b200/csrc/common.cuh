@@ -112,4 +112,14 @@ __device__ __forceinline__ void acc_fence(float (&d)[K]) {
 // barrier over the 128 threads of one consumer warpgroup (ids 1.. are free; 0 is __syncthreads)
 __device__ __forceinline__ void wg_sync(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
 
+// two floats <-> one fp16x2 register (round to nearest)
+__device__ __forceinline__ uint32_t pack_h2(float a, float b) {
+  __half2 h = __floats2half2_rn(a, b);
+  return *reinterpret_cast<uint32_t*>(&h);
+}
+__device__ __forceinline__ float2 unpack_h2(uint32_t u) {
+  __half2 h = *reinterpret_cast<__half2*>(&u);
+  return __half22float2(h);
+}
+
 }  // namespace binb

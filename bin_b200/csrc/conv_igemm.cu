@@ -57,15 +57,6 @@ struct Ctrl {
 };
 static_assert(sizeof(Ctrl) <= 1024, "ctrl block");
 
-__device__ __forceinline__ uint32_t pack_h2(float a, float b) {
-  __half2 h = __floats2half2_rn(a, b);
-  return *reinterpret_cast<uint32_t*>(&h);
-}
-__device__ __forceinline__ float2 unpack_h2(uint32_t u) {
-  __half2 h = *reinterpret_cast<__half2*>(&u);
-  return __half22float2(h);
-}
-
 constexpr int kThreads = 384;   // warpgroup 0: TMA producer (one thread); warpgroups 1, 2: wgmma + epilogue
 
 // PixelShuffle epilogue staging buffer of one consumer warp: one accumulator row set (8 low-res pixels x 128 channels)
@@ -452,30 +443,14 @@ static EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
-int make_p8_tmap(CUtensorMap* m, const bin_act_t& t, int box_rows) {
-  EncodeTiledFn fn = get_encode_fn();
-  if (!fn) return fail(BIN_ERR_CUDA, "cuTensorMapEncodeTiled not available from the driver");
-  if ((reinterpret_cast<uintptr_t>(t.ptr) & 15) != 0) return fail(BIN_ERR_ARG, "P8 tensor not 16-byte aligned");
-  // The (8 channels, W) dims of a P8 plane row are contiguous in memory, so they are described as ONE
-  // dimension of W*8 elements: the box row is then 32 px * 16 B = 512 contiguous bytes (a 16-byte
-  // inner box made the TMA unit the bottleneck).  OOB zero fill works per element, i.e. per pixel.
-  cuuint64_t dims[4] = {(cuuint64_t)t.W * 8, (cuuint64_t)t.H, (cuuint64_t)t.planes, (cuuint64_t)t.B};
-  cuuint64_t strides[3] = {(cuuint64_t)t.W * 16, (cuuint64_t)t.H * t.W * 16, (cuuint64_t)t.planes * t.H * t.W * 16};
-  cuuint32_t box[4] = {(cuuint32_t)kTWH * 8, (cuuint32_t)box_rows, (cuuint32_t)kKPL, 1};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, t.ptr, dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(BIN_ERR_CUDA, "cuTensorMapEncodeTiled failed with code " + std::to_string((int)r));
-  return BIN_OK;
-}
-
-// Generic P8 box: box_px pixels x box_rows rows x box_planes planes (used by the weight-gradient kernel).
-int make_p8_tmap_box(CUtensorMap* m, const bin_act_t& t, int box_px, int box_rows, int box_planes) {
+int make_p8_tmap(CUtensorMap* m, const bin_act_t& t, int box_px, int box_rows, int box_planes) {
   EncodeTiledFn fn = get_encode_fn();
   if (!fn) return fail(BIN_ERR_CUDA, "cuTensorMapEncodeTiled not available from the driver");
   if ((reinterpret_cast<uintptr_t>(t.ptr) & 15) != 0) return fail(BIN_ERR_ARG, "P8 tensor not 16-byte aligned");
   if (box_px * 8 > 256 || box_rows > 256 || box_planes > 256) return fail(BIN_ERR_ARG, "TMA box dimension exceeds 256");
+  // The (8 channels, W) dims of a P8 plane row are contiguous in memory, so they are described as ONE
+  // dimension of W*8 elements: a conv box row is then 32 px * 16 B = 512 contiguous bytes (a 16-byte
+  // inner box made the TMA unit the bottleneck).  OOB zero fill works per element, i.e. per pixel.
   cuuint64_t dims[4] = {(cuuint64_t)t.W * 8, (cuuint64_t)t.H, (cuuint64_t)t.planes, (cuuint64_t)t.B};
   cuuint64_t strides[3] = {(cuuint64_t)t.W * 16, (cuuint64_t)t.H * t.W * 16, (cuuint64_t)t.planes * t.H * t.W * 16};
   cuuint32_t box[4] = {(cuuint32_t)box_px * 8, (cuuint32_t)box_rows, (cuuint32_t)box_planes, 1};
@@ -533,8 +508,8 @@ static int launch_inst(const bin_conv_args_t& a, cudaStream_t s) {
   p.store_planes = a.store_planes > 0 ? a.store_planes : a.cout_pad / 8;
   p.res = reinterpret_cast<const __half*>(a.res.ptr); p.res_planes = a.res.planes; p.res_plane0 = a.res_plane0;
   p.fr = a.fr;
-  BIN_TRY(make_p8_tmap(&p.tmap0, a.in0, C::ROWS));
-  if (a.in1_planes > 0) BIN_TRY(make_p8_tmap(&p.tmap1, a.in1, C::ROWS));
+  BIN_TRY(make_p8_tmap(&p.tmap0, a.in0, kTWH, C::ROWS, kKPL));
+  if (a.in1_planes > 0) BIN_TRY(make_p8_tmap(&p.tmap1, a.in1, kTWH, C::ROWS, kKPL));
   auto kern = conv_igemm_kernel<NT, KS, EPI, SX, X3>;
   static std::atomic<unsigned long long> smem_opted{0};   // per instantiation, per device
   BIN_TRY(ensure_dynamic_smem(kern, kSmemMax, smem_opted));

@@ -2,12 +2,12 @@
 //   sum |a-b| and sum (a-b)^2 (exact, integers), the mean Gaussian-11 SSIM of utils/util.py:211-231 and the mean
 //   box-7 SSIM of skimage <= 0.17 compare_ssim with its defaults.
 //
-// metrics_tile_kernel: one CTA per kTile x kTile block of the image.  It stages the block plus a 5-pixel halo of both
-// images in shared memory, then per channel runs the horizontal passes of both windows (Gaussian in fp64, box in
-// int32: exact) into shared memory and the vertical passes over the valid outputs of the block.  Each CTA writes its
-// four partial sums to the workspace; metrics_reduce_kernel adds them in tile order.  The batch kernels run n pairs of
-// one shape with the same per-tile code and the same tile-order sum, so each pair gets the single call's bits.  The grid depends only on
-// (h, w), every sum has a fixed order, so the result is bit-reproducible and independent of the SM count.
+// metrics_tile_batch_kernel: one CTA per kTile x kTile block of the image and pair.  It stages the block plus a 5-pixel
+// halo of both images in shared memory, then per channel runs the horizontal passes of both windows (Gaussian in fp64,
+// box in int32: exact) into shared memory and the vertical passes over the valid outputs of the block.  Each CTA writes
+// its four partial sums to the workspace; metrics_reduce_batch_kernel adds each pair's in tile order.  A single pair is a
+// batch of one, so each pair of a batch gets the single call's bits.  The grid depends only on (n, h, w), every sum has a
+// fixed order, so the result is bit-reproducible and independent of the SM count.
 #include <stdint.h>
 
 #include "internal.h"
@@ -150,17 +150,12 @@ __device__ __forceinline__ void metrics_tile(const uint8_t* __restrict__ A, cons
   if (tid == 0) part[blockIdx.y * gridDim.x + blockIdx.x] = p;
 }
 
-__global__ void __launch_bounds__(kMetThreads) metrics_tile_kernel(const uint8_t* __restrict__ A, const uint8_t* __restrict__ B,
-                                                                   int h, int w, int c, MetricsPartial* __restrict__ part) {
-  metrics_tile(A, B, h, w, c, false, part);
-}
-
 struct MetricsPairs {
   const uint8_t* a[BIN_METRICS_MAX_BATCH];
   const uint8_t* b[BIN_METRICS_MAX_BATCH];
 };
 
-// blockIdx.z = pair; pair z's tiles occupy part[z * ntiles, (z + 1) * ntiles) in the single-pair kernel's tile order.
+// blockIdx.z = pair; pair z's tiles occupy part[z * ntiles, (z + 1) * ntiles) in row-major tile order.
 __global__ void __launch_bounds__(kMetThreads) metrics_tile_batch_kernel(const MetricsPairs pairs, int h, int w, int c, int bgr,
                                                                          MetricsPartial* __restrict__ part) {
   const int z = blockIdx.z;
@@ -189,12 +184,7 @@ __device__ __forceinline__ void metrics_reduce(const MetricsPartial* __restrict_
   }
 }
 
-__global__ void __launch_bounds__(kRedThreads) metrics_reduce_kernel(const MetricsPartial* __restrict__ part, int ntiles,
-                                                                     double n_gauss, double n_box, double* __restrict__ out4) {
-  metrics_reduce(part, ntiles, n_gauss, n_box, out4);
-}
-
-// One CTA per pair: the same tile-order sum as metrics_reduce_kernel over that pair's slice.
+// One CTA per pair: a tile-order sum over that pair's slice.
 __global__ void __launch_bounds__(kRedThreads) metrics_reduce_batch_kernel(const MetricsPartial* __restrict__ part, int ntiles,
                                                                            double n_gauss, double n_box,
                                                                            double* __restrict__ out) {
@@ -208,56 +198,39 @@ size_t metrics_workspace_bytes(int h, int w) {
   return (size_t)metrics_ntiles(h, w) * sizeof(MetricsPartial);
 }
 
-static int check_metrics_args(const char* fn, int h, int w, int c, const double* out, const void* workspace) {
-  if (!out || !workspace) return fail(BIN_ERR_ARG, std::string(fn) + ": null argument");
-  if (c != 1 && c != 3) return fail(BIN_ERR_ARG, std::string(fn) + ": c must be 1 or 3");
-  if (h < 7 || w < 7) return fail(BIN_ERR_ARG, std::string(fn) + ": h and w must be at least 7 (the 7x7 SSIM window)");
-  if (h > 65535 || w > 65535 || (long long)h * w * c >= (1ll << 31))
-    return fail(BIN_ERR_ARG, std::string(fn) + ": image too large (h, w <= 65535 and h*w*c < 2^31)");
-  if ((reinterpret_cast<uintptr_t>(workspace) & 7) || (reinterpret_cast<uintptr_t>(out) & 7))
-    return fail(BIN_ERR_ARG, std::string(fn) + ": workspace and the output must be 8-byte aligned");
-  return BIN_OK;
-}
-
-int launch_image_metrics_u8(const uint8_t* a, const uint8_t* b, int h, int w, int c, double* out4, void* workspace,
-                            size_t workspace_bytes, cudaStream_t s) {
-  // every check precedes the first CUDA call
-  if (!a || !b) return fail(BIN_ERR_ARG, "image_metrics: null argument");
-  BIN_TRY(check_metrics_args("image_metrics", h, w, c, out4, workspace));
-  if (workspace_bytes < metrics_workspace_bytes(h, w))
-    return fail(BIN_ERR_ARG, "image_metrics: workspace too small (see bin_image_metrics_workspace_bytes)");
-
-  static std::atomic<unsigned long long> smem_mask{0};
-  BIN_TRY(ensure_dynamic_smem(metrics_tile_kernel, (int)sizeof(MetricsSmem), smem_mask));
-  MetricsPartial* part = static_cast<MetricsPartial*>(workspace);
-  const dim3 grid((w + kTile - 1) / kTile, (h + kTile - 1) / kTile);
-  metrics_tile_kernel<<<grid, kMetThreads, sizeof(MetricsSmem), s>>>(a, b, h, w, c, part);
-  BIN_CUDA_OK(cudaGetLastError());
-  const double n_gauss = (h >= 11 && w >= 11) ? (double)c * (h - 10) * (w - 10) : 0.0;
-  const double n_box = (double)c * (h - 6) * (w - 6);
-  metrics_reduce_kernel<<<1, kRedThreads, 0, s>>>(part, metrics_ntiles(h, w), n_gauss, n_box, out4);
-  BIN_CUDA_OK(cudaGetLastError());
-  return BIN_OK;
-}
-
 size_t metrics_batch_workspace_bytes(int n, int h, int w) {
   if (n < 1 || n > BIN_METRICS_MAX_BATCH) return 0;
   return (size_t)n * metrics_workspace_bytes(h, w);
 }
 
-int launch_image_metrics_batch_u8(const uint8_t* const* a_host, const uint8_t* const* b_host, int n, int h, int w, int c,
-                                  int flags, double* out, void* workspace, size_t workspace_bytes, cudaStream_t s) {
+// bin_image_metrics_u8: a batch of one pair.  Its NULL a or b is reported before the one-entry tables exist.
+int launch_image_metrics_u8(const uint8_t* a, const uint8_t* b, int h, int w, int c, double* out4, void* workspace,
+                            size_t workspace_bytes, cudaStream_t s) {
+  if (!a || !b) return fail(BIN_ERR_ARG, "image_metrics: null argument");
+  return launch_image_metrics_batch_u8("image_metrics", &a, &b, 1, h, w, c, 0, out4, workspace, workspace_bytes, s);
+}
+
+int launch_image_metrics_batch_u8(const char* who, const uint8_t* const* a_host, const uint8_t* const* b_host, int n, int h,
+                                  int w, int c, int flags, double* out, void* workspace, size_t workspace_bytes,
+                                  cudaStream_t s) {
   // every check precedes the first CUDA call
-  if (!a_host || !b_host) return fail(BIN_ERR_ARG, "image_metrics_batch: null pointer table");
-  if (n < 1 || n > BIN_METRICS_MAX_BATCH) return fail(BIN_ERR_ARG, "image_metrics_batch: n must be 1..BIN_METRICS_MAX_BATCH");
-  if (flags & ~BIN_METRICS_BGR) return fail(BIN_ERR_ARG, "image_metrics_batch: unknown flag");
-  if ((flags & BIN_METRICS_BGR) && c != 3) return fail(BIN_ERR_ARG, "image_metrics_batch: BIN_METRICS_BGR needs c = 3");
-  BIN_TRY(check_metrics_args("image_metrics_batch", h, w, c, out, workspace));
+  const std::string fn = who;
+  if (!a_host || !b_host) return fail(BIN_ERR_ARG, fn + ": null pointer table");
+  if (n < 1 || n > BIN_METRICS_MAX_BATCH) return fail(BIN_ERR_ARG, fn + ": n must be 1..BIN_METRICS_MAX_BATCH");
+  if (flags & ~BIN_METRICS_BGR) return fail(BIN_ERR_ARG, fn + ": unknown flag");
+  if ((flags & BIN_METRICS_BGR) && c != 3) return fail(BIN_ERR_ARG, fn + ": BIN_METRICS_BGR needs c = 3");
+  if (!out || !workspace) return fail(BIN_ERR_ARG, fn + ": null argument");
+  if (c != 1 && c != 3) return fail(BIN_ERR_ARG, fn + ": c must be 1 or 3");
+  if (h < 7 || w < 7) return fail(BIN_ERR_ARG, fn + ": h and w must be at least 7 (the 7x7 SSIM window)");
+  if (h > 65535 || w > 65535 || (long long)h * w * c >= (1ll << 31))
+    return fail(BIN_ERR_ARG, fn + ": image too large (h, w <= 65535 and h*w*c < 2^31)");
+  if ((reinterpret_cast<uintptr_t>(workspace) & 7) || (reinterpret_cast<uintptr_t>(out) & 7))
+    return fail(BIN_ERR_ARG, fn + ": workspace and the output must be 8-byte aligned");
   if (workspace_bytes < metrics_batch_workspace_bytes(n, h, w))
-    return fail(BIN_ERR_ARG, "image_metrics_batch: workspace too small (see bin_image_metrics_batch_workspace_bytes)");
+    return fail(BIN_ERR_ARG, fn + ": workspace too small (see bin_" + fn + "_workspace_bytes)");
   MetricsPairs pairs = {};
   for (int i = 0; i < n; ++i) {
-    if (!a_host[i] || !b_host[i]) return fail(BIN_ERR_ARG, "image_metrics_batch: null image pointer");
+    if (!a_host[i] || !b_host[i]) return fail(BIN_ERR_ARG, fn + ": null image pointer");
     pairs.a[i] = a_host[i];
     pairs.b[i] = b_host[i];
   }

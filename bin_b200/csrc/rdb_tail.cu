@@ -78,15 +78,6 @@ struct RtCtrl {
 };
 static_assert(sizeof(RtCtrl<96>) <= 512 && sizeof(RtCtrl<64>) <= 512, "ctrl block");
 
-__device__ __forceinline__ uint32_t pack_h2_rt(float a, float b) {
-  __half2 h = __floats2half2_rn(a, b);
-  return *reinterpret_cast<uint32_t*>(&h);
-}
-__device__ __forceinline__ float2 unpack_h2_rt(uint32_t u) {
-  __half2 h = *reinterpret_cast<__half2*>(&u);
-  return __half22float2(h);
-}
-
 template <int G0>
 __global__ void __launch_bounds__(384, 1) rdb_tail_kernel(const __grid_constant__ RdbTailParams p) {
   using Cf = RtCfg<G0>;
@@ -226,7 +217,7 @@ __global__ void __launch_bounds__(384, 1) rdb_tail_kernel(const __grid_constant_
         float f[2];
 #pragma unroll
         for (int e = 0; e < 2; ++e) f[e] = fmaxf(acc_c[4 * i + 2 * h + e] + sb_conv[8 * i + 2 * k4 + e], 0.f);
-        *reinterpret_cast<uint32_t*>(hrow + i * kRtHPlane) = pack_h2_rt(f[0], f[1]);
+        *reinterpret_cast<uint32_t*>(hrow + i * kRtHPlane) = pack_h2(f[0], f[1]);
       }
     }
     fence_proxy_async();                                             // generic-proxy stores -> visible to wgmma
@@ -254,10 +245,10 @@ __global__ void __launch_bounds__(384, 1) rdb_tail_kernel(const __grid_constant_
 #pragma unroll
         for (int i = 0; i < G0 / 8; ++i) {
           const int n = 8 * i + 2 * k4;
-          const float2 g = unpack_h2_rt(res[h][i]);
+          const float2 g = unpack_h2(res[h][i]);
           const size_t off = ((((size_t)b * p.out_planes + p.out_plane0 + i) * p.H + y[h]) * p.W + x[h]) * 8 + 2 * k4;
           *reinterpret_cast<uint32_t*>(p.out + off) =
-              pack_h2_rt((acc_l[4 * i + 2 * h] + sb_lff[n]) + g.x, (acc_l[4 * i + 2 * h + 1] + sb_lff[n + 1]) + g.y);
+              pack_h2((acc_l[4 * i + 2 * h] + sb_lff[n]) + g.x, (acc_l[4 * i + 2 * h + 1] + sb_lff[n + 1]) + g.y);
         }
       }
     }
@@ -266,12 +257,10 @@ __global__ void __launch_bounds__(384, 1) rdb_tail_kernel(const __grid_constant_
 }
 
 // ------------------------------------------------------------------ host side
-int make_p8_tmap(CUtensorMap* m, const bin_act_t& t, int box_rows);   // conv_igemm.cu
-
 template <int G0>
 static int launch_rdb_tail_g(RdbTailParams& p, const bin_act_t& x, const bin_act_t& g, cudaStream_t s) {
-  BIN_TRY(make_p8_tmap(&p.tmap0, x, kRtRows));                // every argument is checked before the first tensor map
-  BIN_TRY(make_p8_tmap(&p.tmap1, g, kRtRows));
+  BIN_TRY(make_p8_tmap(&p.tmap0, x, kTWH, kRtRows, kKPL));    // every argument is checked before the first tensor map
+  BIN_TRY(make_p8_tmap(&p.tmap1, g, kTWH, kRtRows, kKPL));
   static std::atomic<unsigned long long> opted{0};   // per instantiation, per device
   BIN_TRY(ensure_dynamic_smem(rdb_tail_kernel<G0>, RtCfg<G0>::Smem, opted));
   const int sms = num_sms();

@@ -203,8 +203,6 @@ __global__ void __launch_bounds__(256) wgrad_reduce_kernel(const float* __restri
   }
 }
 
-int make_p8_tmap_box(CUtensorMap* m, const bin_act_t& t, int box_px, int box_rows, int box_planes);
-
 template <int N>
 static int run_wgrad(WgradParams p, int smem_bytes, int ci_planes, int kk, int ks, cudaStream_t s, bool det) {
   static std::atomic<unsigned long long> smem_opted{0};   // per instantiation, per device
@@ -231,9 +229,9 @@ static int run_wgrad(WgradParams p, int smem_bytes, int ci_planes, int kk, int k
   return BIN_OK;
 }
 
-int launch_wgrad_impl(const bin_act_t& x0, int x0_plane0, int x0_planes, const bin_act_t& x1, int x1_plane0, int x1_planes,
-                      const bin_act_t& dy, int dy_plane0, int cout, int cin, int ks, const float* scale, float* dw,
-                      float* partial_ws, cudaStream_t s, bool det) {
+int launch_wgrad(const bin_act_t& x0, int x0_plane0, int x0_planes, const bin_act_t& x1, int x1_plane0, int x1_planes,
+                 const bin_act_t& dy, int dy_plane0, int cout, int cin, int ks, const float* scale, float* dw,
+                 float* partial_ws, cudaStream_t s, bool det) {
   if (ks != 1 && ks != 3 && ks != 5) return fail(BIN_ERR_ARG, "wgrad: ksize must be 1, 3 or 5");
   if (!partial_ws) return fail(BIN_ERR_ARG, "wgrad: partial-sum workspace missing");
   // TMA zero-fills a box that runs past its tensor, so a bad plane range or geometry would silently give wrong
@@ -259,9 +257,9 @@ int launch_wgrad_impl(const bin_act_t& x0, int x0_plane0, int x0_planes, const b
   // and then dropped by the reduction's co < cout test)
   n = n <= 64 ? n : n <= 96 ? 96 : n <= 128 ? 128 : 256;
   p.pw = kWgTW + (p.sx ? 0 : 2 * p.pad); p.rows = kWgTH + 2 * p.pad;
-  BIN_TRY(make_p8_tmap_box(&p.xmap0, x0, p.pw, p.rows, 4));
-  if (x1_planes > 0) BIN_TRY(make_p8_tmap_box(&p.xmap1, x1, p.pw, p.rows, 4));
-  BIN_TRY(make_p8_tmap_box(&p.ymap, dy, kWgTW, kWgTH, p.sx ? 4 : n / 8));
+  BIN_TRY(make_p8_tmap(&p.xmap0, x0, p.pw, p.rows, 4));
+  if (x1_planes > 0) BIN_TRY(make_p8_tmap(&p.xmap1, x1, p.pw, p.rows, 4));
+  BIN_TRY(make_p8_tmap(&p.ymap, dy, kWgTW, kWgTH, p.sx ? 4 : n / 8));
   p.x0_plane0 = x0_plane0; p.x0_planes = x0_planes; p.x1_plane0 = x1_plane0; p.x1_planes = x1_planes;
   p.dy_plane0 = dy_plane0; p.n = n; p.cout = cout; p.cin = cin;
   p.B = x0.B; p.H = x0.H; p.W = x0.W;
