@@ -189,19 +189,19 @@ class _Prefetch:
     """cv2.imread of `paths` in order on `threads` host threads, each image copied into pinned memory, at most `depth`
     ahead of the consumer."""
 
-    def __init__(self, paths: Sequence[str], threads: int, depth: int):
+    def __init__(self, paths: Sequence[str], threads: int, depth: int, who: str):
         self._paths = iter(paths)
+        self._who = who
         self._pool = cf.ThreadPoolExecutor(max(threads, 1), thread_name_prefix="bin_b200-decode")
         self._q: collections.deque = collections.deque()
         for _ in range(max(depth, 1)):
             self._submit()
 
-    @staticmethod
-    def _read(path: str) -> torch.Tensor:
+    def _read(self, path: str) -> torch.Tensor:
         import cv2
         img = cv2.imread(path)
         if img is None:
-            raise BinB200Error(f"evaluate_testset: cannot read {path}")
+            raise BinB200Error(f"{self._who}: cannot read {path}")
         return torch.from_numpy(img).pin_memory()
 
     def _submit(self):
@@ -222,7 +222,7 @@ class _Prefetch:
 
 
 # ----------------------------------------------------------------------------- one rank's windows
-def _folder_info(input_path: str, folder: str) -> Tuple[int, int]:
+def folder_info(input_path: str, folder: str, who: str = "evaluate_testset") -> Tuple[int, int]:
     """-> (frame count, first frame number) of a folder (test.py:244, 251-252); the names must run 8 apart."""
     names = sorted(os.listdir(os.path.join(input_path, folder)))
     if not names:
@@ -230,98 +230,86 @@ def _folder_info(input_path: str, folder: str) -> Tuple[int, int]:
     first = int(names[0][:-4])
     want = [str(first + 8 * k).zfill(5) + ".png" for k in range(len(names))]
     if names != want:
-        raise BinB200Error(f"evaluate_testset: the blurry frames of {folder} must be named {want[0]}, {want[1:2]}... 8 "
-                           "apart (test.py:262-287 names its inputs that way)")
+        raise BinB200Error(f"{who}: the blurry frames of {folder} must be named {want[0]}, {want[1:2]}... 8 "
+                           "apart (test.py:262-287 and demo.py:196-205 name their inputs that way)")
     return len(names), first
 
 
-def _schedule(folder_n: int, rng: range) -> List[Tuple[str, object]]:
-    """The order the rank consumes files in: frame p as it arrives, then the GTs of the windows due at it."""
+def _schedule(folder_n: int, rng: range, reads) -> List[Tuple[str, object]]:
+    """The order the rank consumes files in: frame p as it arrives, then the reads(i) of the windows i due at it."""
     plan = VideoPlan(frozenset(), rng, folder_n)
     out = []
     while not plan.complete:
         pos = plan.next_pos
         out.append(("frame", pos))
         for step in plan.arrive():
-            out += [("gt", (step.i, k)) for k in (12, 8, 13) if k in test_py_writes(step.i, folder_n)]
+            out += [("read", p) for p in reads(step.i)]
     return out
 
 
-def _evaluate_rank(win_net, dev, pieces, info, input_path, gt_path, gen_dir, direct_interp, threads):
-    """Run one rank's (folder, window range) pieces -> (records, seconds)."""
-    sched = []                                      # (folder, kind, key, path)
+def window_loop(win_net, dev, pieces, info, frame_path, outputs, *, reads=None, on_window=None, threads: int = 8,
+                who: str = "evaluate_testset") -> float:
+    """One rank's windows, the loop evaluate_testset and demo.run_demo share: each (folder, window range) of `pieces`
+    streamed (stream_video) from frames decoded on `threads` host threads that read ahead, each window's outputs
+    cropped on the device (tensor2img_u8), encoded by the GPU PNG encoder and written by a host thread.  The host never
+    waits on the GPU between windows: window i's PNGs are collected while window i+1 runs.
+
+    info[folder] = (frame count, first frame number); frame_path(folder, pos) names the blurry frame at position pos;
+    outputs(folder, i, n) -> {output index: [files]}: each output window i writes, encoded once and written to every
+    file listed.  reads(folder, i, n) -> [files] window i decodes besides its frames (read ahead with them), and
+    on_window(folder, i, n, (h, w), imgs, decoded, blurry) sees them with the cropped device images and the uint8
+    device frames held by position; what it returns, if not None, is called one window later, once the window's files
+    are queued.  The net computes in its own modes (the caller sets its output selection).  -> seconds taken."""
+    reads = reads or (lambda folder, i, n: ())
+    sched = []                                      # the files in the order they are consumed
     for folder, rng in pieces:
-        n, first = info[folder]
-        wp = lambda i: window_paths(input_path, gt_path, gen_dir, folder, first, i, n, direct_interp)   # noqa: E731
-        for kind, key in _schedule(n, rng):
-            if kind == "frame":
-                p = os.path.join(gt_path if direct_interp else input_path, folder, str(first + 8 * key).zfill(5) + ".png")
-            else:
-                p = wp(key[0]).gt[key[1]]
-            sched.append((folder, kind, key, p))
-    pre = _Prefetch([s[3] for s in sched], threads, 4 * threads + 8)
+        n, _ = info[folder]
+        for kind, key in _schedule(n, rng, lambda i: reads(folder, i, n)):
+            sched.append(frame_path(folder, key) if kind == "frame" else key)
+    pre = _Prefetch(sched, threads, 4 * threads + 8, who)
     writer = cf.ThreadPoolExecutor(1, thread_name_prefix="bin_b200-write")
     writes: List[cf.Future] = []
-    records: List[Record] = []
     pending = None
-    cursor = iter(sched)
-
-    def take(kind, key):
-        _, k, kk, p = next(cursor)
-        assert (k, kk) == (kind, key), ((k, kk), (kind, key))
-        return pre.get(p)
 
     def finish(job):
-        folder, i, hw, ev, host, png, paths = job
-        for path, data in zip(paths, png.result()):
-            writes.append(writer.submit(_write_file, path, data))
-        ev.synchronize()
-        records.append(Record(folder, i, hw[0], hw[1], tuple(tuple(r) for r in host.tolist())))
+        png, names, after = job
+        for paths, data in zip(names, png.result()):
+            for path in paths:
+                writes.append(writer.submit(_write_file, path, data))
+        if after is not None:
+            after()
 
     t0 = time.perf_counter()
     try:
         with torch.cuda.device(dev):
-            stream = torch.cuda.current_stream()
             for folder, rng in pieces:
-                n, first = info[folder]
+                n, _ = info[folder]
                 blurry: Dict[int, torch.Tensor] = {}
                 shape = {}
 
                 def frames():
                     for pos in range(max(rng.start - 2, 0), min(rng.stop + 2, n - 1) + 1):
-                        u8 = take("frame", pos).to(dev, non_blocking=True)
+                        u8 = pre.get(frame_path(folder, pos)).to(dev, non_blocking=True)
                         if not shape:
                             shape["hw"] = tuple(u8.shape[:2])
                             shape["pad"] = test_py_padding(*shape["hw"])
                         elif tuple(u8.shape[:2]) != shape["hw"]:
-                            raise BinB200Error(f"evaluate_testset: the frames of {folder} differ in size")
+                            raise BinB200Error(f"{who}: the frames of {folder} differ in size")
                         blurry[pos] = u8
                         yield upload_frame_u8(u8, shape["pad"], dev)
 
                 for i, outs in stream_video(win_net, frames(), windows=rng, n=n):
                     (h, w), (pl, _, pt, _) = shape["hw"], shape["pad"]
-                    wp = window_paths(input_path, gt_path, gen_dir, folder, first, i, n, direct_interp)
-                    todo = test_py_writes(i, n)
+                    todo = outputs(folder, i, n)
                     imgs = {k: tensor2img_u8(outs[k], crop=(pt, pl, h, w)) for k in todo}
-                    gts = {}
-                    for k in (12, 8, 13):
-                        if k in todo:
-                            gts[k] = take("gt", (i, k)).to(dev, non_blocking=True)
-                            if tuple(gts[k].shape[:2]) != (h, w):
-                                raise BinB200Error(f"evaluate_testset: {wp.gt[k]} is not {h}x{w}")
-                    blur = blurry[min(i + 1, n - 1)]
-                    pairs = [(imgs[k], gts[k]) if k >= 0 else (blur, gts[13]) for k in _scored(i, n)]
-                    sums = image_metrics_batch(pairs, bgr=True)
-                    host = torch.empty(sums.shape, dtype=torch.float64, pin_memory=True)
-                    host.copy_(sums, non_blocking=True)
-                    ev = torch.cuda.Event()
-                    ev.record(stream)
+                    decoded = [pre.get(p) for p in reads(folder, i, n)]
+                    after = None if on_window is None else on_window(folder, i, n, (h, w), imgs, decoded, blurry)
                     png = encode_png_async([imgs[k] for k in todo])
                     for p in [p for p in blurry if p < min(i + 1, n - 1)]:
                         del blurry[p]
                     if pending is not None:
-                        finish(pending)             # window i-1's files and sums, while window i runs
-                    pending = (folder, i, (h, w), ev, host, png, [wp.out[k] for k in todo])
+                        finish(pending)             # window i-1's files, while window i runs
+                    pending = (png, list(todo.values()), after)
             if pending is not None:
                 finish(pending)
             for f in writes:
@@ -330,7 +318,50 @@ def _evaluate_rank(win_net, dev, pieces, info, input_path, gt_path, gen_dir, dir
     finally:
         pre.close()
         writer.shutdown(wait=True)
-    return records, time.perf_counter() - t0
+    return time.perf_counter() - t0
+
+
+def _evaluate_rank(win_net, dev, pieces, info, input_path, gt_path, gen_dir, direct_interp, threads):
+    """Run one rank's (folder, window range) pieces -> (records, seconds)."""
+    records: List[Record] = []
+    paths = lambda folder, i, n: window_paths(input_path, gt_path, gen_dir, folder, info[folder][1], i, n,   # noqa: E731
+                                              direct_interp)
+
+    def frame_path(folder, pos):
+        return os.path.join(gt_path if direct_interp else input_path, folder,
+                            str(info[folder][1] + 8 * pos).zfill(5) + ".png")
+
+    def outputs(folder, i, n):
+        wp = paths(folder, i, n)
+        return {k: [wp.out[k]] for k in test_py_writes(i, n)}
+
+    def reads(folder, i, n):
+        wp = paths(folder, i, n)
+        return [wp.gt[k] for k in (12, 8, 13) if k in test_py_writes(i, n)]
+
+    def score(folder, i, n, hw, imgs, decoded, blurry):
+        wp = paths(folder, i, n)
+        gts = {}
+        for k, g in zip([k for k in (12, 8, 13) if k in imgs], decoded):
+            gts[k] = g.to(dev, non_blocking=True)
+            if tuple(gts[k].shape[:2]) != hw:
+                raise BinB200Error(f"evaluate_testset: {wp.gt[k]} is not {hw[0]}x{hw[1]}")
+        blur = blurry[min(i + 1, n - 1)]
+        pairs = [(imgs[k], gts[k]) if k >= 0 else (blur, gts[13]) for k in _scored(i, n)]
+        sums = image_metrics_batch(pairs, bgr=True)
+        host = torch.empty(sums.shape, dtype=torch.float64, pin_memory=True)
+        host.copy_(sums, non_blocking=True)
+        ev = torch.cuda.Event()
+        ev.record(torch.cuda.current_stream())
+
+        def done():
+            ev.synchronize()
+            records.append(Record(folder, i, hw[0], hw[1], tuple(tuple(r) for r in host.tolist())))
+        return done
+
+    seconds = window_loop(win_net, dev, pieces, info, frame_path, outputs, reads=reads, on_window=score,
+                          threads=threads)
+    return records, seconds
 
 
 def _write_file(path: str, data: bytes) -> None:
@@ -347,10 +378,11 @@ def _gather(local, world: int) -> list:
     return out
 
 
-def _window_net(net):
+def window_nets(net, who: str = "evaluate_testset"):
+    """The BIN window nets inside `net` (the net itself, or the one a wrapper holds)."""
     nets = [m for m in net.modules() if isinstance(m, rdn.RDN_residual_interp_5_input_ConvLSTM_L)]
     if not nets:
-        raise BinB200Error("evaluate_testset: no RDN_residual_interp_5_input_ConvLSTM_L in this module")
+        raise BinB200Error(f"{who}: no RDN_residual_interp_5_input_ConvLSTM_L in this module")
     return nets
 
 
@@ -375,13 +407,13 @@ def evaluate_testset(net, input_path: str, gt_path: str, output_path: str, net_n
             rank, world = 0, 1
     if not 0 <= rank < world:
         raise BinB200Error(f"evaluate_testset: rank {rank} is not in 0..{world - 1}")
-    nets = _window_net(net)
+    nets = window_nets(net)
     dev = next(net.parameters()).device
     flip_test = rdn._ensemble_of(nets[0]) is not None
     result_path = os.path.join(output_path, RESULT_DIR)
     gen_dir = os.path.join(result_path, net_name)
     subdir = sorted(os.listdir(input_path))                                      # test.py:158
-    info = {f: _folder_info(input_path, f) for f in subdir}
+    info = {f: folder_info(input_path, f) for f in subdir}
     pieces = bdist.shard_test_set({f: info[f][0] for f in subdir}, world)[rank]
     for f in subdir:
         os.makedirs(os.path.join(gen_dir, f), exist_ok=True)
