@@ -81,6 +81,19 @@ __device__ __forceinline__ void tma_load_4d(void* smem_dst, const void* tmap, ui
       "l"(tmap), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
 }
+// 4-D tiled store shared -> global into the issuing thread's bulk group; the box's out-of-bounds part is not written.
+// The smem source is 128-byte aligned, and the generic-proxy writes that filled it are ordered before the store by
+// fence_proxy_async() in every writing thread and a barrier.
+__device__ __forceinline__ void tma_store_4d(const void* tmap, const void* smem_src, int c0, int c1, int c2, int c3) {
+  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(tmap),
+               "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// the issuing thread's committed stores have finished reading shared memory (the buffer may be rewritten)
+__device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// the issuing thread's committed stores are complete
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 // 1-D bulk copy global -> shared (size multiple of 16, 16-B aligned both sides).
 __device__ __forceinline__ void bulk_load_1d(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(

@@ -46,6 +46,10 @@ struct ConvCfg {
   // SX: xstack_sum exchange buffers, one per warp pair (2 per warpgroup) and 64-row block (2 per accumulator), so the
   // second block's exchange needs no barrier against the first block's reads
   static constexpr int XS_BYTES = SX ? kMT * 2 * 2 * kXsFloats<NT> * 4 : 0;
+  // fp16 SX P8 epilogue (tma_store below): a consumer warpgroup's staging buffer [NT/8 planes][4 rows][TW px][16 B]
+  static constexpr int ST_PLANE = (kTH / kMT) * TW * 16;
+  static constexpr int ST_BYTES = NT / 8 * ST_PLANE;
+  static_assert(XS_BYTES % 128 == 0 && ST_BYTES % 128 == 0, "TMA store sources must be 128-byte aligned");
   static_assert(!(SX && ROWSPLIT), "SX is only used for 3x3");
   static_assert(NMMA % 16 == 0 && NMMA <= 256, "invalid wgmma N");
 };
@@ -99,6 +103,10 @@ template <int NT, int KS, int EPI, bool SX, bool X3>
 __global__ void __launch_bounds__(kThreads, 1) conv_igemm_kernel(const __grid_constant__ ConvParams p) {
   using C = ConvCfg<NT, KS, SX>;
   static_assert(EPI != BIN_EPI_PIXSHUF || NT == 128, "the PixelShuffle staging buffer holds 4 output planes");
+  // The fp16 x-stacked P8 epilogue (the RDB growth convs) stages each warpgroup's 4 output rows of the tile in shared
+  // memory and writes them with one TMA tensor store over p.tmap_out, whose out-of-bounds clipping stands in for every
+  // pixel validity test but the junk columns.
+  constexpr bool TSTORE = SX && EPI == BIN_EPI_P8 && !X3;
   constexpr int NA = C::NMMA / 2;                              // accumulator registers per thread and 64-row block
   extern __shared__ __align__(1024) uint8_t smem[];
   Ctrl* ctrl = reinterpret_cast<Ctrl*>(smem);
@@ -120,6 +128,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_igemm_kernel(const __grid_co
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&p.tmap0);
     if (p.nch1 > 0) tma_prefetch_desc(&p.tmap1);
+    if (TSTORE) tma_prefetch_desc(&p.tmap_out);
     for (int i = 0; i < kMaxStages; ++i) {
       mbar_init(&ctrl->full[i], 1);
       mbar_init(&ctrl->empty[i], 8);                           // one arrival per consumer warp
@@ -185,6 +194,8 @@ __global__ void __launch_bounds__(kThreads, 1) conv_igemm_kernel(const __grid_co
   const int k4 = lane & 3;                                     // fragment column pair: columns 8 i + 2 k4, +1
   float* xs = reinterpret_cast<float*>(stage0 + (size_t)S * stage_bytes) + (2 * m + (wq >> 1)) * 2 * kXsFloats<NT>;
   uint8_t* psbuf = stage0 + (size_t)S * stage_bytes + (warp - 4) * kPsWarpBytes<X3>;   // PIXSHUF staging buffer
+  uint8_t* stbuf = stage0 + (size_t)S * stage_bytes + C::XS_BYTES + m * C::ST_BYTES;   // TSTORE staging buffer
+  const bool st_leader = (threadIdx.x & 127) == 0;            // TSTORE: the thread that issues the warpgroup's stores
   float acc[2][NA];
   constexpr float kAcc = X3 ? (1.f / 256.f) : 1.f;            // X3 weights are packed scaled by 2^8
   uint32_t s = 0, ph = 0;
@@ -315,6 +326,36 @@ __global__ void __launch_bounds__(kThreads, 1) conv_igemm_kernel(const __grid_co
     // ---------------------------------------------------------- epilogue from the accumulator fragments
     int nh, txi, tyi, b;
     tile_coords(tq, nh, txi, tyi, b);
+    if constexpr (TSTORE) {
+      // The previous tile's store has had this tile's main loop to read the buffer, so this wait should not stall.
+      if (st_leader) bulk_wait_read_all();
+      wg_sync(1 + m);
+#pragma unroll
+      for (int mb = 0; mb < 2; ++mb) {
+        xstack_sum<NT>(acc[mb], xs + mb * kXsFloats<NT>, 3 + 2 * m + (wq >> 1));
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int tx = (wq & 1) * 16 + (lane >> 2) + 8 * h;     // pixel of row 2 mb + wq / 2 of the warpgroup's 4
+          if (tx >= C::TW) continue;                               // junk column
+          uint8_t* dst = stbuf + ((2 * mb + (wq >> 1)) * C::TW + tx) * 16 + 4 * k4;
+#pragma unroll
+          for (int i = 0; i < NT / 8; ++i) {                       // planes past store_planes lie outside the box
+            const int n = nh * NT + 8 * i + 2 * k4;                // NT * nh <= 256: the bias is in shared memory
+            float f0 = acc[mb][4 * i + 2 * h] + sbias[n], f1 = acc[mb][4 * i + 2 * h + 1] + sbias[n + 1];
+            if (p.relu) { f0 = fmaxf(f0, 0.f); f1 = fmaxf(f1, 0.f); }
+            *reinterpret_cast<uint32_t*>(dst + i * C::ST_PLANE) = pack_h2(f0, f1);
+          }
+        }
+      }
+      fence_proxy_async();                                         // generic-proxy writes -> visible to the TMA
+      wg_sync(1 + m);
+      if (st_leader) {
+        tma_store_4d(&p.tmap_out, stbuf, txi * C::TW * 8, tyi * kTH + (kTH / kMT) * m, p.out_plane0 + (nh * NT) / 8,
+                     b - p.b0);
+        bulk_commit();
+      }
+      continue;
+    }
 #pragma unroll
     for (int mb = 0; mb < 2; ++mb) {
       if constexpr (SX) xstack_sum<NT>(acc[mb], xs + mb * kXsFloats<NT>, 3 + 2 * m + (wq >> 1));   // barrier per warp pair
@@ -356,7 +397,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_igemm_kernel(const __grid_co
                   f0 += g2.x; f1 += g2.y;
                 }
               }
-              if constexpr (SX) {                                // the x-stacked kernels keep their own addressing
+              if constexpr (SX) {                                // X3 x-stacked kernel: its own addressing
                 const int op = p.out_plane0 + rel;
                 const size_t off = ((((size_t)b * p.out_planes + (X3 ? x3_plane(op) : op)) * p.H + y) * p.W + x) * 8 + 2 * k4;
                 store_pair<X3>(p.out + off, (size_t)4 * p.H * p.W * 8, f0, f1);
@@ -424,6 +465,9 @@ __global__ void __launch_bounds__(kThreads, 1) conv_igemm_kernel(const __grid_co
       }
     }
   }
+  if constexpr (TSTORE) {
+    if (st_leader) bulk_wait_all();                              // the staging buffers outlive no store
+  }
 }
 
 // ------------------------------------------------------------------ host side
@@ -443,7 +487,8 @@ static EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
-int make_p8_tmap(CUtensorMap* m, const bin_act_t& t, int box_px, int box_rows, int box_planes) {
+int make_p8_tmap(CUtensorMap* m, const bin_act_t& t, int box_px, int box_rows, int box_planes, int b0, int nb, int y0,
+                 int ny) {
   EncodeTiledFn fn = get_encode_fn();
   if (!fn) return fail(BIN_ERR_CUDA, "cuTensorMapEncodeTiled not available from the driver");
   if ((reinterpret_cast<uintptr_t>(t.ptr) & 15) != 0) return fail(BIN_ERR_ARG, "P8 tensor not 16-byte aligned");
@@ -451,11 +496,14 @@ int make_p8_tmap(CUtensorMap* m, const bin_act_t& t, int box_px, int box_rows, i
   // The (8 channels, W) dims of a P8 plane row are contiguous in memory, so they are described as ONE
   // dimension of W*8 elements: a conv box row is then 32 px * 16 B = 512 contiguous bytes (a 16-byte
   // inner box made the TMA unit the bottleneck).  OOB zero fill works per element, i.e. per pixel.
-  cuuint64_t dims[4] = {(cuuint64_t)t.W * 8, (cuuint64_t)t.H, (cuuint64_t)t.planes, (cuuint64_t)t.B};
-  cuuint64_t strides[3] = {(cuuint64_t)t.W * 16, (cuuint64_t)t.H * t.W * 16, (cuuint64_t)t.planes * t.H * t.W * 16};
+  const size_t row = (size_t)t.W * 16, plane = (size_t)t.H * row, image = (size_t)t.planes * plane;
+  void* base = static_cast<uint8_t*>(t.ptr) + (size_t)b0 * image + (size_t)y0 * row;   // stays 16-byte aligned
+  cuuint64_t dims[4] = {(cuuint64_t)t.W * 8, (cuuint64_t)(ny > 0 ? ny : t.H), (cuuint64_t)t.planes,
+                        (cuuint64_t)(nb > 0 ? nb : t.B)};
+  cuuint64_t strides[3] = {row, plane, image};
   cuuint32_t box[4] = {(cuuint32_t)box_px * 8, (cuuint32_t)box_rows, (cuuint32_t)box_planes, 1};
   cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, t.ptr, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                   CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return fail(BIN_ERR_CUDA, "cuTensorMapEncodeTiled failed with code " + std::to_string((int)r));
   return BIN_OK;
@@ -485,7 +533,9 @@ static int launch_inst(const bin_conv_args_t& a, cudaStream_t s) {
   p.div_nh = fast_div(p.nh); p.div_tx = fast_div(p.tiles_x); p.div_ty = fast_div(p.tiles_y);
   p.relu = a.relu;
   const int nchunks = p.nch0 + p.nch1;
-  const int xbytes = C::XS_BYTES + (EPI == BIN_EPI_PIXSHUF ? 8 * kPsWarpBytes<X3> : 0);   // + the consumer warps' staging
+  constexpr bool tma_store = SX && EPI == BIN_EPI_P8 && !X3;   // see conv_igemm_kernel
+  const int xbytes = C::XS_BYTES + (EPI == BIN_EPI_PIXSHUF ? 8 * kPsWarpBytes<X3> : 0) +   // + the consumer warps' staging
+                     (tma_store ? kMT * C::ST_BYTES : 0);
   // keep the whole weight set resident in smem when it leaves room for >= 3 activation stages
   p.resident = (p.nh == 1 && nchunks <= kMaxResidentChunks &&
                 kCtrlBytes + nchunks * C::W_CHUNK + xbytes + 3 * C::A_BYTES + 256 <= kSmemMax) ? 1 : 0;
@@ -510,6 +560,7 @@ static int launch_inst(const bin_conv_args_t& a, cudaStream_t s) {
   p.fr = a.fr;
   BIN_TRY(make_p8_tmap(&p.tmap0, a.in0, kTWH, C::ROWS, kKPL));
   if (a.in1_planes > 0) BIN_TRY(make_p8_tmap(&p.tmap1, a.in1, kTWH, C::ROWS, kKPL));
+  if (tma_store) BIN_TRY(make_p8_tmap(&p.tmap_out, a.out, C::TW, kTH / kMT, p.store_planes, p.b0, nb, p.y0, p.ny));
   auto kern = conv_igemm_kernel<NT, KS, EPI, SX, X3>;
   static std::atomic<unsigned long long> smem_opted{0};   // per instantiation, per device
   BIN_TRY(ensure_dynamic_smem(kern, kSmemMax, smem_opted));

@@ -79,6 +79,7 @@ inline FastDiv fast_div(int d) {   // d >= 1
 
 struct alignas(64) ConvParams {
   CUtensorMap tmap0, tmap1;
+  CUtensorMap tmap_out;                // fp16 x-stacked P8 epilogue: the output over the launch's sub-range (TMA stores)
   int plane0_0, nch0, plane0_1, nch1;  // segment start plane / number of K chunks (X3: 3 per logical chunk)
   int nch0l;                           // logical 32-channel chunks of segment 0
   const __half* w;
@@ -95,8 +96,11 @@ struct alignas(64) ConvParams {
 
 // ------------------------------------------------------------------ conv_igemm.cu
 int launch_conv(const bin_conv_args_t& a, cudaStream_t s);
-// TMA map of a P8 tensor whose box is box_px pixels x box_rows rows x box_planes planes
-int make_p8_tmap(CUtensorMap* m, const bin_act_t& t, int box_px, int box_rows, int box_planes);
+// TMA map of a P8 tensor whose box is box_px pixels x box_rows rows x box_planes planes.  With nb, ny > 0 it covers rows
+// [y0, y0 + ny) of images [b0, b0 + nb) only: coordinates are then relative to (b0, y0), and a box's parts outside that
+// range read as zeros and are not written.
+int make_p8_tmap(CUtensorMap* m, const bin_act_t& t, int box_px, int box_rows, int box_planes, int b0 = 0, int nb = 0,
+                 int y0 = 0, int ny = 0);
 
 // ------------------------------------------------------------------ rdb_tail.cu
 int launch_rdb_tail(int g0, const bin_act_t& x, int x_plane0, const bin_act_t& g, int g_plane0, const void* w_conv,

@@ -239,15 +239,17 @@ __global__ void __launch_bounds__(384, 1) rdb_tail_kernel(const __grid_constant_
     acc_fence(acc_l);
 
     // ---------------------------------------------------------- x' = LFF + b + x
+    const size_t plane = (size_t)p.H * p.W * 8;                     // halves per P8 plane
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       if (valid[h]) {
+        // the pixel's offset once, then one plane stride per plane
+        __half* dst = p.out + ((((size_t)b * p.out_planes + p.out_plane0) * p.H + y[h]) * p.W + x[h]) * 8 + 2 * k4;
 #pragma unroll
         for (int i = 0; i < G0 / 8; ++i) {
           const int n = 8 * i + 2 * k4;
           const float2 g = unpack_h2(res[h][i]);
-          const size_t off = ((((size_t)b * p.out_planes + p.out_plane0 + i) * p.H + y[h]) * p.W + x[h]) * 8 + 2 * k4;
-          *reinterpret_cast<uint32_t*>(p.out + off) =
+          *reinterpret_cast<uint32_t*>(dst + (size_t)i * plane) =
               pack_h2((acc_l[4 * i + 2 * h] + sb_lff[n]) + g.x, (acc_l[4 * i + 2 * h + 1] + sb_lff[n + 1]) + g.y);
         }
       }
