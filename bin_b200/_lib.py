@@ -126,7 +126,7 @@ _SIGS = {
     "bin_u8_to_frame": (C.c_int, [C.c_void_p] + [C.c_int] * 6 + [C.c_void_p, C.c_void_p]),
     "bin_rdb_tail_fwd": (C.c_int, [C.POINTER(Act), C.c_int, C.POINTER(Act), C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                    C.POINTER(Act), C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
-    "bin_adam_step": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int] + [C.c_float] * 8 + [C.c_void_p]),
+    "bin_adam_step": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int] + [C.c_float] * 8 + [C.c_void_p, C.c_void_p]),
     "bin_grad_audit_scratch_bytes": (C.c_size_t, [C.c_int]),
     "bin_grad_audit": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_float, C.c_void_p, C.c_size_t,
                                  C.c_void_p, C.c_void_p]),

@@ -787,10 +787,11 @@ int bin_rdb_tail_fwd(const bin_act_t* x, int x_plane0, const bin_act_t* g, int g
 }
 int bin_adam_step(const bin_adam_tensor_t* table_dev, const int* chunk_prefix_dev, int ntensors, int nchunks, float lr,
                   float beta1, float beta2, float eps, float weight_decay, float bias_correction1,
-                  float bias_correction2, float grad_scale, bin_stream_t s) {
+                  float bias_correction2, float grad_scale, bin_adam_scalars_t* scalars_dev, bin_stream_t s) {
   if (!table_dev || !chunk_prefix_dev) return fail(BIN_ERR_ARG, "adam_step: null argument");
+  if (reinterpret_cast<uintptr_t>(scalars_dev) & 7) return fail(BIN_ERR_ARG, "adam_step: scalars not 8-byte aligned");
   return launch_adam_step(table_dev, chunk_prefix_dev, ntensors, nchunks, lr, beta1, beta2, eps, weight_decay,
-                          bias_correction1, bias_correction2, grad_scale, nullptr, (cudaStream_t)s);
+                          bias_correction1, bias_correction2, grad_scale, nullptr, scalars_dev, (cudaStream_t)s);
 }
 int bin_adam_step_guarded(const bin_adam_tensor_t* table_dev, const int* chunk_prefix_dev, int ntensors, int nchunks,
                           float lr, float beta1, float beta2, float eps, float weight_decay, float bias_correction1,
@@ -798,7 +799,7 @@ int bin_adam_step_guarded(const bin_adam_tensor_t* table_dev, const int* chunk_p
   if (!table_dev || !chunk_prefix_dev || !audit_dev) return fail(BIN_ERR_ARG, "adam_step_guarded: null argument");
   if (reinterpret_cast<uintptr_t>(audit_dev) & 7) return fail(BIN_ERR_ARG, "adam_step_guarded: audit record not 8-byte aligned");
   return launch_adam_step(table_dev, chunk_prefix_dev, ntensors, nchunks, lr, beta1, beta2, eps, weight_decay,
-                          bias_correction1, bias_correction2, grad_scale, audit_dev, (cudaStream_t)s);
+                          bias_correction1, bias_correction2, grad_scale, audit_dev, nullptr, (cudaStream_t)s);
 }
 size_t bin_grad_audit_scratch_bytes(int nchunks) { return grad_audit_scratch_bytes(nchunks); }
 int bin_grad_audit(const bin_adam_tensor_t* table_dev, const int* chunk_prefix_dev, int ntensors, int nchunks,

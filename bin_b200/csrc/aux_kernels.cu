@@ -761,14 +761,42 @@ __device__ __forceinline__ void adam_one(float& p, float g, float& m, float& v, 
   const float denom = sqrtf(v) * inv_sqrt_bc2 + eps;   // (exp_avg_sq.sqrt() / sqrt(bias_correction2)).add_(eps)
   p = p - lr_bc1 * (m / denom);                        // param.addcdiv_(exp_avg, denom, value=-lr / bias_correction1)
 }
-// kGuard: the step obeys the record grad_audit_reduce_kernel left in `audit` (DESIGN 4i).  A block of a skipped step
+// kAdamGuarded: the step obeys the record grad_audit_reduce_kernel left in `audit` (DESIGN 4i).  A block of a skipped step
 // returns before it loads anything else; an applied one scales the gradient by grad_scale * coef, which is grad_scale
 // itself when coef == 1, so an unclipped guarded step writes the plain step's bits.
-template <bool kGuard>
+// adam_one with every rounding spelled out: the fused multiply-adds nvcc forms from adam_one in the plain and guarded
+// kernels.  The device-scalar kernel reads lr_bc1 and inv_sqrt_bc2 from memory, and nvcc contracts adam_one differently
+// there; this form gives it the plain kernel's bits whatever the compiler does.
+__device__ __forceinline__ void adam_one_rn(float& p, float g, float& m, float& v, float lr_bc1, float b1, float b2,
+                                            float eps, float wd, float inv_sqrt_bc2, float gscale) {
+  g = __fmul_rn(g, gscale);
+  if (wd != 0.f) g = __fmaf_rn(wd, p, g);
+  m = __fmaf_rn(__fsub_rn(g, m), __fsub_rn(1.f, b1), m);
+  v = __fmaf_rn(v, b2, __fmul_rn(__fmul_rn(__fsub_rn(1.f, b2), g), g));
+  const float denom = __fmaf_rn(__fsqrt_rn(v), inv_sqrt_bc2, eps);
+  p = __fmaf_rn(-lr_bc1, __fdiv_rn(m, denom), p);
+}
+// kMode: kAdamPlain, kAdamGuarded (the record `audit`), or kAdamDevice (bin_adam_scalars_t: lr_bc1 and inv_sqrt_bc2
+// from adam_scalars_kernel, the guard from the record sc->audit names -- for an unguarded step one that never skips,
+// coef 1).  All three give the same bits (the device form through adam_one_rn).
+enum AdamMode { kAdamPlain = 0, kAdamGuarded = 1, kAdamDevice = 2 };
+template <int kMode>
+__device__ __forceinline__ void adam_update(float& p, float g, float& m, float& v, float lr_bc1, float b1, float b2,
+                                            float eps, float wd, float inv_sqrt_bc2, float gscale) {
+  if (kMode == kAdamDevice) adam_one_rn(p, g, m, v, lr_bc1, b1, b2, eps, wd, inv_sqrt_bc2, gscale);
+  else adam_one(p, g, m, v, lr_bc1, b1, b2, eps, wd, inv_sqrt_bc2, gscale);
+}
+template <int kMode>
 __global__ void adam_step_kernel(const bin_adam_tensor_t* __restrict__ table, const int* __restrict__ chunk_prefix,
                                  int ntensors, float lr_bc1, float b1, float b2, float eps, float wd,
-                                 float inv_sqrt_bc2, float gscale, const bin_grad_audit_t* __restrict__ audit) {
-  if (kGuard) {
+                                 float inv_sqrt_bc2, float gscale, const bin_grad_audit_t* __restrict__ audit,
+                                 const bin_adam_scalars_t* __restrict__ sc) {
+  if (kMode == kAdamDevice) {
+    audit = sc->audit;
+    lr_bc1 = sc->lr_bc1;
+    inv_sqrt_bc2 = sc->inv_sqrt_bc2;
+  }
+  if (kMode != kAdamPlain) {
     if (audit->skip) return;
     gscale = gscale * audit->coef;
   }
@@ -797,26 +825,43 @@ __global__ void adam_step_kernel(const bin_adam_tensor_t* __restrict__ table, co
       float4 p = *reinterpret_cast<float4*>(P + i), m = *reinterpret_cast<float4*>(M + i),
              v = *reinterpret_cast<float4*>(V + i);
       const float4 g = *reinterpret_cast<const float4*>(G + i);
-      adam_one(p.x, g.x, m.x, v.x, lr_bc1, b1, b2, eps, wd, inv_sqrt_bc2, gscale);
-      adam_one(p.y, g.y, m.y, v.y, lr_bc1, b1, b2, eps, wd, inv_sqrt_bc2, gscale);
-      adam_one(p.z, g.z, m.z, v.z, lr_bc1, b1, b2, eps, wd, inv_sqrt_bc2, gscale);
-      adam_one(p.w, g.w, m.w, v.w, lr_bc1, b1, b2, eps, wd, inv_sqrt_bc2, gscale);
+      adam_update<kMode>(p.x, g.x, m.x, v.x, lr_bc1, b1, b2, eps, wd, inv_sqrt_bc2, gscale);
+      adam_update<kMode>(p.y, g.y, m.y, v.y, lr_bc1, b1, b2, eps, wd, inv_sqrt_bc2, gscale);
+      adam_update<kMode>(p.z, g.z, m.z, v.z, lr_bc1, b1, b2, eps, wd, inv_sqrt_bc2, gscale);
+      adam_update<kMode>(p.w, g.w, m.w, v.w, lr_bc1, b1, b2, eps, wd, inv_sqrt_bc2, gscale);
       *reinterpret_cast<float4*>(P + i) = p;
       *reinterpret_cast<float4*>(M + i) = m;
       *reinterpret_cast<float4*>(V + i) = v;
     }
     for (size_t i = end4 + threadIdx.x; i < end; i += blockDim.x) {
       float p = P[i], m = M[i], v = V[i];
-      adam_one(p, G[i], m, v, lr_bc1, b1, b2, eps, wd, inv_sqrt_bc2, gscale);
+      adam_update<kMode>(p, G[i], m, v, lr_bc1, b1, b2, eps, wd, inv_sqrt_bc2, gscale);
       P[i] = p; M[i] = m; V[i] = v;
     }
   } else {
     for (size_t i = base + threadIdx.x; i < end; i += blockDim.x) {
       float p = P[i], m = M[i], v = V[i];
-      adam_one(p, G[i], m, v, lr_bc1, b1, b2, eps, wd, inv_sqrt_bc2, gscale);
+      adam_update<kMode>(p, G[i], m, v, lr_bc1, b1, b2, eps, wd, inv_sqrt_bc2, gscale);
       P[i] = p; M[i] = m; V[i] = v;
     }
   }
+}
+
+// One-thread prologue of the device-scalar step (bin_adam_scalars_t): the scalars the host would pass by value for
+// step + 1, formed the way the host forms them -- 1 - beta^step in fp64, rounded to fp32, then the fp32 quotient and
+// reciprocal square root, each rounded once -- and the step count advanced, or, for a skipped guarded step, the skip
+// counted and nothing else touched.
+__global__ void adam_scalars_kernel(bin_adam_scalars_t* __restrict__ sc) {
+  if (sc->audit->skip) {
+    sc->skipped += 1;
+    return;
+  }
+  const float step = sc->step + 1.f;
+  const float bc1 = (float)(1.0 - pow(sc->beta1, (double)step));
+  const float bc2 = (float)(1.0 - pow(sc->beta2, (double)step));
+  sc->lr_bc1 = __fdiv_rn(sc->lr, bc1);
+  sc->inv_sqrt_bc2 = __fdiv_rn(1.f, __fsqrt_rn(bc2));
+  sc->step = step;
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -1251,16 +1296,26 @@ int launch_u8_to_frame(const uint8_t* img, int h, int w, int pl, int pr, int pt,
 }
 int launch_adam_step(const bin_adam_tensor_t* table, const int* chunk_prefix, int ntensors, int nchunks, float lr,
                      float beta1, float beta2, float eps, float weight_decay, float bias_correction1,
-                     float bias_correction2, float grad_scale, const bin_grad_audit_t* audit, cudaStream_t s) {
+                     float bias_correction2, float grad_scale, const bin_grad_audit_t* audit, bin_adam_scalars_t* sc,
+                     cudaStream_t s) {
+  if (sc) {
+    if (ntensors < 1 || nchunks < 1 || audit) return fail(BIN_ERR_ARG, "adam_step: empty table");
+    adam_scalars_kernel<<<1, 1, 0, s>>>(sc);
+    BIN_CUDA_OK(cudaGetLastError());
+    adam_step_kernel<kAdamDevice><<<nchunks, 256, 0, s>>>(table, chunk_prefix, ntensors, 0.f, beta1, beta2, eps,
+                                                          weight_decay, 0.f, grad_scale, nullptr, sc);
+    BIN_CUDA_OK(cudaGetLastError());
+    return BIN_OK;
+  }
   if (ntensors < 1 || nchunks < 1 || !(bias_correction1 > 0.f) || !(bias_correction2 > 0.f))
     return fail(BIN_ERR_ARG, "adam_step: empty table or non-positive bias correction");
   const float lr_bc1 = lr / bias_correction1, inv_sqrt_bc2 = 1.f / sqrtf(bias_correction2);
   if (audit)
-    adam_step_kernel<true><<<nchunks, 256, 0, s>>>(table, chunk_prefix, ntensors, lr_bc1, beta1, beta2, eps, weight_decay,
-                                                   inv_sqrt_bc2, grad_scale, audit);
+    adam_step_kernel<kAdamGuarded><<<nchunks, 256, 0, s>>>(table, chunk_prefix, ntensors, lr_bc1, beta1, beta2, eps,
+                                                           weight_decay, inv_sqrt_bc2, grad_scale, audit, nullptr);
   else
-    adam_step_kernel<false><<<nchunks, 256, 0, s>>>(table, chunk_prefix, ntensors, lr_bc1, beta1, beta2, eps,
-                                                    weight_decay, inv_sqrt_bc2, grad_scale, nullptr);
+    adam_step_kernel<kAdamPlain><<<nchunks, 256, 0, s>>>(table, chunk_prefix, ntensors, lr_bc1, beta1, beta2, eps,
+                                                         weight_decay, inv_sqrt_bc2, grad_scale, nullptr, nullptr);
   BIN_CUDA_OK(cudaGetLastError());
   return BIN_OK;
 }

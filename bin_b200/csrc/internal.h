@@ -172,7 +172,8 @@ int launch_pixel_loss_bwd(const float* const* a, const float* const* b, float* c
                           size_t n, int kind, float eps, const float* upstream, cudaStream_t s);
 int launch_adam_step(const bin_adam_tensor_t* table, const int* chunk_prefix, int ntensors, int nchunks, float lr,
                      float beta1, float beta2, float eps, float weight_decay, float bias_correction1,
-                     float bias_correction2, float grad_scale, const bin_grad_audit_t* audit, cudaStream_t s);   // audit: NULL = unguarded
+                     float bias_correction2, float grad_scale, const bin_grad_audit_t* audit, bin_adam_scalars_t* sc,
+                     cudaStream_t s);   // audit: NULL = unguarded; sc: NULL = scalars by value
 size_t grad_audit_scratch_bytes(int nchunks);
 int launch_grad_audit(const bin_adam_tensor_t* table, const int* chunk_prefix, int ntensors, int nchunks, float grad_scale,
                       float max_norm, void* scratch, bin_grad_audit_t* audit, cudaStream_t s);

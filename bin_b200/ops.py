@@ -188,12 +188,14 @@ def flipx4_mean(srcs: Sequence[torch.Tensor]) -> List[torch.Tensor]:
     return _flipx4(srcs, False)
 
 
-def train_batch_u8(samples: Sequence[Tuple[Sequence[torch.Tensor], int, int, int]], h: int, w: int) -> torch.Tensor:
+def train_batch_u8(samples: Sequence[Tuple[Sequence[torch.Tensor], int, int, int]], h: int, w: int,
+                   out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Training batch of data/BIN_dataset.py BINDataset as the DataLoader collates it, built on the device.
 
     samples: (frames, top, left, flip) per item; frames = the 17 contiguous uint8 CUDA (H,W,3) BGR images of the item in
     output order (6 LQs, 6 GTenh, 5 GTinp), all of one shape.  Returns one fp32 (17,B,3,h,w) tensor with
-    out[f,b,c,y,x] = frames_b[f][top+y, left + (w-1-x if flip else x), 2-c] / 255, one launch per 16 items."""
+    out[f,b,c,y,x] = frames_b[f][top+y, left + (w-1-x if flip else x), 2-c] / 255, one launch per 16 items.  `out`: a
+    contiguous fp32 tensor of that shape to write into in place (a CUDA graph's static input), else a new one."""
     B = len(samples)
     if B < 1:
         raise _lib.BinB200Error("train_batch_u8: no samples")
@@ -214,8 +216,13 @@ def train_batch_u8(samples: Sequence[Tuple[Sequence[torch.Tensor], int, int, int
         for f, t in enumerate(frames):
             e.src[f] = t.data_ptr()
         e.H, e.W, e.top, e.left, e.flip = shape[0], shape[1], top, left, int(flip)
+    shape = (_lib.BIN_TRAIN_FRAMES, B, 3, h, w)
+    if out is not None and (tuple(out.shape) != shape or out.dtype != torch.float32 or out.device != dev
+                            or not out.is_contiguous()):
+        raise _lib.BinB200Error(f"train_batch_u8: out must be a contiguous fp32 {shape} tensor on {dev}")
     with torch.cuda.device(dev):
-        out = torch.empty((_lib.BIN_TRAIN_FRAMES, B, 3, h, w), dtype=torch.float32, device=dev)
+        if out is None:
+            out = torch.empty(shape, dtype=torch.float32, device=dev)
         for b0 in range(0, B, _lib.BIN_TRAIN_MAX_BATCH):
             n = min(_lib.BIN_TRAIN_MAX_BATCH, B - b0)
             check(lib().bin_train_batch_u8(C.cast(C.byref(tab, b0 * C.sizeof(_lib.TrainSample)), C.POINTER(_lib.TrainSample)),

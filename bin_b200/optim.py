@@ -11,6 +11,9 @@ parameter group over all tensors (`bin_adam_step`) instead of PyTorch's per-op f
 device (`bin_grad_audit`) finds their global norm and any inf or NaN, and `bin_adam_step_guarded` clips by that norm or
 leaves every tensor untouched, without a host synchronisation.  `StepLedger` keeps the host's step count right.
 
+`Adam(..., capturable=True)` is torch's capturable Adam: the step count and the learning rate live on the device, so
+`step()` can be captured in a CUDA graph with the rest of the training step and replayed (DESIGN §4p).
+
 CUDA fp32 parameters only; there is no CPU path."""
 from __future__ import annotations
 
@@ -26,6 +29,9 @@ from ._lib import BinB200Error, check, lib
 ADAM_CHUNK = 4096                                       # BIN_ADAM_CHUNK, include/bin_b200.h
 AUDIT_DTYPE = np.dtype([("sumsq", "<f8"), ("nonfinite", "<u8"), ("first_bad", "<i4"), ("skip", "<i4"),
                         ("norm", "<f4"), ("coef", "<f4")])                     # bin_grad_audit_t
+SCALARS_DTYPE = np.dtype([("beta1", "<f8"), ("beta2", "<f8"), ("audit", "<u8"), ("skipped", "<u8"), ("lr", "<f4"),
+                          ("step", "<f4"), ("lr_bc1", "<f4"), ("inv_sqrt_bc2", "<f4")])   # bin_adam_scalars_t
+_LR, _STEP = 8, 9                                       # their float32 indices in the block
 LOSS_SCALE_MAX = 2048.0                                 # autograd.LOSS_SCALE_TARGET
 BACKOFF_GROWTH_INTERVAL = 1000                          # applied steps in a row that double the loss-scale target
 _log = logging.getLogger(__name__)
@@ -144,17 +150,33 @@ class Adam(torch.optim.Optimizer):
 
     `loss_scale_backoff` (needs `skip_nonfinite`) also halves `autograd.loss_scale_target()` after each skipped step
     and doubles it after 1000 applied steps in a row, within [1, 2048].  The target is process-wide, and what moving
-    it does to convergence has not been measured."""
+    it does to convergence has not been measured.
+
+    `capturable=True` (torch's `capturable`): each parameter group keeps its step count and learning rate in a device
+    block (bin_adam_scalars_t) that the launch reads, and `state[p]["step"]` is a view of that count on the device.
+    `step()` then never synchronises and launches the same kernels every time, so it can be captured in a CUDA graph.
+    It gives the bits of the default optimizer.  The first step of a group must run eagerly (it builds the group's
+    tables); every parameter of a group needs a dense fp32 gradient and all share one step count.  Replay a graph that
+    captured `step()` with `opt.replay(graph)`, not `graph.replay()`: it first copies each group's current `lr` to the
+    device (a stream-ordered copy; a scheduler's change between replays is seen) and afterwards marks the parameters as
+    modified, so that the package's packed-weight caches re-pack them.  betas, eps and weight_decay are baked into the
+    graph.  With the guard, the skip, the clip and the count of skipped steps stay on the device; `resolve()`,
+    `state_dict()` and `load_state_dict()` read them.  `loss_scale_backoff` is refused: the loss-scale target it moves is
+    a host value that a replay would not see.  `state_dict()` gives CPU step tensors, as the default optimizer does, so
+    checkpoints of both load into either, and into torch.optim.Adam."""
 
     def __init__(self, params, lr: float = 1e-3, betas: Tuple[float, float] = (0.9, 0.999), eps: float = 1e-8,
                  weight_decay: float = 0.0, max_grad_norm: Optional[float] = None, skip_nonfinite: bool = False,
-                 loss_scale_backoff: bool = False):
+                 loss_scale_backoff: bool = False, capturable: bool = False):
         if lr < 0 or eps < 0 or weight_decay < 0 or not (0 <= betas[0] < 1 and 0 <= betas[1] < 1):
             raise ValueError("invalid Adam hyper-parameters")
         if max_grad_norm is not None and not max_grad_norm > 0:
             raise ValueError("max_grad_norm must be positive (or None)")
         if loss_scale_backoff and not skip_nonfinite:
             raise ValueError("loss_scale_backoff needs skip_nonfinite=True")
+        if loss_scale_backoff and capturable:
+            raise ValueError("loss_scale_backoff cannot be combined with capturable=True: the loss-scale target is a host "
+                             "value, which a CUDA-graph replay does not see")
         super().__init__(params, dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay))
         self._tables: Dict[object, _Table] = {}           # (group, k), and "audit"
         self.max_grad_norm = None if max_grad_norm is None else float(max_grad_norm)
@@ -166,6 +188,12 @@ class Adam(torch.optim.Optimizer):
             scale = (autograd.loss_scale_target, autograd.set_loss_scale_target)
         self._ledger = StepLedger(scale)
         self._audit_bufs = None                        # (device record, pinned host record, event) of the guard
+        self.capturable = bool(capturable)
+        self._skip_base = 0                            # capturable: skipped steps counted before the current tables
+        self._seen_skipped = 0
+        self._launched = False
+        self._audit_params: List[torch.Tensor] = []
+        self._audit_scale = 1.0
 
     @property
     def skipped_steps(self) -> int:
@@ -177,20 +205,25 @@ class Adam(torch.optim.Optimizer):
         return None if self._ledger.last is None else self._ledger.last.norm
 
     def resolve(self) -> Optional[GradAudit]:
-        """Wait for the guarded step in flight and return its record (the last resolved one when none is in flight)."""
+        """Wait for the guarded step in flight and return its record (the last resolved one when none is in flight).
+        capturable: read the device's record of the last step and its count of skipped steps (a synchronisation)."""
+        if self.capturable:
+            return self._resolve_device()
         return self._ledger.resolve()
 
     def state_dict(self):
         self.resolve()                                 # a saved `step` is exact
         sd = super().state_dict()
         # a `step` tensor of its own per parameter: torch.optim.Adam, stepping from this dict, adds 1 to each entry
-        sd["state"] = {k: {**st, "step": st["step"].clone()} for k, st in sd["state"].items()}
+        # (capturable: a CPU copy of the group's device count, as the default optimizer saves it)
+        sd["state"] = {k: {**st, "step": st["step"].detach().to("cpu", copy=True)} for k, st in sd["state"].items()}
         return sd
 
     def load_state_dict(self, state_dict):
         self.resolve()
         super().load_state_dict(state_dict)
         self._tables.clear()                           # exp_avg / exp_avg_sq / step tensors were replaced
+        self._skip_base, self._seen_skipped = self._ledger.skipped_steps, 0
 
     def add_param_group(self, param_group):
         if hasattr(self, "_tables"):
@@ -198,6 +231,7 @@ class Adam(torch.optim.Optimizer):
         super().add_param_group(param_group)
         if hasattr(self, "_tables"):
             self._tables.clear()
+            self._skip_base, self._seen_skipped = self._ledger.skipped_steps, 0
 
     def _launch(self, tab: _Table, group, step: float, grad_scale: float, audit: Optional[int]) -> None:
         beta1, beta2 = group["betas"]
@@ -205,7 +239,7 @@ class Adam(torch.optim.Optimizer):
                 group["eps"], group["weight_decay"], 1.0 - beta1 ** step, 1.0 - beta2 ** step, grad_scale)
         with torch.cuda.device(tab.dev.device):
             if audit is None:
-                check(lib().bin_adam_step(*args, _stream()))
+                check(lib().bin_adam_step(*args, None, _stream()))
             else:
                 check(lib().bin_adam_step_guarded(*args, audit, _stream()))
         # The kernel writes the parameters through raw device pointers, which autograd's version counter does not see.
@@ -260,6 +294,9 @@ class Adam(torch.optim.Optimizer):
         if closure is not None:
             with torch.enable_grad():
                 loss = closure()
+        if self.capturable:
+            self._step_capturable(grad_scale)
+            return loss
         self.resolve()                                 # the bias corrections below need the number of APPLIED steps
         launches = []                                  # (table, gradients, group, step), launched after the loop
         advanced: List[torch.Tensor] = []              # the step counters this call advances ...
@@ -338,3 +375,164 @@ class Adam(torch.optim.Optimizer):
                     tab.step_value -= 1
             self._ledger.submit(fetch, undo)
         return loss
+
+    # ------------------------------------------------------------------ capturable=True
+    @property
+    def _guarded(self) -> bool:
+        return self.skip_nonfinite or self.max_grad_norm is not None
+
+    def _group_tables(self) -> List[_Table]:
+        return [t for k, t in self._tables.items() if k != "audit"]
+
+    def _capturable_table(self, group) -> _Table:
+        """The table and device scalar block of one parameter group (eager only: it uploads and initialises state)."""
+        params = group["params"]
+        for p in params:
+            if not (p.is_cuda and p.dtype == torch.float32 and p.is_contiguous()):
+                raise BinB200Error("bin_b200.optim.Adam: contiguous fp32 CUDA parameters only (no CPU path)")
+            if p.grad is None or p.grad.is_sparse or p.grad.dtype != torch.float32 or not p.grad.is_contiguous():
+                raise BinB200Error("bin_b200.optim.Adam(capturable=True): every parameter of a group needs a dense, "
+                                   "contiguous fp32 gradient")
+            st = self.state[p]
+            if len(st) == 0:
+                st["step"] = torch.tensor(0.0, dtype=torch.float32)
+                st["exp_avg"] = torch.zeros_like(p, memory_format=torch.preserve_format)
+                st["exp_avg_sq"] = torch.zeros_like(p, memory_format=torch.preserve_format)
+        steps = {float(self.state[p]["step"]) for p in params}
+        if len(steps) != 1:
+            raise BinB200Error("bin_b200.optim.Adam(capturable=True): the parameters of a group must share one step "
+                               f"count; found {sorted(steps)}")
+        dev = params[0].device
+        tab = _Table(params, [self.state[p]["exp_avg"] for p in params], [self.state[p]["exp_avg_sq"] for p in params])
+        with torch.cuda.device(dev):
+            if self._audit_bufs is None or self._audit_bufs[0].device != dev:
+                # the guard's record; unguarded, a record that never skips and clips by 1
+                rec = np.zeros(1, dtype=AUDIT_DTYPE)
+                rec["coef"] = 1.0
+                self._audit_bufs = (torch.from_numpy(rec.view(np.uint8).copy()).to(dev), None, None)
+            blk = np.zeros(1, dtype=SCALARS_DTYPE)
+            blk["beta1"], blk["beta2"] = group["betas"]
+            blk["audit"] = self._audit_bufs[0].data_ptr()
+            blk["lr"], blk["step"] = float(group["lr"]), steps.pop()
+            tab.sc = torch.from_numpy(blk.view(np.float32).copy()).to(dev)
+            tab.upload([p.grad for p in params])
+        tab.lr_value = float(group["lr"])
+        tab.gkey = tuple(p.grad.data_ptr() for p in params)
+        tab.ids = [id(p) for p in params]
+        for p in params:
+            self.state[p]["step"] = tab.sc[_STEP]
+        return tab
+
+    def _static_upload(self, tab: _Table, grads: List[torch.Tensor], capturing: bool) -> None:
+        """Upload the gradient column when the gradient tensors changed.  A captured step must find the gradients its
+        table holds: zero them with zero_grad(set_to_none=False) so that backward accumulates into the same tensors."""
+        key = tuple(g.data_ptr() for g in grads)
+        if key == tab.gkey:
+            return
+        if capturing:
+            raise BinB200Error("bin_b200.optim.Adam(capturable=True): the gradient tensors changed since the last eager "
+                               "step; inside a capture use zero_grad(set_to_none=False) so that they stay the same")
+        tab.upload(grads)
+        tab.gkey = key
+
+    def refresh_lr(self) -> None:
+        """Copy each group's `lr` to its device block where it changed (stream-ordered, no synchronisation).  step() does
+        this itself when it runs eagerly, and replay() before each replay."""
+        if torch.cuda.is_current_stream_capturing():
+            raise BinB200Error("bin_b200.optim.Adam.refresh_lr: not inside a capture (the value would be baked in)")
+        for gi, group in enumerate(self.param_groups):
+            tab = self._tables.get((gi, 0))
+            if tab is not None and tab.lr_value != float(group["lr"]):
+                with torch.cuda.device(tab.sc.device):
+                    tab.sc[_LR].fill_(float(group["lr"]))
+                tab.lr_value = float(group["lr"])
+
+    def replay(self, graph: "torch.cuda.CUDAGraph") -> None:
+        """graph.replay() for a graph that captured step(): each group's current lr goes to the device first, and the
+        parameters' versions are bumped afterwards, as an eager step bumps them, so that every packed-weight cache of
+        the package (forward and backward packs, the inference window's graph) sees the update."""
+        self.refresh_lr()
+        graph.replay()
+        for tab in self._group_tables():
+            torch._C._increment_version(tab.params)
+
+    def _step_capturable(self, grad_scale: float) -> None:
+        capturing = torch.cuda.is_current_stream_capturing()
+        launches = []
+        for gi, group in enumerate(self.param_groups):
+            params = group["params"]
+            if not params:
+                continue
+            tab = self._tables.get((gi, 0))
+            if tab is None or tab.ids != [id(p) for p in params] or tab.pkey != tuple(p.data_ptr() for p in params):
+                if capturing:
+                    raise BinB200Error("bin_b200.optim.Adam(capturable=True): run the first step of a parameter group "
+                                       "(or the first after its parameters changed) eagerly, before a capture")
+                tab = self._tables[(gi, 0)] = self._capturable_table(group)
+            grads = [p.grad for p in params]
+            if any(g is None for g in grads):
+                raise BinB200Error("bin_b200.optim.Adam(capturable=True): every parameter of a group needs a gradient")
+            with torch.cuda.device(tab.dev.device):
+                self._static_upload(tab, grads, capturing)
+            launches.append((tab, grads, group))
+        if not launches:
+            return
+        if not capturing:
+            self.refresh_lr()
+        if self._guarded:
+            self._audit_capturable(launches, grad_scale, capturing)
+        for tab, _, group in launches:
+            beta1, beta2 = group["betas"]
+            with torch.cuda.device(tab.dev.device):
+                check(lib().bin_adam_step(tab.dev.data_ptr(), tab.prefix.data_ptr(), tab.n, tab.nchunks, 0.0, beta1, beta2,
+                                          group["eps"], group["weight_decay"], 1.0, 1.0, grad_scale, tab.sc.data_ptr(),
+                                          _stream()))
+            torch._C._increment_version(tab.params)      # as _launch: the packed-weight caches must see the step
+        self._launched = True
+
+    def _audit_capturable(self, launches, grad_scale: float, capturing: bool) -> None:
+        if len(launches) == 1:
+            tab = launches[0][0]
+        else:
+            ps = [p for t, _, _ in launches for p in t.params]
+            tab = self._tables.get("audit")
+            if tab is None or tab.pkey != tuple(p.data_ptr() for p in ps):
+                if capturing:
+                    raise BinB200Error("bin_b200.optim.Adam(capturable=True): run the first guarded step eagerly")
+                tab = self._tables["audit"] = _Table(ps, [self.state[p]["exp_avg"] for p in ps],
+                                                     [self.state[p]["exp_avg_sq"] for p in ps])
+                tab.gkey = None
+            with torch.cuda.device(tab.dev.device):
+                self._static_upload(tab, [g for _, gs, _ in launches for g in gs], capturing)
+        dev = tab.dev.device
+        if any(t.dev.device != dev for t, _, _ in launches):
+            raise BinB200Error("bin_b200.optim.Adam: the gradient audit needs every parameter on one device")
+        rec_dev = self._audit_bufs[0]
+        with torch.cuda.device(dev):
+            scratch = torch.empty(lib().bin_grad_audit_scratch_bytes(tab.nchunks), dtype=torch.uint8, device=dev)
+            check(lib().bin_grad_audit(tab.dev.data_ptr(), tab.prefix.data_ptr(), tab.n, tab.nchunks, grad_scale,
+                                       math.inf if self.max_grad_norm is None else self.max_grad_norm,
+                                       scratch.data_ptr(), scratch.numel(), rec_dev.data_ptr(), _stream()))
+        self._audit_params = tab.params
+        self._audit_scale = grad_scale
+
+    def _resolve_device(self) -> Optional[GradAudit]:
+        tabs = self._group_tables()
+        if not (self._guarded and self._launched and tabs and self._audit_bufs is not None):
+            return self._ledger.last
+        rec_dev = self._audit_bufs[0]
+        with torch.cuda.device(rec_dev.device):
+            raw = torch.cat([rec_dev, tabs[0].sc.view(torch.uint8)]).cpu().numpy()
+        r = raw[:AUDIT_DTYPE.itemsize].view(AUDIT_DTYPE)[0]
+        skipped = int(raw[AUDIT_DTYPE.itemsize:].view(SCALARS_DTYPE)[0]["skipped"])
+        rec = GradAudit(float(r["sumsq"]), int(r["nonfinite"]), int(r["first_bad"]), bool(r["skip"]),
+                        abs(self._audit_scale) * math.sqrt(float(r["sumsq"])), float(r["coef"]))
+        self.last_nonfinite_param = self._audit_params[rec.first_bad] if rec.skip else None
+        if skipped > self._seen_skipped:
+            _log.warning("bin_b200.optim.Adam: %d step(s) skipped since the last check for non-finite gradients; the "
+                         "last step's first tensor affected is %s", skipped - self._seen_skipped,
+                         "none" if self.last_nonfinite_param is None else tuple(self.last_nonfinite_param.shape))
+        self._seen_skipped = skipped
+        self._ledger.skipped_steps = self._skip_base + skipped
+        self._ledger.last = rec
+        return rec

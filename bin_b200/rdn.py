@@ -207,12 +207,19 @@ class _Backbone(nn.Module):
         """Packed weights of one kind, cached per device and parameter version: "f16" and "x3" feed the forward in
         BIN_PREC_F16 and BIN_PREC_F32X3, "t" (transposed, tap-flipped) the backward's data gradients.  Each kind is its
         own __dict__ slot, assigned whole: replicate() gives an nn.DataParallel replica a shallow copy of the master's
-        __dict__, so a replica packing its own weights (in its own worker thread) never writes into the master's cache."""
+        __dict__, so a replica packing its own weights (in its own worker thread) never writes into the master's cache.
+
+        While the current stream is capturing a CUDA graph the cache is neither read nor written: the pack launch is
+        captured, into a blob of the graph's own pool, so that every replay packs the weights as they are then.  A replay
+        runs no host code, so a cached blob, keyed on versions the host bumps, would hold the weights of before the
+        replayed optimizer step (DESIGN §4p).  The inference window's own graph is the exception: it is keyed on the
+        weight versions and captured again when they change, so the blobs its warm-up cached serve it."""
         ps = self._conv_params()
         key = (kind, ps[0].device.index) + tuple((p.data_ptr(), p._version) for p in ps)
         slot = "_pack_" + kind
+        capturing = torch.cuda.is_current_stream_capturing() and not _capture_keyed_on_versions
         cached = self.__dict__.get(slot)
-        if cached is not None and cached[0] == key:
+        if cached is not None and cached[0] == key and not capturing:
             return cached[1]
         dev = ps[0].device
         if dev.type != "cuda":
@@ -233,7 +240,10 @@ class _Backbone(nn.Module):
             else:
                 blob = torch.empty(L.bin_backbone_packed_bytes(n), dtype=torch.uint8, device=dev)
                 check(L.bin_backbone_pack(n, wp, bp, blob.data_ptr(), ops._stream()))
-        self.__dict__[slot] = (key, blob)
+        if capturing:
+            _CAPTURED_PACKS.append(blob)        # a temporary freed now could be re-allocated before its reader launches
+        else:
+            self.__dict__[slot] = (key, blob)
         return blob
 
     def _forward_frames(self, *frames):
@@ -267,6 +277,8 @@ class RDN_residual_interp_4_1_input(_Backbone):     # RDN.py:282-334
 
 
 _WS = {}
+_capture_keyed_on_versions = False      # set while _forward_graphed captures (see _Backbone._cached_pack)
+_CAPTURED_PACKS: List[torch.Tensor] = []  # weight blobs packed during the capture in progress, until take_workspace
 PRECISIONS = {"fp16": 0, "fp32": 1}
 
 
@@ -330,6 +342,17 @@ def _workspace(dev: torch.device, nbytes: int) -> torch.Tensor:
         cur = torch.empty(nbytes, dtype=torch.uint8, device=dev)
         _WS[key] = cur
     return cur
+
+
+def take_workspace(dev: torch.device) -> list:
+    """Remove and return the scratch buffer of the current stream on `dev` and the weight blobs packed inside a capture
+    (a list, empty if there are none).  At the end of a CUDA graph capture this hands the graph the memory the capture
+    allocated from the graph's pool: the caller keeps it as long as the graph, and no later capture on the same stream
+    shares it."""
+    ws = _WS.pop(_ws_key(dev), None)
+    out = ([] if ws is None else [ws]) + _CAPTURED_PACKS
+    _CAPTURED_PACKS.clear()
+    return out
 
 
 def release_workspaces() -> None:
@@ -610,9 +633,14 @@ class RDN_residual_interp_5_input_ConvLSTM_L(nn.Module):
                     _WS.pop(_ws_key(dev), None)                     # the side stream's scratch buffer is not needed again
                 torch.cuda.current_stream().wait_stream(side)
                 graph = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(graph):
-                    static_out = _window_fwd(self, static_in, live)
-                    ws = _WS.pop(_ws_key(dev), None)                # owned by this entry (graph-private memory pool)
+                global _capture_keyed_on_versions
+                _capture_keyed_on_versions = True
+                try:
+                    with torch.cuda.graph(graph):
+                        static_out = _window_fwd(self, static_in, live)
+                        ws = _WS.pop(_ws_key(dev), None)            # owned by this entry (graph-private memory pool)
+                finally:
+                    _capture_keyed_on_versions = False
                 ent = {"key": key, "graph": graph, "in": static_in, "out": static_out, "ws": ws}
                 self.__dict__["_graph_entry"] = ent
             else:

@@ -18,8 +18,13 @@ Where it departs from the reference: validation crops come from a `random.Random
 validation, where the reference's validation would draw from the global `random` the training crops draw from.  Every
 validation then scores the same crops, and validating does not change the training batches.
 
+With --cuda_graph (one GPU only) iteration 1 runs eagerly, on a side stream, and the step is then captured once in a
+CUDA graph -- zero_grad, the window, the loss, backward, Adam(capturable=True) and the running loss sums -- and
+replayed for every later iteration, the batch built into the graph's static input in place (DESIGN §4p).  The bits
+are the eager run's.  BIN_B200_GRAPH=0 turns capture off.
+
 python -m bin_b200.train -opt <yml> [--checkpointing recompute] [--max_grad_norm X] [--skip_nonfinite]
-[--deterministic] [--from_sharp] [--arch G0,D]; under torchrun each rank trains on its own GPU."""
+[--deterministic] [--from_sharp] [--arch G0,D] [--cuda_graph]; under torchrun each rank trains on its own GPU."""
 from __future__ import annotations
 
 import argparse
@@ -35,7 +40,7 @@ import numpy as np
 import torch
 
 from . import rdn
-from ._lib import BinB200Error
+from ._lib import BIN_TRAIN_FRAMES, BinB200Error
 from .evaluate import load_weights
 from .loss import pixel_loss
 from .metrics import image_metrics_batch
@@ -320,6 +325,16 @@ def build_dataset(root: str, mode: str, device, lq_size, rng, from_sharp: bool) 
     return DeviceBINDataset.from_tree(root, mode=mode, device=device, lq_size=lq_size, rng=rng)
 
 
+def graph_mode(requested: bool, world: int) -> bool:
+    """Whether a run captures its training step: asked for, and not turned off by BIN_B200_GRAPH=0 (as inference's
+    window graph is).  Refused with more than one rank: the step of a DistributedDataParallel run all-reduces through
+    NCCL, which this driver does not capture."""
+    if requested and world > 1:
+        raise BinB200Error(f"--cuda_graph trains on one GPU; this run has {world} ranks (DistributedDataParallel's NCCL "
+                           "all-reduce is not captured)")
+    return requested and rdn._graphs_enabled()
+
+
 # ----------------------------------------------------------------------------- the driver
 class Trainer:
     """One rank's training run.  `run()` trains to the end of the yml's epochs (or `max_iters` iterations in all);
@@ -327,18 +342,20 @@ class Trainer:
 
     rank / world default to the initialised process group, else (0, 1); the device is cuda:<LOCAL_RANK> under a
     process group, else the current device.  sync_debug: a torch.cuda.set_sync_debug_mode level under which every
-    iteration after the first (batch, step, running sums) runs, for checking that it never waits on the device."""
+    iteration after the first (batch, step, running sums) runs, for checking that it never waits on the device.
+    cuda_graph: capture the step after the first iteration and replay it (see the module docstring, `graph_mode`)."""
 
     def __init__(self, opts: Options, *, checkpointing: Optional[str] = None, max_grad_norm: Optional[float] = None,
                  skip_nonfinite: bool = False, deterministic: bool = False, from_sharp: bool = False,
                  arch: Optional[Tuple[int, int]] = None, ratio: int = 100, sync_debug: Optional[str] = None,
-                 stdout: bool = True):
+                 stdout: bool = True, cuda_graph: bool = False):
         self.o = opts
         dist = torch.distributed.is_available() and torch.distributed.is_initialized()
         self.rank = torch.distributed.get_rank() if dist else 0
         self.world = torch.distributed.get_world_size() if dist else 1
         self.dev = torch.device("cuda", int(os.environ.get("LOCAL_RANK", "0")) if dist else torch.cuda.current_device())
         self.sync_debug = sync_debug
+        self.cuda_graph = graph_mode(cuda_graph, self.world)
         self.log = logging.Logger(f"bin_b200.train.{id(self)}", logging.INFO)
         if self.rank == 0:
             os.makedirs(opts.models_dir, exist_ok=True)
@@ -386,7 +403,9 @@ class Trainer:
             else:
                 self.log.warning(f"Params [{k:s}] will not optimize.")
         self.opt = Adam(params, lr=opts.lr, weight_decay=opts.weight_decay, betas=(opts.beta1, opts.beta2),
-                        max_grad_norm=max_grad_norm, skip_nonfinite=skip_nonfinite)
+                        max_grad_norm=max_grad_norm, skip_nonfinite=skip_nonfinite, capturable=self.cuda_graph)
+        if cuda_graph and not self.cuda_graph:
+            self.log.info("BIN_B200_GRAPH=0: the training step runs eagerly")
         self.guarded = max_grad_norm is not None or skip_nonfinite
         self.scheduler = torch.optim.lr_scheduler.ReduceLROnPlateau(self.opt, "min", factor=opts.factor,
                                                                     patience=opts.patience)
@@ -401,6 +420,10 @@ class Trainer:
         with torch.cuda.device(self.dev):
             self.loss_sums = torch.zeros(NOUT + 1, dtype=torch.float32, device=self.dev)
         self.loss_count = 0
+        # --cuda_graph: the static batch buffer every batch is built into, then the graph and what it owns
+        self._static: Optional[torch.Tensor] = None
+        self._graph: Optional[torch.cuda.CUDAGraph] = None
+        self._graph_keep: tuple = ()
 
     # ------------------------------------------------------------------ checkpoints
     def _resume(self, path: str) -> None:
@@ -442,14 +465,54 @@ class Trainer:
         self.opt.step()
         return loss, losses
 
+    def _iterate(self, batch: Dict) -> None:
+        """One training iteration on `batch`, the running loss sums included: eager, or a replay of the captured step
+        (the first iteration of a --cuda_graph run is its eager warm-up, and the capture follows it)."""
+        if not self.cuda_graph:
+            loss, losses = self.train_step(batch)
+            self.loss_sums += torch.stack(list(losses) + [loss.detach()])
+        elif self._graph is not None:
+            self.opt.replay(self._graph)
+        else:
+            self._warm_up_and_capture(batch)
+
+    def _warm_up_and_capture(self, batch: Dict) -> None:
+        """Run `batch` eagerly on a side stream (a real step, with the eager bits; it also makes the tables, the packed
+        weights and the kernels' shared-memory opt-ins), then capture one step on the static batch buffer.  A capture
+        records without running, so it applies no update.  The gradients stay the warm-up's tensors: zero_grad(
+        set_to_none=False) inside the graph, and backward accumulates into them.  The graph owns the scratch workspaces
+        the side stream and the capture allocated."""
+        side = torch.cuda.Stream(self.dev)
+        side.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(side):
+            loss, losses = self.train_step(batch)
+            self.loss_sums += torch.stack(list(losses) + [loss.detach()])
+            rdn.take_workspace(self.dev)
+        torch.cuda.current_stream().wait_stream(side)
+        graph, capture = torch.cuda.CUDAGraph(), torch.cuda.Stream(self.dev)
+        with torch.cuda.graph(graph, stream=capture):
+            self.opt.zero_grad(set_to_none=False)
+            outs = self.model(*[batch["LQs"][:, k] for k in range(6)])
+            loss, losses = pixel_loss(outs, gt_list(batch), self.o.pixel_criterion, nframes=6, version=self.o.version)
+            (self.o.pixel_weight * loss).backward()
+            self.opt.step()
+            self.loss_sums += torch.stack(list(losses) + [loss.detach()])
+            ws = rdn.take_workspace(self.dev)
+        del outs, loss, losses
+        self._graph, self._graph_keep = graph, (ws, capture)
+
     def _batches(self) -> Iterator[Dict]:
-        """The batches of the epoch the next iteration is in, from the next one on."""
+        """The batches of the epoch the next iteration is in, from the next one on (with --cuda_graph, each built into
+        the one static batch buffer the captured step reads)."""
         epoch, done = divmod(self.step, self.iters_per_epoch)
         self.sampler.set_epoch(epoch)
         it = iter(self.sampler)
         for _ in range(done * self.B):
             next(it)
-        return self.train_set.batches(it, self.B)
+        if self.cuda_graph and self._static is None:
+            h, w = self.train_set.h, self.train_set.w
+            self._static = torch.empty((BIN_TRAIN_FRAMES, self.B, 3, h, w), dtype=torch.float32, device=self.dev)
+        return self.train_set.batches(it, self.B, self._static)
 
     def run(self, max_iters: Optional[int] = None) -> None:
         """Train to the end of the last epoch, or until `max_iters` iterations in all have run."""
@@ -466,8 +529,7 @@ class Trainer:
                     if self.sync_debug is not None and not first:
                         torch.cuda.set_sync_debug_mode(self.sync_debug)
                     try:
-                        loss, losses = self.train_step(next(batches))
-                        self.loss_sums += torch.stack(list(losses) + [loss.detach()])
+                        self._iterate(next(batches))
                     finally:
                         torch.cuda.set_sync_debug_mode(mode)
                     first = False
@@ -560,10 +622,14 @@ def main(argv=None) -> None:
                     help="synthesise the blurry frames from <root>/<mode>/<folder> (DeviceClip.from_sharp)")
     ap.add_argument("--arch", type=_arch, default=None, help="backbone G0,D of a light window, e.g. 64,6")
     ap.add_argument("--ratio", type=int, default=100, help="DistIterSampler's epoch enlargement under torchrun")
+    ap.add_argument("--cuda_graph", action="store_true",
+                    help="capture the training step in a CUDA graph after the first iteration and replay it (one GPU)")
     args = ap.parse_args(argv)
+    world = int(os.environ.get("WORLD_SIZE", "1"))
+    graph_mode(args.cuda_graph, world)
     opts = load_options(args.opt)
 
-    distributed = int(os.environ.get("WORLD_SIZE", "1")) > 1
+    distributed = world > 1
     local = int(os.environ.get("LOCAL_RANK", "0"))
     torch.cuda.set_device(local)
     if distributed:
@@ -571,7 +637,7 @@ def main(argv=None) -> None:
     try:
         t = Trainer(opts, checkpointing=args.checkpointing, max_grad_norm=args.max_grad_norm,
                     skip_nonfinite=args.skip_nonfinite, deterministic=args.deterministic, from_sharp=args.from_sharp,
-                    arch=args.arch, ratio=args.ratio)
+                    arch=args.arch, ratio=args.ratio, cuda_graph=args.cuda_graph)
         try:
             t.run()
         finally:

@@ -127,14 +127,15 @@ class DeviceBINDataset:
         for _ in range(count):
             self._draw(0)
 
-    def batch(self, indices: Sequence[int]) -> Dict:
+    def batch(self, indices: Sequence[int], out: Optional[torch.Tensor] = None) -> Dict:
         """default_collate of [ds[i] for i in indices], with the draws made in that order: 'LQs' (B,6,3,h,w), 'GTenh'
         (B,6,3,h,w), 'GTinp' (B,5,3,h,w) fp32 views of one (17,B,3,h,w) buffer, so `LQs[:, k]` is a contiguous
-        (B,3,h,w) batch; 'key' a list of B strings."""
+        (B,3,h,w) batch; 'key' a list of B strings.  `out`: that buffer, written in place (the static input of a
+        captured training step), else a new one."""
         if len(indices) < 1:
             raise BinB200Error("DeviceBINDataset.batch: no indices")
         drawn = [self._draw(i) for i in indices]
-        buf = ops.train_batch_u8([s for s, _ in drawn], self.h, self.w)
+        buf = ops.train_batch_u8([s for s, _ in drawn], self.h, self.w, out)
         return {"LQs": buf[0:N_LQ].transpose(0, 1), "GTenh": buf[N_LQ:N_LQ + N_ENH].transpose(0, 1),
                 "GTinp": buf[N_LQ + N_ENH:].transpose(0, 1), "key": [k for _, k in drawn]}
 
@@ -143,16 +144,16 @@ class DeviceBINDataset:
         b = self.batch([i])
         return {"LQs": b["LQs"][0], "GTenh": b["GTenh"][0], "GTinp": b["GTinp"][0], "key": b["key"][0]}
 
-    def batches(self, sampler: Iterable[int], batch_size: int) -> Iterator[Dict]:
+    def batches(self, sampler: Iterable[int], batch_size: int, out: Optional[torch.Tensor] = None) -> Iterator[Dict]:
         """DataLoader(batch_size, sampler, drop_last=True) over any iterable of indices (e.g. the reference's
-        DistIterSampler)."""
+        DistIterSampler); `out` as for batch()."""
         if batch_size < 1:
             raise BinB200Error("DeviceBINDataset.batches: batch_size must be >= 1")
         chunk = []
         for i in sampler:
             chunk.append(i)
             if len(chunk) == batch_size:
-                yield self.batch(chunk)
+                yield self.batch(chunk, out)
                 chunk = []
 
     @classmethod

@@ -314,7 +314,8 @@ int bin_u8_to_frame(const uint8_t* img, int h, int w, int pad_l, int pad_r, int 
  * chunk_prefix[t] = number of BIN_ADAM_CHUNK-element blocks before tensor t, chunk_prefix[ntensors] = nchunks.
  * Semantics of torch.optim.Adam(amsgrad=False, maximize=False): g' = grad_scale*g + weight_decay*p;
  * m += (g'-m)(1-beta1); v = beta2 v + (1-beta2) g'^2; p -= lr/bias_correction1 * m / (sqrt(v)/sqrt(bias_correction2) + eps)
- * with bias_correction_i = 1 - beta_i^step computed by the caller (as torch does, on the host). */
+ * with bias_correction_i = 1 - beta_i^step computed by the caller (as torch does, on the host), or on the device from
+ * a bin_adam_scalars_t block, below. */
 #define BIN_ADAM_CHUNK 4096
 typedef struct {
   float* p;                 /* parameter (updated in place)        */
@@ -323,9 +324,6 @@ typedef struct {
   float* v;                 /* exp_avg_sq                          */
   unsigned long long n;     /* elements                            */
 } bin_adam_tensor_t;
-int bin_adam_step(const bin_adam_tensor_t* table_dev, const int* chunk_prefix_dev, int ntensors, int nchunks, float lr,
-                  float beta1, float beta2, float eps, float weight_decay, float bias_correction1,
-                  float bias_correction2, float grad_scale, bin_stream_t s);
 
 /* ---- guarded optimizer step: a device-side audit of all gradients, then an Adam step that obeys it --------------- */
 /* bin_grad_audit makes one pass over the g column of an Adam table (two launches: one block per chunk, then one block)
@@ -339,6 +337,27 @@ typedef struct {
   float norm;                   /* |grad_scale| * sqrt(sumsq): the global L2 norm of the gradients Adam would see    */
   float coef;                   /* min(1, max_norm / (norm + 1e-6)) as torch's clip_grad_norm_; 1 if max_norm is inf  */
 } bin_grad_audit_t;
+/* The per-step scalars of a step that a CUDA graph replays (bin_b200.optim.Adam(capturable=True), DESIGN §4p): one
+ * 8-byte aligned block per parameter group in device memory.  The caller writes beta1, beta2, audit, skipped and step
+ * once and lr whenever it changes; the launch reads them on the device, so a replay takes the current learning rate and
+ * the next step count.  A one-thread prologue of the launch forms lr_bc1 = lr / float(1 - beta1^(step+1)) and
+ * inv_sqrt_bc2 = 1 / sqrt(float(1 - beta2^(step+1))), the fp64 powers rounded to fp32 as the caller's by-value
+ * arguments are, and stores step + 1 -- unless `audit` says skip: then step stays, skipped grows by one and p, m and v
+ * keep their bits.  An applied step scales the gradients by grad_scale * coef. */
+typedef struct {
+  double beta1, beta2;             /* the betas in fp64, as the host's bias corrections use them                      */
+  const bin_grad_audit_t* audit;   /* the record (of bin_grad_audit) this step obeys; unguarded: skip 0, coef 1      */
+  unsigned long long skipped;      /* steps the audit skipped                                                         */
+  float lr;                        /* learning rate                                                                    */
+  float step;                      /* steps applied so far (torch's state['step'])                                     */
+  float lr_bc1, inv_sqrt_bc2;      /* written by the launch                                                            */
+} bin_adam_scalars_t;
+/* bin_adam_step: one launch over every tensor of the table.  scalars_dev NULL: lr and the bias corrections are taken
+ * by value (bias_correction_i > 0), as torch forms them on the host.  Otherwise those three arguments are ignored and
+ * the step reads bin_adam_scalars_t on the device (8-byte aligned); the launch is then two kernels. */
+int bin_adam_step(const bin_adam_tensor_t* table_dev, const int* chunk_prefix_dev, int ntensors, int nchunks, float lr,
+                  float beta1, float beta2, float eps, float weight_decay, float bias_correction1,
+                  float bias_correction2, float grad_scale, bin_adam_scalars_t* scalars_dev, bin_stream_t s);
 /* Bytes of per-chunk partial sums (device, 16-byte aligned); 0 if nchunks < 1. */
 size_t bin_grad_audit_scratch_bytes(int nchunks);
 /* table / chunk_prefix as bin_adam_step takes them; one table may span every parameter group, so that one record

@@ -36,7 +36,8 @@ tab = ours._tables[(0, 0)]
 from bin_b200._lib import check, lib           # noqa: E402
 st = torch.cuda.current_stream().cuda_stream
 res["ours_kernel_ms"] = timed(lambda: check(lib().bin_adam_step(tab.dev.data_ptr(), tab.prefix.data_ptr(), tab.n, tab.nchunks,
-                                                                1e-4, 0.9, 0.99, 1e-8, 0.0, 0.1, 0.01, 1.0, st)), iters=50)
+                                                                1e-4, 0.9, 0.99, 1e-8, 0.0, 0.1, 0.01, 1.0, None, st)),
+                                      iters=50)
 res["torch_fused_ms"] = timed(torch.optim.Adam(ps, lr=1e-4, betas=(0.9, 0.99), fused=True).step)
 res["torch_foreach_ms"] = timed(torch.optim.Adam(ps, lr=1e-4, betas=(0.9, 0.99), foreach=True).step)
 res["ours_GBps_algorithmic"] = n * 28 / res["ours_kernel_ms"] / 1e6          # 16 B read + 12 B written per parameter

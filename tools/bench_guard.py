@@ -56,7 +56,7 @@ adam_args = (tab.dev.data_ptr(), tab.prefix.data_ptr(), tab.n, tab.nchunks, 1e-4
 
 
 def plain():
-    check(lib().bin_adam_step(*adam_args, st))
+    check(lib().bin_adam_step(*adam_args, None, st))
 
 
 def audit():
