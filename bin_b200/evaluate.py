@@ -187,22 +187,26 @@ def _write_log(path: str, messages: Sequence[str]) -> None:
 # ----------------------------------------------------------------------------- decoding
 class _Prefetch:
     """cv2.imread of `paths` in order on `threads` host threads, each image copied into pinned memory, at most `depth`
-    ahead of the consumer."""
+    ahead of the consumer.  `read(path)` -> numpy image replaces cv2.imread when given."""
 
-    def __init__(self, paths: Sequence[str], threads: int, depth: int, who: str):
+    def __init__(self, paths: Sequence[str], threads: int, depth: int, who: str, read=None):
         self._paths = iter(paths)
         self._who = who
+        self._decode = read or self._imread
         self._pool = cf.ThreadPoolExecutor(max(threads, 1), thread_name_prefix="bin_b200-decode")
         self._q: collections.deque = collections.deque()
         for _ in range(max(depth, 1)):
             self._submit()
 
-    def _read(self, path: str) -> torch.Tensor:
+    def _imread(self, path: str) -> np.ndarray:
         import cv2
         img = cv2.imread(path)
         if img is None:
             raise BinB200Error(f"{self._who}: cannot read {path}")
-        return torch.from_numpy(img).pin_memory()
+        return img
+
+    def _read(self, path: str) -> torch.Tensor:
+        return torch.from_numpy(self._decode(path)).pin_memory()
 
     def _submit(self):
         p = next(self._paths, None)
