@@ -7,6 +7,12 @@ every ReLU input is at least DELTA away from 0; check_no_relu_near_zero asserts 
 runs.  oracle_grads is fp64 autograd through arch_oracle.backbone, optionally with the fp16-storage emulation of
 bin_oracle (activations and loss-scaled gradients rounded to fp16 where the CUDA path stores them).
 
+no_flip_window_sd does the same for a whole six-frame window: each of the four canonical backbones is rebuilt on the
+calls the window makes of it, in dataflow order, so that later stages are built on what earlier ones give.
+window_oracle_grads is fp64 autograd through that window, either along the reference's own dataflow or along the
+library's batched schedule (bin_b200.rdn._window_schedule), where the fp16-storage emulation rounds the gradients of all
+the calls of a stage at one scale, as the library does.
+
 check_gradients holds a set of gradients to the bar of the whole-backbone tests: per tensor,
 e <= k_emu * e_emu + 1e-3 * max|ref|, with e the CUDA error against fp64, e_emu the emulating oracle's and k_emu = 4
 for the bias of growth convs 0-2 (whose dY is summed in fp16, in place, over several launches, where the oracle rounds
@@ -114,6 +120,99 @@ def oracle_grads(pool, calls_idx, cots, sd, emulate, device="cuda"):
     grads = torch.autograd.grad(loss, fr + [leaves[k] for k in names], allow_unused=True)
     grads = [torch.zeros_like(t) if g is None else g for g, t in zip(grads, fr + [leaves[k] for k in names])]
     return [o.detach() for o in outs], list(grads[:len(fr)]), dict(zip(names, grads[len(fr):]))
+
+
+CANON = tuple(O.BACKBONE_ALIASES)        # the window's four distinct backbones, model1_1 .. model4_1, in stage order
+
+
+def _window_run(F, stage, lstm):
+    """The window's 17 backbone calls and 6 ConvLSTM cells on the six frames F, in the library's schedule: the 5 frame
+    pairs as stage 1, then bin_b200.rdn._window_schedule.  stage(name, calls) runs the calls of the backbone `name`
+    (one of CANON) and returns their outputs; lstm(group) runs the cells (k, x) of a hand-off and returns their h."""
+    from types import SimpleNamespace
+
+    from bin_b200 import rdn
+    s1 = stage("model1_1", [(F[a], F[a + 1]) for a in range(5)])
+    return list(rdn._window_schedule(stage, lstm, SimpleNamespace(**{m: m for m in CANON}), F, s1))
+
+
+def no_flip_window_sd(seed, g0, d, frames):
+    """A window state_dict (net.model = RDN_residual_interp_5_input(lstm=True, GO=g0, D=d)) whose every backbone has no
+    ReLU input near 0 on the calls the window makes of it: the ConvLSTM gates of A.synth_state_dict(seed, g0, d), and
+    each canonical backbone rebuilt by no_flip_sd on its calls (duplicates removed: the 5 / 6 / 4 / 2 calls of the
+    library's schedule), in dataflow order and fp64, each stage's inputs computed with the fp32 weights of the stages
+    before it.  Aliases (O.BACKBONE_ALIASES) share the tensors.  frames: the six frames; fp32 weights on the CPU."""
+    dev = frames[0].device
+    sd = {k: v for k, v in A.synth_state_dict(seed, g0, d).items() if not k.startswith("model.")}
+    cells = {k: v.to(dev, torch.float64) for k, v in sd.items()}
+    built = {}
+
+    def stage(name, calls):
+        calls = [[f.to(dev, torch.float64) for f in c] for c in calls]
+        bsd = no_flip_sd(O.BACKBONE_NFRAMES[name], seed * 1000 + 100 + CANON.index(name), calls, g0, d)
+        check_no_relu_near_zero(calls, bsd)
+        built[name] = bsd
+        bsd = {k: v.double() for k, v in bsd.items()}
+        return [A.backbone(c, bsd) for c in calls]
+
+    _window_run([f.to(dev, torch.float64) for f in frames], stage,
+                lambda group: [O.convlstm(x, cells, O.LSTM_NAMES[k])[0] for k, x in group])
+    for canon, aliases in O.BACKBONE_ALIASES.items():
+        bsd = {k: v.cpu() for k, v in built[canon].items()}
+        for a in aliases:
+            sd.update({f"model.{a}.{k}": v for k, v in bsd.items()})
+    return sd
+
+
+@contextlib.contextmanager
+def _no_fp16_emulation():
+    prev = O._EMULATE_FP16, O._EMULATE_FP16_GRADS
+    O._EMULATE_FP16 = O._EMULATE_FP16_GRADS = False
+    try:
+        yield
+    finally:
+        O._EMULATE_FP16, O._EMULATE_FP16_GRADS = prev
+
+
+def window_oracle_grads(frames, cots, sd, emulate, device="cuda", batched=None, wrap=None):
+    """fp64 autograd through the six-frame window on `device` (optionally with the fp16-storage emulation of activations
+    and gradients): (the 14 outputs, the 6 frame gradients, {parameter name: gradient}), one gradient for each distinct
+    tensor of sd under its first name, the names of net.named_parameters(): aliases share one leaf.
+
+    cots: the 14 cotangents (None leaves an output out of the loss), or a function of the 14 outputs that returns the
+    loss.  batched (default: emulate) chooses the dataflow.  False: A.window_forward, the reference's own 20 backbone
+    calls, independent of the code under test.  True: the library's schedule (_window_run), each stage's calls
+    concatenated along the batch and run as one A.backbone, so that the emulation's _round_grad_fp16 sees one tensor per
+    stage and rounds every call at the loudest call's scale, as bin_grad_scale does; the ConvLSTM cells run without fp16
+    rounding of their weights, like the library's fp32 cell.  wrap(stage, lstm, F) -> (stage, lstm) replaces the batched
+    schedule's stage and cell functions, F being the six frame leaves (a test injects window-glue faults with it)."""
+    batched = emulate if batched is None else batched
+    uniq, full = {}, {}
+    for k, v in sd.items():
+        if v.data_ptr() not in uniq:
+            uniq[v.data_ptr()] = (k, v.to(device, torch.float64).requires_grad_(True))
+        full[k] = uniq[v.data_ptr()][1]
+    fr = [f.to(device, torch.float64).requires_grad_(True) for f in frames]
+
+    def stage(name, calls):
+        B = calls[0][0].shape[0]
+        slots = [torch.cat([c[j] for c in calls]) for j in range(len(calls[0]))]
+        return list(A.backbone(slots, O.sub_sd(full, f"model.{name}")).split(B))
+
+    def lstm(group):
+        with _no_fp16_emulation():
+            return [O.convlstm(x, full, O.LSTM_NAMES[k])[0] for k, x in group]
+
+    if wrap is not None:
+        stage, lstm = wrap(stage, lstm, fr)
+    with O.emulate_fp16_storage(grads=True) if emulate else contextlib.nullcontext():
+        outs = _window_run(fr, stage, lstm) if batched else A.window_forward(fr, full)
+    loss = cots(outs) if callable(cots) else sum((o * c.to(device, torch.float64)).sum()
+                                                 for o, c in zip(outs, cots) if c is not None)
+    names, leaves = zip(*uniq.values())
+    grads = torch.autograd.grad(loss, fr + list(leaves), allow_unused=True)
+    grads = [torch.zeros_like(t) if g is None else g for g, t in zip(grads, fr + list(leaves))]
+    return [o.detach() for o in outs], grads[:len(fr)], dict(zip(names, grads[len(fr):]))
 
 
 def k_emu(key):
