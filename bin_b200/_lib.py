@@ -122,6 +122,12 @@ _SIGS = {
                                         C.c_void_p, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p]),
     "bin_pixel_loss_bwd": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_int,
                                     C.c_size_t, C.c_int, C.c_float, C.c_void_p, C.c_void_p]),
+    "bin_ssim_loss_scratch_bytes": (C.c_size_t, [C.c_int] * 4),
+    "bin_ssim_loss_maps_bytes": (C.c_size_t, [C.c_int] * 4),
+    "bin_ssim_loss_fwd": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)] + [C.c_int] * 4
+                          + [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "bin_ssim_loss_bwd": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_void_p, C.POINTER(C.c_void_p),
+                                    C.POINTER(C.c_void_p)] + [C.c_int] * 4 + [C.c_void_p, C.c_void_p]),
     "bin_tensor2img_u8": (C.c_int, [C.c_void_p] + [C.c_int] * 6 + [C.c_void_p, C.c_void_p]),
     "bin_u8_to_frame": (C.c_int, [C.c_void_p] + [C.c_int] * 6 + [C.c_void_p, C.c_void_p]),
     "bin_rdb_tail_fwd": (C.c_int, [C.POINTER(Act), C.c_int, C.POINTER(Act), C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,

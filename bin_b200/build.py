@@ -10,8 +10,8 @@ import tempfile
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libbin_b200.so")
-SOURCES = ["conv_igemm.cu", "rdb_tail.cu", "aux_kernels.cu", "wgrad.cu", "metrics.cu", "png.cu", "api.cu"]
-HEADERS = ["common.cuh", "wgmma.cuh", "xstack.cuh", "internal.h", os.path.join("..", "..", "include", "bin_b200.h")]
+SOURCES = ["conv_igemm.cu", "rdb_tail.cu", "aux_kernels.cu", "wgrad.cu", "metrics.cu", "ssim_loss.cu", "png.cu", "api.cu"]
+HEADERS = ["common.cuh", "gauss11.cuh", "wgmma.cuh", "xstack.cuh", "internal.h", os.path.join("..", "..", "include", "bin_b200.h")]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = [*ARCH, "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v"]
 

@@ -588,6 +588,19 @@ int bin_pixel_loss_bwd(const float* const* a_host, const float* const* b_host, f
   if (!a_host || !b_host || !da_host || !upstream) return fail(BIN_ERR_ARG, "pixel_loss_bwd: null argument");
   return launch_pixel_loss_bwd(a_host, b_host, da_host, db_host, npairs, n, kind, eps, upstream, (cudaStream_t)s);
 }
+size_t bin_ssim_loss_scratch_bytes(int npairs, int planes, int h, int w) {
+  return ssim_loss_scratch_bytes(npairs, planes, h, w);
+}
+size_t bin_ssim_loss_maps_bytes(int npairs, int planes, int h, int w) { return ssim_loss_maps_bytes(npairs, planes, h, w); }
+int bin_ssim_loss_fwd(const float* const* a_host, const float* const* b_host, int npairs, int planes, int h, int w,
+                      float* ssim_sum, float* maps, int flags, void* scratch, size_t scratch_bytes, bin_stream_t s) {
+  return launch_ssim_loss_fwd(a_host, b_host, npairs, planes, h, w, ssim_sum, maps, flags, scratch, scratch_bytes,
+                              (cudaStream_t)s);
+}
+int bin_ssim_loss_bwd(const float* const* a_host, const float* const* b_host, const float* maps, float* const* da_host,
+                      float* const* db_host, int npairs, int planes, int h, int w, const float* upstream, bin_stream_t s) {
+  return launch_ssim_loss_bwd(a_host, b_host, maps, da_host, db_host, npairs, planes, h, w, upstream, (cudaStream_t)s);
+}
 int bin_tensor2img_u8(const float* x, int Hs, int Ws, int top, int left, int h, int w, uint8_t* out, bin_stream_t s) {
   if (!x || !out) return fail(BIN_ERR_ARG, "tensor2img: null argument");
   return launch_tensor2img_u8(x, Hs, Ws, top, left, h, w, out, (cudaStream_t)s);

@@ -196,6 +196,14 @@ int launch_image_metrics_batch_u8(const char* who, const uint8_t* const* a_host,
                                   int w, int c, int flags, double* out, void* workspace, size_t workspace_bytes,
                                   cudaStream_t s);
 
+// ------------------------------------------------------------------ ssim_loss.cu
+size_t ssim_loss_scratch_bytes(int npairs, int planes, int h, int w);
+size_t ssim_loss_maps_bytes(int npairs, int planes, int h, int w);
+int launch_ssim_loss_fwd(const float* const* a, const float* const* b, int npairs, int planes, int h, int w, float* sums,
+                         float* maps, int flags, void* scratch, size_t scratch_bytes, cudaStream_t s);
+int launch_ssim_loss_bwd(const float* const* a, const float* const* b, const float* maps, float* const* da,
+                         float* const* db, int npairs, int planes, int h, int w, const float* upstream, cudaStream_t s);
+
 // ------------------------------------------------------------------ png.cu
 size_t png_max_bytes(int h, int w);
 size_t png_workspace_bytes(int n, int h, int w);

@@ -10,6 +10,7 @@
 // fixed order, so the result is bit-reproducible and independent of the SM count.
 #include <stdint.h>
 
+#include "gauss11.cuh"
 #include "internal.h"
 
 namespace binb {
@@ -19,11 +20,6 @@ constexpr int kHalo = 5;                  // Gaussian radius (the box radius, 3,
 constexpr int kRows = kTile + 2 * kHalo;  // staged rows / columns
 constexpr int kMetThreads = 256;
 constexpr int kRedThreads = 512;
-
-// cv2.getGaussianKernel(11, 1.5) bit for bit (OpenCV's bit-exact kernel differs from exp()/sum in the last bits).
-__constant__ double kGauss11[11] = {0x1.0d956b52a1d6ep-10, 0x1.f1fe01ae5a5b5p-8, 0x1.26eb175d83f66p-5, 0x1.bff0fe8e98418p-4,
-                                    0x1.b43c3f52b19f3p-3,  0x1.106560aa892bfp-2, 0x1.b43c3f52b19f3p-3, 0x1.bff0fe8e98418p-4,
-                                    0x1.26eb175d83f66p-5,  0x1.f1fe01ae5a5b5p-8, 0x1.0d956b52a1d6ep-10};
 
 struct MetricsPartial {
   unsigned long long abs_sum, sq_sum;

@@ -6,6 +6,7 @@ write around bin_model, with every step of the hot path on the GPU:
     sequential with one process, DistIterSampler under torchrun (restated here as `DistIterSampler`);
   * step: bin_model.optimize_parameters (bin_model.py:130-141): zero_grad, the window on LQs[:, 0..5], loss.pixel_loss
     of the 14 outputs against get_info's GT list with the cycle terms, x pixel_weight, backward, optim.Adam.step;
+    pixel_criterion 'cb+ssim' adds train.ssim_weight * (1 - SSIM) to every term (DESIGN §4r);
   * the per-output losses are running sums on the device, read only at print_freq iterations, so an ordinary iteration
     does not synchronise the host with the device;
   * validation every val_freq iterations at batch 1: the 14 losses and their mean, PSNR and SSIM of each output
@@ -42,7 +43,7 @@ import torch
 from . import rdn
 from ._lib import BIN_TRAIN_FRAMES, BinB200Error
 from .evaluate import load_weights
-from .loss import pixel_loss
+from .loss import CB_SSIM, cycle_pairs_for, pixel_loss, pixel_ssim_loss
 from .metrics import image_metrics_batch
 from .optim import Adam
 from .streaming import tensor2img_u8
@@ -88,6 +89,7 @@ class Options:
     print_freq: int
     save_freq: int
     ignored: List[str] = field(default_factory=list)
+    ssim_weight: Optional[float] = None   # train.ssim_weight: read, and required, with pixel_criterion cb+ssim only
 
     @property
     def experiments_root(self) -> str:
@@ -120,7 +122,7 @@ def _path(p) -> Optional[str]:
 def parse_options(opt: dict) -> Options:
     """The honoured keys of a parsed train yml.  Raises BinB200Error naming the key for what this driver does not do:
     another model than bin_stage4, nframes other than 6, another lr_scheme than ReduceLROnPlateau, ft_tsa_only, an
-    unknown pixel_criterion."""
+    unknown pixel_criterion, cb+ssim without train.ssim_weight."""
     if _get(opt, "network_G.which_model_G") != "bin_stage4":
         raise BinB200Error(f"network_G.which_model_G: {_get(opt, 'network_G.which_model_G')!r} is not trained here; "
                            "only bin_stage4 is")
@@ -132,8 +134,10 @@ def parse_options(opt: dict) -> Options:
     if _get(opt, "train.ft_tsa_only", None):
         raise BinB200Error("train.ft_tsa_only is not supported")
     crit = _get(opt, "train.pixel_criterion")
-    if crit not in ("l1", "l2", "cb"):
-        raise BinB200Error(f"train.pixel_criterion: {crit!r} is not one of l1, l2, cb (bin_model.py:54-61)")
+    if crit not in ("l1", "l2", "cb", CB_SSIM):
+        raise BinB200Error(f"train.pixel_criterion: {crit!r} is not one of l1, l2, cb (bin_model.py:54-61) or "
+                           f"{CB_SSIM}")
+    ssim_weight = float(_get(opt, "train.ssim_weight")) if crit == CB_SSIM else None
     val = _get(opt, "datasets.val", None)
     return Options(
         name=str(_get(opt, "name")),
@@ -163,7 +167,8 @@ def parse_options(opt: dict) -> Options:
         manual_seed=int(_get(opt, "train.manual_seed")),
         print_freq=int(float(_get(opt, "logger.print_freq"))),
         save_freq=int(float(_get(opt, "logger.save_checkpoint_freq"))),
-        ignored=[k for k in IGNORED if _get(opt, k, None) is not None])
+        ignored=[k for k in IGNORED if _get(opt, k, None) is not None],
+        ssim_weight=ssim_weight)
 
 
 def load_options(path: str) -> Options:
@@ -246,11 +251,15 @@ def gt_list(batch: Dict) -> List[torch.Tensor]:
 
 
 # ----------------------------------------------------------------------------- logs
-def train_message(epoch: int, step: int, lr: float, avg: Sequence[float], guard: Optional[Tuple[int, float]]) -> str:
+def train_message(epoch: int, step: int, lr: float, avg: Sequence[float], guard: Optional[Tuple[int, float]],
+                  ssim_loss: Optional[float] = None) -> str:
     """avg: the 14 per-output losses and their mean (get_current_log('train')'s '0'..'13', 'Al'), averaged since the
-    last message; guard: (skipped steps, last grad norm) when the step is guarded."""
+    last message; guard: (skipped steps, last grad norm) when the step is guarded; ssim_loss: with cb+ssim, the SSIM
+    part of the loss (ssim_weight * (1 - SSIM), the mean over the 14 outputs; Video_base_model's 'ssim_loss')."""
     msg = "<epoch:{:3d}, iter:{:8,d}, lr:{:.3e}> ".format(epoch, step, lr)
     msg += "".join("{:s}: {:.4e} ".format(k, v) for k, v in zip([str(i) for i in range(NOUT)] + ["Al"], avg))
+    if ssim_loss is not None:
+        msg += "ssim_loss: {:.4e} ".format(ssim_loss)
     if guard is not None:
         skipped, norm = guard
         msg += "skipped: {:d} grad_norm: {} ".format(skipped, "n/a" if norm is None else "{:.4e}".format(norm))
@@ -417,8 +426,10 @@ class Trainer:
         self.step = 0
         if opts.resume_state:
             self._resume(opts.resume_state)
-        with torch.cuda.device(self.dev):
-            self.loss_sums = torch.zeros(NOUT + 1, dtype=torch.float32, device=self.dev)
+        self.ssim = opts.pixel_criterion == CB_SSIM
+        self._ssim_part: Optional[torch.Tensor] = None
+        with torch.cuda.device(self.dev):     # 14 losses, their mean and, with cb+ssim, the SSIM part
+            self.loss_sums = torch.zeros(NOUT + 1 + self.ssim, dtype=torch.float32, device=self.dev)
         self.loss_count = 0
         # --cuda_graph: the static batch buffer every batch is built into, then the graph and what it owns
         self._static: Optional[torch.Tensor] = None
@@ -456,11 +467,24 @@ class Trainer:
         self.log.info("Saving models and training states.")
 
     # ------------------------------------------------------------------ one iteration
+    def _loss(self, outs, batch: Dict) -> Tuple[torch.Tensor, List[torch.Tensor]]:
+        """The criterion of the yml on the 14 outputs.  With cb+ssim it also leaves the step's SSIM part (the mean
+        over the 14 outputs of ssim_weight * (1 - SSIM)) in self._ssim_part, on the device."""
+        if not self.ssim:
+            return pixel_loss(outs, gt_list(batch), self.o.pixel_criterion, nframes=6, version=self.o.version)
+        loss, losses, means = pixel_ssim_loss(outs, gt_list(batch), self.o.ssim_weight,
+                                              cycle_pairs=cycle_pairs_for(6, self.o.version))
+        self._ssim_part = self.o.ssim_weight * (1.0 - torch.stack(means).mean())
+        return loss, losses
+
+    def _sums_row(self, loss: torch.Tensor, losses: List[torch.Tensor]) -> torch.Tensor:
+        return torch.stack(list(losses) + [loss.detach()] + ([self._ssim_part] if self.ssim else []))
+
     def train_step(self, batch: Dict) -> Tuple[torch.Tensor, List[torch.Tensor]]:
         """bin_model.optimize_parameters on one batch: -> (loss, the 14 per-output losses), on the device."""
         self.opt.zero_grad(set_to_none=True)
         outs = self.model(*[batch["LQs"][:, k] for k in range(6)])
-        loss, losses = pixel_loss(outs, gt_list(batch), self.o.pixel_criterion, nframes=6, version=self.o.version)
+        loss, losses = self._loss(outs, batch)
         (self.o.pixel_weight * loss).backward()
         self.opt.step()
         return loss, losses
@@ -470,7 +494,7 @@ class Trainer:
         (the first iteration of a --cuda_graph run is its eager warm-up, and the capture follows it)."""
         if not self.cuda_graph:
             loss, losses = self.train_step(batch)
-            self.loss_sums += torch.stack(list(losses) + [loss.detach()])
+            self.loss_sums += self._sums_row(loss, losses)
         elif self._graph is not None:
             self.opt.replay(self._graph)
         else:
@@ -486,19 +510,20 @@ class Trainer:
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):
             loss, losses = self.train_step(batch)
-            self.loss_sums += torch.stack(list(losses) + [loss.detach()])
+            self.loss_sums += self._sums_row(loss, losses)
             rdn.take_workspace(self.dev)
         torch.cuda.current_stream().wait_stream(side)
         graph, capture = torch.cuda.CUDAGraph(), torch.cuda.Stream(self.dev)
         with torch.cuda.graph(graph, stream=capture):
             self.opt.zero_grad(set_to_none=False)
             outs = self.model(*[batch["LQs"][:, k] for k in range(6)])
-            loss, losses = pixel_loss(outs, gt_list(batch), self.o.pixel_criterion, nframes=6, version=self.o.version)
+            loss, losses = self._loss(outs, batch)
             (self.o.pixel_weight * loss).backward()
             self.opt.step()
-            self.loss_sums += torch.stack(list(losses) + [loss.detach()])
+            self.loss_sums += self._sums_row(loss, losses)
             ws = rdn.take_workspace(self.dev)
         del outs, loss, losses
+        self._ssim_part = None
         self._graph, self._graph_keep = graph, (ws, capture)
 
     def _batches(self) -> Iterator[Dict]:
@@ -561,7 +586,8 @@ class Trainer:
         if self.guarded:
             self.opt.resolve()
             guard = (self.opt.skipped_steps, self.opt.last_grad_norm)
-        self.log.info(train_message(self.epoch, self.step, self.opt.param_groups[0]["lr"], avg, guard))
+        self.log.info(train_message(self.epoch, self.step, self.opt.param_groups[0]["lr"], avg[:NOUT + 1], guard,
+                                    avg[NOUT + 1] if self.ssim else None))
         self.loss_sums.zero_()
         self.loss_count = 0
 
@@ -580,7 +606,7 @@ class Trainer:
                 continue
             b = vs.batch([i])
             outs = self.net(*[b["LQs"][:, k] for k in range(6)])
-            loss, lst = pixel_loss(outs, gt_list(b), self.o.pixel_criterion, nframes=6, version=self.o.version)
+            loss, lst = self._loss(outs, b)
             pairs = [(tensor2img_u8(outs[k][0]), tensor2img_u8(g[0])) for k, g in enumerate(gt_list(b))]
             rows.append(image_metrics_batch(pairs))
             losses.append(torch.stack(lst + [loss]))

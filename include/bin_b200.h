@@ -301,6 +301,25 @@ int bin_pixel_loss_fwd_ex(const float* const* a_host, const float* const* b_host
 int bin_pixel_loss_bwd(const float* const* a_host, const float* const* b_host, float* const* da_host, float* const* db_host,
                        int npairs, size_t n, int kind, float eps, const float* upstream, bin_stream_t s);
 
+/* ---- fused SSIM loss (pixel_criterion 'cb+ssim', DESIGN §4r) ------------------------------------------------ */
+/* npairs (<= BIN_MAX_LOSS_PAIRS) pairs of fp32 images of one shape: `planes` planes (B * C) of h x w each, h, w >= 11.
+ * ssim_sum[k] (device fp32[npairs]) = the sum over planes and the (h-10)(w-10) valid positions of the SSIM map of
+ * utils/util.py:211-231 (window outer(g, g), g = cv2.getGaussianKernel(11, 1.5)) with C1 = 0.01^2, C2 = 0.03^2: data
+ * range 1.  The mean SSIM is ssim_sum[k] / (planes (h-10)(w-10)).  maps (device, >= bin_ssim_loss_maps_bytes, or NULL):
+ * the per-position derivatives the backward reads.  flags: BIN_DETERMINISTIC sums each CTA's partial in index order
+ * through scratch (device, >= bin_ssim_loss_scratch_bytes; NULL fails with BIN_ERR_ARG, small with BIN_ERR_WORKSPACE);
+ * 0 adds the partials with float atomics (scratch unused). */
+size_t bin_ssim_loss_scratch_bytes(int npairs, int planes, int h, int w);
+size_t bin_ssim_loss_maps_bytes(int npairs, int planes, int h, int w);
+int bin_ssim_loss_fwd(const float* const* a_host, const float* const* b_host, int npairs, int planes, int h, int w,
+                      float* ssim_sum, float* maps, int flags, void* scratch, size_t scratch_bytes, bin_stream_t s);
+/* da_k += upstream[k] * d ssim_sum[k] / d a_k and db_k += upstream[k] * d ssim_sum[k] / d b_k (upstream: device
+ * fp32[npairs]; maps: what bin_ssim_loss_fwd wrote for the same a, b).  ADDS to da / db, so it follows
+ * bin_pixel_loss_bwd's writes on the same stream; db_host or single entries may be NULL.  The da / db buffers must not
+ * alias one another.  Each element has one writer: the result does not depend on the run. */
+int bin_ssim_loss_bwd(const float* const* a_host, const float* const* b_host, const float* maps, float* const* da_host,
+                      float* const* db_host, int npairs, int planes, int h, int w, const float* upstream, bin_stream_t s);
+
 /* ---- image boundary of the caller loop (SURVEY 8f rank 2) ------------------------------------ */
 /* utils/util.py:113-137 tensor2img + the crop of test.py:394-402 for ONE (3,Hs,Ws) fp32 RGB image:
  * clamp [0,1], *255, round-half-even, uint8 HWC BGR of the (top,left,h,w) window -> out (h*w*3 bytes, device). */
