@@ -19,6 +19,7 @@ from __future__ import annotations
 
 import logging
 import math
+from collections import defaultdict
 from typing import Callable, Dict, List, NamedTuple, Optional, Tuple
 
 import numpy as np
@@ -163,7 +164,15 @@ class Adam(torch.optim.Optimizer):
     graph.  With the guard, the skip, the clip and the count of skipped steps stay on the device; `resolve()`,
     `state_dict()` and `load_state_dict()` read them.  `loss_scale_backoff` is refused: the loss-scale target it moves is
     a host value that a replay would not see.  `state_dict()` gives CPU step tensors, as the default optimizer does, so
-    checkpoints of both load into either, and into torch.optim.Adam."""
+    checkpoints of both load into either, and into torch.optim.Adam.
+
+    `reset_state()`, or assigning a new `state` (`opt.state = defaultdict(dict)`, what the reference's
+    `MultiStepLR_Restart(clear_state=True)` does to torch.optim.Adam), drops every parameter's state: the next step
+    starts the moments and the step count from zero and gives the bits of a fresh Adam on the current parameters
+    (DESIGN §4s).  `step()` and `replay()` notice a reassigned `state`.  The moments and step counts are zeroed in place
+    (the moments, and capturable's device step count, stream-ordered) and the new `state` is bound to those tensors, so
+    the tables and a captured graph keep their pointers and no iteration synchronises; a guarded step still in flight is
+    resolved first (one host wait).  The device's count of skipped steps is kept."""
 
     def __init__(self, params, lr: float = 1e-3, betas: Tuple[float, float] = (0.9, 0.999), eps: float = 1e-8,
                  weight_decay: float = 0.0, max_grad_norm: Optional[float] = None, skip_nonfinite: bool = False,
@@ -194,6 +203,7 @@ class Adam(torch.optim.Optimizer):
         self._launched = False
         self._audit_params: List[torch.Tensor] = []
         self._audit_scale = 1.0
+        self._state_ref = self.state                   # the `state` the tables were built for (a new one is a reset)
 
     @property
     def skipped_steps(self) -> int:
@@ -222,8 +232,43 @@ class Adam(torch.optim.Optimizer):
     def load_state_dict(self, state_dict):
         self.resolve()
         super().load_state_dict(state_dict)
+        self._state_ref = self.state
         self._tables.clear()                           # exp_avg / exp_avg_sq / step tensors were replaced
         self._skip_base, self._seen_skipped = self._ledger.skipped_steps, 0
+
+    def reset_state(self) -> None:
+        """Drop every parameter's Adam state, as `opt.state = defaultdict(dict)` does (see the class docstring)."""
+        self.state = defaultdict(dict)
+        self._apply_reset()
+
+    def _apply_reset(self) -> None:
+        """Make the optimizer follow a `state` replaced since the last step: the moments and step counts of the old
+        state are zeroed in place and bound to the new one, so the tables (and a captured graph) keep their pointers and
+        no table is rebuilt.  Eager the zeroing is on the host (step counts) and stream-ordered (moments); capturable
+        the device step count of each group is filled with 0, stream-ordered too."""
+        if self.state is self._state_ref:
+            return
+        if torch.cuda.is_current_stream_capturing():
+            raise BinB200Error("bin_b200.optim.Adam: the optimizer's state was reset; run a step (or replay()) before a "
+                               "capture, so that the reset is not baked into the graph")
+        self._ledger.resolve()                         # a skipped step's undo must act on the counters before they are zeroed
+        old = self._state_ref
+        seen = set()
+        for st in old.values():
+            t = st["step"]                             # shared by a group's parameters (eager fast path, capturable)
+            if (t.device, t.data_ptr()) not in seen:
+                seen.add((t.device, t.data_ptr()))
+                with torch.cuda.device(t.device if t.is_cuda else None):
+                    t.zero_()
+        for tab in self._group_tables():
+            tab.step_value = 0.0
+        moments = [st[k] for st in old.values() for k in ("exp_avg", "exp_avg_sq")]
+        for dev in {m.device for m in moments}:
+            with torch.cuda.device(dev):
+                torch._foreach_zero_([m for m in moments if m.device == dev])
+        for p, st in old.items():
+            self.state[p] = {"step": st["step"], "exp_avg": st["exp_avg"], "exp_avg_sq": st["exp_avg_sq"]}
+        self._state_ref = self.state
 
     def add_param_group(self, param_group):
         if hasattr(self, "_tables"):
@@ -294,6 +339,7 @@ class Adam(torch.optim.Optimizer):
         if closure is not None:
             with torch.enable_grad():
                 loss = closure()
+        self._apply_reset()
         if self.capturable:
             self._step_capturable(grad_scale)
             return loss
@@ -450,7 +496,9 @@ class Adam(torch.optim.Optimizer):
     def replay(self, graph: "torch.cuda.CUDAGraph") -> None:
         """graph.replay() for a graph that captured step(): each group's current lr goes to the device first, and the
         parameters' versions are bumped afterwards, as an eager step bumps them, so that every packed-weight cache of
-        the package (forward and backward packs, the inference window's graph) sees the update."""
+        the package (forward and backward packs, the inference window's graph) sees the update.  A `state` reset since
+        the last step or replay is applied first."""
+        self._apply_reset()
         self.refresh_lr()
         graph.replay()
         for tab in self._group_tables():

@@ -12,6 +12,8 @@ write around bin_model, with every step of the hot path on the GPU:
   * validation every val_freq iterations at batch 1: the 14 losses and their mean, PSNR and SSIM of each output
     (utils/util.py calculate_psnr / calculate_ssim on tensor2img images), windows sharded over the ranks and the sums
     all-reduced; ReduceLROnPlateau steps on the mean validation loss;
+  * lr_scheme MultiStepLR or CosineAnnealingLR_Restart (lr_scheduler.py): update_learning_rate(step, warmup_iter)
+    before every iteration, step 1-based, so iteration k runs with the scheduler at last_epoch k (DESIGN §4s);
   * checkpoints `<iter>_G.pth` (base_model.save_network) and `<iter>.state` (save_training_state), and resume from
     them at the exact batch, crop and flip the saved run would have drawn next.
 
@@ -33,7 +35,9 @@ import logging
 import math
 import os
 import random
+import re
 import sys
+import warnings
 from dataclasses import dataclass, field
 from typing import Dict, Iterator, List, Optional, Sequence, Tuple
 
@@ -44,12 +48,14 @@ from . import rdn
 from ._lib import BIN_TRAIN_FRAMES, BinB200Error
 from .evaluate import load_weights
 from .loss import CB_SSIM, cycle_pairs_for, pixel_loss, pixel_ssim_loss
+from .lr_scheduler import CosineAnnealingLR_Restart, MultiStepLR_Restart, warm_up
 from .metrics import image_metrics_batch
 from .optim import Adam
 from .streaming import tensor2img_u8
 from .trainset import DeviceBINDataset, DeviceClip
 
 NOUT = 14
+PLATEAU, MULTISTEP, COSINE = "ReduceLROnPlateau", "MultiStepLR", "CosineAnnealingLR_Restart"
 # bin_model.get_info (nframes 6, bin_model.py:530-534): output k is scored against I_GT_OF[k]; feed_data maps I(2m+1) to
 # GTenh[:, m] and I(2m) to GTinp[:, m-1] (bin_model.py:164-174)
 I_GT_OF = (2, 4, 6, 8, 3, 5, 7, 4, 6, 5, 10, 9, 8, 7)
@@ -81,8 +87,8 @@ class Options:
     weight_decay: float
     pixel_criterion: str
     pixel_weight: float
-    factor: float
-    patience: int
+    factor: Optional[float]              # ReduceLROnPlateau only (None with the other schemes)
+    patience: Optional[int]
     epochs: int
     val_freq: int
     manual_seed: int
@@ -90,6 +96,15 @@ class Options:
     save_freq: int
     ignored: List[str] = field(default_factory=list)
     ssim_weight: Optional[float] = None   # train.ssim_weight: read, and required, with pixel_criterion cb+ssim only
+    lr_scheme: str = PLATEAU               # train.lr_scheme (DESIGN §4s); the keys below are read with MultiStepLR and
+    lr_steps: Optional[List[int]] = None   # CosineAnnealingLR_Restart only
+    lr_gamma: Optional[float] = None
+    clear_state: bool = False
+    T_period: Optional[List[int]] = None
+    eta_min: Optional[float] = None
+    restarts: Optional[List[int]] = None   # as the yml gives them (None: unset); a restart r happens at iteration r + 1
+    restart_weights: Optional[List[float]] = None
+    warmup_iter: int = -1
 
     @property
     def experiments_root(self) -> str:
@@ -119,18 +134,59 @@ def _path(p) -> Optional[str]:
     return None if p in (None, "") else os.path.expanduser(str(p))
 
 
+def _schedule_options(opt: dict, scheme: str) -> dict:
+    """The keys of MultiStepLR / CosineAnnealingLR_Restart, checked so that no configuration on which
+    bin_model's scheduler would fail part-way through training starts (DESIGN §4s)."""
+    def need(key: str):
+        v = _get(opt, "train." + key, None)
+        if v is None:
+            raise BinB200Error(f"train.{key} is missing: train.lr_scheme {scheme} needs it")
+        return v
+
+    def ints(key: str, v) -> List[int]:
+        if not isinstance(v, (list, tuple)):
+            raise BinB200Error(f"train.{key} must be a list (train.lr_scheme {scheme}), got {v!r}")
+        return [int(float(x)) for x in v]
+
+    restarts, weights = _get(opt, "train.restarts", None), _get(opt, "train.restart_weights", None)
+    restarts = ints("restarts", restarts) if restarts is not None else None
+    if weights is not None and not isinstance(weights, (list, tuple)):
+        raise BinB200Error(f"train.restart_weights must be a list (train.lr_scheme {scheme}), got {weights!r}")
+    weights = [float(w) for w in weights] if weights is not None else None
+    n_restarts, n_weights = len(restarts or [0]), len(weights or [1])       # unset or empty: one restart, weight 1
+    if n_restarts != n_weights:
+        raise BinB200Error(f"train.restarts ({n_restarts} restart(s)) and train.restart_weights ({n_weights} "
+                           f"weight(s)) differ in length: train.lr_scheme {scheme} pairs them")
+    out = dict(lr_scheme=scheme, restarts=restarts, restart_weights=weights,
+               warmup_iter=int(float(_get(opt, "train.warmup_iter", -1))))
+    if scheme == MULTISTEP:
+        out.update(lr_steps=ints("lr_steps", need("lr_steps")), lr_gamma=float(need("lr_gamma")),
+                   clear_state=bool(_get(opt, "train.clear_state", False)))
+    else:
+        T_period = ints("T_period", need("T_period"))
+        if len(T_period) < n_restarts + 1:
+            raise BinB200Error(f"train.T_period has {len(T_period)} entr{'y' if len(T_period) == 1 else 'ies'}; "
+                               f"train.lr_scheme {scheme} with {n_restarts} restart(s) needs {n_restarts + 1}"
+                               + ("" if restarts else " (with train.restarts unset, iteration 1 is a restart)"))
+        out.update(T_period=T_period, eta_min=float(need("eta_min")))
+    return out
+
+
 def parse_options(opt: dict) -> Options:
     """The honoured keys of a parsed train yml.  Raises BinB200Error naming the key for what this driver does not do:
-    another model than bin_stage4, nframes other than 6, another lr_scheme than ReduceLROnPlateau, ft_tsa_only, an
-    unknown pixel_criterion, cb+ssim without train.ssim_weight."""
+    another model than bin_stage4, nframes other than 6, an lr_scheme other than ReduceLROnPlateau, MultiStepLR and
+    CosineAnnealingLR_Restart or one missing a key it needs, ft_tsa_only, an unknown pixel_criterion, cb+ssim without
+    train.ssim_weight."""
     if _get(opt, "network_G.which_model_G") != "bin_stage4":
         raise BinB200Error(f"network_G.which_model_G: {_get(opt, 'network_G.which_model_G')!r} is not trained here; "
                            "only bin_stage4 is")
     if int(_get(opt, "network_G.nframes")) != 6:
         raise BinB200Error("network_G.nframes: only 6 (the 14-output bin_stage4 window) is trained here")
-    if _get(opt, "train.lr_scheme") != "ReduceLROnPlateau":
-        raise BinB200Error(f"train.lr_scheme: {_get(opt, 'train.lr_scheme')!r} is not supported; only "
-                           "ReduceLROnPlateau is")
+    scheme = _get(opt, "train.lr_scheme")
+    if scheme not in (PLATEAU, MULTISTEP, COSINE):
+        raise BinB200Error(f"train.lr_scheme: {scheme!r} is not supported; {PLATEAU}, {MULTISTEP} and {COSINE} are "
+                           "(bin_model.py:103-125)")
+    schedule = _schedule_options(opt, scheme) if scheme != PLATEAU else {}
     if _get(opt, "train.ft_tsa_only", None):
         raise BinB200Error("train.ft_tsa_only is not supported")
     crit = _get(opt, "train.pixel_criterion")
@@ -160,15 +216,16 @@ def parse_options(opt: dict) -> Options:
         weight_decay=float(_get(opt, "train.weight_decay_G", 0) or 0),     # bin_model.py:65
         pixel_criterion=crit,
         pixel_weight=float(_get(opt, "train.pixel_weight")),
-        factor=float(_get(opt, "train.factor")),
-        patience=int(_get(opt, "train.patience")),
+        factor=float(_get(opt, "train.factor")) if scheme == PLATEAU else None,
+        patience=int(_get(opt, "train.patience")) if scheme == PLATEAU else None,
         epochs=int(_get(opt, "train.epoch")),
         val_freq=int(float(_get(opt, "train.val_freq"))),
         manual_seed=int(_get(opt, "train.manual_seed")),
         print_freq=int(float(_get(opt, "logger.print_freq"))),
         save_freq=int(float(_get(opt, "logger.save_checkpoint_freq"))),
         ignored=[k for k in IGNORED if _get(opt, k, None) is not None],
-        ssim_weight=ssim_weight)
+        ssim_weight=ssim_weight,
+        **schedule)
 
 
 def load_options(path: str) -> Options:
@@ -334,6 +391,28 @@ def build_dataset(root: str, mode: str, device, lq_size, rng, from_sharp: bool) 
     return DeviceBINDataset.from_tree(root, mode=mode, device=device, lq_size=lq_size, rng=rng)
 
 
+def make_scheduler(opt: torch.optim.Optimizer, o: Options):
+    """bin_model.__init__'s scheduler for the yml's lr_scheme (bin_model.py:103-125)."""
+    if o.lr_scheme == MULTISTEP:
+        return MultiStepLR_Restart(opt, o.lr_steps, restarts=o.restarts, weights=o.restart_weights, gamma=o.lr_gamma,
+                                   clear_state=o.clear_state)
+    if o.lr_scheme == COSINE:
+        return CosineAnnealingLR_Restart(opt, o.T_period, restarts=o.restarts, weights=o.restart_weights,
+                                         eta_min=o.eta_min)
+    return torch.optim.lr_scheduler.ReduceLROnPlateau(opt, "min", factor=o.factor, patience=o.patience)
+
+
+def scheduler_kind(sd: dict) -> str:
+    """The lr_scheme whose scheduler wrote the state dict `sd` (its class's own keys tell them apart)."""
+    if "T_period" in sd:
+        return COSINE
+    if "milestones" in sd and "restart_weights" in sd:
+        return MULTISTEP
+    if "patience" in sd and "factor" in sd:
+        return PLATEAU
+    return "unknown"
+
+
 def graph_mode(requested: bool, world: int) -> bool:
     """Whether a run captures its training step: asked for, and not turned off by BIN_B200_GRAPH=0 (as inference's
     window graph is).  Refused with more than one rank: the step of a DistributedDataParallel run all-reduces through
@@ -347,7 +426,7 @@ def graph_mode(requested: bool, world: int) -> bool:
 # ----------------------------------------------------------------------------- the driver
 class Trainer:
     """One rank's training run.  `run()` trains to the end of the yml's epochs (or `max_iters` iterations in all);
-    `net` is the unwrapped module, `opt` the optimizer, `scheduler` the ReduceLROnPlateau.
+    `net` is the unwrapped module, `opt` the optimizer, `scheduler` the yml's lr_scheme (make_scheduler).
 
     rank / world default to the initialised process group, else (0, 1); the device is cuda:<LOCAL_RANK> under a
     process group, else the current device.  sync_debug: a torch.cuda.set_sync_debug_mode level under which every
@@ -416,8 +495,7 @@ class Trainer:
         if cuda_graph and not self.cuda_graph:
             self.log.info("BIN_B200_GRAPH=0: the training step runs eagerly")
         self.guarded = max_grad_norm is not None or skip_nonfinite
-        self.scheduler = torch.optim.lr_scheduler.ReduceLROnPlateau(self.opt, "min", factor=opts.factor,
-                                                                    patience=opts.patience)
+        self.scheduler = make_scheduler(self.opt, opts)
         self.model = self.net
         if self.world > 1:
             from torch.nn.parallel import DistributedDataParallel
@@ -445,6 +523,10 @@ class Trainer:
         if len(state["optimizers"]) != 1 or len(state["schedulers"]) != 1:
             raise BinB200Error(f"resume: {path} holds {len(state['optimizers'])} optimizers and "
                                f"{len(state['schedulers'])} schedulers; this driver has one of each")
+        saved = scheduler_kind(state["schedulers"][0])
+        if saved != self.o.lr_scheme:
+            raise BinB200Error(f"resume: {path} holds a {saved} scheduler, but the yml's train.lr_scheme is "
+                               f"{self.o.lr_scheme}")
         self.opt.load_state_dict(state["optimizers"][0])
         self.scheduler.load_state_dict(state["schedulers"][0])
         resume_position(int(state["epoch"]), int(state["iter"]), self.iters_per_epoch)
@@ -554,6 +636,8 @@ class Trainer:
                     if self.sync_debug is not None and not first:
                         torch.cuda.set_sync_debug_mode(self.sync_debug)
                     try:
+                        if o.lr_scheme != PLATEAU:
+                            self._update_learning_rate()
                         self._iterate(next(batches))
                     finally:
                         torch.cuda.set_sync_debug_mode(mode)
@@ -565,7 +649,8 @@ class Trainer:
                         self._print()
                     if "val" in ev and self.val_set is not None:
                         log = self.validate()
-                        self.scheduler.step(log[4])
+                        if o.lr_scheme == PLATEAU:
+                            self.scheduler.step(log[4])
                         self.log.info(val_message(self.epoch, self.step, log))
                     if "save" in ev:
                         self.save()
@@ -574,6 +659,15 @@ class Trainer:
                 self.save()
             torch.cuda.synchronize(self.dev)
         self.log.info("End of training.")
+
+    def _update_learning_rate(self) -> None:
+        """base_model.update_learning_rate(step, warmup_iter) before iteration `step` (1-based) runs: the scheduler
+        steps to last_epoch == step, then the warm-up.  The loop steps the scheduler before the optimizer on purpose,
+        so torch's warning about that order is not shown."""
+        with warnings.catch_warnings():
+            warnings.filterwarnings("ignore", message=re.escape("Detected call of `lr_scheduler.step()` before"))
+            self.scheduler.step()
+        warm_up(self.opt, self.step + 1, self.o.warmup_iter)
 
     @property
     def epoch(self) -> int:
